@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native ParticleSfM hot paths.
+"""bench.py — headline benchmark of the H100-native ParticleSfM hot paths.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--config 2..5]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one global bundle adjustment (HP2) of the BASELINE.json target workload
@@ -18,11 +19,17 @@ rotations + focal length refined).  `--config N` runs BASELINE.json's configs[N-
            result — all inside the timed region.
 The line also carries the HP1 number (trajectory optimiser, pts/s) under "traj_opt".
 
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step returned to its caller
+(the refined state, with N GPUs the points of every rank gathered; the step summary; rank 0's HP1 output)
+as DIR/<name>.npy, so that two builds can be compared output for output on the same seeded inputs.  With
+`--impl reference` the ba_* files hold the CPU arm's last solve.  HP1 is bit-reproducible; HP2 sums with
+unordered fp64 atomics, so two runs of the same build agree to ~1e-13 relative, not bit for bit.
+
 `--impl reference` times the CPU arm — the oracle's restatement of the reference's algorithm
 (Ceres LM + SPARSE_SCHUR: block-sparse Schur complement, band Cholesky; OpenMP, the best thread
 count of {8,16,32,64} <= min(ncpu, 64) — the reference's cap, sfm/main_sfm.py:144 — found by a
 short calibration, see cpu_threads()) — on the SAME workload, full size; the sample
-is only shrunk (and said so) when a full-size solve would not fit the driver's time budget.
+is only shrunk (and said so) when a full-size solve would not fit REFERENCE_BUDGET_S.
 """
 import argparse
 import ctypes as C
@@ -65,7 +72,57 @@ def read_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s; not measured)"
+
+
+def smi_device(index):
+    """nvidia-smi's name for CUDA device `index` of this process: its PCI address.  CUDA_VISIBLE_DEVICES renumbers
+    CUDA's ordinals but not nvidia-smi's indices, so an ordinal may name another GPU there."""
+    import torch
+    p = torch.cuda.get_device_properties(index)
+    return f"{p.pci_domain_id:08X}:{p.pci_bus_id:02X}:{p.pci_device_id:02X}.0"
+
+
+def gpu_info(device):
+    """Name and power limit of the device the numbers were measured on (part of every absolute number);
+    `device` as smi_device() gives it."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", device, "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
+    except (OSError, subprocess.SubprocessError):
+        return None
+    c = [x.strip() for x in out.split(",")]
+    return {"name": c[0], "power_limit": c[1], "sm_max_clock": c[2]} if len(c) == 3 else None
+
+
+DUMP_BYTES = 64 << 20            # --dump-outputs: at most this much in all
+
+
+def ba_outputs(p, s):
+    """What a caller of the BA solve receives: the refined state of problem p and the summary s."""
+    return {"ba_qvec": p.qvec, "ba_tvec": p.tvec, "ba_xyz": p.xyz, "ba_cam_params": p.cam_params,
+            "ba_summary": [s.initial_cost, s.final_cost, s.num_iterations, s.termination]}
+
+
+def dump_outputs(d, arrays):
+    """Writes each array as d/<name>.npy (float64, float32 when given so), at most DUMP_BYTES in all.  The
+    smallest arrays are written first; an array larger than an equal share of what is left is replaced by a
+    fixed, seeded sample of its rows, whose row numbers are written beside it as d/<name>_rows.npy."""
+    os.makedirs(d, exist_ok=True)
+    arrays = {k: np.asarray(v) for k, v in arrays.items()}
+    arrays = {k: v.astype(np.float32 if v.dtype == np.float32 else np.float64) for k, v in arrays.items()}
+    left = DUMP_BYTES
+    for i, name in enumerate(sorted(arrays, key=lambda k: arrays[k].nbytes)):
+        a = arrays[name]
+        share = left // (len(arrays) - i)
+        if a.nbytes > share:
+            k = max(1, share // (a.nbytes // a.shape[0] + 8))
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=k, replace=False))
+            np.save(os.path.join(d, f"{name}_rows.npy"), rows.astype(np.float64))
+            left -= 8 * k
+            a = a[rows]
+        np.save(os.path.join(d, f"{name}.npy"), a)
+        left -= a.nbytes
 
 
 class ClockSampler:
@@ -73,10 +130,10 @@ class ClockSampler:
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
 
-    def __init__(self, index=0):
+    def __init__(self, device):
         self.f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
         try:
-            self.p = subprocess.Popen(["nvidia-smi", "-i", str(index), f"--query-gpu={self.Q}",
+            self.p = subprocess.Popen(["nvidia-smi", "-i", device, f"--query-gpu={self.Q}",
                                        "--format=csv,noheader,nounits", "-lms", "20"], stdout=self.f,
                                       stderr=subprocess.DEVNULL)
         except OSError:
@@ -149,8 +206,8 @@ _CPU_THREADS = None
 
 def cpu_threads(w=None):
     """Threads of the CPU arm.  The reference takes min(cpu_count, 64) (ctx_init, sfm/main_sfm.py:144); on a
-    two-socket host the memory-bound sweeps stop scaling well before that (measured on the GPU box, 2 x 32
-    cores: 16 threads 3.2 M obs/s, 64 threads 1.9, profiles/r02_cpu_threads.md), so the arm is given the
+    two-socket host the memory-bound sweeps stop scaling well before that (on a 2 x 32-core
+    host the full workload ran faster on 16 threads than on 64), so the arm is given the
     BEST count of {8, 16, 32, 64} <= cpu_count, found with a short calibration solve on 1/10 of the
     workload — the CPU arm must not lose to its own thread count."""
     global _CPU_THREADS
@@ -245,13 +302,15 @@ def run_reference(args, rank, cfg):
                    "linear_solver": "exact step: block-sparse Schur complement + band Cholesky (SPARSE_SCHUR restatement, "
                                     "reference rule for <= 1000 images)",
                    "implementation": "oracle/ba_oracle.c (C + OpenMP, -O3 AVX2/FMA): the reference's algorithm restated — "
-                                     "Ceres/COLMAP cannot be built in this image (DESIGN.md §9)"},
+                                     "Ceres/COLMAP are not available to build (DESIGN.md §9)"},
         "lm_iterations_per_step": iters / len(times),
         "obs_iterations_per_sec": M * iters / total,
         "cpu_baseline": {"value": val, "unit": "observations/s", "cores": cores, "kind": "port", "sample": sample},
         "e2e": {"value": val, "unit": "observations/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
     }
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, ba_outputs(p, s))
     print(json.dumps(line), flush=True)
 
 
@@ -268,6 +327,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-traj", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -282,6 +343,7 @@ def main():
     if lib.psfm_device_count() <= 0:
         raise SystemExit("bench.py: no CUDA device — the product has no CPU path (use --impl reference for the CPU arm)")
     _lib.check(lib.psfm_set_device(local_rank), "psfm_set_device")
+    smi = smi_device(local_rank)
     dist = None
     if world > 1:
         import torch
@@ -327,7 +389,7 @@ def main():
         S.set_state(*init)
         return S.run(o)
 
-    sampler = ClockSampler(local_rank) if rank == 0 else None
+    sampler = ClockSampler(smi) if rank == 0 else None
     for _ in range(args.warmup):
         step()
     barrier()
@@ -348,6 +410,10 @@ def main():
     iters = sum(s.num_iterations for s in summaries) / len(summaries)
     lin_its = sum(s.num_linear_iterations for s in summaries) / len(summaries)
     S.get_state()
+    if args.dump_outputs and dist is not None:
+        from particlesfm_b200 import distributed
+        distributed.merge_points(prob, dist, world)      # every rank's points: the dump means the same at any N
+    dumps = ba_outputs(prob, s_last)
     ate = syn.umeyama_ate(syn.camera_centres(prob.qvec, prob.tvec), truth["centres"])
 
     # ---------------- rooflines (live CUDA events of this run) ----------------
@@ -388,22 +454,12 @@ def main():
         kernels["k_schur_pairs (image-pair blocks of the Schur complement)"] = dict(bound="hbm", ms=sum(s.schur_pairs_ms for s in summaries), n=n_expl,
                                                                                     bytes=288.0 * M_local + 8.0 * pairs_local)
 
-    # measured DRAM traffic per launch (ncu --set full capture of the headline workload at 1 GPU, this round's kernels)
-    traffic = {}
-    try:
-        if world == 1 and args.config == "target" and not args.points:
-            with open(os.path.join(ROOT, "profiles", "traffic_r02b.json")) as f:
-                traffic = json.load(f)
-    except (OSError, ValueError):
-        traffic = {}
-
     def roof(name):
         k = kernels[name]
         if k["n"] == 0 or k["ms"] <= 0:
             return None
         avg = k["ms"] / k["n"]
-        d = {"kernel": name, "bound": k["bound"], "avg_launch_ms": avg, "launches": k["n"], "share_of_step": k["ms"] / (1e3 * t_local),
-             "traffic": traffic.get(name.split(" ")[0])}
+        d = {"kernel": name, "bound": k["bound"], "avg_launch_ms": avg, "launches": k["n"], "share_of_step": k["ms"] / (1e3 * t_local)}
         if k["bound"] == "fp64":
             d.update({"peak": fp64_peak_tflops, "unit": "TFLOP/s", "peak_source": "measured in this run (psfm_measure_dfma: chip-wide DFMA rate x 2)",
                       "algorithmic_flops_per_launch": k["flops"], "achieved": k["flops"] / (avg * 1e-3) / 1e12})
@@ -469,7 +525,7 @@ def main():
                                      1: "exact step: explicit Schur complement + band Cholesky on the device (reference rule for <= 1000 images)"}
                    [s_last.linear_solver_used],
                    "parallelism": f"points sharded over {world} GPU(s); NCCL all-reduce of the camera-side accumulators / reduced system",
-                   "l2": "per-step working set (observations, linearisation, pair entries: ~0.7 GB) is larger than the 126 MB L2; no flush needed"},
+                   "l2": "per-step working set (observations, linearisation, pair entries: ~0.7 GB) is larger than the 50 MB L2; no flush needed"},
         "lm_iterations_per_step": iters, "pcg_iterations_per_step": lin_its,
         "obs_iterations_per_sec": M_total * sum(s.num_iterations for s in summaries) / t_total,
         "device_ms_per_step": sum(s.device_ms for s in summaries) / len(summaries),
@@ -478,6 +534,7 @@ def main():
         "e2e": {"value": e2e_val, "unit": "observations/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
                 "ms_per_step": 1e3 * sum(e2e_times) / len(e2e_times) if e2e_times else None},
         "gpu_launches": int(launches),
+        "gpu": gpu_info(smi),
         "clocks": clocks,
         "fp64_roof": {"dfma_per_s": dfma.value, "tflops": fp64_peak_tflops, "dependent_dfma_latency_cycles": dlat.value,
                       "how": "psfm_measure_dfma: 8 independent DFMA chains per thread, 8 CTAs x 256 threads per SM, best of 4"},
@@ -501,6 +558,7 @@ def main():
             if k >= args.warmup:
                 ts.append(time.perf_counter() - t0)
                 dev_ms.append(ssum.solve_ms)
+        dumps["traj_out"] = out
         t_call = max_over_ranks(statistics.mean(ts))
         t_dev = max_over_ranks(statistics.mean(dev_ms) * 1e-3)
         traj_bytes = 104.0 * n + 8.0 * TR["height"] * TR["width"]
@@ -525,6 +583,8 @@ def main():
             line["traj_opt"]["cpu_baseline"] = {"value": n / (time.perf_counter() - t0), "unit": "trajectories/s", "cores": 8,
                                                 "kind": "port", "sample": "same call, 8 threads (trajectory_optimize.cpp:79)"}
     if rank == 0:
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, dumps)
         print(json.dumps(line), flush=True)
     if dist is not None:
         lib.psfm_dist_finalize()

@@ -1,5 +1,5 @@
 /*
- * psfm_b200.h — C ABI of the B200-native ParticleSfM optimisation hot paths.
+ * psfm_b200.h — C ABI of the H100-native ParticleSfM optimisation hot paths.
  *
  * Two paths, nothing else (SURVEY.md §8):
  *

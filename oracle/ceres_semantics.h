@@ -4,7 +4,7 @@
  * TEST INFRASTRUCTURE (oracle).  Recalled from the published Ceres 2.0.0 sources
  * (internal/ceres/{trust_region_minimizer,levenberg_marquardt_strategy,dogleg_strategy,
  * conjugate_gradients_solver,corrector,loss_function}.cc, include/ceres/solver.h);
- * the sources are not in this container — see SURVEY.md Appendix A.
+ * the sources are not in the reference repository — see SURVEY.md Appendix A.
  */
 #ifndef PSFM_CERES_SEMANTICS_H_
 #define PSFM_CERES_SEMANTICS_H_

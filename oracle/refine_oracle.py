@@ -18,7 +18,7 @@ reference's Track / Point2D objects):
                              Retriangulate: out of scope, they change 0 observations here) and
                              AdjustGlobalBundle :215-243 / sfm/global_mapper.cc:402-448.
 
-COLMAP helpers that are NOT under /root/reference (COLMAP bd84ad6, base/projection.cc,
+COLMAP helpers that are NOT in the reference repository (COLMAP bd84ad6, base/projection.cc,
 base/triangulation.cc) are restated from their published source:
   HasPointPositiveDepth(P, X)            = P.row(2) . [X; 1] >= DBL_EPSILON
   CalculateSquaredReprojectionError      = DBL_MAX when (R X + t).z < DBL_EPSILON, else

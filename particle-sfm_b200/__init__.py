@@ -1,4 +1,4 @@
-"""B200-native ParticleSfM optimisation hot paths (HP1 path-consistency trajectory
+"""H100-native ParticleSfM optimisation hot paths (HP1 path-consistency trajectory
 optimiser, HP2 global bundle adjustment).  See DESIGN.md.
 
 The CUDA library is loaded lazily (first use); there is no CPU fallback: without the

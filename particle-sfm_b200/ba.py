@@ -45,7 +45,7 @@ class SolverOptions:
     max_num_consecutive_invalid_steps: int = 10
     max_consecutive_nonmonotonic_steps: int = 10   # inert: use_nonmonotonic_steps stays false
     num_threads: int = -1                          # meaningless on the GPU; kept for the surface
-    # B200 extensions (not in the reference): which reduced-system solve to use
+    # extensions (not in the reference): which reduced-system solve to use
     linear_solver: int = _abi.SOLVER_AUTO
     eta: float = 0.1
 

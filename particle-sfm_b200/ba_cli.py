@@ -1,4 +1,4 @@
-"""psfm_ba — global bundle adjustment of a COLMAP model directory on the B200 (HP2, boundary B3).
+"""psfm_ba — global bundle adjustment of a COLMAP model directory on the GPU (HP2, boundary B3).
 
     python -m particlesfm_b200.ba_cli --input_path M --output_path M' [options]
 

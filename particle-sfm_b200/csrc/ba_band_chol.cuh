@@ -203,10 +203,10 @@ __device__ __forceinline__ void bc_wait(const int* flag, int v) {
 }
 
 // bar.sync 0 from role-specific loops: every thread of the CTA executes the same NUMBER of
-// barriers, from different program counters.  Measured on B200: one warp runs dependent scalar
-// code at ~5 cycles per instruction, so what a role does per pivot is counted in instructions —
-// the first version (all roles interleaved in one unrolled body, index arithmetic per pivot)
-// took 1900 cycles per pivot.  Hence: per-role loops, compile-time shared-memory offsets,
+// barriers, from different program counters.  One warp runs dependent scalar code at several
+// cycles per instruction, so what a role does per pivot is counted in instructions — a first
+// version (all roles interleaved in one unrolled body, index arithmetic per pivot) was several
+// times slower per pivot.  Hence: per-role loops, compile-time shared-memory offsets,
 // one element per helper lane, no early exit.
 __device__ __forceinline__ void bc_bar() { asm volatile("bar.sync 0;\n" ::: "memory"); }
 
@@ -666,8 +666,8 @@ __device__ __forceinline__ void bc_pbar(int n) { asm volatile("bar.sync 2, %0;\n
 
 template <int MAXT, int TR, int TC>
 __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
-  // TR x TC: tile of a worker thread inside a 6 x 6 block (6 x 6: one thread per block; 3 x 6: two; 3 x 3: four).  Measured on B200
-  // (PSFM_CHOL_PROFILE): a warp executes ~1 instruction per 4.6 cycles whatever the dependences, so a step costs
+  // TR x TC: tile of a worker thread inside a 6 x 6 block (6 x 6: one thread per block; 3 x 6: two; 3 x 3: four).  A warp issues
+  // about one instruction per several cycles whatever the dependences (PSFM_CHOL_PROFILE shows it), so a step costs
   // what its LONGEST warp executes — many thin threads beat few fat ones as long as the CTA has room for them.
   extern __shared__ __align__(16) double bc_smem[];
   __shared__ int s_fail;
@@ -1197,7 +1197,7 @@ inline void band_chol_launch(BandCholArgs c, cudaStream_t st) {
     }                                                                                                              \
     k_band_chol6<MT, TRV, TCV><<<grid, MT, smem, st>>>(c);                                                               \
   } while (0)
-    // thin threads while the CTA has room for them (measured, profiles/r02_band_chol_notes.md), else one fat thread
+    // thin threads while the CTA has room for them (PSFM_CHOL_PROFILE shows why), else one fat thread
     // per block; the threads after the workers and the panel group are the loader (>= 32)
     static const int tile = getenv("PSFM_CHOL_TILE") ? atoi(getenv("PSFM_CHOL_TILE")) : 0;     // measurement: 33 | 36 | 66
     const int ng2 = ((2 * nblk + 31) & ~31) + np;

@@ -1,4 +1,4 @@
-// ba_kernels.cuh — sm_100a tile kernels of HP2 (global bundle adjustment), FACTORED-JACOBIAN
+// ba_kernels.cuh — sm_90a tile kernels of HP2 (global bundle adjustment), FACTORED-JACOBIAN
 // formulation.
 //
 // Replaces what ceres::Solve does inside BundleAdjuster::Solve

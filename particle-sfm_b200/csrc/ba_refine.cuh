@@ -14,7 +14,7 @@
 // (rebuild_structure in ba_solver.cu).  The reference's sequential DeleteObservation calls have
 // order-independent per-point outcomes, written here in closed form (oracle/refine_oracle.py
 // states and tests the same closed forms against hand-computed cases).
-// COLMAP helpers not under /root/reference (base/projection.cc, base/triangulation.cc @bd84ad6)
+// COLMAP helpers not in the reference repository (base/projection.cc, base/triangulation.cc @bd84ad6)
 // are restated: HasPointPositiveDepth (depth >= DBL_EPSILON), CalculateSquaredReprojectionError
 // (DBL_MAX when depth < DBL_EPSILON), CalculateTriangulationAngle (law of cosines, min(a, pi - a)).
 #pragma once

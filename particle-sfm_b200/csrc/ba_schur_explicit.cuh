@@ -259,10 +259,9 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
   const int tid = threadIdx.x;
   const double inv_f = (a.intr >= 1) ? 1.0 / __ldg(a.K) : 0.0;
   // Pair tasks of this tile -> lanes: two lanes share a task (q = 2 task + part; entries e0 + part, stride 2).
-  // Measured and dropped (round 2, profiles/r02_schur_tile_notes.md): runs cut into units of <= 8 entries so that
-  // all 8 warps carry pairs (more REDs: 1.11 -> 1.88 ms), three lanes per task (7 trips instead of 11 on the
-  // tile's critical path: 0.98 -> 1.05 ms) — the pair loop is bound by its fp64 instruction count, not by the
-  // longest lane.
+  // Tried and dropped, both slower: runs cut into units of <= 8 entries so that all 8 warps carry pairs (more
+  // REDs), three lanes per task (7 trips instead of 11 on the tile's critical path) — the pair loop is bound by
+  // its fp64 instruction count, not by the longest lane.
   constexpr int lpt = 2;
   const int nq = (a.dbg & 2) ? 0 : 2 * nt;
   auto lane_task = [&](int q, int& tq, int& par) -> bool {

@@ -421,11 +421,13 @@ int build_structure(psfm_ba_solver* S) {
     PSFM_LAUNCH_CHECK();
   }
   // pipeline form: packed tile headers, tile-relative point starts, 32-bit segment offsets
-  S->pipe = T > 0 && !getenv("PSFM_NO_PIPE");
-  if (S->pipe) {
+  {
     int dev = 0;
     PSFM_CUDA(cudaGetDevice(&dev));
     PSFM_CUDA(cudaDeviceGetAttribute(&S->sm_count, cudaDevAttrMultiProcessorCount, dev));
+  }
+  S->pipe = T > 0 && !getenv("PSFM_NO_PIPE");
+  if (S->pipe) {
     S->d_tile_hdr.alloc(2 * (size_t)T, st); S->d_pstart_rel.alloc((size_t)P + 1, st);
     S->d_cseg_off32.alloc((size_t)S->nseg + 1, st); S->d_seg_pose.alloc(PSFM_SPS * (size_t)S->nseg + 2, st); S->d_seg_pose.zero(st);
     k_pipe_headers<<<grid_for(T), 256, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_cseg_ptr.p, T, S->d_tile_hdr.p);
@@ -1366,9 +1368,9 @@ StepOut compute_step(psfm_ba_solver* S, const RunCfg& c, double radius, int* npr
     const size_t lin_smem = S->tile == 256 ? pipe_smem_linearize<256>(S->cap_ns, S->cap_np) : pipe_smem_linearize<512>(S->cap_ns, S->cap_np);
     auto bs_bytes = [&]() { return S->tile == 256 ? pipe_smem_back_substitute<256>(S->cap_ns, S->cap_np) : pipe_smem_back_substitute<512>(S->cap_ns, S->cap_np); };
     // fused cost (opt-in, PSFM_FUSED_COST=1): the candidate pose table (8 F doubles) lives in shared memory; at least
-    // two CTAs per SM must fit.  Measured on the bench workload: 16.61 ms per solve fused against 16.57 ms with the
-    // separate k_cost pass — the table and the second 16-byte stage cost the third resident CTA, which cancels the
-    // 0.085 ms of k_cost.  Kept for problems with few images; off by default.
+    // two CTAs per SM must fit.  Measured on the bench workload on an H100 SXM (700 W limit): 21.6 / 22.9 ms per solve
+    // fused against 21.0 / 21.8 ms with the separate k_cost pass (two runs each) — the table and the second 16-byte
+    // stage cost the third resident CTA, which more than cancels k_cost.  Kept for problems with few images; off by default.
     g_bs_fuse_F = no_fuse ? 0 : S->F;
     if (g_bs_fuse_F && !(pipe_ok(S, bs_bytes()) && (S->tile != 256 || 2 * (bs_bytes() + 1024) <= (size_t)227 * 1024))) g_bs_fuse_F = 0;
     const size_t bs_smem = bs_bytes();
@@ -1387,7 +1389,7 @@ StepOut compute_step(psfm_ba_solver* S, const RunCfg& c, double radius, int* npr
     ca.pose = S->d_pose[1 - S->cur].p; ca.X = S->d_X[1 - S->cur].p; ca.K = S->d_K[1 - S->cur].p;
     ca.loss.type = c.o.loss_function_type; ca.loss.a = c.o.loss_function_scale;
     ca.acc_cost = S->d_step.p + 3;
-    const unsigned g = (unsigned)std::min<size_t>(((size_t)S->M + 255) / 256, 148 * 8);
+    const unsigned g = (unsigned)std::min<size_t>(((size_t)S->M + 255) / 256, (size_t)S->sm_count * 8);
     k_cost<<<g, 256, 0, S->stream>>>(S->tc(), ca);
     PSFM_LAUNCH_CHECK();
   }

@@ -146,7 +146,7 @@ TrajectorySet set_from_dict(const std::map<int, py::dict>& in) {
 }  // namespace
 
 PYBIND11_MODULE(particlesfm, m) {
-  m.doc() = "point trajectories + path-consistency optimiser (B200 build)";
+  m.doc() = "point trajectories + path-consistency optimiser (H100 build)";
   m.def("optimize_location", &optimize_location, py::arg("uv12"), py::arg("uv_ref1"), py::arg("uv_ref2"),
         py::arg("ref2_scale"), py::arg("flow12_map"), py::arg("total_num"), py::arg("width"), py::arg("height"));
 

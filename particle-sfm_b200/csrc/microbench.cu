@@ -1,6 +1,6 @@
 // microbench.cu — measured fp64 roof of the device this library runs on.
 //
-// The driver's MEASURED_PEAKS.json carries an HBM copy bandwidth and a bf16 tensor rate; the
+// An optional MEASURED_PEAKS.json carries an HBM copy bandwidth and a bf16 tensor rate; the
 // kernels of this library compute in fp64 (the reference is Ceres: double everywhere), and the
 // ones that are not HBM-bound (the Schur-complement pair products, the band factorisation) are
 // bounded by the fp64 FMA pipe.  bench.py reports their roofline against THIS measurement:

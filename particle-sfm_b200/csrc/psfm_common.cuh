@@ -1,4 +1,4 @@
-// psfm_common.cuh — shared helpers of the sm_100a library (error handling, launch
+// psfm_common.cuh — shared helpers of the sm_90a library (error handling, launch
 // accounting, block reductions).  Product code: no CPU path lives here.
 #pragma once
 #include <cuda_runtime.h>

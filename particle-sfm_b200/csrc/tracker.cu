@@ -15,7 +15,7 @@
 //     out = fma(v_se, w n, fma(v_sw, e n, fma(v_ne, w s, v_nw * (e s))))
 // in float32 — established by comparing a numpy emulation with torch on 10^5 random samples (0 bit
 // differences; the plain sum and the other fma orders differ in ~70 % of the samples), and re-checked
-// against torch itself on the GPU box by tests/test_gpu_tracker.py.  Every float32 operation below is
+// against torch itself on the GPU by tests/test_gpu_tracker.py.  Every float32 operation below is
 // an explicit round-to-nearest intrinsic, immune to -fmad.  torch.norm over the 2 flow channels is
 // sqrt(a*a + b*b) without fma.  The distance transform is only ever compared with the integer
 // sample_ratio: dist > r  <=>  no occupied pixel within squared distance r^2 — exact in integers.

@@ -1,4 +1,4 @@
-// traj_solver.cu — HP1: path-consistency trajectory optimiser on sm_100a.
+// traj_solver.cu — HP1: path-consistency trajectory optimiser on sm_90a.
 //
 // Drop-in target: particlesfm::optimize_location
 //   (reference point_trajectory/optimize/src/trajectory_optimize.cpp:30-96): N residual

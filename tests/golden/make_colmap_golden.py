@@ -1,8 +1,8 @@
 """Writes tests/golden/colmap_model/{cameras,images,points3D}.bin with the REFERENCE's own
-writer (/root/reference/sfm/colmap_utils/read_write_model.py:447-456, imported read-only) from
+writer (the reference's sfm/colmap_utils/read_write_model.py:447-456, imported read-only) from
 the values of colmap_model_def.py, and checks that the reference's reader gets them back.
 
-    python tests/golden/make_colmap_golden.py       # only in the build container
+    PSFM_REFERENCE=/path/to/particle-sfm python tests/golden/make_colmap_golden.py
 """
 import os
 import sys
@@ -11,7 +11,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
-sys.path.insert(0, "/root/reference/sfm/colmap_utils")
+sys.path.insert(0, os.path.join(os.environ["PSFM_REFERENCE"], "sfm", "colmap_utils"))
 
 
 def main():

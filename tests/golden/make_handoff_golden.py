@@ -1,9 +1,9 @@
 """Generates tests/golden/handoff_small.npz by running the REFERENCE's own
-`traj_to_matches` (/root/reference/sfm/matches_from_flow.py:51-118, imported read-only) on
+`traj_to_matches` (the reference's sfm/matches_from_flow.py:51-118, imported read-only) on
 a small synthetic track file.  Pins keypoint order / indices, match lists and their order
 and the pair-list order of particlesfm_b200.handoff.traj_to_matches.
 
-    python tests/golden/make_handoff_golden.py       # only in the build container
+    PSFM_REFERENCE=/path/to/particle-sfm python tests/golden/make_handoff_golden.py
 """
 import os
 import sys
@@ -11,7 +11,7 @@ import tempfile
 
 import numpy as np
 
-REF = "/root/reference"
+REF = os.environ["PSFM_REFERENCE"]            # a ParticleSfM checkout
 
 
 def make_tracks(num_images=36, num_traj=160, seed=21):

@@ -1,8 +1,8 @@
 """Generates tests/golden/import_small.npz by running the REFERENCE's import_keypoints_matches
-(/root/reference/sfm/import_feature_matches.py:76-104) on a COLMAP database created by the reference's own
+(the reference's sfm/import_feature_matches.py:76-104) on a COLMAP database created by the reference's own
 COLMAPDatabase (sfm/colmap_utils/database.py), with `traj_to_matches` replaced by a function that returns the
 match data of tests/golden/handoff_small.npz's trajectories (the reference function reads trajectory FILES; the
-rest — keypoint shift, pair de-duplication, blobs — runs unmodified).  Run in the build container only:
+rest — keypoint shift, pair de-duplication, blobs — runs unmodified).  Needs a ParticleSfM checkout at $PSFM_REFERENCE:
     python tests/golden/make_import_golden.py
 """
 import os
@@ -16,8 +16,8 @@ import numpy as np
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference/sfm")
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.path.join(os.environ["PSFM_REFERENCE"], "sfm"))
+sys.path.insert(0, os.environ["PSFM_REFERENCE"])
 
 
 def main():

@@ -1,11 +1,11 @@
 """Generates tests/golden/tracker_small.npz by running the REFERENCE's own Python tracker
-(/root/reference/point_trajectory/track_optimize.py, imported read-only) on a small synthetic
+(the reference's point_trajectory/track_optimize.py, imported read-only) on a small synthetic
 flow sequence.  The reference's native module is replaced by a stub whose `Trajectory` is
 this repo's pybind11 class and whose `optimize_location` is the CPU oracle (the reference's
 Ceres build is unavailable here — SURVEY.md §8c), so the fixture pins the TRACKER semantics
 (sampling, survival test, re-seeding, id order), not the optimiser.
 
-    python tests/golden/make_tracker_golden.py       # only in the build container
+    PSFM_REFERENCE=/path/to/particle-sfm python tests/golden/make_tracker_golden.py
 """
 import os
 import sys
@@ -16,7 +16,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "particle-sfm_b200"))
-REF = "/root/reference"
+REF = os.environ["PSFM_REFERENCE"]            # a ParticleSfM checkout
 
 
 def make_sequence(n_frames=7, h=36, w=52, seed=11):

@@ -35,7 +35,7 @@ def test_bit_exact_vs_oracle(gpu, n, h, w, seed):
                                         (5000, 128, 256, 4), (70001, 218, 512, 5)])
 def test_against_reference_dump_when_present(gpu, n, h, w, seed):
     """Outputs of the REAL reference module (Ceres 2.0.0), dumped by oracle/ref_recipe/dump_ref_vectors.py
-    on a machine that can build it.  Not available in this image: skipped until the files exist."""
+    on a machine that can build it.  Skipped until the files exist."""
     import hashlib
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", f"ref_traj_{n}_{h}_{w}_{seed}.npz")
     if not os.path.exists(path):

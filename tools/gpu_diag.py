@@ -1,4 +1,4 @@
-"""Step-by-step diagnostic for GPU box runs (prints, never swallows)."""
+"""Step-by-step diagnostic for GPU runs (prints, never swallows)."""
 import ctypes as C
 import os
 import sys
