@@ -276,6 +276,8 @@ typedef struct {
   int64_t num_pair_entries;          /* observation pairs of the Schur complement on this rank */
   int32_t num_pair_tasks;            /* (tile, image pair) runs of those entries */
   int32_t explicit_fused;            /* 1: k_schur_tile, 0: k_schur_w + k_schur_pairs */
+  int32_t explicit_dense_tiles;      /* k_schur_tile tiles whose pair blocks are one dense tensor-core
+                                        product (the others run the pair loop) */
 } psfm_ba_summary;
 
 void psfm_ba_default_options(psfm_ba_options* o);          /* bundle_adjustment.h defaults */

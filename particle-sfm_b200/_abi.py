@@ -139,6 +139,7 @@ class BASummary(C.Structure):
         ("num_pair_entries", C.c_int64),
         ("num_pair_tasks", C.c_int32),
         ("explicit_fused", C.c_int32),
+        ("explicit_dense_tiles", C.c_int32),
     ]
 
     def as_dict(self):

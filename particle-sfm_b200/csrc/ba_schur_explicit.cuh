@@ -248,16 +248,115 @@ struct StArgs {
   double* Sband;                 // [nrep][F * (span + 1) * 36]
   size_t band_stride;
   int nrep_mask;
-  int dbg;      // PSFM_SCHUR_FLAGS (measurement only): 1 = no band REDs, 2 = no pair loop
+  int span;
+  const unsigned char* tile_dense;   // [T] pair phase of the tile: TILE_PAIRS_LOOP | _DENSE | _DENSE_DUP
+  int dbg;      // PSFM_SCHUR_FLAGS (measurement only): 1 = no band REDs, 2 = no pair phase
 };
 
+// ---- dense pair phase (tensor cores)
+//
+// For a point p with H~_p = L_p L_p' (3x3 Cholesky) and its observation i, Z_i = W_i L_p (6 x 3);
+// then (W_i H~) W_j' = Z_i Z_j', and a tile's pair blocks are the block-upper part of Z Z' with
+// Z = (6 ns) x (3 np): block (image segment s, point p) = sum of Z_i over the observations of p in
+// s (two observations of p in one image give Z_i + Z_j, i.e. all their cross terms).  Z is staged
+// in the dead reduction rows, zero-padded to 16-row blocks and 8-column pairs of k-steps, in the
+// fragment order of mma.m16n8k4.f64: lane l of a warp holds Z[8 q + l / 4][4 k + l % 4] of 8-row
+// block q at k-step k, and for Z Z' the A and B operands use that same layout.  Element
+// (row, col) lives at ((q * KB2 + k / 2) * 32 + (l ^ (q & 7))) * 2 + k % 2: one LDS.128 per lane
+// reads two k-steps of a fragment, a warp reads 512 contiguous bytes (no bank conflicts).  The XOR
+// spreads the stores: the observations of one point are rows 6 s + r, all of one parity, and would
+// otherwise write one bank.
+enum : unsigned char { TILE_PAIRS_LOOP = 0, TILE_PAIRS_DENSE = 1, TILE_PAIRS_DENSE_DUP = 2 };
+
+__host__ __device__ inline int dense_z_kb2(int np) { return (3 * np + 7) >> 3; }
+__host__ __device__ inline int dense_z_rb(int ns) { return (6 * ns + 15) >> 4; }
+// doubles of the staged Z of a tile with ns image segments and np points
+__host__ __device__ inline size_t dense_z_doubles(int ns, int np) { return (size_t)dense_z_rb(ns) * dense_z_kb2(np) * 128; }
+
+__device__ __forceinline__ void dmma_16x8x4(double (&d)[4], double a0, double a1, double b) {
+  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+      : "d"(a0), "d"(a1), "d"(b));
+}
+
+// L = chol(H~) of a packed symmetric 3x3 [h00 h01 h02 h11 h12 h22], L packed [l00 l10 l11 l20 l21 l22];
+// false when a pivot is not positive and finite
+__device__ __forceinline__ bool chol3(const double (&h)[6], double (&l)[6]) {
+  const double d0 = h[0];
+  l[0] = sqrt(d0);
+  l[1] = h[1] / l[0];
+  l[3] = h[2] / l[0];
+  const double d1 = h[3] - l[1] * l[1];
+  l[2] = sqrt(d1);
+  l[4] = (h[4] - l[3] * l[1]) / l[2];
+  const double d2 = h[5] - l[3] * l[3] - l[4] * l[4];
+  l[5] = sqrt(d2);
+  auto ok = [](double d) { return d > 0.0 && !isinf(d); };
+  return ok(d0) && ok(d1) && ok(d2);
+}
+
+// Z Z' of the staged tile -> band blocks.  Warps take 16 x 16 output blocks (I <= J) of the
+// block-upper part; per k-step pair 4 LDS.128 and 4 DMMA.16x8x4.  An element (r, c) goes to
+// Sband[img(r)][img(c) - img(r)][r % 6][c % 6] when img(r) <= img(c) and its 8-row tile is not
+// below the column's; a diagonal image block straddling two 8-row tiles also takes the mirror of
+// the upper tile's elements (the lower tile is not computed).  Exact zeros (images that share no
+// point of the tile) are not sent.
+template <int TILE>
+__device__ __forceinline__ void dense_pairs_mma(const double* __restrict__ zf, const int* __restrict__ cimg, int ns, int np,
+                                                double* __restrict__ band, int span, bool red) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int R = 6 * ns, RB = dense_z_rb(ns), KB2 = dense_z_kb2(np);
+  const int nblk = RB * (RB + 1) / 2;
+  const double2* z2 = reinterpret_cast<const double2*>(zf);
+  for (int blk = warp; blk < nblk; blk += TILE / 32) {
+    int I = 0, rem = blk;
+    while (rem >= RB - I) { rem -= RB - I; ++I; }
+    const int J = I + rem;
+    const double2* pa0 = z2 + (size_t)(2 * I) * KB2 * 32 + (lane ^ ((2 * I) & 7));
+    const double2* pa1 = z2 + (size_t)(2 * I + 1) * KB2 * 32 + (lane ^ ((2 * I + 1) & 7));
+    const double2* pb0 = z2 + (size_t)(2 * J) * KB2 * 32 + (lane ^ ((2 * J) & 7));
+    const double2* pb1 = z2 + (size_t)(2 * J + 1) * KB2 * 32 + (lane ^ ((2 * J + 1) & 7));
+    double acc[2][4];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[h][e] = 0.0;
+#pragma unroll 2
+    for (int k = 0; k < KB2; ++k) {
+      const double2 a0 = pa0[32 * k], a1 = pa1[32 * k], b0 = pb0[32 * k], b1 = pb1[32 * k];
+      dmma_16x8x4(acc[0], a0.x, a1.x, b0.x);
+      dmma_16x8x4(acc[1], a0.x, a1.x, b1.x);
+      dmma_16x8x4(acc[0], a0.y, a1.y, b0.y);
+      dmma_16x8x4(acc[1], a0.y, a1.y, b1.y);
+    }
+    if (!red) continue;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const double v = acc[h][e];
+        const int r = 16 * I + (lane >> 2) + 8 * (e >> 1), c = 16 * J + 8 * h + 2 * (lane & 3) + (e & 1);
+        if (v == 0.0 || r >= R || c >= R || (r >> 3) > (c >> 3)) continue;
+        const int sr = r / 6, sc = c / 6;
+        if (sr > sc) continue;
+        const int ia = cimg[sr], d = cimg[sc] - ia;
+        if (d > span) continue;
+        double* blkp = band + ((size_t)ia * (span + 1) + d) * 36;
+        atomicAdd(blkp + 6 * (r - 6 * sr) + (c - 6 * sc), v);
+        if (sr == sc && (r >> 3) < (c >> 3)) atomicAdd(blkp + 6 * (c - 6 * sc) + (r - 6 * sr), v);
+      }
+  }
+}
+
 // One tile of the fused Schur kernel; shared memory holds the staged inputs (see linearize_tile).
+// rep is the tile's index.
 template <int TILE, bool ROT>
 __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs& a, TileSmem<TILE>& sm, const TileInfo& ti,
                                                 const bool act, const int ls, const int lp, const double a00, const double a02,
                                                 const double a12, const int rep, const int t0, const int nt) {
   const int tid = threadIdx.x;
   const double inv_f = (a.intr >= 1) ? 1.0 / __ldg(a.K) : 0.0;
+  const unsigned char mode = (a.dbg & 2) ? TILE_PAIRS_LOOP : __ldg(a.tile_dense + rep);
   // Pair tasks of this tile -> lanes: two lanes share a task (q = 2 task + part; entries e0 + part, stride 2).
   // Tried and dropped, both slower: runs cut into units of <= 8 entries so that all 8 warps carry pairs (more
   // REDs), three lanes per task (7 trips instead of 11 on the tile's critical path) — the pair loop is bound by
@@ -283,6 +382,7 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
   double rec[18];
 #pragma unroll
   for (int k = 0; k < 18; ++k) rec[k] = 0.0;
+  bool pivot_bad = false;
   if (act) {
     ObsGeom g;
     load_geom<TILE>(sm, ls, lp, g);
@@ -290,6 +390,10 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
     double hv[6], wkp[3], wh[3];
 #pragma unroll
     for (int k = 0; k < 6; ++k) hv[k] = sm.prow(3 + k)[lp];
+    if (mode != TILE_PAIRS_LOOP) {
+      double lh[6];
+      pivot_bad = !chol3(hv, lh);
+    }
 #pragma unroll
     for (int k = 0; k < 3; ++k) { wkp[k] = sm.prow(9 + k)[lp]; wh[k] = sm.prow(12 + k)[lp]; }
     double jp[2][3], jc[2][6], Q[2][3];
@@ -340,7 +444,8 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
 #pragma unroll
     for (int r = (ROT ? 0 : 3); r < 6; ++r) sv[(21 + r) * PSFM_SVS] = -(jc[0][r] * pw0 + jc[1][r] * pw1);   // -(W w^)
   }
-  __syncthreads();
+  // a point whose H~ has no Cholesky factor sends the whole tile to the pair loop
+  const bool dense = !__syncthreads_or(pivot_bad) && mode != TILE_PAIRS_LOOP;
   {
     double* dst = a.acc_cam + (size_t)(rep & (NREP - 1)) * a.rep_stride;
     tile_reduce_images<TILE>(sm, ti, NVX2, [&](int k, int img, double acc) {
@@ -348,6 +453,51 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
     });
   }
   __syncthreads();
+  double* band = a.Sband + (size_t)(rep & a.nrep_mask) * a.band_stride;
+  if (dense) {
+    // the reduction rows are dead: stage Z (zero blocks where a point has no observation)
+    double* zf = sm.sv;
+    const int nz2 = (int)(dense_z_doubles(ti.ns, ti.np) / 2);
+    for (int k = tid; k < nz2; k += TILE) reinterpret_cast<double2*>(zf)[k] = make_double2(0.0, 0.0);
+    __syncthreads();
+    if (act) {
+      // Z_i = Jc' (Jp L): Jc from the record as in the per-observation phase above; L is recomputed
+      // here rather than kept live through the reduction (register pressure)
+      double hv[6], lh[6];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) hv[k] = sm.prow(3 + k)[lp];
+      chol3(hv, lh);
+      const double w0 = rec[3], w1 = rec[4], w2 = rec[5];
+      double jl[2][3], jc[2][6];
+#pragma unroll
+      for (int m = 0; m < 2; ++m) {
+        const double p0 = rec[12 + 3 * m], p1 = rec[13 + 3 * m], p2 = rec[14 + 3 * m];
+        jl[m][0] = p0 * lh[0] + p1 * lh[1] + p2 * lh[3];
+        jl[m][1] = p1 * lh[2] + p2 * lh[4];
+        jl[m][2] = p2 * lh[5];
+      }
+      if (ROT) {
+        jc[0][0] = 2.0 * a02 * w1; jc[0][1] = 2.0 * (a00 * w2 - a02 * w0); jc[0][2] = -2.0 * a00 * w1;
+        jc[1][0] = 2.0 * (a12 * w1 - a00 * w2); jc[1][1] = -2.0 * a12 * w0; jc[1][2] = 2.0 * a00 * w0;
+      }
+      jc[0][3] = a00; jc[0][4] = 0.0; jc[0][5] = a02;
+      jc[1][3] = 0.0; jc[1][4] = a00; jc[1][5] = a12;
+      const int KB2 = dense_z_kb2(ti.np);
+#pragma unroll
+      for (int r = (ROT ? 0 : 3); r < 6; ++r)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          const int row = 6 * ls + r, col = 3 * lp + k;
+          const int q = row >> 3;
+          double* z = zf + (((q * KB2 + (col >> 3)) * 32 + (((row & 7) * 4 + (col & 3)) ^ (q & 7))) * 2 + ((col >> 2) & 1));
+          const double v = jc[0][r] * jl[0][k] + jc[1][r] * jl[1][k];
+          if (mode == TILE_PAIRS_DENSE_DUP) atomicAdd(z, v); else *z = v;
+        }
+    }
+    __syncthreads();
+    dense_pairs_mma<TILE>(zf, sm.cimg, ti.ns, ti.np, band, a.span, !(a.dbg & 1));
+    return;
+  }
   // first entries of the first pass (three in flight per lane: one trip is shorter than an L2 round trip)
   unsigned int uf0 = 0u, uf1 = 0u, uf2 = 0u;
   {
@@ -364,7 +514,6 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
     for (int k = 0; k < 9; ++k) o[k] = make_double2(rec[2 * k], rec[2 * k + 1]);
   }
   __syncthreads();
-  double* band = a.Sband + (size_t)(rep & a.nrep_mask) * a.band_stride;
   // Pair tasks.  Block(i, j) = (W_i H~) W_j' = Jc_i' M Jc_j with the 2x2 M = Q_i Jp_j': per
   // entry 12 16-byte shared-memory loads (ncu, round 2: 64 % of the L1 data-pipe cycles with 24 8-byte loads at a
   // 19-double stride, the busiest unit of the kernel) and ~110 flops.  Two lanes per task (even | odd entries), the full 6x6 block in
@@ -554,6 +703,23 @@ __global__ void k_pair_fill_tile(const int* pt_ptr, const int* obs_pt, const int
     keys[o] = khi | a;
     vals[o] = ((unsigned)(j - base) << 16) | (unsigned)(k - base);
   }
+}
+
+// pair phase of every tile: dense (Z Z' on tensor cores) when allowed and its Z fits the reduction rows
+// (zcap doubles), else the pair loop; tiles with two observations of a point in one image accumulate
+// Z with shared-memory atomics.  ndense counts the dense tiles.
+__global__ void k_tile_pairs_mode(const int* tile_start, const int* tile_pt, const int* cseg_ptr, const int* obs_pt,
+                                  const int* obs_img, int T, size_t zcap, int allow, unsigned char* mode, int* ndense) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= T) return;
+  unsigned char m = TILE_PAIRS_LOOP;
+  if (allow && dense_z_doubles(cseg_ptr[t + 1] - cseg_ptr[t], tile_pt[t + 1] - tile_pt[t]) <= zcap) {
+    m = TILE_PAIRS_DENSE;
+    for (int j = tile_start[t] + 1; j < tile_start[t + 1]; ++j)
+      if (obs_pt[j] == obs_pt[j - 1] && obs_img[j] == obs_img[j - 1]) { m = TILE_PAIRS_DENSE_DUP; break; }
+    atomicAdd(ndense, 1);
+  }
+  mode[t] = m;
 }
 
 // first entry of every tile (entries are written in observation order, tiles are observation ranges)

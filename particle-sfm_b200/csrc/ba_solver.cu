@@ -172,6 +172,8 @@ struct psfm_ba_solver {
   DBuf<int> d_task_slot, d_tile_task;
   DBuf<int2> d_task_rng;
   DBuf<double> d_xband, d_bandrep;      // d_xband = [xcam F*NVX2 | Sband band_n] (one all-reduce)
+  DBuf<unsigned char> d_tile_pairs;     // [T] pair phase of each tile (TILE_PAIRS_*)
+  int ndense = 0;                       // tiles whose pair phase is the dense product
   // single-CTA sliding-window band Cholesky (ba_band_chol.cuh): compact band matrix, factor, scratch
   bool band_chol = false;
   BandWork bwk;             // plan + buffers of k_band_chol
@@ -984,7 +986,7 @@ void ensure_pairs(psfm_ba_solver* S) {
     S->fused = h < 0.5;
   }
   if (M == 0 && S->fused) {   // nothing to contribute: zero accumulators that still take part in the all-reduces
-    S->ntasks = 0;
+    S->ntasks = 0; S->ndense = 0;
     S->band_n = (size_t)F * (S->span + 1) * 36; S->band_nrep = 1;
     S->d_xband.alloc((size_t)F * NVX2 + S->band_n, st);
     S->d_bandrep.alloc(S->band_n, st); S->d_bandrep.zero(st);
@@ -1073,6 +1075,21 @@ void ensure_pairs(psfm_ba_solver* S) {
     }
     k_tile_tasks<<<grid_for((size_t)T + 1), 256, 0, st>>>(key2_out.p, nt, T, S->d_tile_task.p);
     PSFM_LAUNCH_CHECK();
+    {
+      // PSFM_SCHUR_PAIRS=loop keeps every tile on the pair loop (measurement and tests); by default every
+      // tile whose Z fits the reduction rows takes the dense product
+      const char* e = getenv("PSFM_SCHUR_PAIRS");
+      const int allow = (e && !strcmp(e, "loop")) ? 0 : 1;
+      const size_t zcap = (size_t)NVX2 * (S->tile + 1);
+      DBuf<int> nd; nd.alloc(1, st); nd.zero(st);
+      S->d_tile_pairs.alloc((size_t)std::max(T, 1), st);
+      if (T > 0) {
+        k_tile_pairs_mode<<<grid_for(T), 256, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_cseg_ptr.p, S->d_obs_pt.p,
+                                                       S->d_obs_img.p, T, zcap, allow, S->d_tile_pairs.p, nd.p);
+        PSFM_LAUNCH_CHECK();
+      }
+      PSFM_CUDA(cudaMemcpyAsync(&S->ndense, nd.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    }
     S->band_n = (size_t)F * (S->span + 1) * 36;
     int nrep = 8;   // the pair-task REDs are spread over many band blocks: few replicas suffice (fold cost grows with them)
     while (nrep > 1 && S->band_n * nrep * sizeof(double) > ((size_t)256 << 20)) nrep >>= 1;
@@ -1237,6 +1254,7 @@ void do_explicit_solve_fused(psfm_ba_solver* S, const RunCfg& c, double radius) 
   w.K = S->d_K[S->cur].p; w.acc_cam = S->d_xcamrep.p; w.rep_stride = nx; w.intr = c.intr;
   w.entries = S->d_tentries.p; w.task_slot = S->d_task_slot.p; w.task_rng = S->d_task_rng.p; w.tile_task = S->d_tile_task.p;
   w.Sband = S->d_bandrep.p; w.band_stride = S->band_n; w.nrep_mask = S->band_nrep - 1;
+  w.span = S->span; w.tile_dense = S->d_tile_pairs.p;
   { static const int dbg = getenv("PSFM_SCHUR_FLAGS") ? atoi(getenv("PSFM_SCHUR_FLAGS")) : 0; w.dbg = dbg; }
   auto mark = [&](std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& v, bool begin) {
     cudaEvent_t e = S->events.get();
@@ -1586,6 +1604,7 @@ int run_impl(psfm_ba_solver* S, const psfm_ba_options* opts, psfm_ba_summary* ou
   for (auto& e : S->ev_chol) { PSFM_CUDA(cudaEventElapsedTime(&ms, e.first, e.second)); s.cholesky_ms += ms; }
   s.num_explicit_solves = (int)S->ev_chol.size();
   s.num_pair_entries = S->npairs; s.num_pair_tasks = S->ntasks; s.explicit_fused = S->fused ? 1 : 0;
+  s.explicit_dense_tiles = S->fused ? S->ndense : 0;
   s.num_linearize = (int)S->ev_lin.size();
   s.num_schur_products = (int)S->ev_sp.size();
   s.num_iterations = iteration;
