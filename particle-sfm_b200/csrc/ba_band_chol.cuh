@@ -187,8 +187,6 @@ struct BandCholArgs {
   int* sync;                // [2] = epoch once: 0 the hand-over is written, 1 the middle x and the intrinsics are written
   int epoch;
   int blk6;                 // k_band_chol6 (plan)
-  int flags;                // timing experiments (PSFM_CHOL_FLAGS; results invalid): 1 no output of L, 2 no reciprocal, 4 no publish, 8 barrier + pivot load only, 16 no row streaming
-  long long* prof;          // optional [8]: SM cycles of factorisation | corner + staging | back substitution, pivots (side 0)
 };
 
 __device__ __forceinline__ void bc_post(int* flag, int v) {
@@ -226,10 +224,9 @@ __device__ __forceinline__ double bc_rcp(double d) {
 // hand-shake of the two-sided form, back substitution.  Called by every thread of the CTA.
 template <int RP>
 __device__ __forceinline__ void bc_tail(const BandCholArgs& a, const BandSide& sd, const int side, double* stage, int& s_fail,
-                                        double* s_xI, const double* s_c4, const long long tk0, const long long tk1) {
+                                        double* s_xI, const double* s_c4) {
   const int tid = threadIdx.x, lane = tid & 31;
   const int nb = sd.nb, npiv = sd.npiv, bw = a.bw, LS = bw + 1;
-  const int nsteps = npiv;
   // 1 / sqrt(d): normalisation of the stored columns, applied while staging the back substitution
   for (int j = tid; j < npiv; j += blockDim.x) sd.dinv[j] = rsqrt(__ldcg(sd.dinv + j));
   // ---- arrow corner: 3 x 3 intrinsics block and its right-hand side (thread of block {Wb, Wb})
@@ -321,7 +318,6 @@ __device__ __forceinline__ void bc_tail(const BandCholArgs& a, const BandSide& s
 #pragma unroll
   for (int m = 0; m < BC_MAXSLOT; ++m) yy[m] = (tid < 32 && m < ms) ? y0(32 * (ctop - m) + lane) : 0.0;
   __syncthreads();
-  const long long tk2 = a.prof ? clock64() : 0;
   for (int c = ctop, n = 0; c >= 0; --c, ++n) {
     const double* buf = stage + (n & 1) * CH;
     if (tid >= 32) {
@@ -363,10 +359,6 @@ __device__ __forceinline__ void bc_tail(const BandCholArgs& a, const BandSide& s
     }
     __syncthreads();
     if (c == cpost && tid == 0) bc_post(a.sync + 1, a.epoch);
-  }
-  if (a.prof && tid == 0 && side == 0) {
-    const long long tk3 = clock64();
-    a.prof[0] = tk1 - tk0; a.prof[1] = tk2 - tk1; a.prof[2] = tk3 - tk2; a.prof[3] = nsteps;
   }
 }
 
@@ -427,7 +419,6 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
 #pragma unroll
     for (int i = 0; i < BS; ++i) colbuf[bc_idx(BS * P) + i] = v[i][0];
   }
-  const long long tk0 = a.prof ? clock64() : 0;
   const int nsteps = ((npiv + UN - 1) / UN) * UN;
   const int jsplit = jswitch >= 0 ? jswitch : nsteps;      // end of phase 0
   bool bad = false;
@@ -446,12 +437,10 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) { rg[i] = live ? __ldg(src) : 0.0; src += RS; }
     int kk = e;                                            // (e - pj) mod W for band entries
-    const bool no_out = (a.flags & 1) != 0, no_ring = (a.flags & 16) != 0;
     const int ce = bc_idx(e);                              // where position e of the pivot column lives
     // entry (j + kk, kk) of Lr: one element back per pivot, W (LS + 1) forward when kk wraps
     double* lp = sd.Lr + (size_t)e * LS + e;
     double* la = sd.La + (size_t)(live && !band ? e - W : 0) * nb;
-    long long p_own = 0, p_wait = 0, tlast = a.prof ? clock64() : 0;
     // two phases (before | after the hand-over of the two-sided form) around ONE copy of the pivot loop:
     // the hand-over code stays out of the loop body (instruction cache), the one-sided form has an empty phase 1
 #pragma unroll 1
@@ -463,20 +452,14 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
 #pragma unroll
       for (int u = 0; u < UN; ++u) {
         const int j = j0 + u;
-        if (!no_ring) {
-          if (live) ring[u * BC_CSM + bc_idx(pos)] = rg[u & 3];   // row j + W -> slot u
-          rg[u & 3] = live ? __ldg(src) : 0.0;                    // row j + W + 4
+        if (live) {
+          ring[u * BC_CSM + bc_idx(pos)] = rg[u & 3];             // row j + W -> slot u
+          rg[u & 3] = __ldg(src);                                 // row j + W + 4
         }
         src += RS;
         if (band && ++pos == W) pos = 0;
-        if (a.prof) { const long long t = clock64(); p_own += t - tlast; tlast = t; }
         bc_bar();
-        if (a.prof) {
-          const double dd = colbuf[(u & 1) * BC_CSM];        // first use after the barrier: the wait shows up here
-          const long long t = clock64();
-          p_wait += t - tlast + (dd == 1.25e-300 ? 1 : 0); tlast = t;
-        }
-        if (j < nb && !no_out) {
+        if (j < nb) {
           const double val = colbuf[(u & 1) * BC_CSM + ce];
           if (band) {
             if (kk <= bw && j + kk < nb) *lp = val;
@@ -492,14 +475,12 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
       }
     }
     }
-    if (a.prof && tid == ldr0) { a.prof[4] = p_own; a.prof[5] = p_wait; }
   } else {
     // ---- workers (and idle threads of the last worker warp: barriers only)
     const double* sP = colbuf + bc_idx(BS * P);
     const double* sQ = colbuf + bc_idx(BS * Q);
     int pj0 = 0, pjp = 0;                                  // pivot position of step u = 0 of the body, and its padded index
     int Pj = 0;
-    long long p_own = 0, p_wait = 0, tlast = a.prof ? clock64() : 0;
 #pragma unroll 1
     for (int phase = 0; phase < 2; ++phase) {
       if (phase == 1 && jswitch >= 0) {
@@ -536,13 +517,11 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
       for (int u = 0; u < UN; ++u) {
         const int ij = u % BS;
         const int par = (u & 1) * BC_CSM, parn = ((u + 1) & 1) * BC_CSM, slot = u * BC_CSM;
-        if (a.prof) { const long long t = clock64(); p_own += t - tlast; tlast = t; }
         bc_bar();
         const double d = colbuf[par + pjp + u];            // 8 consecutive positions never straddle a padding gap
         bad |= !(d > 0.0 && d <= 1.7976931348623157e308);
-        if (a.prof) { const long long t = clock64(); p_wait += t - tlast + (bad ? 0 : 0); tlast = t; }
-        if (worker && !(a.flags & 8)) {
-          const double invd = (a.flags & 2) ? 1.0 - 1e-3 * d : bc_rcp(d);
+        if (worker) {
+          const double invd = bc_rcp(d);
           double cp[BS], tq[BS];
 #pragma unroll
           for (int i = 0; i < BS; i += 2) {
@@ -576,8 +555,7 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
           int Pjn = Pj;
           if (ij == BS - 1) { Pjn = Pj + 1; if (Pjn == Wb) Pjn = 0; }
           double* cbn = colbuf + parn;
-          if (a.flags & 4) {
-          } else if (Q == Pjn) {
+          if (Q == Pjn) {
 #pragma unroll
             for (int i = 0; i < BS; i += 2) *reinterpret_cast<double2*>(cbn + bc_idx(BS * P) + i) = make_double2(v[i][ijn], v[i + 1][ijn]);
           } else if (P == Pjn) {
@@ -594,11 +572,8 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
       pjp = bc_idx(pj0);
     }
     }
-    if (a.prof && tid == 0) { a.prof[6] = p_own; a.prof[7] = p_wait; }
   }
   __syncthreads();
-  const long long tk1 = a.prof ? clock64() : 0;
-  if (a.prof && tid == 0 && side == 0) { a.prof[0] = tk1 - tk0; a.prof[3] = nsteps; }
   if (bad) s_fail = 1;
   if (a.two && side == 1) {
     // hand-over: what is left in the window (rows n1 .. n1 + W - 1 of the reversed matrix, zero on input)
@@ -630,7 +605,7 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
       for (int k = 0; k < 4; ++k) s_c4[4 * i + k] = v[i][k];
   }
   __syncthreads();
-  bc_tail<1>(a, sd, side, stage, s_fail, s_xI, s_c4, tk0, tk1);
+  bc_tail<1>(a, sd, side, stage, s_fail, s_xI, s_c4);
 }
 
 // ------------------------------------------------------------------ block-6 form with look-ahead (k_band_chol6)
@@ -667,7 +642,7 @@ __device__ __forceinline__ void bc_pbar(int n) { asm volatile("bar.sync 2, %0;\n
 template <int MAXT, int TR, int TC>
 __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
   // TR x TC: tile of a worker thread inside a 6 x 6 block (6 x 6: one thread per block; 3 x 6: two; 3 x 3: four).  A warp issues
-  // about one instruction per several cycles whatever the dependences (PSFM_CHOL_PROFILE shows it), so a step costs
+  // about one instruction per several cycles whatever the dependences (measured with clock64 per role), so a step costs
   // what its LONGEST warp executes — many thin threads beat few fat ones as long as the CTA has room for them.
   extern __shared__ __align__(16) double bc_smem[];
   __shared__ int s_fail;
@@ -701,7 +676,6 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
   const int RB = 6 * RS;
   const double* __restrict__ Ab = sd.Ab;
   if (tid == 0) s_fail = 0;
-  const long long tk0 = a.prof ? clock64() : 0;
   bool bad = false;
   const int kb0 = 0, ke0 = jsw >= 0 ? jsw : nsteps;     // phase 0; phase 1 (two-sided, side 0): jsw .. nsteps
 
@@ -824,7 +798,6 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
         }
       }
     };
-    long long p_own = 0, p_wait = 0, tlast = a.prof ? clock64() : 0, q_upd = 0, q_rec = 0, q_pub = 0;
 #pragma unroll 1
     for (int phase = 0; phase < 2; ++phase) {
       const int kb = phase == 0 ? kb0 : jsw, ke = phase == 0 ? ke0 : nsteps;
@@ -866,21 +839,15 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
         const int cn = c + 1 == Wb ? 0 : c + 1, cn2 = cn + 1 == Wb ? 0 : cn + 1;
         if (act) {
           const bool ic = (P == c || Q == c), icn = (P == cn || Q == cn);
-          long long t0 = a.prof ? clock64() : 0;
           if (ic) { if (!icn || last) recycle(k, c, cn); }
           else if (!icn || last) update(Ypan + (k & 1) * PB, Zpan + (k & 1) * PB);
-          if (a.prof) { const long long t1 = clock64(); if (ic) q_rec += t1 - t0; else q_upd += t1 - t0; t0 = t1; }
           if (!last && !ic && !icn && (P == cn2 || Q == cn2)) publish(Raw + (k & 1) * PB, cn2);
-          if (a.prof) q_pub += clock64() - t0;
         }
         output(k, c);
-        if (a.prof) { const long long t = clock64(); p_own += t - tlast; tlast = t; }
         bc_gbar(NG2);
-        if (a.prof) { const long long t = clock64(); p_wait += t - tlast; tlast = t; }
         c = cn;
       }
     }
-    if (a.prof && tid == 0 && side == 0) { a.prof[6] = p_own; a.prof[7] = p_wait; a.prof[8] = q_upd; a.prof[9] = q_rec; a.prof[10] = q_pub; }
     if (act && a.two && side == 1) {
       // hand-over: what is left in the window (rows n1 .. n1 + W - 1 of the reversed matrix, zero on input) is the
       // update of the middle block by this side's pivots; reversed row n1 + m is middle row W - 1 - m
@@ -922,7 +889,6 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
 #pragma unroll
       for (int m = 0; m < 6; ++m) dst[m] = rg[-m];
     };
-    long long p_own = 0, p_wait = 0, tlast = a.prof ? clock64() : 0, q_pbar = 0, q_chol = 0, q_out = 0;
     // col = row (p, ar) of the fully updated pivot column block at position cp: factor the diagonal block (LDL'
     // recurrence, every thread redundantly: one reciprocal per pivot on the chain), solve the row on the fly,
     // publish y and z = y / d
@@ -932,9 +898,7 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
 #pragma unroll
         for (int m = 0; m < 6; m += 2) o[m >> 1] = make_double2(col[m], col[m + 1]);
       }
-      long long tq = a.prof ? clock64() : 0;
       bc_pbar(NP);
-      if (a.prof) { const long long t = clock64(); q_pbar += t - tq; tq = t; }
       double Dl[6][6], w[6][6], invd[6];
       {
         double dfull[36];
@@ -967,14 +931,12 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
         yo[j] = t;
         z[j] = t * invd[j];
       }
-      if (a.prof) { const long long t = clock64(); q_chol += t - tq + (z[5] == 1.25e-300 ? 1 : 0); tq = t; }
       if (pact) {
         double2* oy = reinterpret_cast<double2*>(Ydst + p * B6_PBS + 6 * ar);
         double2* oz = reinterpret_cast<double2*>(Zdst + p * B6_PBS + 6 * ar);
 #pragma unroll
         for (int m = 0; m < 6; m += 2) { oy[m >> 1] = make_double2(yo[m], yo[m + 1]); oz[m >> 1] = make_double2(z[m], z[m + 1]); }
       }
-      if (a.prof) q_out += clock64() - tq;
     };
 #pragma unroll 1
     for (int phase = 0; phase < 2; ++phase) {
@@ -1019,13 +981,10 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
           }
           finish(cn, col, Ypan + ((k + 1) & 1) * PB, Zpan + ((k + 1) & 1) * PB);
         }
-        if (a.prof) { const long long t = clock64(); p_own += t - tlast; tlast = t; }
         bc_gbar(NG2);
-        if (a.prof) { const long long t = clock64(); p_wait += t - tlast; tlast = t; }
         c = cn;
       }
     }
-    if (a.prof && tid == NW && side == 0) { a.prof[4] = p_own; a.prof[5] = p_wait; a.prof[11] = q_pbar; a.prof[12] = q_chol; a.prof[13] = q_out; }
   } else {
     // ------------------------------------------------------------ loader warps: block row k + Wb of Ab -> ring slot k & 3,
     //      one step before it is used, loaded from global memory one step before that (registers in between)
@@ -1070,11 +1029,10 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
   }
   if (a.two && side == 1) __threadfence();
   __syncthreads();
-  const long long tk1 = a.prof ? clock64() : 0;
   if (bad) s_fail = 1;
   if (a.two && side == 1 && tid == 0) bc_post(a.sync, a.epoch);
   __syncthreads();
-  bc_tail<2>(a, sd, side, bc_smem, s_fail, s_xI, s_c4, tk0, tk1);
+  bc_tail<2>(a, sd, side, bc_smem, s_fail, s_xI, s_c4);
 }
 
 // threads of the kernel for window W with BS x BS blocks
@@ -1171,15 +1129,12 @@ struct BandWork {
     c.two = pl.two; c.nbg = pl.nb; c.nbp = pl.nbp; c.k0 = pl.k0;
     c.bw = pl.bw; c.W = pl.W; c.RS = pl.RS; c.ns = ns; c.blk6 = pl.blk6;
     c.x = x; c.fail = fail; c.D = D.p; c.sync = sync.p; c.epoch = ++epoch;
-    c.prof = nullptr;
     return c;
   }
 };
 
 // one launch: one CTA, or two for the two-sided form
-inline void band_chol_launch(BandCholArgs c, cudaStream_t st) {
-  static const int flags = getenv("PSFM_CHOL_FLAGS") ? atoi(getenv("PSFM_CHOL_FLAGS")) : 0;
-  c.flags = flags;
+inline void band_chol_launch(const BandCholArgs& c, cudaStream_t st) {
   const int grid = c.two ? 2 : 1;
   if (c.blk6) {
     const int Wb = c.W / 6, nblk = (Wb + 1) * (Wb + 2) / 2;
@@ -1187,7 +1142,6 @@ inline void band_chol_launch(BandCholArgs c, cudaStream_t st) {
     const int ng4 = ((4 * nblk + 31) & ~31) + np, ng1 = ((nblk + 31) & ~31) + np;
     const size_t fact = sizeof(double) * (7 * (size_t)(Wb + 1) * B6_PBS + 36 + 4 * 6 * (size_t)c.RS);
     const size_t smem = std::max(fact, band_chol_smem(c.bw));
-    static const bool fat = getenv("PSFM_CHOL_FAT") != nullptr;     // measurement: one thread per block everywhere
 #define PSFM_BC6_GO(MT, TRV, TCV)                                                                                      \
   do {                                                                                                             \
     static size_t attr = 0;                                                                                        \
@@ -1197,12 +1151,11 @@ inline void band_chol_launch(BandCholArgs c, cudaStream_t st) {
     }                                                                                                              \
     k_band_chol6<MT, TRV, TCV><<<grid, MT, smem, st>>>(c);                                                               \
   } while (0)
-    // thin threads while the CTA has room for them (PSFM_CHOL_PROFILE shows why), else one fat thread
-    // per block; the threads after the workers and the panel group are the loader (>= 32)
-    static const int tile = getenv("PSFM_CHOL_TILE") ? atoi(getenv("PSFM_CHOL_TILE")) : 0;     // measurement: 33 | 36 | 66
+    // thin threads while the CTA has room for them (see k_band_chol6), else one fat thread per block; the threads
+    // after the workers and the panel group are the loader (>= 32)
     const int ng2 = ((2 * nblk + 31) & ~31) + np;
-    if (!fat && tile != 36 && tile != 66 && ng4 + 32 <= 512) PSFM_BC6_GO(512, 3, 3);
-    else if (!fat && tile != 66 && ng2 + 32 <= 384) PSFM_BC6_GO(384, 3, 6);
+    if (ng4 + 32 <= 512) PSFM_BC6_GO(512, 3, 3);
+    else if (ng2 + 32 <= 384) PSFM_BC6_GO(384, 3, 6);
     else if (ng1 + 64 <= 256) PSFM_BC6_GO(256, 6, 6);
     else if (ng1 + 64 <= 512) PSFM_BC6_GO(512, 6, 6);
     else PSFM_BC6_GO(640, 6, 6);

@@ -830,12 +830,8 @@ struct BackArgs {
   const double* xs;     // [6F + 3C] s o y_c  (y_c = reduced-system solution; step_c = -y_c)
   const double* K;
   double* Xc;           // [3P] candidate points
-  double* acc;          // [0] sum m(r + m/2)   [1] |dX|^2   [2] |Xc|^2   [3] candidate cost (fused form only)
+  double* acc;          // [0] sum m(r + m/2)   [1] |dX|^2   [2] |Xc|^2
   int intr;
-  // fused candidate cost (k_back_substitute_p only; null: k_cost runs afterwards)
-  const double* pose_c;   // [F*8] candidate poses q(4) t(3) pad — k_apply_cams runs BEFORE the back-substitution then
-  const double* K_c;      // [C*3] candidate intrinsics
-  LossP loss;
 };
 
 // One tile of the back-substitution.  Shared memory (sm.simg, sm.sx, sm.spt rows 0..11, sm.pstart) holds the tile's
@@ -844,8 +840,7 @@ template <int TILE, bool ROT>
 __device__ __forceinline__ void back_substitute_tile(const TileCtx& tc, const BackArgs& a, TileSmem<TILE>& sm, const TileInfo& ti,
                                                      const bool act, const int ls, const int lp, const double a00, const double a02,
                                                      const double a12, const double r0, const double r1, const double* xk,
-                                                     const double inv_f, const double* pose_sm = nullptr,
-                                                     const double2 xy = double2{0.0, 0.0}, double* racc = nullptr) {
+                                                     const double inv_f, double* racc = nullptr) {
   const int tid = threadIdx.x;
   ObsGeom g;
   double u0 = 0, u1 = 0, jf0 = 0, jf1 = 0, sq = 0;
@@ -897,33 +892,14 @@ __device__ __forceinline__ void back_substitute_tile(const TileCtx& tc, const Ba
     const double m1 = -(u1 + a00 * y1 + a12 * y2);
     mm = m0 * (r0 + 0.5 * m0) + m1 * (r1 + 0.5 * m1);
   }
-  // candidate cost of this observation (ComputeCandidatePointAndEvaluateCost): pose and intrinsics of the candidate,
-  // point X - y_p of the tile (sm.sw still holds y_p)
-  double cc = 0.0;
-  if (pose_sm != nullptr && act) {
-    const int img = sm.cimg[ls], cam = __ldg(tc.img_cam + img);
-    const double2* pp = reinterpret_cast<const double2*>(pose_sm + 8 * (size_t)img);
-    const double2 qa = pp[0], qb = pp[1], ta = pp[2], tb = pp[3];
-    const double q0 = qa.x, q1 = qa.y, q2 = qb.x, q3 = qb.y;
-    const double X0 = sm.sxyz[3 * lp] + (-sm.sw[lp]), X1 = sm.sxyz[3 * lp + 1] + (-sm.sw[cnp + lp]), X2 = sm.sxyz[3 * lp + 2] + (-sm.sw[2 * cnp + lp]);
-    const double p0 = (1.0 - 2.0 * (q2 * q2 + q3 * q3)) * X0 + 2.0 * (q1 * q2 - q0 * q3) * X1 + 2.0 * (q1 * q3 + q0 * q2) * X2 + ta.x;
-    const double p1 = 2.0 * (q1 * q2 + q0 * q3) * X0 + (1.0 - 2.0 * (q1 * q1 + q3 * q3)) * X1 + 2.0 * (q2 * q3 - q0 * q1) * X2 + ta.y;
-    const double p2 = 2.0 * (q1 * q3 - q0 * q2) * X0 + 2.0 * (q2 * q3 + q0 * q1) * X1 + (1.0 - 2.0 * (q1 * q1 + q2 * q2)) * X2 + tb.x;
-    const double iz = 1.0 / p2;
-    const double f = __ldg(a.K_c + 3 * cam), cx = __ldg(a.K_c + 3 * cam + 1), cy = __ldg(a.K_c + 3 * cam + 2);
-    const double e0 = f * p0 * iz + cx - xy.x, e1 = f * p1 * iz + cy - xy.y;
-    double rho0, rho1;
-    loss_eval(a.loss, e0 * e0 + e1 * e1, rho0, rho1);
-    cc = 0.5 * rho0;
-  }
-  double v[4] = {mm, dx2, xc2, cc};
+  double v[3] = {mm, dx2, xc2};
   if (racc != nullptr) {       // persistent kernel: per-thread sums (shared memory, stride TILE) across its tiles, one reduction at the end
 #pragma unroll
-    for (int k = 0; k < 4; ++k) racc[k * TILE + tid] += v[k];
+    for (int k = 0; k < 3; ++k) racc[k * TILE + tid] += v[k];
     return;
   }
-  const double s = block_sum_multi<4>(v, sm.sred);
-  if (tid < (pose_sm != nullptr ? 4 : 3)) atomicAdd(a.acc + tid, s);
+  const double s = block_sum_multi<3>(v, sm.sred);
+  if (tid < 3) atomicAdd(a.acc + tid, s);
 }
 
 template <int TILE, bool ROT>

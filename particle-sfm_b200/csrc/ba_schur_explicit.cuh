@@ -243,14 +243,13 @@ struct StArgs {
   int intr;
   const unsigned int* entries;   // (li << 16) | lj, tile-local indices, sorted by (tile, a, b)
   const int* task_slot;          // [ntasks] band-block slot a * (span + 1) + (b - a)
-  const int2* task_rng;          // [ntasks] entry range (begin, end) of the task; tasks of a tile ordered longest first
+  const int2* task_rng;          // [ntasks] entry range (begin, end) of the task; tasks of a tile ordered by image pair
   const int* tile_task;          // [T + 1] task range of the tile
   double* Sband;                 // [nrep][F * (span + 1) * 36]
   size_t band_stride;
   int nrep_mask;
   int span;
   const unsigned char* tile_dense;   // [T] pair phase of the tile: TILE_PAIRS_LOOP | _DENSE | _DENSE_DUP
-  int dbg;      // PSFM_SCHUR_FLAGS (measurement only): 1 = no band REDs, 2 = no pair phase
 };
 
 // ---- dense pair phase (tensor cores)
@@ -303,7 +302,7 @@ __device__ __forceinline__ bool chol3(const double (&h)[6], double (&l)[6]) {
 // point of the tile) are not sent.
 template <int TILE>
 __device__ __forceinline__ void dense_pairs_mma(const double* __restrict__ zf, const int* __restrict__ cimg, int ns, int np,
-                                                double* __restrict__ band, int span, bool red) {
+                                                double* __restrict__ band, int span) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int R = 6 * ns, RB = dense_z_rb(ns), KB2 = dense_z_kb2(np);
   const int nblk = RB * (RB + 1) / 2;
@@ -329,7 +328,6 @@ __device__ __forceinline__ void dense_pairs_mma(const double* __restrict__ zf, c
       dmma_16x8x4(acc[0], a0.y, a1.y, b0.y);
       dmma_16x8x4(acc[1], a0.y, a1.y, b1.y);
     }
-    if (!red) continue;
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -356,13 +354,13 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
                                                 const double a12, const int rep, const int t0, const int nt) {
   const int tid = threadIdx.x;
   const double inv_f = (a.intr >= 1) ? 1.0 / __ldg(a.K) : 0.0;
-  const unsigned char mode = (a.dbg & 2) ? TILE_PAIRS_LOOP : __ldg(a.tile_dense + rep);
+  const unsigned char mode = __ldg(a.tile_dense + rep);
   // Pair tasks of this tile -> lanes: two lanes share a task (q = 2 task + part; entries e0 + part, stride 2).
   // Tried and dropped, both slower: runs cut into units of <= 8 entries so that all 8 warps carry pairs (more
   // REDs), three lanes per task (7 trips instead of 11 on the tile's critical path) — the pair loop is bound by
   // its fp64 instruction count, not by the longest lane.
   constexpr int lpt = 2;
-  const int nq = (a.dbg & 2) ? 0 : 2 * nt;
+  const int nq = 2 * max(nt, 0);      // nt >= 0; with the clamp ptxas spills 20 B less in k_schur_tile_p<*, true>
   auto lane_task = [&](int q, int& tq, int& par) -> bool {
     par = q & 1; tq = q >> 1;
     return q < nq;
@@ -495,7 +493,7 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
         }
     }
     __syncthreads();
-    dense_pairs_mma<TILE>(zf, sm.cimg, ti.ns, ti.np, band, a.span, !(a.dbg & 1));
+    dense_pairs_mma<TILE>(zf, sm.cimg, ti.ns, ti.np, band, a.span);
     return;
   }
   // first entries of the first pass (three in flight per lane: one trip is shorter than an L2 round trip)
@@ -610,15 +608,12 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
     // combine the lanes of a task: lane `par` ends up with the sums of ITS share of the 36 elements (every
     // lane sends what its reader owns), then one RED per element
     double* dst = band + (size_t)slot * 36;
-    const bool red = valid && !(a.dbg & 1);
-    {
 #pragma unroll
-      for (int i = 0; i < 18; ++i) {
-        const double mine = par ? acc[18 + i] : acc[i];
-        const double x = par ? acc[i] : acc[18 + i];
-        const double v = mine + __shfl_xor_sync(0xffffffffu, x, 1);
-        if (red && (ROT || v != 0.0)) atomicAdd(dst + 18 * par + i, v);
-      }
+    for (int i = 0; i < 18; ++i) {
+      const double mine = par ? acc[18 + i] : acc[i];
+      const double x = par ? acc[i] : acc[18 + i];
+      const double v = mine + __shfl_xor_sync(0xffffffffu, x, 1);
+      if (valid && (ROT || v != 0.0)) atomicAdd(dst + 18 * par + i, v);
     }
   }
 }
@@ -728,51 +723,26 @@ __global__ void k_tile_entry_offsets(const int* tile_start, const int* ptr, int 
   if (t <= T) seg[t] = ptr[tile_start[t]];
 }
 
-// A run of equal keys (one image pair of one tile) is cut into UNITS of at most `chunk` entries, all
-// of (nearly) the same length; a unit is what two lanes of k_schur_tile accumulate in registers.
-// Without the cut the longest run of a tile (every point of the tile sees both images) sets the trip
-// count of its warp while the other warps wait at the end-of-tile barrier.
-__global__ void k_unit_count(const int* ucount, int nruns, int chunk, int* nunits) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t > nruns) return;
-  nunits[t] = t < nruns ? (ucount[t] + chunk - 1) / chunk : 0;
-}
-// units of a tile are processed longest first (lanes of a warp then run similar trip counts and the
-// short units fill the last pass): sort key (tile, ~count), payload = (slot, entry range)
-__global__ void k_unit_fill(const unsigned long long* ukeys, const int* ucount, const int* beg, const int* ubeg, int nruns,
-                            int fbits, int span, int by_pair, unsigned long long* key2, int* idx, int* slot, int2* rng) {
+// One task per run of equal (tile, image a, image b) keys, in key order: band-block slot and entry range
+// [beg, beg + count) of the run (beg: exclusive scan of the run lengths)
+__global__ void k_pair_tasks(const unsigned long long* run_key, const int* run_count, const int* run_beg, int nruns,
+                             int fbits, int span, int* slot, int2* rng) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= nruns) return;
-  const unsigned long long k = ukeys[t], mask = (1ull << fbits) - 1;
+  const unsigned long long k = run_key[t], mask = (1ull << fbits) - 1;
   const int b = (int)(k & mask), a = (int)((k >> fbits) & mask);
-  const unsigned long long tile = k >> (2 * fbits);
-  const int n = ubeg[t + 1] - ubeg[t], cnt = ucount[t], base = cnt / n, rem = cnt % n;
-  int e = beg[t];
-  for (int c = 0; c < n; ++c) {
-    const int len = base + (c < rem), u = ubeg[t] + c;
-    key2[u] = (tile << 32) | (by_pair ? (unsigned long long)(unsigned)u : (unsigned long long)(0xffffffffu - (unsigned)len));
-    idx[u] = u;
-    slot[u] = a * (span + 1) + (b - a);
-    rng[u] = make_int2(e, e + len);
-    e += len;
-  }
-}
-__global__ void k_task_gather(const int* order, const int* slot_in, const int2* rng_in, int ntasks, int* slot_out, int2* rng_out) {
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= ntasks) return;
-  const int o = order[t];
-  slot_out[t] = slot_in[o];
-  rng_out[t] = rng_in[o];
+  slot[t] = a * (span + 1) + (b - a);
+  rng[t] = make_int2(run_beg[t], run_beg[t] + run_count[t]);
 }
 
-// tile -> first unit (lower bound over the sorted (tile, ~count) keys)
-__global__ void k_tile_tasks(const unsigned long long* key2_sorted, int ntasks, int T, int* tile_task) {
+// tile -> first task (lower bound over the tiles of the sorted run keys)
+__global__ void k_tile_tasks(const unsigned long long* run_key, int nruns, int fbits, int T, int* tile_task) {
   const int tile = blockIdx.x * blockDim.x + threadIdx.x;
   if (tile > T) return;
-  int lo = 0, hi = ntasks;
+  int lo = 0, hi = nruns;
   while (lo < hi) {
     const int mid = (lo + hi) >> 1;
-    if ((int)(key2_sorted[mid] >> 32) < tile) lo = mid + 1; else hi = mid;
+    if ((long long)(run_key[mid] >> (2 * fbits)) < tile) lo = mid + 1; else hi = mid;
   }
   tile_task[tile] = lo;
 }
@@ -906,7 +876,6 @@ struct CholArgs {
   double* Lp;                 // [npanel][rmax][CB]  solved rows below each panel (the factor's off-diagonal part)
   double* Ld;                 // [npanel][CB][CB]    diagonal blocks of the factor
   int rmax;                   // rows reserved per panel in Lp
-  unsigned long long* prof;   // optional [8]: SM cycles of CTA 0 per phase (PSFM_CHOL_PROFILE)
 };
 
 // Grid-wide barrier for the few (co-resident, cooperative launch) CTAs of k_chol_blocked: one
@@ -996,20 +965,11 @@ __global__ void __launch_bounds__(256) k_chol_blocked(const CholArgs a) {
   double* A = a.A;
   if (tid == 0) s_bad = 0;
   __syncthreads();
-  const bool prof = a.prof != nullptr && blockIdx.x == 0 && tid == 0;
-  long long tk = prof ? clock64() : 0;
-#define PSFM_CHOL_TICK(slot)                                   \
-  if (prof) {                                                  \
-    const long long now_ = clock64();                          \
-    a.prof[slot] += (unsigned long long)(now_ - tk);           \
-    tk = now_;                                                 \
-  }
   for (int c0 = 0; c0 < ns; c0 += CB) {
     const int w = min(CB, ns - c0), c1 = c0 + w;
     // ---- (1) diagonal block, redundantly per CTA: warp 0 factors it in registers
     if (tid < CB && chol_diag_warp(A + (size_t)c0 * lda + c0, lda, w, sD, sDinv)) s_bad = 1;
     __syncthreads();
-    PSFM_CHOL_TICK(0);
     if (s_bad) break;     // uniform across the grid: every CTA factors the same block
     // ---- rows below the panel that can be non-zero
     const int rb = (c1 < a.nb) ? min(a.nb, c1 + a.bw) : c1;
@@ -1084,9 +1044,7 @@ __global__ void __launch_bounds__(256) k_chol_blocked(const CholArgs a) {
         }
       }
     }
-    PSFM_CHOL_TICK(3);
     chol_grid_barrier(a.bar, bar_target);
-    PSFM_CHOL_TICK(4);
   }
   if (blockIdx.x != 0) return;
   if (tid == 0) *a.fail = s_bad;
@@ -1149,8 +1107,6 @@ __global__ void __launch_bounds__(256) k_chol_blocked(const CholArgs a) {
     }
     __syncthreads();
   }
-  PSFM_CHOL_TICK(5);
-#undef PSFM_CHOL_TICK
 }
 
 }  // namespace ba

@@ -159,7 +159,6 @@ struct psfm_ba_solver {
   long long npairs = 0;
   DBuf<unsigned long long> d_entries;
   DBuf<int> d_blk_key, d_chunk_blk, d_cholfail;
-  DBuf<unsigned long long> d_cholprof;
   DBuf<unsigned int> d_cholbar;
   DBuf<double> d_cholLp, d_cholLd;
   DBuf<long long> d_chunk_beg;
@@ -229,6 +228,17 @@ void d2h_sync(cudaStream_t st, T* dst, const T* src, size_t n) {
 }
 
 inline unsigned grid_for(size_t n, int block = 256) { return (unsigned)((n + block - 1) / block); }
+
+// a host scalar reduced over the ranks with op (dist::allreduce_max | dist::allreduce_sum); v itself on one rank
+double reduce_over_ranks(cudaStream_t st, double v, void (*op)(double*, size_t, cudaStream_t)) {
+  if (dist::world_size() == 1) return v;
+  DBuf<double> d; d.alloc(1, st);
+  k_fill<<<1, 32, 0, st>>>(d.p, v, 1); PSFM_LAUNCH_CHECK();
+  op(d.p, 1, st);
+  double h = 0.0;
+  d2h_sync(st, &h, d.p, 1);
+  return h;
+}
 
 // Configuration and the caller's observations -> device (once per solver).
 int upload_problem(psfm_ba_solver* S, const psfm_ba_problem* pb) {
@@ -353,21 +363,14 @@ int build_structure(psfm_ba_solver* S) {
   int P = 0, maxL = 0;
   while (P < Pt && h_cs[P] > 0) ++P;           // observed points come first
   for (int j = 0; j < P; ++j) maxL = std::max(maxL, h_cs[j]);
-  if (dist::world_size() > 1) {   // every rank takes the same code paths: the longest track of ANY shard decides
-    DBuf<double> mx; mx.alloc(1, st);
-    k_fill<<<1, 32, 0, st>>>(mx.p, (double)maxL, 1); PSFM_LAUNCH_CHECK();
-    dist::allreduce_max(mx.p, 1, st);
-    double h = 0.0;
-    PSFM_CUDA(cudaMemcpyAsync(&h, mx.p, sizeof(double), cudaMemcpyDeviceToHost, st));
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    maxL = (int)(h + 0.5);
-  }
+  // every rank takes the same code paths: the longest track of ANY shard decides
+  maxL = (int)(reduce_over_ranks(st, maxL, dist::allreduce_max) + 0.5);
   S->P = P; S->maxL = maxL;
   S->pt_orig.assign(h_order.begin(), h_order.begin() + P);
   // A track lives in one tile and a tile's per-image staging grows with the images it spans: beyond
   // 512 observations the shared memory of an SM (227 KB) no longer holds a tile.
   if (maxL > 512) { set_error("a track with more than 512 observations is not supported"); return PSFM_ERR_UNSUPPORTED; }
-  S->tile = (maxL <= 256 && !getenv("PSFM_TILE512")) ? 256 : 512;
+  S->tile = maxL <= 256 ? 256 : 512;
   // tiles: whole points, <= tile observations (greedy, host: P iterations)
   const int TILE = S->tile;
   std::vector<int> pt_ptr(P + 1, 0), tile_start, tile_pt;
@@ -494,14 +497,15 @@ void alloc_work(psfm_ba_solver* S) {
     }                                                                                                      \
   } while (0)
 
-// persistent pipelined tile kernels: grid = SMs x resident CTAs (capped by the tile count)
-#define PSFM_PIPE_LAUNCH(KERNEL, SMEM_FN, S, ROT, PS, ARGS)                                                 \
+// persistent pipelined tile kernels: grid = SMs x resident CTAs (capped by the tile count); SMEM: dynamic shared
+// memory of the kernel at the solver's tile width
+#define PSFM_PIPE_LAUNCH(KERNEL, SMEM, S, ROT, PS, ARGS)                                                    \
   do {                                                                                                     \
     const TileCtx _tc = (S)->tc();                                                                         \
+    const size_t smem = (SMEM);                                                                            \
     auto _go = [&](auto tile_c, auto rot_c) {                                                              \
       constexpr int TL = decltype(tile_c)::value;                                                          \
       constexpr bool RT = decltype(rot_c)::value;                                                          \
-      const size_t smem = SMEM_FN<TL>((S)->cap_ns, (S)->cap_np);                                           \
       static size_t attr_bytes = 0;                                                                        \
       static int occ = 0;                                                                                  \
       if (smem > attr_bytes || occ == 0) {                                                                 \
@@ -694,7 +698,7 @@ void do_linearize(psfm_ba_solver* S, const RunCfg& c, bool timed) {
   if (pipe_ok(S, pipe_smem)) {
     PipeSrc ps = pipe_src(S);
     ps.obs_xy = S->d_obs_xy.p;
-    PSFM_PIPE_LAUNCH(k_linearize_p, pipe_smem_linearize, S, c.rot, ps, a);
+    PSFM_PIPE_LAUNCH(k_linearize_p, pipe_smem, S, c.rot, ps, a);
   } else {
     PSFM_TILE_LAUNCH(k_linearize, 18, 3, S, c.rot, a);
   }
@@ -908,7 +912,7 @@ __global__ void k_point_span(const int* pt_ptr, const int* obs_img, int P, int* 
 // k_band_chol, the reduced system never exists as a dense matrix.
 void setup_band_chol(psfm_ba_solver* S) {
   const BandPlan pl = band_chol_plan(6 * S->F, S->bw, S->span);
-  S->band_chol = S->fused && pl.W > 0 && !getenv("PSFM_OLD_CHOL");
+  S->band_chol = S->fused && pl.W > 0;
   if (!S->band_chol) {
     S->d_S.alloc((size_t)(S->NS + 1) * (S->NS + 1), S->stream);
     return;
@@ -947,28 +951,14 @@ void ensure_pairs(psfm_ba_solver* S) {
     PSFM_CUDA(cudaMemcpyAsync(&h_span, span.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     PSFM_CUDA(cudaStreamSynchronize(st));
     S->npairs = total;
-    if (dist::world_size() > 1) {   // every rank must use the same band: max span over all shards
-      DBuf<double> sp; sp.alloc(1, st);
-      k_fill<<<1, 32, 0, st>>>(sp.p, (double)h_span, 1); PSFM_LAUNCH_CHECK();
-      dist::allreduce_max(sp.p, 1, st);
-      double hs = 0.0;
-      PSFM_CUDA(cudaMemcpyAsync(&hs, sp.p, sizeof(double), cudaMemcpyDeviceToHost, st));
-      PSFM_CUDA(cudaStreamSynchronize(st));
-      h_span = (int)(hs + 0.5);
-    }
+    // every rank must use the same band: max span over all shards
+    h_span = (int)(reduce_over_ranks(st, h_span, dist::allreduce_max) + 0.5);
     S->bw = 6 * h_span + 5;
   }
-  {
-    // an error on one rank is an error on all of them (nobody is left waiting in an all-reduce)
-    double too_many = S->npairs >= (1ll << 31) ? 1.0 : 0.0;
-    if (dist::world_size() > 1) {
-      DBuf<double> fl; fl.alloc(1, st);
-      k_fill<<<1, 32, 0, st>>>(fl.p, too_many, 1); PSFM_LAUNCH_CHECK();
-      dist::allreduce_max(fl.p, 1, st);
-      PSFM_CUDA(cudaMemcpyAsync(&too_many, fl.p, sizeof(double), cudaMemcpyDeviceToHost, st));
-      PSFM_CUDA(cudaStreamSynchronize(st));
-    }
-    if (too_many > 0.5) { set_error("too many observation pairs for the explicit Schur complement"); throw CudaFail{PSFM_ERR_UNSUPPORTED}; }
+  // an error on one rank is an error on all of them (nobody is left waiting in an all-reduce)
+  if (reduce_over_ranks(st, S->npairs >= (1ll << 31) ? 1.0 : 0.0, dist::allreduce_max) > 0.5) {
+    set_error("too many observation pairs for the explicit Schur complement");
+    throw CudaFail{PSFM_ERR_UNSUPPORTED};
   }
   S->span = (S->bw - 5) / 6;
   {
@@ -976,15 +966,8 @@ void ensure_pairs(psfm_ba_solver* S) {
     const size_t smem = S->tile == 256 ? smem256 : smem512;
     S->fused = smem <= 227 * 1024 && !getenv("PSFM_SCHUR_UNFUSED");
   }
-  if (dist::world_size() > 1) {   // fused and unfused paths all-reduce different buffers: one decision for all ranks
-    DBuf<double> fl; fl.alloc(1, st);
-    k_fill<<<1, 32, 0, st>>>(fl.p, S->fused ? 0.0 : 1.0, 1); PSFM_LAUNCH_CHECK();
-    dist::allreduce_max(fl.p, 1, st);
-    double h = 0.0;
-    PSFM_CUDA(cudaMemcpyAsync(&h, fl.p, sizeof(double), cudaMemcpyDeviceToHost, st));
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    S->fused = h < 0.5;
-  }
+  // fused and unfused paths all-reduce different buffers: one decision for all ranks
+  S->fused = reduce_over_ranks(st, S->fused ? 0.0 : 1.0, dist::allreduce_max) < 0.5;
   if (M == 0 && S->fused) {   // nothing to contribute: zero accumulators that still take part in the all-reduces
     S->ntasks = 0; S->ndense = 0;
     S->band_n = (size_t)F * (S->span + 1) * 36; S->band_nrep = 1;
@@ -1010,7 +993,6 @@ void ensure_pairs(psfm_ba_solver* S) {
     // ---- tile-local tasks for k_schur_tile
     const int T = S->T;
     int fb = 1; while ((1 << fb) < F) ++fb;
-    int tb = 1; while ((1ll << tb) < (long long)T + 1) ++tb;
     DBuf<unsigned long long> k64, k64_out, uk64;
     DBuf<unsigned int> v32;
     k64.alloc(NPr, st); k64_out.alloc(NPr, st); v32.alloc(NPr, st); S->d_tentries.alloc(NPr, st);
@@ -1036,44 +1018,22 @@ void ensure_pairs(psfm_ba_solver* S) {
       DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
       cub::DeviceRunLengthEncode::Encode(tmp.p, need, k64_out.p, uk64.p, ucount.p, nruns.p, (int)NPr, st);
     }
+    // one task per run, i.e. per image pair of a tile; the runs are in (tile, a, b) order
     int nr = 0;
     PSFM_CUDA(cudaMemcpyAsync(&nr, nruns.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     PSFM_CUDA(cudaStreamSynchronize(st));
-    // runs -> units of <= chunk entries (k_unit_count / k_unit_fill)
-    int chunk = 1 << 30;
-    if (const char* e = getenv("PSFM_TASK_CHUNK")) chunk = std::max(1, atoi(e));
-    const int by_pair = getenv("PSFM_TASK_BY_LENGTH") ? 0 : 1;
-    DBuf<int> beg0, nun, ubeg;
-    beg0.alloc((size_t)nr + 1, st); nun.alloc((size_t)nr + 1, st); ubeg.alloc((size_t)nr + 1, st);
-    PSFM_CUDA(cudaMemsetAsync(ucount.p + nr, 0, sizeof(int), st));
-    k_unit_count<<<grid_for((size_t)nr + 1), 256, 0, st>>>(ucount.p, nr, chunk, nun.p); PSFM_LAUNCH_CHECK();
-    {
-      size_t need = 0, need2 = 0;
-      cub::DeviceScan::ExclusiveSum(nullptr, need, ucount.p, beg0.p, nr + 1, st);
-      cub::DeviceScan::ExclusiveSum(nullptr, need2, nun.p, ubeg.p, nr + 1, st);
-      DBuf<unsigned char> tmp; tmp.alloc(std::max(need, need2) + 256, st);
-      cub::DeviceScan::ExclusiveSum(tmp.p, need, ucount.p, beg0.p, nr + 1, st);
-      cub::DeviceScan::ExclusiveSum(tmp.p, need2, nun.p, ubeg.p, nr + 1, st);
-    }
-    int nt = 0;
-    PSFM_CUDA(cudaMemcpyAsync(&nt, ubeg.p + nr, sizeof(int), cudaMemcpyDeviceToHost, st));
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    S->ntasks = nt;
-    S->d_task_slot.alloc(nt, st); S->d_task_rng.alloc(nt, st); S->d_tile_task.alloc((size_t)T + 1, st);
-    DBuf<int> slot0, idx0, order;
-    DBuf<int2> rng0;
-    DBuf<unsigned long long> key2, key2_out;
-    slot0.alloc(nt, st); rng0.alloc(nt, st); idx0.alloc(nt, st); order.alloc(nt, st); key2.alloc(nt, st); key2_out.alloc(nt, st);
-    if (nt) {
-      k_unit_fill<<<grid_for(nr), 256, 0, st>>>(uk64.p, ucount.p, beg0.p, ubeg.p, nr, fb, S->span, by_pair, key2.p, idx0.p, slot0.p, rng0.p);
-      PSFM_LAUNCH_CHECK();
+    S->ntasks = nr;
+    S->d_task_slot.alloc(nr, st); S->d_task_rng.alloc(nr, st); S->d_tile_task.alloc((size_t)T + 1, st);
+    if (nr) {
+      DBuf<int> beg; beg.alloc(nr, st);
       size_t need = 0;
-      cub::DeviceRadixSort::SortPairs(nullptr, need, key2.p, key2_out.p, idx0.p, order.p, nt, 0, 32 + tb, st);
+      cub::DeviceScan::ExclusiveSum(nullptr, need, ucount.p, beg.p, nr, st);
       DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
-      cub::DeviceRadixSort::SortPairs(tmp.p, need, key2.p, key2_out.p, idx0.p, order.p, nt, 0, 32 + tb, st);
-      k_task_gather<<<grid_for(nt), 256, 0, st>>>(order.p, slot0.p, rng0.p, nt, S->d_task_slot.p, S->d_task_rng.p); PSFM_LAUNCH_CHECK();
+      cub::DeviceScan::ExclusiveSum(tmp.p, need, ucount.p, beg.p, nr, st);
+      k_pair_tasks<<<grid_for(nr), 256, 0, st>>>(uk64.p, ucount.p, beg.p, nr, fb, S->span, S->d_task_slot.p, S->d_task_rng.p);
+      PSFM_LAUNCH_CHECK();
     }
-    k_tile_tasks<<<grid_for((size_t)T + 1), 256, 0, st>>>(key2_out.p, nt, T, S->d_tile_task.p);
+    k_tile_tasks<<<grid_for((size_t)T + 1), 256, 0, st>>>(uk64.p, nr, fb, T, S->d_tile_task.p);
     PSFM_LAUNCH_CHECK();
     {
       // PSFM_SCHUR_PAIRS=loop keeps every tile on the pair loop (measurement and tests); by default every
@@ -1191,9 +1151,6 @@ void launch_cholesky(psfm_ba_solver* S) {
       if (S->d_cholLd.n < (size_t)npanel * CB * CB) S->d_cholLd.alloc((size_t)npanel * CB * CB, st);
       ca.Lp = S->d_cholLp.p; ca.Ld = S->d_cholLd.p; ca.rmax = rmax;
     }
-    static const bool want_prof = getenv("PSFM_CHOL_PROFILE") != nullptr;
-    if (want_prof && S->d_cholprof.n == 0) { S->d_cholprof.alloc(8, st); S->d_cholprof.zero(st); }
-    ca.prof = want_prof ? S->d_cholprof.p : nullptr;
     void* kargs[] = {(void*)&ca};
     // few CTAs when the band is narrow (cheaper grid barriers), all SMs for a dense system
     const int tiles = (std::min(bw + 2, nbnd) + (S->NS + 1 - nbnd) + CB - 1) / CB;
@@ -1202,13 +1159,6 @@ void launch_cholesky(psfm_ba_solver* S) {
     PSFM_LAUNCH_CHECK();
   }
   { cudaEvent_t e = S->events.get(); PSFM_CUDA(cudaEventRecord(e, st)); S->ev_chol.back().second = e; }
-  if (S->d_cholprof.n) {   // debugging aid: cumulative SM cycles of CTA 0 per phase
-    unsigned long long h[8];
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    PSFM_CUDA(cudaMemcpy(h, S->d_cholprof.p, sizeof(h), cudaMemcpyDeviceToHost));
-    fprintf(stderr, "[psfm chol cycles] diag %llu rows %llu sync %llu trail %llu sync %llu backsub %llu\n",
-            h[0], h[1], h[2], h[3], h[4], h[5]);
-  }
 }
 
 // single-CTA register-window band Cholesky (ba_band_chol.cuh): assemble the compact band matrix,
@@ -1226,21 +1176,7 @@ void launch_band_cholesky(psfm_ba_solver* S) {
   b.Ab = S->bwk.ab(0); b.Ab1 = S->bwk.ab(1); b.C4 = S->bwk.C4.p; b.fail = S->d_cholfail.p;
   k_band_assemble<<<grid_for((size_t)(pl.rows[0] + pl.rows[1]) * pl.RS), 256, 0, st>>>(b);
   PSFM_LAUNCH_CHECK();
-  BandCholArgs c = S->bwk.args(S->d_x.p, S->NS, S->d_cholfail.p);
-  static const bool want_prof = getenv("PSFM_CHOL_PROFILE") != nullptr;
-  if (want_prof && S->d_cholprof.n < 16) { S->d_cholprof.alloc(16, st); S->d_cholprof.zero(st); }
-  c.prof = want_prof ? reinterpret_cast<long long*>(S->d_cholprof.p) : nullptr;
-  band_chol_launch(c, st);
-  if (want_prof) {
-    long long h[16];
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    PSFM_CUDA(cudaMemcpy(h, S->d_cholprof.p, sizeof(h), cudaMemcpyDeviceToHost));
-    if (c.blk6) fprintf(stderr, "[psfm chol6 cycles/step] worker0 update %.0f recycle %.0f publish %.0f | panel pbar %.0f chol+solve %.0f out %.0f (steps %lld)\n",
-                        h[8] / (h[3] / 6.0), h[9] / (h[3] / 6.0), h[10] / (h[3] / 6.0), h[11] / (h[3] / 6.0), h[12] / (h[3] / 6.0), h[13] / (h[3] / 6.0), h[3] / 6);
-    const double np_ = (double)std::max(1ll, h[3]);
-    fprintf(stderr, "[psfm band chol cycles] factor %lld (%lld pivots, %.0f / pivot) corner+stage %lld backsub %lld | per pivot own/wait: helper %.0f/%.0f worker0 %.0f/%.0f\n",
-            h[0], h[3], (double)h[0] / np_, h[1], h[2], h[4] / np_, h[5] / np_, h[6] / np_, h[7] / np_);
-  }
+  band_chol_launch(S->bwk.args(S->d_x.p, S->NS, S->d_cholfail.p), st);
   { cudaEvent_t e = S->events.get(); PSFM_CUDA(cudaEventRecord(e, st)); S->ev_chol.back().second = e; }
 }
 
@@ -1255,7 +1191,6 @@ void do_explicit_solve_fused(psfm_ba_solver* S, const RunCfg& c, double radius) 
   w.entries = S->d_tentries.p; w.task_slot = S->d_task_slot.p; w.task_rng = S->d_task_rng.p; w.tile_task = S->d_tile_task.p;
   w.Sband = S->d_bandrep.p; w.band_stride = S->band_n; w.nrep_mask = S->band_nrep - 1;
   w.span = S->span; w.tile_dense = S->d_tile_pairs.p;
-  { static const int dbg = getenv("PSFM_SCHUR_FLAGS") ? atoi(getenv("PSFM_SCHUR_FLAGS")) : 0; w.dbg = dbg; }
   auto mark = [&](std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& v, bool begin) {
     cudaEvent_t e = S->events.get();
     PSFM_CUDA(cudaEventRecord(e, st));
@@ -1266,7 +1201,7 @@ void do_explicit_solve_fused(psfm_ba_solver* S, const RunCfg& c, double radius) 
   if (pipe_ok(S, pipe_smem) && !getenv("PSFM_NO_PIPE_SCHUR")) {
     PipeSrc ps = pipe_src(S);
     ps.obs_a = S->d_a.p; ps.p6 = S->d_hinv.p; ps.p3a = S->d_wk.p; ps.p3b = S->d_w.p;
-    PSFM_PIPE_LAUNCH(k_schur_tile_p, pipe_smem_schur_tile, S, c.rot, ps, w);
+    PSFM_PIPE_LAUNCH(k_schur_tile_p, pipe_smem, S, c.rot, ps, w);
   } else {
     PSFM_TILE_LAUNCH(k_schur_tile, NVX2, 15, S, c.rot, w);
   }
@@ -1348,7 +1283,7 @@ StepOut compute_step(psfm_ba_solver* S, const RunCfg& c, double radius, int* npr
     max_it = c.o.exact_max_iterations > 0 ? c.o.exact_max_iterations
                                           : std::min(20000, std::max(1000, 5 * S->NS));
   }
-  const bool explicit_ok = c.solver == PSFM_BA_SOLVER_EXACT_SCHUR && c.intr <= 1 && !getenv("PSFM_EXACT_PCG") &&
+  const bool explicit_ok = c.solver == PSFM_BA_SOLVER_EXACT_SCHUR && c.intr <= 1 &&
                            (size_t)S->NS * S->NS * sizeof(double) <= ((size_t)4 << 30);
   if (explicit_ok) ensure_pairs(S);
   const bool fused = explicit_ok && S->fused;
@@ -1364,8 +1299,6 @@ StepOut compute_step(psfm_ba_solver* S, const RunCfg& c, double radius, int* npr
   // candidate: points (inside the back-substitution), poses/intrinsics, cost
   S->d_step.zero(S->stream);          // [0..3] step scalars, [4..5] the camera share (k_apply_cams): one memset
   scale_vec(S, S->d_x.p, nullptr);
-  // candidate poses / intrinsics first: they only need the reduced-system solution, and the pipelined
-  // back-substitution can then evaluate the candidate cost in the same sweep (no k_cost pass over the observations)
   ApplyArgs a;
   a.yc = S->d_x.p; a.scale_c = S->d_scale_c.p; a.active = S->d_active.p;
   a.pose = S->d_pose[S->cur].p; a.K = S->d_K[S->cur].p;
@@ -1377,32 +1310,21 @@ StepOut compute_step(psfm_ba_solver* S, const RunCfg& c, double radius, int* npr
   BackArgs b;
   b.L = lin_of(S); b.pose16 = S->d_pose16.p; b.X = S->d_X[S->cur].p; b.ht = S->d_hinv.p; b.wt = S->d_w.p;
   b.xs = S->d_xs.p; b.K = S->d_K[S->cur].p; b.Xc = S->d_X[1 - S->cur].p; b.acc = S->d_step.p; b.intr = c.intr;
-  b.pose_c = nullptr; b.K_c = S->d_K[1 - S->cur].p;
-  b.loss.type = c.o.loss_function_type; b.loss.a = c.o.loss_function_scale;
-  bool cost_fused = false;
   {
-    g_bs_nxs = S->NS;
-    static const bool no_pipe = getenv("PSFM_NO_PIPE_BACK") != nullptr, no_fuse = getenv("PSFM_FUSED_COST") == nullptr;
     const size_t lin_smem = S->tile == 256 ? pipe_smem_linearize<256>(S->cap_ns, S->cap_np) : pipe_smem_linearize<512>(S->cap_ns, S->cap_np);
-    auto bs_bytes = [&]() { return S->tile == 256 ? pipe_smem_back_substitute<256>(S->cap_ns, S->cap_np) : pipe_smem_back_substitute<512>(S->cap_ns, S->cap_np); };
-    // fused cost (opt-in, PSFM_FUSED_COST=1): the candidate pose table (8 F doubles) lives in shared memory; at least
-    // two CTAs per SM must fit.  Measured on the bench workload on an H100 SXM (700 W limit): 21.6 / 22.9 ms per solve
-    // fused against 21.0 / 21.8 ms with the separate k_cost pass (two runs each) — the table and the second 16-byte
-    // stage cost the third resident CTA, which more than cancels k_cost.  Kept for problems with few images; off by default.
-    g_bs_fuse_F = no_fuse ? 0 : S->F;
-    if (g_bs_fuse_F && !(pipe_ok(S, bs_bytes()) && (S->tile != 256 || 2 * (bs_bytes() + 1024) <= (size_t)227 * 1024))) g_bs_fuse_F = 0;
-    const size_t bs_smem = bs_bytes();
-    if (!no_pipe && pipe_ok(S, lin_smem) && pipe_ok(S, bs_smem)) {     // seg_pose exists iff the sweep was pipelined
+    const size_t bs_smem = S->tile == 256 ? pipe_smem_back_substitute<256>(S->cap_ns, S->cap_np, S->NS)
+                                          : pipe_smem_back_substitute<512>(S->cap_ns, S->cap_np, S->NS);
+    if (pipe_ok(S, lin_smem) && pipe_ok(S, bs_smem)) {     // seg_pose exists iff the sweep was pipelined
       PipeSrc ps = pipe_src(S);
       ps.obs_xy = reinterpret_cast<const double2*>(S->d_r.p); ps.obs_a = S->d_a.p; ps.p6 = S->d_hinv.p; ps.p3a = S->d_w.p;
-      if (g_bs_fuse_F) { ps.obs_xy2 = S->d_obs_xy.p; b.pose_c = S->d_pose[1 - S->cur].p; cost_fused = true; }
-      PSFM_PIPE_LAUNCH(k_back_substitute_p, pipe_smem_back_substitute, S, c.rot, ps, b);
+      PSFM_PIPE_LAUNCH(k_back_substitute_p, bs_smem, S, c.rot, ps, b);
     } else {
-      g_bs_fuse_F = 0;
       PSFM_TILE_LAUNCH(k_back_substitute, 3, 12, S, c.rot, b);
     }
   }
-  if (S->M && !cost_fused) {
+  // candidate cost over the observations (a fused form inside the back-substitution was measured slower on an H100
+  // SXM at a 700 W limit: 21.6 / 22.9 ms per solve against 21.0 / 21.8 ms with this separate pass)
+  if (S->M) {
     CostArgs ca;
     ca.pose = S->d_pose[1 - S->cur].p; ca.X = S->d_X[1 - S->cur].p; ca.K = S->d_K[1 - S->cur].p;
     ca.loss.type = c.o.loss_function_type; ca.loss.a = c.o.loss_function_scale;
@@ -1431,14 +1353,7 @@ StepOut compute_step(psfm_ba_solver* S, const RunCfg& c, double radius, int* npr
 
 int count_observed_points_all_ranks(psfm_ba_solver* S) {
   // every point lives on exactly one rank
-  if (dist::world_size() == 1) return S->P;
-  S->d_x2.zero(S->stream);
-  k_fill<<<1, 32, 0, S->stream>>>(S->d_x2.p, (double)S->P, 1);
-  PSFM_LAUNCH_CHECK();
-  dist::allreduce_sum(S->d_x2.p, 1, S->stream);
-  d2h(S, &S->hs->x2, S->d_x2.p, 1);
-  PSFM_CUDA(cudaStreamSynchronize(S->stream));
-  return (int)(S->hs->x2 + 0.5);
+  return (int)(reduce_over_ranks(S->stream, S->P, dist::allreduce_sum) + 0.5);
 }
 
 // Sharded problems: whether an image / a camera has observations — i.e. whether Ceres would add
@@ -1464,13 +1379,7 @@ void sync_observed_flags(psfm_ba_solver* S) {
 }
 
 int total_observations_all_ranks(psfm_ba_solver* S) {
-  if (dist::world_size() == 1) return S->M;
-  k_fill<<<1, 32, 0, S->stream>>>(S->d_x2.p, (double)S->M, 1);
-  PSFM_LAUNCH_CHECK();
-  dist::allreduce_sum(S->d_x2.p, 1, S->stream);
-  d2h(S, &S->hs->x2, S->d_x2.p, 1);
-  PSFM_CUDA(cudaStreamSynchronize(S->stream));
-  return (int)(S->hs->x2 + 0.5);
+  return (int)(reduce_over_ranks(S->stream, S->M, dist::allreduce_sum) + 0.5);
 }
 
 void print_summary(const psfm_ba_summary& s) {

@@ -64,8 +64,7 @@ struct PipeSrc {
   const double* seg_pose;           // [nseg][PSFM_SPS]  R (9) | t (3) | pad of the segment's image
   // what the kernel wants staged besides the structure
   const double2* obs_xy;            // [M] or null (16-byte records: the image coordinates, or the residual pairs)
-  const double2* obs_xy2;           // [M] or null (a second 16-byte record array)
-  const double* obs_a;              // [3][M] or null
+  const double* obs_a;             // [3][M] or null
   const double* X;                  // [3P]
   const double* p6;                 // [6][P] or null   -> spt rows 3..8
   const double* p3a;                // [3][P] or null   -> spt rows 9..11
@@ -102,13 +101,12 @@ __global__ void k_pipe_off32(const unsigned short* cseg_off, int nseg, int* off3
 // multiples of 16) are the same for both stages; the pointers below already include the tile's leads.
 template <int TILE>
 struct PipeLayout {
-  int o_xy, o_xy2, o_a, o_simg, o_xyz, o_spt, o_pstart, o_coff, o_cimg, o_lseg, o_lpt, o_perm, bytes;
+  int o_xy, o_a, o_simg, o_xyz, o_spt, o_pstart, o_coff, o_cimg, o_lseg, o_lpt, o_perm, bytes;
   int pstr;          // doubles per spt row (even, >= cap_np + 2)
   __host__ __device__ static int r16(int b) { return (b + 15) & ~15; }
-  __host__ __device__ PipeLayout(bool has_xy, bool has_a, int npt, int cns, int cnp, bool has_xy2 = false) {
+  __host__ __device__ PipeLayout(bool has_xy, bool has_a, int npt, int cns, int cnp) {
     int b = 0;
     o_xy = b; if (has_xy) b += 16 * TILE;
-    o_xy2 = b; if (has_xy2) b += 16 * TILE;
     o_a = b; if (has_a) b += 3 * 8 * (TILE + 2);
     o_simg = b; b += r16(8 * PSFM_SPS * cns);
     o_xyz = b; b += r16(8 * (3 * cnp + 2));
@@ -127,7 +125,6 @@ struct PipeLayout {
 template <int TILE>
 struct PipeStage {
   const double2* xy;            // [TILE]
-  const double2* xy2;           // [TILE]
   const double *a0, *a1, *a2;   // [TILE] each
   double* simg;                 // [cap_ns][PSFM_SPS]
   double* sxyz;                 // [np][3]
@@ -135,13 +132,12 @@ struct PipeStage {
   int *pstart, *coff, *cimg;
   const unsigned short *lseg, *lpt, *perm;
   int pstr, plead0, plead1;
-  static __host__ __device__ size_t bytes(bool has_xy, bool has_a, int npt, int cns, int cnp, bool has_xy2 = false) {
-    return (size_t)PipeLayout<TILE>(has_xy, has_a, npt, cns, cnp, has_xy2).bytes;
+  static __host__ __device__ size_t bytes(bool has_xy, bool has_a, int npt, int cns, int cnp) {
+    return (size_t)PipeLayout<TILE>(has_xy, has_a, npt, cns, cnp).bytes;
   }
   // mpar / ppar: parity of M and P (SoA row k of an [.][M] array starts at element k * M)
   __device__ __forceinline__ void view(unsigned char* sb, const PipeLayout<TILE>& L, int base, int pt0, int cs0, int mpar, int ppar) {
     xy = reinterpret_cast<const double2*>(sb + L.o_xy);
-    xy2 = reinterpret_cast<const double2*>(sb + L.o_xy2);
     const double* ab = reinterpret_cast<const double*>(sb + L.o_a);
     a0 = ab + (base & 1);
     a1 = ab + (TILE + 2) + ((base + mpar) & 1);
@@ -188,7 +184,6 @@ __device__ __forceinline__ PipeDesc pipe_desc(const TileCtx& tc, const PipeSrc& 
   else if (lane <= 20) { if (ps.p3a) set(ps.p3a + (size_t)(lane - 18) * P, 8, 1, 1, L.o_spt + (6 + lane - 18) * 8 * L.pstr); }
   else if (lane <= 23) { if (ps.p3b) set(ps.p3b + (size_t)(lane - 21) * P, 8, 1, 1, L.o_spt + (9 + lane - 21) * 8 * L.pstr); }
   else if (lane == 24) set(ps.tile_hdr, 32, 3, 1, 0);
-  else if (lane == 25) { if (ps.obs_xy2) set(ps.obs_xy2, 16, 0, 1, L.o_xy2); }
   return d;
 }
 
@@ -218,7 +213,7 @@ __device__ __forceinline__ void pipe_run(const TileCtx& tc, const PipeSrc& ps, u
   int tile = blockIdx.x;
   if (tile >= tc.T) return;
   const bool has_xy = ps.obs_xy != nullptr, has_a = ps.obs_a != nullptr;
-  const PipeLayout<TILE> L(has_xy, has_a, npt, cns, cnp, ps.obs_xy2 != nullptr);
+  const PipeLayout<TILE> L(has_xy, has_a, npt, cns, cnp);
   const int mpar = tc.M & 1, ppar = tc.P & 1;
   const bool issuer = tid < 32;
   // the descriptors live in shared memory (the pair loop of the Schur kernel has no registers to spare)
@@ -310,8 +305,7 @@ __global__ void __launch_bounds__(TILE, (TILE == 256 ? 3 : 1)) k_back_substitute
   __shared__ __align__(16) int4 hdr_ring[4][2];
   __shared__ __align__(8) unsigned long long bars[2];
   const int cns = tc.cap_ns, cnp = tc.cap_np;
-  const bool fuse = a.pose_c != nullptr;          // candidate cost in the same sweep (ps.obs_xy2 = image coordinates)
-  const size_t sb = PipeStage<TILE>::bytes(true, true, 12, cns, cnp, fuse);
+  const size_t sb = PipeStage<TILE>::bytes(true, true, 12, cns, cnp);
   TileSmem<TILE> sm;
   sm.cap_ns = cns; sm.cap_np = cnp;
   sm.sv = reinterpret_cast<double*>(smem_raw + 2 * sb);
@@ -320,19 +314,16 @@ __global__ void __launch_bounds__(TILE, (TILE == 256 ? 3 : 1)) k_back_substitute
   sm.sx = sm.sred + 9 * 32;
   double* xs_all = sm.sx + 6 * (size_t)cns;
   const int nxs = 6 * tc.F + 3 * tc.C;
-  // [F][8] candidate poses (fused cost only), read as 16-byte pairs: round the address up (sv has an odd length)
-  double* pose_all = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(xs_all + nxs) + 15) & ~(uintptr_t)15);
   for (int j = threadIdx.x; j < nxs; j += TILE) xs_all[j] = __ldg(a.xs + j);
-  if (fuse)
-    for (int j = threadIdx.x; j < 8 * tc.F; j += TILE) pose_all[j] = __ldg(a.pose_c + j);
   double xk[3] = {0, 0, 0};
   double inv_f = 0.0;
   if (a.intr >= 1) {
     xk[0] = __ldg(a.xs + 6 * (size_t)tc.F); xk[1] = __ldg(a.xs + 6 * (size_t)tc.F + 1); xk[2] = __ldg(a.xs + 6 * (size_t)tc.F + 2);
     inv_f = 1.0 / __ldg(a.K);
   }
-  double* racc = pose_all + (fuse ? 8 * (size_t)tc.F : 0);       // [4][TILE] running sums of this CTA's threads
-  for (int k = 0; k < 4; ++k) racc[k * TILE + threadIdx.x] = 0.0;
+  // [3][TILE] running sums of this CTA's threads, 16-byte aligned (ptxas then needs 107 instead of 121 registers at TILE 512)
+  double* racc = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(xs_all + nxs) + 15) & ~(uintptr_t)15);
+  for (int k = 0; k < 3; ++k) racc[k * TILE + threadIdx.x] = 0.0;
   __syncthreads();
   pipe_run<TILE>(tc, ps, smem_raw, hdr_ring, bars, 12, cns, cnp, [&](const TileInfo& ti, const PipeStage<TILE>& s, int tile) {
     view_stage<TILE>(sm, s);
@@ -340,34 +331,31 @@ __global__ void __launch_bounds__(TILE, (TILE == 256 ? 3 : 1)) k_back_substitute
     const bool act = tid < ti.n;
     int ls = 0, lp = 0;
     double a00 = 0, a02 = 0, a12 = 0, r0 = 0, r1 = 0;
-    double2 xy = make_double2(0.0, 0.0);
     if (act) {
       ls = s.lseg[tid]; lp = s.lpt[tid];
       a00 = s.a0[tid]; a02 = s.a1[tid]; a12 = s.a2[tid];
       const double2 rr = s.xy[tid];
       r0 = rr.x; r1 = rr.y;
-      if (fuse) xy = s.xy2[tid];
     }
     for (int j = tid; j < ti.ns * 6; j += TILE) {
       const int sg = j / 6, k = j - 6 * sg;
       sm.sx[k * cns + sg] = xs_all[6 * s.cimg[sg] + k];
     }
     __syncthreads();
-    back_substitute_tile<TILE, ROT>(tc, a, sm, ti, act, ls, lp, a00, a02, a12, r0, r1, xk, inv_f, fuse ? pose_all : nullptr, xy, racc);
+    back_substitute_tile<TILE, ROT>(tc, a, sm, ti, act, ls, lp, a00, a02, a12, r0, r1, xk, inv_f, racc);
   });
   if ((int)blockIdx.x < tc.T) {
-    double v[4] = {racc[threadIdx.x], racc[TILE + threadIdx.x], racc[2 * TILE + threadIdx.x], racc[3 * TILE + threadIdx.x]};
-    const double s = block_sum_multi<4>(v, sm.sred);
-    if (threadIdx.x < (fuse ? 4 : 3)) atomicAdd(a.acc + threadIdx.x, s);
+    double v[3] = {racc[threadIdx.x], racc[TILE + threadIdx.x], racc[2 * TILE + threadIdx.x]};
+    const double s = block_sum_multi<3>(v, sm.sred);
+    if (threadIdx.x < 3) atomicAdd(a.acc + threadIdx.x, s);
   }
 }
 
-inline int g_bs_nxs = 0;      // 6 F + 3 C of the solver being launched (set by the caller: the launch macro passes two sizes)
-inline int g_bs_fuse_F = 0;   // > 0: the candidate cost is fused (pose table of F images in shared memory)
+// nxs: length of the scaled camera step (6 F + 3 C)
 template <int TILE>
-inline size_t pipe_smem_back_substitute(int cns, int cnp) {
-  return 2 * PipeStage<TILE>::bytes(true, true, 12, cns, cnp, g_bs_fuse_F > 0) +
-         sizeof(double) * (3 * (TILE + 1) + 4 * (size_t)cnp + 9 * 32 + 6 * (size_t)cns + (size_t)g_bs_nxs + 2 + 8 * (size_t)g_bs_fuse_F + 4 * TILE);
+inline size_t pipe_smem_back_substitute(int cns, int cnp, int nxs) {
+  return 2 * PipeStage<TILE>::bytes(true, true, 12, cns, cnp) +
+         sizeof(double) * (3 * (TILE + 1) + 4 * (size_t)cnp + 9 * 32 + 6 * (size_t)cns + (size_t)nxs + 2 + 3 * TILE);
 }
 
 }  // namespace ba
