@@ -4,19 +4,22 @@
 // SPARSE_SCHUR, bundle_adjustment.cc:276-286): Ceres' SchurEliminator forms
 //     S = F'F + D_c^2 - sum_p (F'E)_p (E'E + D_p^2)^-1 (E'F)_p
 // and factorises it.  This file does the same on the GPU:
+//   pair structure   all (i, j) observation pairs of a point keyed by (tile, image a, image b),
+//                    one TASK per run of equal keys (built once per problem with a segmented
+//                    sort / run-length encode); both paths below run these tasks
 //   k_schur_tile[_p] FUSED path: per observation the compact factors [D | w | Q = Jp H~ | Jp]
 //                    stay in shared memory; per-image cross blocks / focal column / rhs
 //                    correction; the tile's pair tasks sum (W_i H~) W_j' = Jc_i' (Q_i Jp_j') Jc_j
 //                    into the band-block accumulator Sband[a][b - a][36]
-//   pair structure   all (i, j) observation pairs of a point keyed by (tile, image a, image b)
-//                    (built once per problem with radix sort / run-length encode)
-//   k_schur_w, k_schur_pairs   unfused fallback through HBM (W, W H~ per observation, AoS),
-//                    used when a tile's staging does not fit in shared memory
-//   k_schur_assemble dense symmetric S (6F+3C)^2 with Jacobi scaling, LM diagonal, gauge
-//   k_chol_blocked   cooperative blocked banded(+arrow) Cholesky and the triangular solves,
-//                    band = 6 * (longest image span of a track) — video tracks make S banded
+//   k_schur_w, k_schur_pairs   unfused fallback, used when a tile's staging does not fit the
+//                    fused kernel's shared memory: the same per-image sums and the same pair
+//                    tasks into the same Sband, with W, W H~ per observation through HBM (AoS)
+//   reduced system   [per-image sums | Sband] is all-reduced, then either assembled into a
+//                    compact band matrix for k_band_chol (ba_band_chol.cuh) or, when the band is
+//                    too wide, into dense S (k_schur_assemble_*) for k_chol_blocked: cooperative
+//                    blocked banded(+arrow) Cholesky, band = 6 * (longest image span of a track)
 // Everything accumulates with the UNSCALED factored Jacobian (see ba_kernels.cuh); the
-// scaling diag(s) is applied in k_schur_assemble.
+// scaling diag(s) is applied when the reduced system is assembled.
 #pragma once
 #include <cooperative_groups.h>
 #include <cub/cub.cuh>
@@ -27,7 +30,11 @@
 namespace psfm {
 namespace ba {
 
-constexpr int NVX = 21;   // k_schur_w per-image sums: rot-t cross block (9) | F'G focal (6) | -(W H~) Wk' (6)
+// per-image sums, stride NVX2 in the accumulator of both paths: rot-t cross block (9) | F'G focal (6) |
+// -(W H~) Wk' (6) | -(W w^) rot (3) | t (3).  k_schur_w stages and sends only the first NVX rows (its
+// shared memory is what the fallback has to fit); its rhs correction comes from k_schur_prep instead.
+constexpr int NVX = 21;
+constexpr int NVX2 = 27;
 
 // ------------------------------------------------------------------ per-observation W, W H~
 
@@ -40,7 +47,7 @@ struct SwArgs {
   const double* K;
   double* W;            // [M][18]  rows: rot 0..2, t 0..2 ; 3 values per row
   double* WH;           // [M][18]
-  double* acc_cam;      // [NREP][F][NVX]
+  double* acc_cam;      // [NREP][F][NVX2], rows NVX.. untouched
   size_t rep_stride;
   int intr;
 };
@@ -128,7 +135,7 @@ __global__ void __launch_bounds__(TILE, (TILE == 256 ? 2 : 1)) k_schur_w(const T
   __syncthreads();
   double* dst = a.acc_cam + (size_t)(blockIdx.x & (NREP - 1)) * a.rep_stride;
   tile_reduce_images<TILE>(sm, ti, NVX, [&](int k, int img, double acc) {
-    if (acc != 0.0) atomicAdd(dst + (size_t)img * NVX + k, acc);
+    if (acc != 0.0) atomicAdd(dst + (size_t)img * NVX2 + k, acc);
   });
 }
 
@@ -147,70 +154,56 @@ __global__ void k_pair_count(const int* pt_ptr, const int* obs_pt, const int* ob
   cnt[j] = c;
 }
 
-__global__ void k_pair_fill(const int* pt_ptr, const int* obs_pt, const int* obs_img, const int* ptr, int M, int F,
-                            unsigned int* keys, unsigned long long* vals) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= M) return;
-  const int p = obs_pt[j];
-  const int b = pt_ptr[p], e = pt_ptr[p + 1];
-  const int a = obs_img[j];
-  size_t o = (size_t)ptr[j];
-  for (int k = j; k < e; ++k, ++o) {
-    keys[o] = (unsigned)a * (unsigned)F + (unsigned)obs_img[k];
-    vals[o] = ((unsigned long long)(unsigned)j << 32) | (unsigned)k;
-  }
-  for (int k = j - 1; k >= b && obs_img[k] == a; --k, ++o) {
-    keys[o] = (unsigned)a * (unsigned)F + (unsigned)a;
-    vals[o] = ((unsigned long long)(unsigned)j << 32) | (unsigned)k;
-  }
-}
-
 // ------------------------------------------------------------------ block products
 
 struct PairArgs {
-  const unsigned long long* entries;   // (i << 32) | j, sorted by image pair
-  const int* chunk_blk;                // [nchunks] block id
-  const long long* chunk_beg;          // [nchunks + 1] entry range of the chunk
-  const double* W;                     // [M][18]
-  const double* WH;                    // [M][18]
-  double* Sblk;                        // [nblocks][36]  += sum (W_i H~) W_j'
+  const unsigned int* entries;   // the fused path's pair tasks (see StArgs)
+  const int* task_slot;
+  const int2* task_rng;
+  const int* tile_task;
+  const int* tile_start;         // [T + 1] first observation of the tile: entries hold tile-local indices
+  const double* W;               // [M][18]
+  const double* WH;              // [M][18]
+  double* Sband;                 // [nrep][band_stride]  += sum (W_i H~) W_j'
+  size_t band_stride;
+  int nrep_mask;
 };
 
+// One CTA per tile, one thread per pair task: the task's sum over its entries in registers, one RED per
+// element into the tile's Sband replica.  A task has few entries (one for each point that sees both
+// images), too few to pay for a reduction across lanes.
 __global__ void __launch_bounds__(128) k_schur_pairs(const PairArgs a) {
-  __shared__ double sred[36 * 4];
-  const int ch = blockIdx.x;
-  const long long beg = a.chunk_beg[ch], end = a.chunk_beg[ch + 1];
-  double acc[36];
+  const int t = blockIdx.x;
+  const size_t base = (size_t)__ldg(a.tile_start + t);
+  const int q1 = __ldg(a.tile_task + t + 1);
+  double* band = a.Sband + (size_t)(t & a.nrep_mask) * a.band_stride;
+  for (int q = __ldg(a.tile_task + t) + threadIdx.x; q < q1; q += blockDim.x) {
+    const int2 rg = __ldg(a.task_rng + q);
+    double acc[36];
 #pragma unroll
-  for (int k = 0; k < 36; ++k) acc[k] = 0.0;
-  for (long long e = beg + threadIdx.x; e < end; e += 128) {
-    const unsigned long long ij = a.entries[e];
-    const size_t i = (size_t)(ij >> 32), j = (size_t)(ij & 0xffffffffull);
-    const double2* wh = reinterpret_cast<const double2*>(a.WH + 18 * i);
-    const double2* wj = reinterpret_cast<const double2*>(a.W + 18 * j);
-    double A[18], B[18];
+    for (int k = 0; k < 36; ++k) acc[k] = 0.0;
+    for (int e = rg.x; e < rg.y; ++e) {
+      const unsigned int u = __ldg(a.entries + e);
+      const size_t i = base + (u >> 16), j = base + (u & 0xffffu);
+      const double2* wh = reinterpret_cast<const double2*>(a.WH + 18 * i);
+      const double2* wj = reinterpret_cast<const double2*>(a.W + 18 * j);
+      double A[18], B[18];
 #pragma unroll
-    for (int k = 0; k < 9; ++k) {
-      const double2 u = __ldg(wh + k), v = __ldg(wj + k);
-      A[2 * k] = u.x; A[2 * k + 1] = u.y;
-      B[2 * k] = v.x; B[2 * k + 1] = v.y;
+      for (int k = 0; k < 9; ++k) {
+        const double2 x = __ldg(wh + k), y = __ldg(wj + k);
+        A[2 * k] = x.x; A[2 * k + 1] = x.y;
+        B[2 * k] = y.x; B[2 * k + 1] = y.y;
+      }
+#pragma unroll
+      for (int r = 0; r < 6; ++r)
+#pragma unroll
+        for (int c = 0; c < 6; ++c)
+          acc[6 * r + c] += A[3 * r] * B[3 * c] + A[3 * r + 1] * B[3 * c + 1] + A[3 * r + 2] * B[3 * c + 2];
     }
+    double* dst = band + (size_t)__ldg(a.task_slot + q) * 36;
 #pragma unroll
-    for (int r = 0; r < 6; ++r)
-#pragma unroll
-      for (int c = 0; c < 6; ++c)
-        acc[6 * r + c] += A[3 * r] * B[3 * c] + A[3 * r + 1] * B[3 * c + 1] + A[3 * r + 2] * B[3 * c + 2];
-  }
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < 36; ++k) {
-    const double s = warp_sum(acc[k]);
-    if (lane == 0) sred[k * 4 + wid] = s;
-  }
-  __syncthreads();
-  if (threadIdx.x < 36) {
-    const double s = sred[threadIdx.x * 4] + sred[threadIdx.x * 4 + 1] + sred[threadIdx.x * 4 + 2] + sred[threadIdx.x * 4 + 3];
-    atomicAdd(a.Sblk + 36 * (size_t)a.chunk_blk[ch] + threadIdx.x, s);
+    for (int k = 0; k < 36; ++k)
+      if (acc[k] != 0.0) atomicAdd(dst + k, acc[k]);
   }
 }
 
@@ -226,7 +219,6 @@ __global__ void __launch_bounds__(128) k_schur_pairs(const PairArgs a) {
 // block, focal column, rhs correction -W w^) are reduced per image segment as in the other
 // tile kernels.
 
-constexpr int NVX2 = 27;   // NVX (21) | -(W w^) rot (3) | t (3)
 constexpr int PS = 18;     // shared-memory stride of one observation's record: 9 x 16 bytes, read with LDS.128 — eight
                            // consecutive records tile the 32 banks, so the records of one point (consecutive) do not collide
 
@@ -773,13 +765,10 @@ __global__ void k_schur_assemble_band(const BandAsmArgs a) {
 // ------------------------------------------------------------------ assembly of the dense reduced system
 
 struct AsmArgs {
-  const double* Sblk;       // [nblocks][36]
-  const int* blk_key;       // [nblocks] a * F + b  (a <= b)
-  int nblocks;
   const double* lin_cam;    // [F][NVL]  rot F'F (6) | t F'F (6) | ...
   const double* lin_intr;   // [C][NVI]
   const double* prep_intr;  // [C][NVI]
-  const double* xcam;       // [F][xstride] per-image sums of k_schur_w (NVX) / k_schur_tile (NVX2)
+  const double* xcam;       // [F][xstride] per-image sums (NVX2)
   int xstride;
   const double* scale_c;    // [NS]
   const double* Dc2;        // [NS]
@@ -790,19 +779,7 @@ struct AsmArgs {
   double* S;                // [lda][lda] row-major, zeroed
 };
 
-// off-diagonal / diagonal pair blocks: S[6a+r][6b+c] -= s s' Sblk (mirrored)
-__global__ void k_schur_assemble_blocks(const AsmArgs a) {
-  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= (size_t)a.nblocks * 36) return;
-  const int blk = (int)(t / 36), e = (int)(t % 36), r = e / 6, c = e % 6;
-  const int ia = a.blk_key[blk] / a.F, ib = a.blk_key[blk] % a.F;
-  const size_t row = 6 * (size_t)ia + r, col = 6 * (size_t)ib + c;
-  const double v = -a.scale_c[row] * a.scale_c[col] * a.Sblk[t];
-  atomicAdd(a.S + row * a.lda + col, v);
-  if (ia != ib) atomicAdd(a.S + col * a.lda + row, v);
-}
-
-// rank-local per-image parts: rot-t cross block of F'F and the focal column
+// per-image parts: rot-t cross block of F'F and the focal column
 __global__ void k_schur_assemble_local(const AsmArgs a) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   const int NS = a.lda, F = a.F;

@@ -155,15 +155,13 @@ struct psfm_ba_solver {
   // not yet all-reduced): linearize_and_measure computes it for gradient_max_norm, compute_step reuses it
   bool pb_fresh = false;
   double pb_radius = 0.0;
-  int nblocks = 0, nchunks = 0, bw = 0;
+  int bw = 0;
   long long npairs = 0;
-  DBuf<unsigned long long> d_entries;
-  DBuf<int> d_blk_key, d_chunk_blk, d_cholfail;
+  DBuf<int> d_cholfail;
   DBuf<unsigned int> d_cholbar;
   DBuf<double> d_cholLp, d_cholLd;
-  DBuf<long long> d_chunk_beg;
-  DBuf<double> d_W, d_WH, d_xcam, d_xcamrep, d_Sblk, d_S;
-  // fused tile path (k_schur_tile): tile-local pair tasks and the band-block accumulator
+  DBuf<double> d_W, d_WH, d_xcamrep, d_S;   // d_W, d_WH: per-observation W, W H~ of the unfused path
+  // tile-local pair tasks and the band-block accumulator (both paths); fused: k_schur_tile, else k_schur_w + k_schur_pairs
   bool fused = false;
   int span = 0, ntasks = 0, band_nrep = 1;
   size_t band_n = 0;
@@ -742,7 +740,7 @@ void cam_finalize(psfm_ba_solver* S, const RunCfg& c, double radius, bool fused)
   PSFM_LAUNCH_CHECK();
 }
 
-// fused_explicit: the rhs correction comes out of k_schur_tile (do_explicit_solve_fused), the
+// fused_explicit: the rhs correction comes out of k_schur_tile (do_explicit_solve), the
 // Schur-Jacobi blocks are not needed; only the point blocks and the intrinsics sums are made here
 void do_reduced_setup(psfm_ba_solver* S, const RunCfg& c, double radius, bool fused_explicit = false) {
   if (!(S->pb_fresh && S->pb_radius == radius)) {
@@ -908,11 +906,11 @@ __global__ void k_point_span(const int* pt_ptr, const int* obs_img, int P, int* 
   if (e > b) atomicMax(span_max, obs_img[e - 1] - obs_img[b]);
 }
 
-// The fused path ends in Sband: when the band is narrow enough for the register window of
+// Both paths end in Sband: when the band is narrow enough for the register window of
 // k_band_chol, the reduced system never exists as a dense matrix.
 void setup_band_chol(psfm_ba_solver* S) {
   const BandPlan pl = band_chol_plan(6 * S->F, S->bw, S->span);
-  S->band_chol = S->fused && pl.W > 0;
+  S->band_chol = pl.W > 0;
   if (!S->band_chol) {
     S->d_S.alloc((size_t)(S->NS + 1) * (S->NS + 1), S->stream);
     return;
@@ -920,15 +918,14 @@ void setup_band_chol(psfm_ba_solver* S) {
   S->bwk.alloc(pl, S->stream);
 }
 
-// (i, j) observation pairs of every point grouped by image pair — built once per problem
+// (i, j) observation pairs of every point as pair tasks, one per image pair of a tile, and the
+// accumulators of the exact solve (both Schur paths) — built once per problem
 void ensure_pairs(psfm_ba_solver* S) {
   if (S->pairs_ready) return;
   PhaseTimer tm;
   cudaStream_t st = S->stream;
   const int M = S->M, F = S->F;
   DBuf<int> cnt, span;
-  DBuf<unsigned int> keys, keys_out, ukeys;
-  DBuf<unsigned long long> vals;
   DBuf<int> ucount, nruns;
   cnt.alloc((size_t)M + 1, st); span.alloc(1, st); span.zero(st);
   PSFM_CUDA(cudaMemsetAsync(cnt.p + M, 0, sizeof(int), st));
@@ -966,11 +963,12 @@ void ensure_pairs(psfm_ba_solver* S) {
     const size_t smem = S->tile == 256 ? smem256 : smem512;
     S->fused = smem <= 227 * 1024 && !getenv("PSFM_SCHUR_UNFUSED");
   }
-  // fused and unfused paths all-reduce different buffers: one decision for all ranks
+  // the fused path sums the rhs correction into d_xband, the unfused one into d_prep (k_schur_prep), and each
+  // reads it back from its own accumulator after the all-reduce: one decision for all ranks
   S->fused = reduce_over_ranks(st, S->fused ? 0.0 : 1.0, dist::allreduce_max) < 0.5;
-  if (M == 0 && S->fused) {   // nothing to contribute: zero accumulators that still take part in the all-reduces
-    S->ntasks = 0; S->ndense = 0;
-    S->band_n = (size_t)F * (S->span + 1) * 36; S->band_nrep = 1;
+  S->band_n = (size_t)F * (S->span + 1) * 36;
+  if (M == 0) {   // nothing to contribute: zero accumulators that still take part in the all-reduces
+    S->ntasks = 0; S->ndense = 0; S->band_nrep = 1;
     S->d_xband.alloc((size_t)F * NVX2 + S->band_n, st);
     S->d_bandrep.alloc(S->band_n, st); S->d_bandrep.zero(st);
     S->d_xcamrep.alloc((size_t)NREP * F * NVX2, st); S->d_xcamrep.zero(st);
@@ -989,131 +987,77 @@ void ensure_pairs(psfm_ba_solver* S) {
     DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
     cub::DeviceScan::ExclusiveSum(tmp.p, need, cnt.p, ptr32.p, M + 1, st);
   }
-  if (S->fused) {
-    // ---- tile-local tasks for k_schur_tile
-    const int T = S->T;
-    int fb = 1; while ((1 << fb) < F) ++fb;
-    DBuf<unsigned long long> k64, k64_out, uk64;
-    DBuf<unsigned int> v32;
-    k64.alloc(NPr, st); k64_out.alloc(NPr, st); v32.alloc(NPr, st); S->d_tentries.alloc(NPr, st);
-    k_pair_fill_tile<<<grid_for(M), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_pt.p, S->d_obs_img.p, ptr32.p, M,
-                                                   S->d_tile_start.p, T, fb, k64.p, v32.p);
+  const int T = S->T;
+  int fb = 1; while ((1 << fb) < F) ++fb;
+  DBuf<unsigned long long> k64, k64_out, uk64;
+  DBuf<unsigned int> v32;
+  k64.alloc(NPr, st); k64_out.alloc(NPr, st); v32.alloc(NPr, st); S->d_tentries.alloc(NPr, st);
+  k_pair_fill_tile<<<grid_for(M), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_pt.p, S->d_obs_img.p, ptr32.p, M,
+                                                 S->d_tile_start.p, T, fb, k64.p, v32.p);
+  PSFM_LAUNCH_CHECK();
+  {
+    // k_pair_fill_tile writes the entries in observation order, i.e. already tile by tile: what is left is a
+    // sort of each tile's ~1.6 k entries by their image pair (the low 2 fb bits) — one pass through shared
+    // memory per tile instead of four passes of a global 64-bit radix sort over 39 M pairs
+    DBuf<int> seg; seg.alloc((size_t)T + 1, st);
+    k_tile_entry_offsets<<<grid_for((size_t)T + 1), 256, 0, st>>>(S->d_tile_start.p, ptr32.p, T, seg.p); PSFM_LAUNCH_CHECK();
+    size_t need = 0;
+    cub::DeviceSegmentedRadixSort::SortPairs(nullptr, need, k64.p, k64_out.p, v32.p, S->d_tentries.p, (int)NPr, T, seg.p, seg.p + 1, 0, 2 * fb, st);
+    DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
+    cub::DeviceSegmentedRadixSort::SortPairs(tmp.p, need, k64.p, k64_out.p, v32.p, S->d_tentries.p, (int)NPr, T, seg.p, seg.p + 1, 0, 2 * fb, st);
+  }
+  k64.release(); v32.release();
+  uk64.alloc(NPr, st); ucount.alloc(NPr + 1, st); nruns.alloc(1, st);
+  {
+    size_t need = 0;
+    cub::DeviceRunLengthEncode::Encode(nullptr, need, k64_out.p, uk64.p, ucount.p, nruns.p, (int)NPr, st);
+    DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
+    cub::DeviceRunLengthEncode::Encode(tmp.p, need, k64_out.p, uk64.p, ucount.p, nruns.p, (int)NPr, st);
+  }
+  // one task per run, i.e. per image pair of a tile; the runs are in (tile, a, b) order
+  int nr = 0;
+  PSFM_CUDA(cudaMemcpyAsync(&nr, nruns.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  PSFM_CUDA(cudaStreamSynchronize(st));
+  S->ntasks = nr;
+  S->d_task_slot.alloc(nr, st); S->d_task_rng.alloc(nr, st); S->d_tile_task.alloc((size_t)T + 1, st);
+  if (nr) {
+    DBuf<int> beg; beg.alloc(nr, st);
+    size_t need = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, need, ucount.p, beg.p, nr, st);
+    DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
+    cub::DeviceScan::ExclusiveSum(tmp.p, need, ucount.p, beg.p, nr, st);
+    k_pair_tasks<<<grid_for(nr), 256, 0, st>>>(uk64.p, ucount.p, beg.p, nr, fb, S->span, S->d_task_slot.p, S->d_task_rng.p);
     PSFM_LAUNCH_CHECK();
-    {
-      // k_pair_fill_tile writes the entries in observation order, i.e. already tile by tile: what is left is a
-      // sort of each tile's ~1.6 k entries by their image pair (the low 2 fb bits) — one pass through shared
-      // memory per tile instead of four passes of a global 64-bit radix sort over 39 M pairs
-      DBuf<int> seg; seg.alloc((size_t)T + 1, st);
-      k_tile_entry_offsets<<<grid_for((size_t)T + 1), 256, 0, st>>>(S->d_tile_start.p, ptr32.p, T, seg.p); PSFM_LAUNCH_CHECK();
-      size_t need = 0;
-      cub::DeviceSegmentedRadixSort::SortPairs(nullptr, need, k64.p, k64_out.p, v32.p, S->d_tentries.p, (int)NPr, T, seg.p, seg.p + 1, 0, 2 * fb, st);
-      DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
-      cub::DeviceSegmentedRadixSort::SortPairs(tmp.p, need, k64.p, k64_out.p, v32.p, S->d_tentries.p, (int)NPr, T, seg.p, seg.p + 1, 0, 2 * fb, st);
-    }
-    k64.release(); v32.release();
-    uk64.alloc(NPr, st); ucount.alloc(NPr + 1, st); nruns.alloc(1, st);
-    {
-      size_t need = 0;
-      cub::DeviceRunLengthEncode::Encode(nullptr, need, k64_out.p, uk64.p, ucount.p, nruns.p, (int)NPr, st);
-      DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
-      cub::DeviceRunLengthEncode::Encode(tmp.p, need, k64_out.p, uk64.p, ucount.p, nruns.p, (int)NPr, st);
-    }
-    // one task per run, i.e. per image pair of a tile; the runs are in (tile, a, b) order
-    int nr = 0;
-    PSFM_CUDA(cudaMemcpyAsync(&nr, nruns.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    S->ntasks = nr;
-    S->d_task_slot.alloc(nr, st); S->d_task_rng.alloc(nr, st); S->d_tile_task.alloc((size_t)T + 1, st);
-    if (nr) {
-      DBuf<int> beg; beg.alloc(nr, st);
-      size_t need = 0;
-      cub::DeviceScan::ExclusiveSum(nullptr, need, ucount.p, beg.p, nr, st);
-      DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
-      cub::DeviceScan::ExclusiveSum(tmp.p, need, ucount.p, beg.p, nr, st);
-      k_pair_tasks<<<grid_for(nr), 256, 0, st>>>(uk64.p, ucount.p, beg.p, nr, fb, S->span, S->d_task_slot.p, S->d_task_rng.p);
+  }
+  k_tile_tasks<<<grid_for((size_t)T + 1), 256, 0, st>>>(uk64.p, nr, fb, T, S->d_tile_task.p);
+  PSFM_LAUNCH_CHECK();
+  {
+    // PSFM_SCHUR_PAIRS=loop keeps every tile on the pair loop (measurement and tests); by default every
+    // tile whose Z fits the reduction rows takes the dense product
+    const char* e = getenv("PSFM_SCHUR_PAIRS");
+    const int allow = (e && !strcmp(e, "loop")) ? 0 : 1;
+    const size_t zcap = (size_t)NVX2 * (S->tile + 1);
+    DBuf<int> nd; nd.alloc(1, st); nd.zero(st);
+    S->d_tile_pairs.alloc((size_t)std::max(T, 1), st);
+    if (T > 0) {
+      k_tile_pairs_mode<<<grid_for(T), 256, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_cseg_ptr.p, S->d_obs_pt.p,
+                                                     S->d_obs_img.p, T, zcap, allow, S->d_tile_pairs.p, nd.p);
       PSFM_LAUNCH_CHECK();
     }
-    k_tile_tasks<<<grid_for((size_t)T + 1), 256, 0, st>>>(uk64.p, nr, fb, T, S->d_tile_task.p);
-    PSFM_LAUNCH_CHECK();
-    {
-      // PSFM_SCHUR_PAIRS=loop keeps every tile on the pair loop (measurement and tests); by default every
-      // tile whose Z fits the reduction rows takes the dense product
-      const char* e = getenv("PSFM_SCHUR_PAIRS");
-      const int allow = (e && !strcmp(e, "loop")) ? 0 : 1;
-      const size_t zcap = (size_t)NVX2 * (S->tile + 1);
-      DBuf<int> nd; nd.alloc(1, st); nd.zero(st);
-      S->d_tile_pairs.alloc((size_t)std::max(T, 1), st);
-      if (T > 0) {
-        k_tile_pairs_mode<<<grid_for(T), 256, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_cseg_ptr.p, S->d_obs_pt.p,
-                                                       S->d_obs_img.p, T, zcap, allow, S->d_tile_pairs.p, nd.p);
-        PSFM_LAUNCH_CHECK();
-      }
-      PSFM_CUDA(cudaMemcpyAsync(&S->ndense, nd.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    }
-    S->band_n = (size_t)F * (S->span + 1) * 36;
-    int nrep = 8;   // the pair-task REDs are spread over many band blocks: few replicas suffice (fold cost grows with them)
-    while (nrep > 1 && S->band_n * nrep * sizeof(double) > ((size_t)256 << 20)) nrep >>= 1;
-    S->band_nrep = nrep;
-    S->d_xband.alloc((size_t)F * NVX2 + S->band_n, st);
-    S->d_bandrep.alloc(S->band_n * nrep, st); S->d_bandrep.zero(st);
-    S->d_xcamrep.alloc((size_t)NREP * F * NVX2, st); S->d_xcamrep.zero(st);
-    S->d_cholfail.alloc(1, st);
-    setup_band_chol(S);
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    S->pairs_ready = true;
-    tm.mark("tile pair tasks (explicit Schur, fused)");
-    return;
+    PSFM_CUDA(cudaMemcpyAsync(&S->ndense, nd.p, sizeof(int), cudaMemcpyDeviceToHost, st));
   }
-  keys.alloc(NPr, st); keys_out.alloc(NPr, st); vals.alloc(NPr, st); S->d_entries.alloc(NPr, st);
-  k_pair_fill<<<grid_for(M), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_pt.p, S->d_obs_img.p, ptr32.p, M, F, keys.p, vals.p);
-  PSFM_LAUNCH_CHECK();
-  int kbits = 1; while ((1ull << kbits) < (unsigned long long)F * F) ++kbits;
-  {
-    size_t need = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, need, keys.p, keys_out.p, vals.p, S->d_entries.p, (int)NPr, 0, kbits, st);
-    DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
-    cub::DeviceRadixSort::SortPairs(tmp.p, need, keys.p, keys_out.p, vals.p, S->d_entries.p, (int)NPr, 0, kbits, st);
-  }
-  // run-length encode -> image-pair blocks
-  ukeys.alloc(NPr, st); ucount.alloc(NPr, st); nruns.alloc(1, st);
-  {
-    size_t need = 0;
-    cub::DeviceRunLengthEncode::Encode(nullptr, need, keys_out.p, ukeys.p, ucount.p, nruns.p, (int)NPr, st);
-    DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
-    cub::DeviceRunLengthEncode::Encode(tmp.p, need, keys_out.p, ukeys.p, ucount.p, nruns.p, (int)NPr, st);
-  }
-  int nb = 0;
-  PSFM_CUDA(cudaMemcpyAsync(&nb, nruns.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  PSFM_CUDA(cudaStreamSynchronize(st));
-  S->nblocks = nb;
-  std::vector<unsigned int> h_keys(nb);
-  std::vector<int> h_cnt(nb);
-  PSFM_CUDA(cudaMemcpyAsync(h_keys.data(), ukeys.p, sizeof(unsigned) * nb, cudaMemcpyDeviceToHost, st));
-  PSFM_CUDA(cudaMemcpyAsync(h_cnt.data(), ucount.p, sizeof(int) * nb, cudaMemcpyDeviceToHost, st));
-  PSFM_CUDA(cudaStreamSynchronize(st));
-  // chunks of <= 4096 entries of one block
-  const int CH = 4096;
-  std::vector<int> chunk_blk, blk_key(nb);
-  std::vector<long long> chunk_beg;
-  long long off = 0;
-  for (int b = 0; b < nb; ++b) {
-    blk_key[b] = (int)h_keys[b];
-    for (int c0 = 0; c0 < h_cnt[b]; c0 += CH) { chunk_blk.push_back(b); chunk_beg.push_back(off + c0); }
-    off += h_cnt[b];
-  }
-  chunk_beg.push_back(off);
-  // a chunk ends where the next begins, except at block boundaries: store explicit ends by
-  // making chunk_beg[k+1] the end of chunk k (chunks are consecutive in entry order)
-  S->nchunks = (int)chunk_blk.size();
-  S->d_blk_key.alloc(nb, st); S->d_blk_key.upload(blk_key.data(), nb, st);
-  S->d_chunk_blk.alloc(S->nchunks, st); S->d_chunk_blk.upload(chunk_blk.data(), S->nchunks, st);
-  S->d_chunk_beg.alloc((size_t)S->nchunks + 1, st); S->d_chunk_beg.upload(chunk_beg.data(), (size_t)S->nchunks + 1, st);
-  S->d_W.alloc(18 * (size_t)M, st); S->d_WH.alloc(18 * (size_t)M, st);
-  S->d_xcam.alloc((size_t)F * NVX, st); S->d_xcamrep.alloc((size_t)NREP * F * NVX, st); S->d_xcamrep.zero(st);
-  S->d_Sblk.alloc((size_t)nb * 36, st); S->d_S.alloc((size_t)(S->NS + 1) * (S->NS + 1), st); S->d_cholfail.alloc(1, st);
+  int nrep = 8;   // the pair-task REDs are spread over many band blocks: few replicas suffice (fold cost grows with them)
+  while (nrep > 1 && S->band_n * nrep * sizeof(double) > ((size_t)256 << 20)) nrep >>= 1;
+  S->band_nrep = nrep;
+  S->d_xband.alloc((size_t)F * NVX2 + S->band_n, st);
+  S->d_bandrep.alloc(S->band_n * nrep, st); S->d_bandrep.zero(st);
+  S->d_xcamrep.alloc((size_t)NREP * F * NVX2, st); S->d_xcamrep.zero(st);
+  S->d_cholfail.alloc(1, st);
+  if (!S->fused) { S->d_W.alloc(18 * (size_t)M, st); S->d_WH.alloc(18 * (size_t)M, st); }
+  setup_band_chol(S);
   PSFM_CUDA(cudaStreamSynchronize(st));
   S->pairs_ready = true;
-  tm.mark("pair structure (explicit Schur)");
+  tm.mark("tile pair tasks (explicit Schur)");
 }
 
 // blocked band(+arrow) Cholesky of d_S (rhs carried as the extra row) -> d_x; d_cholfail[0] = 1 on a
@@ -1181,90 +1125,66 @@ void launch_band_cholesky(psfm_ba_solver* S) {
 }
 
 
-// exact reduced-system solve, fused tile path: k_schur_tile -> band blocks -> (band matrix | dense S) -> Cholesky
-void do_explicit_solve_fused(psfm_ba_solver* S, const RunCfg& c, double radius) {
+// exact reduced-system solve: the Schur kernels (fused k_schur_tile | k_schur_w + k_schur_pairs) -> per-image sums
+// and band blocks -> all-reduce -> (band matrix | dense S) -> Cholesky; solution in d_x (d_cholfail on failure)
+void do_explicit_solve(psfm_ba_solver* S, const RunCfg& c, double radius) {
   cudaStream_t st = S->stream;
   const size_t nx = (size_t)S->F * NVX2;
-  StArgs w;
-  w.L = lin_of(S); w.pose16 = S->d_pose16.p; w.X = S->d_X[S->cur].p; w.ht = S->d_hinv.p; w.wt = S->d_w.p; w.wk = S->d_wk.p;
-  w.K = S->d_K[S->cur].p; w.acc_cam = S->d_xcamrep.p; w.rep_stride = nx; w.intr = c.intr;
-  w.entries = S->d_tentries.p; w.task_slot = S->d_task_slot.p; w.task_rng = S->d_task_rng.p; w.tile_task = S->d_tile_task.p;
-  w.Sband = S->d_bandrep.p; w.band_stride = S->band_n; w.nrep_mask = S->band_nrep - 1;
-  w.span = S->span; w.tile_dense = S->d_tile_pairs.p;
   auto mark = [&](std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& v, bool begin) {
     cudaEvent_t e = S->events.get();
     PSFM_CUDA(cudaEventRecord(e, st));
     if (begin) v.push_back({e, nullptr}); else v.back().second = e;
   };
-  mark(S->ev_sw, true);
-  const size_t pipe_smem = S->tile == 256 ? pipe_smem_schur_tile<256>(S->cap_ns, S->cap_np) : pipe_smem_schur_tile<512>(S->cap_ns, S->cap_np);
-  if (pipe_ok(S, pipe_smem) && !getenv("PSFM_NO_PIPE_SCHUR")) {
-    PipeSrc ps = pipe_src(S);
-    ps.obs_a = S->d_a.p; ps.p6 = S->d_hinv.p; ps.p3a = S->d_wk.p; ps.p3b = S->d_w.p;
-    PSFM_PIPE_LAUNCH(k_schur_tile_p, pipe_smem, S, c.rot, ps, w);
+  if (S->fused) {
+    StArgs w;
+    w.L = lin_of(S); w.pose16 = S->d_pose16.p; w.X = S->d_X[S->cur].p; w.ht = S->d_hinv.p; w.wt = S->d_w.p; w.wk = S->d_wk.p;
+    w.K = S->d_K[S->cur].p; w.acc_cam = S->d_xcamrep.p; w.rep_stride = nx; w.intr = c.intr;
+    w.entries = S->d_tentries.p; w.task_slot = S->d_task_slot.p; w.task_rng = S->d_task_rng.p; w.tile_task = S->d_tile_task.p;
+    w.Sband = S->d_bandrep.p; w.band_stride = S->band_n; w.nrep_mask = S->band_nrep - 1;
+    w.span = S->span; w.tile_dense = S->d_tile_pairs.p;
+    mark(S->ev_sw, true);
+    const size_t pipe_smem = S->tile == 256 ? pipe_smem_schur_tile<256>(S->cap_ns, S->cap_np) : pipe_smem_schur_tile<512>(S->cap_ns, S->cap_np);
+    if (pipe_ok(S, pipe_smem) && !getenv("PSFM_NO_PIPE_SCHUR")) {
+      PipeSrc ps = pipe_src(S);
+      ps.obs_a = S->d_a.p; ps.p6 = S->d_hinv.p; ps.p3a = S->d_wk.p; ps.p3b = S->d_w.p;
+      PSFM_PIPE_LAUNCH(k_schur_tile_p, pipe_smem, S, c.rot, ps, w);
+    } else {
+      PSFM_TILE_LAUNCH(k_schur_tile, NVX2, 15, S, c.rot, w);
+    }
+    mark(S->ev_sw, false);
   } else {
-    PSFM_TILE_LAUNCH(k_schur_tile, NVX2, 15, S, c.rot, w);
+    SwArgs w;
+    w.L = lin_of(S); w.pose16 = S->d_pose16.p; w.X = S->d_X[S->cur].p; w.ht = S->d_hinv.p; w.wk = S->d_wk.p;
+    w.K = S->d_K[S->cur].p; w.W = S->d_W.p; w.WH = S->d_WH.p; w.acc_cam = S->d_xcamrep.p; w.rep_stride = nx; w.intr = c.intr;
+    mark(S->ev_sw, true);
+    PSFM_TILE_LAUNCH(k_schur_w, NVX, 12, S, c.rot, w);
+    mark(S->ev_sw, false);
+    PairArgs pa;
+    pa.entries = S->d_tentries.p; pa.task_slot = S->d_task_slot.p; pa.task_rng = S->d_task_rng.p; pa.tile_task = S->d_tile_task.p;
+    pa.tile_start = S->d_tile_start.p; pa.W = S->d_W.p; pa.WH = S->d_WH.p;
+    pa.Sband = S->d_bandrep.p; pa.band_stride = S->band_n; pa.nrep_mask = S->band_nrep - 1;
+    mark(S->ev_pairs, true);
+    if (S->T > 0) { k_schur_pairs<<<S->T, 128, 0, st>>>(pa); PSFM_LAUNCH_CHECK(); }
+    mark(S->ev_pairs, false);
   }
-  mark(S->ev_sw, false);
   mark(S->ev_chol, true);
   k_fold_replicas2<<<grid_for(nx + S->band_n), 256, 0, st>>>(S->d_xband.p, S->d_xcamrep.p, nx, NREP, S->d_bandrep.p, S->band_n, S->band_nrep);
   PSFM_LAUNCH_CHECK();
   dist::allreduce_sum(S->d_xband.p, S->d_xband.n, st);
-  cam_finalize(S, c, radius, true);
+  // the unfused path's rhs correction is already in d_rhs (do_reduced_setup); rows 21.. of its sums are zero
+  if (S->fused) cam_finalize(S, c, radius, true);
   if (S->band_chol) { launch_band_cholesky(S); return; }
   S->d_S.zero(st);
   BandAsmArgs ba_;
   ba_.Sband = S->d_xband.p + nx; ba_.scale_c = S->d_scale_c.p; ba_.F = S->F; ba_.span = S->span; ba_.lda = S->NS + 1; ba_.S = S->d_S.p;
   k_schur_assemble_band<<<grid_for(S->band_n), 256, 0, st>>>(ba_); PSFM_LAUNCH_CHECK();
   AsmArgs a;
-  a.Sblk = nullptr; a.blk_key = nullptr; a.nblocks = 0;
   a.lin_cam = S->d_lin.p; a.lin_intr = S->d_lin.p + (size_t)S->F * NVL;
   a.prep_intr = S->d_prep.p + (size_t)S->F * NVL; a.xcam = S->d_xband.p; a.xstride = NVX2;
   a.scale_c = S->d_scale_c.p; a.Dc2 = S->d_Dc2.p; a.active = S->d_active.p;
   a.rhs = S->d_rhs.p;
   a.F = S->F; a.C = S->C; a.NS = S->NS; a.lda = S->NS + 1; a.S = S->d_S.p;
   k_schur_assemble_local<<<grid_for(S->F, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
-  k_schur_assemble_global<<<grid_for(S->F + S->C, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
-  k_schur_assemble_finish<<<grid_for(S->NS, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
-  launch_cholesky(S);
-}
-
-// exact reduced-system solve: explicit S, banded Cholesky; solution in d_x (d_cholfail on failure)
-void do_explicit_solve(psfm_ba_solver* S, const RunCfg& c) {
-  ensure_pairs(S);
-  cudaStream_t st = S->stream;
-  SwArgs w;
-  w.L = lin_of(S); w.pose16 = S->d_pose16.p; w.X = S->d_X[S->cur].p; w.ht = S->d_hinv.p; w.wk = S->d_wk.p;
-  w.K = S->d_K[S->cur].p; w.W = S->d_W.p; w.WH = S->d_WH.p; w.acc_cam = S->d_xcamrep.p;
-  w.rep_stride = (size_t)S->F * NVX; w.intr = c.intr;
-  auto mark = [&](std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& v, bool begin) {
-    cudaEvent_t e = S->events.get();
-    PSFM_CUDA(cudaEventRecord(e, st));
-    if (begin) v.push_back({e, nullptr}); else v.back().second = e;
-  };
-  mark(S->ev_sw, true);
-  PSFM_TILE_LAUNCH(k_schur_w, NVX, 12, S, c.rot, w);
-  mark(S->ev_sw, false);
-  fold_replicas(S, S->d_xcam.p, S->d_xcamrep.p, (size_t)S->F * NVX, nullptr, nullptr);
-  S->d_Sblk.zero(st);
-  PairArgs pa;
-  pa.entries = S->d_entries.p; pa.chunk_blk = S->d_chunk_blk.p; pa.chunk_beg = S->d_chunk_beg.p;
-  pa.W = S->d_W.p; pa.WH = S->d_WH.p; pa.Sblk = S->d_Sblk.p;
-  mark(S->ev_pairs, true);
-  if (S->nchunks) { k_schur_pairs<<<S->nchunks, 128, 0, st>>>(pa); PSFM_LAUNCH_CHECK(); }
-  mark(S->ev_pairs, false);
-  mark(S->ev_chol, true);
-  S->d_S.zero(st);
-  AsmArgs a;
-  a.Sblk = S->d_Sblk.p; a.blk_key = S->d_blk_key.p; a.nblocks = S->nblocks;
-  a.lin_cam = S->d_lin.p; a.lin_intr = S->d_lin.p + (size_t)S->F * NVL;
-  a.prep_intr = S->d_prep.p + (size_t)S->F * NVL; a.xcam = S->d_xcam.p; a.xstride = NVX;
-  a.scale_c = S->d_scale_c.p; a.Dc2 = S->d_Dc2.p; a.active = S->d_active.p;
-  a.rhs = S->d_rhs.p;
-  a.F = S->F; a.C = S->C; a.NS = S->NS; a.lda = S->NS + 1; a.S = S->d_S.p;
-  if (S->nblocks) { k_schur_assemble_blocks<<<grid_for((size_t)S->nblocks * 36), 256, 0, st>>>(a); PSFM_LAUNCH_CHECK(); }
-  k_schur_assemble_local<<<grid_for(S->F, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
-  dist::allreduce_sum(S->d_S.p, S->d_S.n, st);
   k_schur_assemble_global<<<grid_for(S->F + S->C, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
   k_schur_assemble_finish<<<grid_for(S->NS, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
   launch_cholesky(S);
@@ -1289,7 +1209,7 @@ StepOut compute_step(psfm_ba_solver* S, const RunCfg& c, double radius, int* npr
   const bool fused = explicit_ok && S->fused;
   do_reduced_setup(S, c, radius, fused);
   if (explicit_ok) {
-    if (fused) do_explicit_solve_fused(S, c, radius); else do_explicit_solve(S, c);
+    do_explicit_solve(S, c, radius);
     so.pcg_flag = PCG_SUCCESS;     // the factorisation's verdict comes back with the step scalars below
     iters = 1;
   } else {

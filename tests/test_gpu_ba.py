@@ -204,24 +204,35 @@ def test_exact_mode_principal_point_falls_back_to_tight_pcg(gpu):
     assert abs(s1.final_cost - s0.final_cost) <= 1e-6 * s0.final_cost
 
 
-def _mixed_track_problem(frames, long_len, seed):
-    """A few tracks of `long_len` observations (select the 512-wide tiles) plus short ones."""
-    a, _ = syn.make_ba_problem(frames, 24, long_len, seed=seed)
+def _mixed_track_problem(frames, long_len, seed, singles=0):
+    """A few tracks of `long_len` observations (select the 512-wide tiles) plus short ones, plus
+    `singles` points observed once, all in the last image: points are tiled in order of their
+    first image, so these come last and fill whole tiles of single-observation points."""
+    a, truth = syn.make_ba_problem(frames, 24, long_len, seed=seed)
     b, _ = syn.make_ba_problem(frames, 600, 8, seed=seed + 1)
-    return _abi.BAProblem(a.qvec, a.tvec, np.concatenate([a.xyz, b.xyz]), a.cam_params,
-                          np.concatenate([a.obs_image, b.obs_image]),
-                          np.concatenate([a.obs_point, b.obs_point + a.num_points]),
-                          np.concatenate([a.obs_xy, b.obs_xy]), a.image_camera,
-                          a.pose_constant, a.tvec_constant_mask, a.camera_constant)
+    rng = np.random.default_rng(seed + 2)
+    X = rng.uniform(-2.5, 2.5, (singles, 3))
+    Xc = X @ syn.qvec_to_rotmat(truth["qvec"][-1]).T + truth["tvec"][-1]
+    f, cx, cy = a.cam_params[0]
+    xy = f * Xc[:, :2] / Xc[:, 2:] + [cx, cy] + rng.normal(0.0, 0.5, (singles, 2))
+    P = a.num_points + b.num_points
+    return _abi.BAProblem(a.qvec, a.tvec, np.concatenate([a.xyz, b.xyz, X + rng.normal(0.0, 0.05, X.shape)]),
+                          a.cam_params,
+                          np.concatenate([a.obs_image, b.obs_image, np.full(singles, frames - 1)]),
+                          np.concatenate([a.obs_point, b.obs_point + a.num_points, P + np.arange(singles)]),
+                          np.concatenate([a.obs_xy, b.obs_xy, xy.astype(np.float32).astype(np.float64)]),
+                          a.image_camera, a.pose_constant, a.tvec_constant_mask, a.camera_constant)
 
 
-@pytest.mark.parametrize("frames,long_len,fused", [(320, 300, 1), (520, 500, 1)])
+@pytest.mark.parametrize("frames,long_len,fused", [(320, 300, 1), (520, 500, 1), (320, 300, 0)])
 def test_exact_mode_wide_tiles(gpu, frames, long_len, fused):
     """Tracks of 300 / 500 observations run the fused Schur kernel on 512-wide tiles (per-image
-    staging for up to 520 images next to the per-observation records in shared memory); the
-    unfused k_schur_w + k_schur_pairs path is covered by test_code_paths_agree.  Both sizes
-    must reproduce the oracle's exact step."""
-    p = _mixed_track_problem(frames, long_len, seed=30)
+    staging for up to 520 images next to the per-observation records in shared memory).  With
+    1100 single-observation points appended (fused=0) one tile holds 512 points next to the 300
+    images of a long track: the fused kernel's staging no longer fits in shared memory and the
+    solver falls back to k_schur_w + k_schur_pairs.  Every case must reproduce the oracle's exact
+    step."""
+    p = _mixed_track_problem(frames, long_len, seed=30, singles=0 if fused else 1100)
     o = _opts(True, True, _abi.SOLVER_EXACT_SCHUR)
     o.max_num_iterations = 3
     p0, p1 = p.copy(), p.copy()

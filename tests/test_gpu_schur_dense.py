@@ -1,7 +1,8 @@
 """The two pair phases of the fused Schur tile kernel: the per-entry loop and the dense Z Z'
-product on fp64 tensor cores (PSFM_SCHUR_PAIRS=loop | dense) are the same Schur complement
-summed in a different order.  They must give the same LM trajectory and the same parameters
-to the drift bound of test_run_to_run_drift_is_bounded."""
+product on fp64 tensor cores (PSFM_SCHUR_PAIRS=loop | dense), and the unfused fallback
+(PSFM_SCHUR_UNFUSED=1: k_schur_w + k_schur_pairs over the same pair tasks) are the same Schur
+complement summed in a different order.  They must give the same LM trajectory and the same
+parameters to the drift bound of test_run_to_run_drift_is_bounded."""
 import numpy as np
 import pytest
 
@@ -48,15 +49,18 @@ def test_dense_and_loop_pair_phases_agree(gpu, monkeypatch, kind, rot, focal):
     prob = _problem(kind)
     o = _opts(rot, focal)
     out = {}
-    for arm in ("loop", "dense"):
-        monkeypatch.setenv("PSFM_SCHUR_PAIRS", arm)
+    for arm in ("loop", "dense", "unfused"):
+        env = ("PSFM_SCHUR_UNFUSED", "1") if arm == "unfused" else ("PSFM_SCHUR_PAIRS", arm)
+        monkeypatch.setenv(*env)
         p = prob.copy()
         out[arm] = (ba.solve_problem(p, o), p)
-    monkeypatch.delenv("PSFM_SCHUR_PAIRS")
-    (sl, pl), (sd, pd) = out["loop"], out["dense"]
-    assert sl.explicit_fused == 1 and sd.explicit_fused == 1
-    assert sl.explicit_dense_tiles == 0 and sd.explicit_dense_tiles > 0
-    assert sd.num_iterations == sl.num_iterations and sd.termination == sl.termination
-    assert abs(sd.final_cost - sl.final_cost) <= 1e-11 * sl.final_cost
-    for a, b in ((pd.qvec, pl.qvec), (pd.tvec, pl.tvec), (pd.xyz, pl.xyz), (pd.cam_params, pl.cam_params)):
-        assert _rel(a, b) < 1e-9
+        monkeypatch.delenv(env[0])
+    (sl, pl), (sd, pd), (su, pu) = out["loop"], out["dense"], out["unfused"]
+    assert sl.explicit_fused == 1 and sd.explicit_fused == 1 and su.explicit_fused == 0
+    assert sl.explicit_dense_tiles == 0 and sd.explicit_dense_tiles > 0 and su.explicit_dense_tiles == 0
+    assert sl.num_pair_tasks > 0 and sd.num_pair_tasks == sl.num_pair_tasks and su.num_pair_tasks == sl.num_pair_tasks
+    for s, q in ((sd, pd), (su, pu)):
+        assert s.num_iterations == sl.num_iterations and s.termination == sl.termination
+        assert abs(s.final_cost - sl.final_cost) <= 1e-11 * sl.final_cost
+        for a, b in ((q.qvec, pl.qvec), (q.tvec, pl.tvec), (q.xyz, pl.xyz), (q.cam_params, pl.cam_params)):
+            assert _rel(a, b) < 1e-9
