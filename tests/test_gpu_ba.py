@@ -54,8 +54,8 @@ def test_linear_step_matches_cholesky(gpu, rot, focal):
         sc0, sp0, _ = oracle.ba_linear_step(prob, o, radius, _abi.SOLVER_EXACT_SCHUR)
         sc1, sp1, it = ba.ResidentSolver(prob).linear_step(o, radius)
         assert it > 0
-        assert _rel(sc1, sc0) < 1e-6, (rot, focal, radius, _rel(sc1, sc0))
-        assert _rel(sp1, sp0) < 1e-6
+        assert _rel(sc1, sc0) < 1e-9, (rot, focal, radius, _rel(sc1, sc0))
+        assert _rel(sp1, sp0) < 1e-9
 
 
 def test_iterative_linear_step_matches_oracle_pcg(gpu):
