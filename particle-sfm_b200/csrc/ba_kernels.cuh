@@ -542,7 +542,12 @@ struct PtsArgs {
   int P;
   double* ht;          // [6][P] H~ = diag(s_p) (s_p E'E s_p + D^2)^-1 diag(s_p)
   double* wt;          // [3][P] w^ = H~ E'r
-  double* acc_intr;    // [NVI] -(G'E) H~ (E'G) (6) | -(G'E) w^ (3)   (unscaled in the intrinsics)
+  // factor of H~ for the fused exact Schur kernel (null: not written).  With s_p E'E s_p + D^2 = L L',
+  // G = diag(s_p) L^-T is upper triangular and G G' = H~
+  double* gf;          // [6][P] G packed [g00 g01 g02 g11 g12 g22]
+  double* gv;          // [3][P] G' (focal row of G'E)
+  double* gu;          // [3][P] G' E'r
+  double* acc_intr;   // [NVI] -(G'E) H~ (E'G) (6) | -(G'E) w^ (3)   (unscaled in the intrinsics)
   double* acc_fail;    // [1] > 0 when a block is not positive definite
   double* gmax;        // [1] max |gradient| over point parameters (atomic max)
 };
@@ -582,6 +587,17 @@ __global__ void __launch_bounds__(256) k_point_blocks(const PtsArgs a) {
     double v00 = i00 * i00 + i10 * i10 + i20 * i20, v01 = i10 * i11 + i20 * i21, v02 = i20 * i22,
            v11 = i11 * i11 + i21 * i21, v12 = i21 * i22, v22 = i22 * i22;
     if (bad) { fail = 1.0; v00 = v11 = v22 = 1.0; v01 = v02 = v12 = 0.0; }
+    if (a.gf) {
+      // G = diag(s) L^-T (diag(s) where the inverse above was replaced by the identity)
+      double f00 = s0, f01 = 0.0, f02 = 0.0, f11 = s1, f12 = 0.0, f22 = s2;
+      if (!bad) { f00 = s0 * i00; f01 = s0 * i10; f02 = s0 * i20; f11 = s1 * i11; f12 = s1 * i21; f22 = s2 * i22; }
+      a.gf[p] = f00; a.gf[P + p] = f01; a.gf[2 * P + p] = f02;
+      a.gf[3 * P + p] = f11; a.gf[4 * P + p] = f12; a.gf[5 * P + p] = f22;
+      a.gu[p] = f00 * g0; a.gu[P + p] = f01 * g0 + f11 * g1; a.gu[2 * P + p] = f02 * g0 + f12 * g1 + f22 * g2;
+      double k0 = 0.0, k1 = 0.0, k2 = 0.0;
+      if (a.intr >= 1) { k0 = a.wk[p]; k1 = a.wk[P + p]; k2 = a.wk[2 * P + p]; }
+      a.gv[p] = f00 * k0; a.gv[P + p] = f01 * k0 + f11 * k1; a.gv[2 * P + p] = f02 * k0 + f12 * k1 + f22 * k2;
+    }
     // H~ = diag(s) Hinv diag(s)
     v00 *= s0 * s0; v01 *= s0 * s1; v02 *= s0 * s2; v11 *= s1 * s1; v12 *= s1 * s2; v22 *= s2 * s2;
     a.ht[p] = v00; a.ht[P + p] = v01; a.ht[2 * P + p] = v02;

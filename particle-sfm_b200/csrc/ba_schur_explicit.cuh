@@ -7,8 +7,8 @@
 //   pair structure   all (i, j) observation pairs of a point keyed by (tile, image a, image b),
 //                    one TASK per run of equal keys (built once per problem with a segmented
 //                    sort / run-length encode); both paths below run these tasks
-//   k_schur_tile[_p] FUSED path: per observation the compact factors [D | w | Q = Jp H~ | Jp]
-//                    stay in shared memory; per-image cross blocks / focal column / rhs
+//   k_schur_tile[_p] FUSED path: per observation Z_i = W_i G (dense tiles, H~ = G G') or the compact
+//                    factors [D | w | Q = Jp H~ | Jp] (pair loop) stay in shared memory; per-image cross blocks / focal column / rhs
 //                    correction; the tile's pair tasks sum (W_i H~) W_j' = Jc_i' (Q_i Jp_j') Jc_j
 //                    into the band-block accumulator Sband[a][b - a][36]
 //   k_schur_w, k_schur_pairs   unfused fallback, used when a tile's staging does not fit the
@@ -226,9 +226,9 @@ struct StArgs {
   Lin L;
   const double* pose16;
   const double* X;
-  const double* ht;     // [6][P]
-  const double* wt;     // [3][P] w^ = H~ g^
-  const double* wk;     // [9][P] G'E per point (focal row used)
+  const double* gf;     // [6][P] G, H~ = G G' (k_point_blocks)
+  const double* gv;     // [3][P] G' (focal row of G'E)
+  const double* gu;     // [3][P] G' g^, so that w^ = H~ g^ = G gu
   const double* K;
   double* acc_cam;      // [NREP][F][NVX2]
   size_t rep_stride;
@@ -246,7 +246,7 @@ struct StArgs {
 
 // ---- dense pair phase (tensor cores)
 //
-// For a point p with H~_p = L_p L_p' (3x3 Cholesky) and its observation i, Z_i = W_i L_p (6 x 3);
+// For a point p with H~_p = G_p G_p' (G_p from k_point_blocks) and its observation i, Z_i = W_i G_p (6 x 3);
 // then (W_i H~) W_j' = Z_i Z_j', and a tile's pair blocks are the block-upper part of Z Z' with
 // Z = (6 ns) x (3 np): block (image segment s, point p) = sum of Z_i over the observations of p in
 // s (two observations of p in one image give Z_i + Z_j, i.e. all their cross terms).  Z is staged
@@ -268,22 +268,6 @@ __device__ __forceinline__ void dmma_16x8x4(double (&d)[4], double a0, double a1
   asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
       : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
       : "d"(a0), "d"(a1), "d"(b));
-}
-
-// L = chol(H~) of a packed symmetric 3x3 [h00 h01 h02 h11 h12 h22], L packed [l00 l10 l11 l20 l21 l22];
-// false when a pivot is not positive and finite
-__device__ __forceinline__ bool chol3(const double (&h)[6], double (&l)[6]) {
-  const double d0 = h[0];
-  l[0] = sqrt(d0);
-  l[1] = h[1] / l[0];
-  l[3] = h[2] / l[0];
-  const double d1 = h[3] - l[1] * l[1];
-  l[2] = sqrt(d1);
-  l[4] = (h[4] - l[3] * l[1]) / l[2];
-  const double d2 = h[5] - l[3] * l[3] - l[4] * l[4];
-  l[5] = sqrt(d2);
-  auto ok = [](double d) { return d > 0.0 && !isinf(d); };
-  return ok(d0) && ok(d1) && ok(d2);
 }
 
 // Z Z' of the staged tile -> band blocks.  Warps take 16 x 16 output blocks (I <= J) of the
@@ -367,36 +351,31 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
   double* sv = sm.sv + tid;
 #pragma unroll
   for (int k = 0; k < NVX2; ++k) sv[k * PSFM_SVS] = 0.0;
-  // compact per-observation factors kept for the pair phase (W = Jc' Jp and W H~ = Jc' Q are
-  // never formed in memory):  rec = [a00 a02 a12 | w (3) | Q = Jp H~ (2x3) | Jp (2x3)]
+  // per-observation factors kept through the reduction (W = Jc' Jp and W H~ are never formed in memory):
+  //   pair loop   rec = [a00 a02 a12 | w (3) | Q = Jp H~ (2x3) | Jp (2x3)]
+  //   dense       rec = Z_i = Jc' (Jp G)  (6x3, row-major)
   double rec[18];
 #pragma unroll
   for (int k = 0; k < 18; ++k) rec[k] = 0.0;
-  bool pivot_bad = false;
   if (act) {
     ObsGeom g;
     load_geom<TILE>(sm, ls, lp, g);
     const int cnp = sm.cap_np;
-    double hv[6], wkp[3], wh[3];
+    double gm[6];
 #pragma unroll
-    for (int k = 0; k < 6; ++k) hv[k] = sm.prow(3 + k)[lp];
-    if (mode != TILE_PAIRS_LOOP) {
-      double lh[6];
-      pivot_bad = !chol3(hv, lh);
-    }
-#pragma unroll
-    for (int k = 0; k < 3; ++k) { wkp[k] = sm.prow(9 + k)[lp]; wh[k] = sm.prow(12 + k)[lp]; }
-    double jp[2][3], jc[2][6], Q[2][3];
+    for (int k = 0; k < 6; ++k) gm[k] = sm.prow(3 + k)[lp];
+    double jp[2][3], jc[2][6], jg[2][3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
       jp[0][k] = a00 * g.R[k] + a02 * g.R[6 + k];
       jp[1][k] = a00 * g.R[3 + k] + a12 * g.R[6 + k];
     }
+    // JG = Jp G (G upper triangular, packed [g00 g01 g02 g11 g12 g22]); W H~ v = Jc' JG (G' v) for any v
 #pragma unroll
     for (int m = 0; m < 2; ++m) {
-      Q[m][0] = jp[m][0] * hv[0] + jp[m][1] * hv[1] + jp[m][2] * hv[2];
-      Q[m][1] = jp[m][0] * hv[1] + jp[m][1] * hv[3] + jp[m][2] * hv[4];
-      Q[m][2] = jp[m][0] * hv[2] + jp[m][1] * hv[4] + jp[m][2] * hv[5];
+      jg[m][0] = jp[m][0] * gm[0];
+      jg[m][1] = jp[m][0] * gm[1] + jp[m][1] * gm[3];
+      jg[m][2] = jp[m][0] * gm[2] + jp[m][1] * gm[4] + jp[m][2] * gm[5];
     }
     if (ROT) {
       jc[0][0] = 2.0 * a02 * g.w[1]; jc[0][1] = 2.0 * (a00 * g.w[2] - a02 * g.w[0]); jc[0][2] = -2.0 * a00 * g.w[1];
@@ -407,35 +386,47 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
     }
     jc[0][3] = a00; jc[0][4] = 0.0; jc[0][5] = a02;
     jc[1][3] = 0.0; jc[1][4] = a00; jc[1][5] = a12;
-    rec[0] = a00; rec[1] = a02; rec[2] = a12;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) { rec[3 + k] = g.w[k]; rec[6 + k] = Q[0][k]; rec[9 + k] = Q[1][k]; rec[12 + k] = jp[0][k]; rec[15 + k] = jp[1][k]; }
     if (ROT) {   // rot-t cross block of F'F: (Jr' Jt)[r][c]
 #pragma unroll
       for (int r = 0; r < 3; ++r)
 #pragma unroll
         for (int c = 0; c < 3; ++c) sv[(3 * r + c) * PSFM_SVS] = jc[0][r] * jc[0][3 + c] + jc[1][r] * jc[1][3 + c];
     }
-    // per-image sums that need W = Jc' Jp and W H~ = Jc' Q contracted with a per-point 3-vector v:
-    // (W v)[r] = jc0[r] (jp0.v) + jc1[r] (jp1.v),   (W H~ v)[r] = jc0[r] (Q0.v) + jc1[r] (Q1.v)
     if (a.intr >= 1) {
       const double zf = (g.w[2] + g.tz) * inv_f;
       const double jf0 = -a02 * zf, jf1 = -a12 * zf;
-      const double qk0 = Q[0][0] * wkp[0] + Q[0][1] * wkp[1] + Q[0][2] * wkp[2];
-      const double qk1 = Q[1][0] * wkp[0] + Q[1][1] * wkp[1] + Q[1][2] * wkp[2];
+      const double gk[3] = {sm.prow(9)[lp], sm.prow(10)[lp], sm.prow(11)[lp]};
+      const double qk0 = jg[0][0] * gk[0] + jg[0][1] * gk[1] + jg[0][2] * gk[2];
+      const double qk1 = jg[1][0] * gk[0] + jg[1][1] * gk[1] + jg[1][2] * gk[2];
 #pragma unroll
       for (int r = 0; r < 6; ++r) {
         sv[(9 + r) * PSFM_SVS] = jc[0][r] * jf0 + jc[1][r] * jf1;            // F'G
         sv[(15 + r) * PSFM_SVS] = -(jc[0][r] * qk0 + jc[1][r] * qk1);          // -(W H~) Wk'
       }
     }
-    const double pw0 = jp[0][0] * wh[0] + jp[0][1] * wh[1] + jp[0][2] * wh[2];
-    const double pw1 = jp[1][0] * wh[0] + jp[1][1] * wh[1] + jp[1][2] * wh[2];
+    const double gg[3] = {sm.prow(12)[lp], sm.prow(13)[lp], sm.prow(14)[lp]};
+    const double pw0 = jg[0][0] * gg[0] + jg[0][1] * gg[1] + jg[0][2] * gg[2];
+    const double pw1 = jg[1][0] * gg[0] + jg[1][1] * gg[1] + jg[1][2] * gg[2];
 #pragma unroll
     for (int r = (ROT ? 0 : 3); r < 6; ++r) sv[(21 + r) * PSFM_SVS] = -(jc[0][r] * pw0 + jc[1][r] * pw1);   // -(W w^)
+    if (mode == TILE_PAIRS_LOOP) {
+      rec[0] = a00; rec[1] = a02; rec[2] = a12;
+#pragma unroll
+      for (int m = 0; m < 2; ++m) {   // Q = JG G'
+        rec[6 + 3 * m] = jg[m][0] * gm[0] + jg[m][1] * gm[1] + jg[m][2] * gm[2];
+        rec[7 + 3 * m] = jg[m][1] * gm[3] + jg[m][2] * gm[4];
+        rec[8 + 3 * m] = jg[m][2] * gm[5];
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { rec[3 + k] = g.w[k]; rec[12 + k] = jp[0][k]; rec[15 + k] = jp[1][k]; }
+    } else {
+#pragma unroll
+      for (int r = 0; r < 6; ++r)
+#pragma unroll
+        for (int k = 0; k < 3; ++k) rec[3 * r + k] = jc[0][r] * jg[0][k] + jc[1][r] * jg[1][k];
+    }
   }
-  // a point whose H~ has no Cholesky factor sends the whole tile to the pair loop
-  const bool dense = !__syncthreads_or(pivot_bad) && mode != TILE_PAIRS_LOOP;
+  __syncthreads();
   {
     double* dst = a.acc_cam + (size_t)(rep & (NREP - 1)) * a.rep_stride;
     tile_reduce_images<TILE>(sm, ti, NVX2, [&](int k, int img, double acc) {
@@ -444,44 +435,26 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
   }
   __syncthreads();
   double* band = a.Sband + (size_t)(rep & a.nrep_mask) * a.band_stride;
-  if (dense) {
-    // the reduction rows are dead: stage Z (zero blocks where a point has no observation)
+  if (mode != TILE_PAIRS_LOOP) {
+    // the reduction rows are dead: stage Z there
     double* zf = sm.sv;
-    const int nz2 = (int)(dense_z_doubles(ti.ns, ti.np) / 2);
+    const int KB2 = dense_z_kb2(ti.np), zrows = 16 * dense_z_rb(ti.ns), zcols = 8 * KB2;
+    auto zat = [&](int row, int col) -> double* {
+      const int q = row >> 3;
+      return zf + (((q * KB2 + (col >> 3)) * 32 + (((row & 7) * 4 + (col & 3)) ^ (q & 7))) * 2 + ((col >> 2) & 1));
+    };
+    // zero blocks where a point has no observation; two observations of a point in one image
+    // (TILE_PAIRS_DENSE_DUP) add into one block
+    const int nz2 = zrows * zcols / 2;
     for (int k = tid; k < nz2; k += TILE) reinterpret_cast<double2*>(zf)[k] = make_double2(0.0, 0.0);
     __syncthreads();
     if (act) {
-      // Z_i = Jc' (Jp L): Jc from the record as in the per-observation phase above; L is recomputed
-      // here rather than kept live through the reduction (register pressure)
-      double hv[6], lh[6];
 #pragma unroll
-      for (int k = 0; k < 6; ++k) hv[k] = sm.prow(3 + k)[lp];
-      chol3(hv, lh);
-      const double w0 = rec[3], w1 = rec[4], w2 = rec[5];
-      double jl[2][3], jc[2][6];
-#pragma unroll
-      for (int m = 0; m < 2; ++m) {
-        const double p0 = rec[12 + 3 * m], p1 = rec[13 + 3 * m], p2 = rec[14 + 3 * m];
-        jl[m][0] = p0 * lh[0] + p1 * lh[1] + p2 * lh[3];
-        jl[m][1] = p1 * lh[2] + p2 * lh[4];
-        jl[m][2] = p2 * lh[5];
-      }
-      if (ROT) {
-        jc[0][0] = 2.0 * a02 * w1; jc[0][1] = 2.0 * (a00 * w2 - a02 * w0); jc[0][2] = -2.0 * a00 * w1;
-        jc[1][0] = 2.0 * (a12 * w1 - a00 * w2); jc[1][1] = -2.0 * a12 * w0; jc[1][2] = 2.0 * a00 * w0;
-      }
-      jc[0][3] = a00; jc[0][4] = 0.0; jc[0][5] = a02;
-      jc[1][3] = 0.0; jc[1][4] = a00; jc[1][5] = a12;
-      const int KB2 = dense_z_kb2(ti.np);
-#pragma unroll
-      for (int r = (ROT ? 0 : 3); r < 6; ++r)
+      for (int r = 0; r < 6; ++r)
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
-          const int row = 6 * ls + r, col = 3 * lp + k;
-          const int q = row >> 3;
-          double* z = zf + (((q * KB2 + (col >> 3)) * 32 + (((row & 7) * 4 + (col & 3)) ^ (q & 7))) * 2 + ((col >> 2) & 1));
-          const double v = jc[0][r] * jl[0][k] + jc[1][r] * jl[1][k];
-          if (mode == TILE_PAIRS_DENSE_DUP) atomicAdd(z, v); else *z = v;
+          double* z = zat(6 * ls + r, 3 * lp + k);
+          if (mode == TILE_PAIRS_DENSE_DUP) atomicAdd(z, rec[3 * r + k]); else *z = rec[3 * r + k];
         }
     }
     __syncthreads();
@@ -628,8 +601,8 @@ __global__ void __launch_bounds__(TILE, (TILE == 256 ? 2 : 1)) k_schur_tile(cons
     a00 = a.L.a[i]; a02 = a.L.a[M + i]; a12 = a.L.a[2 * M + i];
   }
   const int t0 = __ldg(a.tile_task + blockIdx.x), nt = __ldg(a.tile_task + blockIdx.x + 1) - t0;
-  // per point: X (0..2), H~ (3..8), focal row of G'E (9..11), w^ (12..14)
-  tile_fill_smem<TILE>(tc, sm, ti, a.pose16, nullptr, a.X, a.ht, a.wk, true, a.wt);
+  // per point: X (0..2), G (3..8), G' (focal row of G'E) (9..11), G' g^ (12..14)
+  tile_fill_smem<TILE>(tc, sm, ti, a.pose16, nullptr, a.X, a.gf, a.gv, true, a.gu);
   schur_tile_body<TILE, ROT>(tc, a, sm, ti, act, ls, lp, a00, a02, a12, blockIdx.x, t0, nt);
 }
 

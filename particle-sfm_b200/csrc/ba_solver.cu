@@ -169,6 +169,7 @@ struct psfm_ba_solver {
   DBuf<int> d_task_slot, d_tile_task;
   DBuf<int2> d_task_rng;
   DBuf<double> d_xband, d_bandrep;      // d_xband = [xcam F*NVX2 | Sband band_n] (one all-reduce)
+  DBuf<double> d_gf, d_gv, d_gu;        // fused path: factor G of H~ and G' (focal row of G'E), G' E'r (k_point_blocks)
   DBuf<unsigned char> d_tile_pairs;     // [T] pair phase of each tile (TILE_PAIRS_*)
   int ndense = 0;                       // tiles whose pair phase is the dense product
   // single-CTA sliding-window band Cholesky (ba_band_chol.cuh): compact band matrix, factor, scratch
@@ -713,6 +714,8 @@ void do_point_blocks(psfm_ba_solver* S, const RunCfg& c, double radius) {
   a.radius = radius; a.min_diag = c.o.min_lm_diagonal; a.max_diag = c.o.max_lm_diagonal;
   a.intr = c.intr; a.P = S->P;
   a.ht = S->d_hinv.p; a.wt = S->d_w.p;
+  const bool gfac = S->pairs_ready && S->fused;
+  a.gf = gfac ? S->d_gf.p : nullptr; a.gv = S->d_gv.p; a.gu = S->d_gu.p;
   a.acc_intr = S->d_prep.p + (size_t)S->F * NVL;
   a.acc_fail = S->d_prep.p + (size_t)S->F * NVL + (size_t)S->C * NVI;
   a.gmax = S->d_gmax.p;
@@ -966,6 +969,10 @@ void ensure_pairs(psfm_ba_solver* S) {
   // the fused path sums the rhs correction into d_xband, the unfused one into d_prep (k_schur_prep), and each
   // reads it back from its own accumulator after the all-reduce: one decision for all ranks
   S->fused = reduce_over_ranks(st, S->fused ? 0.0 : 1.0, dist::allreduce_max) < 0.5;
+  if (S->fused) {
+    S->d_gf.alloc(6 * (size_t)S->P, st); S->d_gv.alloc(3 * (size_t)S->P, st); S->d_gu.alloc(3 * (size_t)S->P, st);
+    S->pb_fresh = false;     // point blocks computed before the factor had a buffer: recompute them with it
+  }
   S->band_n = (size_t)F * (S->span + 1) * 36;
   if (M == 0) {   // nothing to contribute: zero accumulators that still take part in the all-reduces
     S->ntasks = 0; S->ndense = 0; S->band_nrep = 1;
@@ -1137,7 +1144,7 @@ void do_explicit_solve(psfm_ba_solver* S, const RunCfg& c, double radius) {
   };
   if (S->fused) {
     StArgs w;
-    w.L = lin_of(S); w.pose16 = S->d_pose16.p; w.X = S->d_X[S->cur].p; w.ht = S->d_hinv.p; w.wt = S->d_w.p; w.wk = S->d_wk.p;
+    w.L = lin_of(S); w.pose16 = S->d_pose16.p; w.X = S->d_X[S->cur].p; w.gf = S->d_gf.p; w.gv = S->d_gv.p; w.gu = S->d_gu.p;
     w.K = S->d_K[S->cur].p; w.acc_cam = S->d_xcamrep.p; w.rep_stride = nx; w.intr = c.intr;
     w.entries = S->d_tentries.p; w.task_slot = S->d_task_slot.p; w.task_rng = S->d_task_rng.p; w.tile_task = S->d_tile_task.p;
     w.Sband = S->d_bandrep.p; w.band_stride = S->band_n; w.nrep_mask = S->band_nrep - 1;
@@ -1146,7 +1153,7 @@ void do_explicit_solve(psfm_ba_solver* S, const RunCfg& c, double radius) {
     const size_t pipe_smem = S->tile == 256 ? pipe_smem_schur_tile<256>(S->cap_ns, S->cap_np) : pipe_smem_schur_tile<512>(S->cap_ns, S->cap_np);
     if (pipe_ok(S, pipe_smem) && !getenv("PSFM_NO_PIPE_SCHUR")) {
       PipeSrc ps = pipe_src(S);
-      ps.obs_a = S->d_a.p; ps.p6 = S->d_hinv.p; ps.p3a = S->d_wk.p; ps.p3b = S->d_w.p;
+      ps.obs_a = S->d_a.p; ps.p6 = S->d_gf.p; ps.p3a = S->d_gv.p; ps.p3b = S->d_gu.p;
       PSFM_PIPE_LAUNCH(k_schur_tile_p, pipe_smem, S, c.rot, ps, w);
     } else {
       PSFM_TILE_LAUNCH(k_schur_tile, NVX2, 15, S, c.rot, w);
