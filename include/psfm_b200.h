@@ -385,7 +385,9 @@ int psfm_measure_dfma(double* dfma_per_second, double* dependent_latency_cycles)
      A   [n][n] row-major symmetric, n = nb + 3: A[i][j] == 0 for |i - j| > bw among the
          first nb rows/columns, the last 3 rows/columns are dense (the shared camera)
      b   [n]     x [n] receives the solution.  Returns PSFM_OK, PSFM_ERR_INVALID when the
-   matrix is not positive definite, PSFM_ERR_UNSUPPORTED when bw exceeds the register window. */
+   matrix is not positive definite, PSFM_ERR_UNSUPPORTED when nb is not a multiple of 6 of at
+   least 18, or when the block window (min(bw, nb - 1) + 5) / 6 + 1 exceeds 25 blocks and
+   nb / 6 does too. */
 int psfm_ba_band_solve(const double* A, const double* b, int32_t nb, int32_t bw, double* x);
 
 /* ------------------------------------------------------------------------- */

@@ -1,4 +1,4 @@
-// ba_band_chol.cuh — the reduced camera system of a VIDEO (banded + arrow) solved by ONE CTA.
+// ba_band_chol.cuh — the reduced camera system of a VIDEO (banded + arrow) solved by one CTA (or two).
 //
 // Exact-Schur mode (reference rule for <= 1000 images, bundle_adjustment.cc:276-286; Ceres
 // SchurComplementSolver semantics, SURVEY.md A.6): S y = rhs with S = 6F x 6F banded (half
@@ -10,20 +10,15 @@
 //
 //   k_band_assemble  band blocks + per-image sums -> compact scaled band matrix Ab (each entry
 //                    written exactly once; the dense (6F+3)^2 S is never formed or zeroed)
-//   k_band_chol      right-looking Cholesky on a sliding W x W window (W >= bw + 1, multiple
-//                    of 4).  Index i lives at circular position i mod W; the symmetric window
-//                    is held as unordered pairs of positions {p, q}, one 4 x 4 block of pairs
-//                    per thread.  Per pivot j: the owners of column j publish it to shared
-//                    memory, ONE __syncthreads, every thread applies the rank-1 update to its
-//                    block (1/d recomputed redundantly: no second barrier), the freed slots are
-//                    refilled with row j + W, which a streaming warp copies 4 pivots ahead with
-//                    cp.async into an 8-row ring (already permuted to window positions); an
-//                    output warp writes the finished column of L.  Each role runs its OWN small
-//                    loop (bar.sync from three program counters).  The 4 arrow rows (3 intrinsics + the rhs, so
-//                    that L^-1 b falls out of the same sweep) are one more block row; their 4x4
-//                    corner one more thread.  Then L' x = y by warp 0 in axpy form (per pivot:
-//                    one multiply, one shuffle, one fma on the chain), the rows of L staged
-//                    chunk-wise into shared memory by the other warps.
+//   k_band_chol6     right-looking Cholesky on a sliding window of Wb 6 x 6 image blocks (W = 6 Wb > bw,
+//                    3 <= Wb <= 25), one BLOCK pivot per step: block index I lives at ring position I mod Wb,
+//                    the symmetric window is held as unordered pairs of positions {P, Q}, a tile of one 6 x 6
+//                    block per worker thread.  Workers, panel group and loader each run their OWN small loop
+//                    (named barriers from different program counters; see the comment above the kernel).
+//                    The 4 arrow rows (3 intrinsics + the rhs, so that L^-1 b falls out of the same sweep)
+//                    are one more block row of the window.  Then L' x = y by warp 0 in axpy form (per pivot:
+//                    one multiply, one shuffle, one fma on the chain), the rows of L staged chunk-wise into
+//                    shared memory by the other warps (bc_tail).
 //                    TWO-SIDED form (gridDim.x = 2, matrices of >= 4 windows): the chain of nb dependent
 //                    pivots is cut in two.  CTA 0 factors the leading k0 pivots of A top-down, CTA 1
 //                    the trailing n1 pivots bottom-up (the same code on the index-reversed matrix);
@@ -34,32 +29,20 @@
 //                    corner.  The back substitution mirrors it: CTA 0 solves the middle rows first
 //                    and releases them, then both CTAs walk outwards.  Same arithmetic per pivot as
 //                    the one-sided form, different (but fixed) elimination order.
-// tools/emu_band_chol.py is a thread-level numpy emulation of the one-sided window logic.
+// Block windows wider than 25 images, and systems of fewer than 3 images, go to the dense S + k_chol_blocked route.
 #pragma once
 #include "ba_schur_explicit.cuh"
 
 namespace psfm {
 namespace ba {
 
-constexpr int BC_RING = 8;        // ring of upcoming rows (streamed 4 pivots ahead)
-constexpr int BC_MAXW = 152;      // window limit: (W/4 + 1)(W/4 + 2)/2 workers + W + 4 helper lanes <= 1024 threads
-constexpr int BC_CSM = 184;       // FIXED shared-memory row stride of colbuf / ring (addresses become immediates):
-                                  // bc_idx(BC_MAXW + 7) < 184
-// Window position p lives at double index p + 2 (p / 16): 16 bytes of padding after every 128.
-// A warp's lanes read 32 consecutive bytes each (their block of 4 positions) with two LDS.128; at a
-// plain 32-byte stride the lanes q and q + 4 of a quarter warp hit the same banks (2-way conflict:
-// measured, the workers were bound by shared-memory wavefronts), with the padding they do not.
-__host__ __device__ __forceinline__ constexpr int bc_idx(int p) { return p + ((p >> 4) << 1); }
-
 constexpr int BC_MAXSLOT = 7;     // 1 + ceil(bw / 32) register slots of the back substitution
 
 // Split of the pivot chain (band_chol_plan): one-sided (two = 0) or two-sided.
 struct BandPlan {
-  int nb, bw, W, RS;
+  int nb, bw, W, RS;        // nb multiple of 6, W = 6 Wb with 3 <= Wb <= 25 (W = 0: no band plan)
   int two;                  // 1: two CTAs
-  int blk6;                 // 1: block-6 kernel k_band_chol6 (nb and bw + 1 multiples of 6, 3 <= W / 6 <= 25)
-  int nbp;                  // nb rounded up to 8 (identity padding rows)
-  int k0, n1;               // pivots factored top-down before the hand-over | bottom-up; k0 + W + n1 = nbp
+  int k0, n1;               // pivots factored top-down before the hand-over | bottom-up; k0 + W + n1 = nb
   int nbs[2];               // rows of the matrix each side sees: k0 + W | n1 + W   (one-sided: nb | 0)
   int npiv[2];              // pivots each side factors:           k0 + W | n1       (one-sided: nb | 0)
   int rows[2];              // rows of Ab each side may touch (band_chol_rows)
@@ -81,7 +64,7 @@ struct BandAsmArgs2 {
   double* Ab;               // side 0 [rows[0]][RS]: Ab[r][k] = A[r][r - k] (k <= bw), Ab[r][W + a] = A[nb + a][r], a < 3; Ab[r][W + 3] = rhs[r]
   double* Ab1;              // side 1 [rows[1]][RS]: the same of the index-reversed matrix, middle block and middle arrow zero
   double* C4;               // [2][4][4] arrow corner: intrinsics block (3 x 3) | rhs entries in row / column 3; side 1: zero
-  int* fail;                // cleared here, set by k_band_chol
+  int* fail;                // cleared here, set by k_band_chol6
 };
 
 // packed index of element (r, c) of a symmetric 3 x 3 stored as 00 01 02 11 12 22
@@ -150,8 +133,8 @@ __global__ void k_band_assemble(const BandAsmArgs2 a) {
     }
     a.Ab[t] = v;
   } else if (t < n0 + n1) {
-    // index-reversed matrix B[r'][c'] = A[nbp-1-r'][nbp-1-c']: its lower element (r', r' - e) is the
-    // lower element (R, R - e) of A with R = nbp - 1 - (r' - e).  Rows / columns >= n1 are the middle
+    // index-reversed matrix B[r'][c'] = A[nb-1-r'][nb-1-c']: its lower element (r', r' - e) is the
+    // lower element (R, R - e) of A with R = nb - 1 - (r' - e).  Rows / columns >= n1 are the middle
     // block, which side 0 owns: zero here, so that what is left in the window is the pure update.
     const size_t u = t - n0;
     const int r = (int)(u / RS), e = (int)(u % RS);
@@ -160,9 +143,9 @@ __global__ void k_band_assemble(const BandAsmArgs2 a) {
       v = (e == 0) ? 1.0 : 0.0;
     } else if (e < W) {
       const int c = r - e;
-      if (e <= pl.bw && c >= 0 && !(r >= pl.n1 && c >= pl.n1)) v = band_entry(a, pl.nbp - 1 - c, e);
+      if (e <= pl.bw && c >= 0 && !(r >= pl.n1 && c >= pl.n1)) v = band_entry(a, pl.nb - 1 - c, e);
     } else if (r < pl.n1) {
-      v = arrow_entry(a, pl.nbp - 1 - r, e - W);
+      v = arrow_entry(a, pl.nb - 1 - r, e - W);
     }
     a.Ab1[u] = v;
   }
@@ -171,7 +154,7 @@ __global__ void k_band_assemble(const BandAsmArgs2 a) {
 struct BandSide {
   const double* Ab;
   const double* C4;
-  int nb, npiv;             // rows of this side's matrix | pivots it factors (multiple of 8 in the two-sided form)
+  int nb, npiv;             // rows of this side's matrix | pivots it factors (multiple of 6)
   double* Lr;               // [nb][bw + 1]  UNNORMALISED columns: Lr[r][k] = A~[r][r - k] (= L[r][r - k] sqrt(d[r - k]))
   double* La;               // [4][nb]       unnormalised arrow rows (row 3 = rhs)
   double* dinv;             // [nb]          pivots d[j], replaced by 1 / sqrt(d[j]) after the factorisation
@@ -179,14 +162,15 @@ struct BandSide {
 
 struct BandCholArgs {
   BandSide s[2];            // blockIdx.x = side
-  int two, nbg, nbp, k0;    // two-sided | rows of the whole matrix | padded to 8 | pivots of side 0 before the hand-over
-  int bw, W, RS, ns;        // ns: length of x (slots past nbg + 3 — other cameras — are zeroed)
+  // two-sided | value of the sync flags for this launch | rows of the whole matrix | pivots of side 0 before the
+  // hand-over.  The field order matters to k_band_chol6's register allocation under its 128-register cap: with
+  // bw .. ns at other offsets, ptxas spilled inside the factorisation loop of the 512-thread 3 x 3 instantiation.
+  int two, epoch, nb, k0;
+  int bw, W, RS, ns;        // ns: length of x (slots past nb + 3 — other cameras — are zeroed)
   double* x;                // [ns]
   int* fail;                // OR of both sides (cleared by k_band_assemble)
   double* D;                // hand-over of side 1: [W][W] update of the middle block (A orientation) | [4][W] arrow | [16] corner
   int* sync;                // [2] = epoch once: 0 the hand-over is written, 1 the middle x and the intrinsics are written
-  int epoch;
-  int blk6;                 // k_band_chol6 (plan)
 };
 
 __device__ __forceinline__ void bc_post(int* flag, int v) {
@@ -200,14 +184,6 @@ __device__ __forceinline__ void bc_wait(const int* flag, int v) {
   } while (x != v);
 }
 
-// bar.sync 0 from role-specific loops: every thread of the CTA executes the same NUMBER of
-// barriers, from different program counters.  One warp runs dependent scalar code at several
-// cycles per instruction, so what a role does per pivot is counted in instructions — a first
-// version (all roles interleaved in one unrolled body, index arithmetic per pivot) was several
-// times slower per pivot.  Hence: per-role loops, compile-time shared-memory offsets,
-// one element per helper lane, no early exit.
-__device__ __forceinline__ void bc_bar() { asm volatile("bar.sync 0;\n" ::: "memory"); }
-
 // 1 / d to full double precision (not correctly rounded): MUFU seed + two Newton steps — about
 // half the dependent latency of the IEEE division, which sits on the pivot-to-pivot chain
 __device__ __forceinline__ double bc_rcp(double d) {
@@ -219,10 +195,9 @@ __device__ __forceinline__ double bc_rcp(double d) {
   return fma(r, e, r);
 }
 
-// Everything after the factorisation, shared by k_band_chol and k_band_chol6: normalisation, the 3 x 3 arrow corner
-// (s_c4: the 4 x 4 corner block of the window, written to shared memory by its owner before the caller's barrier),
-// hand-shake of the two-sided form, back substitution.  Called by every thread of the CTA.
-template <int RP>
+// Everything after the factorisation: normalisation, the 3 x 3 arrow corner (s_c4: the 4 x 4 corner block of the
+// window, written to shared memory by its owner before the caller's barrier), hand-shake of the two-sided form, back
+// substitution.  Called by every thread of the CTA.
 __device__ __forceinline__ void bc_tail(const BandCholArgs& a, const BandSide& sd, const int side, double* stage, int& s_fail,
                                         double* s_xI, const double* s_c4) {
   const int tid = threadIdx.x, lane = tid & 31;
@@ -253,12 +228,12 @@ __device__ __forceinline__ void bc_tail(const BandCholArgs& a, const BandSide& s
       if (a.two && tid == 0) bc_post(a.sync + 1, a.epoch);     // side 1 must not wait for ever
       return;
     }
-    for (int s = a.nbg + tid; s < a.ns; s += blockDim.x) a.x[s] = (s < a.nbg + 3) ? s_xI[s - a.nbg] : 0.0;
+    for (int s = a.nb + tid; s < a.ns; s += blockDim.x) a.x[s] = (s < a.nb + 3) ? s_xI[s - a.nb] : 0.0;
   } else {
     // the middle x and the intrinsics come from side 0
     if (tid == 0) {
       bc_wait(a.sync + 1, a.epoch);
-      for (int k = 0; k < 3; ++k) s_xI[k] = __ldcg(a.x + a.nbg + k);
+      for (int k = 0; k < 3; ++k) s_xI[k] = __ldcg(a.x + a.nb + k);
     }
     __syncthreads();
   }
@@ -279,8 +254,9 @@ __device__ __forceinline__ void bc_tail(const BandCholArgs& a, const BandSide& s
   // dependent load pair per element the staging, not the substitution chain, set the pace (measured: 7.5 k cycles
   // per 32-row chunk against 1.3 k for the chain)
   auto stage_chunk = [&](int c, double* buf, int w0, int nw) {
-    // RP rows per pass (2 in the block-6 kernel): with 8 warps (the block-6 kernel) a warp stages ~5 rows of a chunk, one global-memory
-    // latency each would outlast the substitution chain of the chunk
+    // RP rows per pass: with 8 warps a warp stages ~5 rows of a chunk, one global-memory latency each would outlast
+    // the substitution chain of the chunk
+    constexpr int RP = 2;
     for (int j0 = w0; j0 < 32; j0 += RP * nw) {
       double lv[RP][BC_MAXSLOT], dv[RP][BC_MAXSLOT];
 #pragma unroll
@@ -326,9 +302,9 @@ __device__ __forceinline__ void bc_tail(const BandCholArgs& a, const BandSide& s
       const double fresh = (c > 0) ? y0(32 * (c - ms) + lane) : 0.0;     // slot ms - 1 of the next chunk
       const int jl = 32 * c + lane;
       const double dl = (jl < npiv) ? __ldcg(sd.dinv + jl) : 0.0;
-      // global index of local row jl: side 0 jl, side 1 nbp - 1 - jl; rows past nbg are identity padding (x = 0)
-      const int gl = side ? a.nbp - 1 - jl : jl;
-      const bool inx = jl < nb && gl >= 0 && gl < a.nbg;
+      // global index of local row jl: side 0 jl, side 1 a.nb - 1 - jl; rows >= this side's nb (last chunk) write nothing
+      const int gl = side ? a.nb - 1 - jl : jl;
+      const bool inx = jl < nb && gl >= 0 && gl < a.nb;
       const double xk = (jl >= npiv && inx) ? __ldcg(a.x + gl) : 0.0;   // known x (side 1: middle rows)
       const bool wr = jl < npiv && inx;
       double* xw = a.x + (inx ? gl : 0);
@@ -362,256 +338,10 @@ __device__ __forceinline__ void bc_tail(const BandCholArgs& a, const BandSide& s
   }
 }
 
-// Roles: workers (one BS x BS block of window slots each), helper lanes (one element each:
-// stream entry e of the upcoming rows into the ring with cp.async, 4 pivots ahead, and write
-// entry e of the finished column to global memory).
-template <int BS, int MAXT>
-__global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
-  extern __shared__ __align__(16) double bc_smem[];
-  __shared__ int s_fail;
-  __shared__ double s_xI[4];
-  __shared__ double s_c4[16];
-  constexpr int UN = 8;                     // pivots per unrolled body: ring slot and colbuf parity are compile-time
-  const int side = blockIdx.x;
-  // this side's pointers in registers (indexing the parameter block with blockIdx.x would turn every use into a
-  // dependent constant-bank load inside the pivot loop)
-  BandSide sd;
-  sd.Ab = side ? a.s[1].Ab : a.s[0].Ab; sd.C4 = side ? a.s[1].C4 : a.s[0].C4;
-  sd.nb = side ? a.s[1].nb : a.s[0].nb; sd.npiv = side ? a.s[1].npiv : a.s[0].npiv;
-  sd.Lr = side ? a.s[1].Lr : a.s[0].Lr; sd.La = side ? a.s[1].La : a.s[0].La; sd.dinv = side ? a.s[1].dinv : a.s[0].dinv;
-  const int W = a.W, Wb = W / BS, RS = a.RS, nb = sd.nb, npiv = sd.npiv, bw = a.bw, LS = bw + 1;
-  const int jswitch = (a.two && side == 0) ? a.k0 : -1;
-  double* colbuf = bc_smem;                 // [2][BC_CSM]   pivot column by window position (double buffered)
-  double* ring = colbuf + 2 * BC_CSM;       // [BC_RING][BC_CSM] upcoming rows, permuted to window positions
-  double* stage = ring + BC_RING * BC_CSM;  // [2][32][LSP] coefficients of the back substitution
-  const int tid = threadIdx.x;
-  const int NT = (Wb + 1) * (Wb + 2) / 2;
-  const int ldr0 = (NT + 31) & ~31;         // first helper thread; blockDim.x = ldr0 + 32 * ceil((W + 4) / 32)
-  const bool worker = tid < NT, helper = tid >= ldr0;
-  int P = 0, Q = 0;
-  if (worker) {
-    P = (int)((sqrtf(8.f * (float)tid + 1.f) - 1.f) * 0.5f);
-    while ((P + 1) * (P + 2) / 2 <= tid) ++P;
-    while (P * (P + 1) / 2 > tid) --P;
-    Q = tid - P * (P + 1) / 2;
-  }
-  if (tid == 0) s_fail = 0;
-  for (int t = tid; t < (2 + BC_RING) * BC_CSM; t += blockDim.x) colbuf[t] = 0.0;
-  // initial window: indices 0 .. W-1
-  double v[BS][BS];
-#pragma unroll
-  for (int i = 0; i < BS; ++i)
-#pragma unroll
-    for (int k = 0; k < BS; ++k) {
-      double x = 0.0;
-      if (worker) {
-        if (P < Wb) {
-          const int rp = BS * P + i, rq = BS * Q + k, hi = max(rp, rq), lo = min(rp, rq);
-          x = __ldg(sd.Ab + (size_t)hi * RS + (hi - lo));
-        } else if (Q < Wb) { if (i < 4) x = __ldg(sd.Ab + (size_t)(BS * Q + k) * RS + W + i); }
-        else if (i < 4 && k < 4) x = __ldg(sd.C4 + 4 * i + k);
-      }
-      v[i][k] = x;
-    }
-  __syncthreads();
-  // column 0
-  if (worker && Q == 0) {
-#pragma unroll
-    for (int i = 0; i < BS; ++i) colbuf[bc_idx(BS * P) + i] = v[i][0];
-  }
-  const int nsteps = ((npiv + UN - 1) / UN) * UN;
-  const int jsplit = jswitch >= 0 ? jswitch : nsteps;      // end of phase 0
-  bool bad = false;
-
-  if (helper) {
-    // ---- element e: entry e of row r of Ab (column r - e) goes to window position (r - e) mod W of ring
-    //      slot r mod 8; entries W .. W+3 are the arrow and keep their position.  After the barrier of
-    //      pivot j, position e of the pivot column is entry (e - pj) mod W of column j of L (unnormalised).
-    const int e = tid - ldr0;
-    const bool band = e < W, live = e < W + 4;
-    const double* src = sd.Ab + (size_t)W * RS + e;       // row W
-    int pos = band ? (e == 0 ? 0 : W - e) : e;            // (W - e) mod W: position of entry e of row W
-    // rows travel global -> register (4 pivots ahead) -> ring: plain loads, NOT cp.async — a pending
-    // LDGSTS is a pending shared-memory write, and bar.sync drains those (measured: ~600 cycles / pivot)
-    double rg[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { rg[i] = live ? __ldg(src) : 0.0; src += RS; }
-    int kk = e;                                            // (e - pj) mod W for band entries
-    const int ce = bc_idx(e);                              // where position e of the pivot column lives
-    // entry (j + kk, kk) of Lr: one element back per pivot, W (LS + 1) forward when kk wraps
-    double* lp = sd.Lr + (size_t)e * LS + e;
-    double* la = sd.La + (size_t)(live && !band ? e - W : 0) * nb;
-    // two phases (before | after the hand-over of the two-sided form) around ONE copy of the pivot loop:
-    // the hand-over code stays out of the loop body (instruction cache), the one-sided form has an empty phase 1
-#pragma unroll 1
-    for (int phase = 0; phase < 2; ++phase) {
-    if (phase == 1 && jswitch >= 0) { bc_bar(); bc_bar(); }    // hand-over of side 1 (workers, below)
-    const int jend = phase == 0 ? jsplit : nsteps;
-#pragma unroll 1
-    for (int j0 = phase == 0 ? 0 : jsplit; j0 < jend; j0 += UN) {
-#pragma unroll
-      for (int u = 0; u < UN; ++u) {
-        const int j = j0 + u;
-        if (live) {
-          ring[u * BC_CSM + bc_idx(pos)] = rg[u & 3];             // row j + W -> slot u
-          rg[u & 3] = __ldg(src);                                 // row j + W + 4
-        }
-        src += RS;
-        if (band && ++pos == W) pos = 0;
-        bc_bar();
-        if (j < nb) {
-          const double val = colbuf[(u & 1) * BC_CSM + ce];
-          if (band) {
-            if (kk <= bw && j + kk < nb) *lp = val;
-            if (kk == 0) sd.dinv[j] = val;                 // the pivot itself
-          } else if (live) {
-            la[j] = val;
-          }
-        }
-        if (band) {
-          if (--kk < 0) { kk = W - 1; lp += (size_t)W * (LS + 1); }
-          lp -= 1;
-        }
-      }
-    }
-    }
-  } else {
-    // ---- workers (and idle threads of the last worker warp: barriers only)
-    const double* sP = colbuf + bc_idx(BS * P);
-    const double* sQ = colbuf + bc_idx(BS * Q);
-    int pj0 = 0, pjp = 0;                                  // pivot position of step u = 0 of the body, and its padded index
-    int Pj = 0;
-#pragma unroll 1
-    for (int phase = 0; phase < 2; ++phase) {
-      if (phase == 1 && jswitch >= 0) {
-        // two-sided form: the window now holds rows k0 .. k0 + W - 1 with the updates of the pivots above;
-        // add side 1's updates of the same rows (pivots below), then publish column k0 again
-        if (tid == 0) bc_wait(a.sync, a.epoch);
-        bc_bar();
-        if (worker) {
-          const int kw = a.k0 % W;
-          const double* DA = a.D + (size_t)W * W;
-#pragma unroll
-          for (int i = 0; i < BS; ++i)
-#pragma unroll
-            for (int k = 0; k < BS; ++k) {
-              const int mk = (BS * Q + k - kw + W) % W;      // position -> row of the middle block
-              if (P < Wb) v[i][k] += __ldcg(a.D + (size_t)((BS * P + i - kw + W) % W) * W + mk);
-              else if (Q < Wb) { if (i < 4) v[i][k] += __ldcg(DA + (size_t)i * W + mk); }
-              else if (i < 4 && k < 4) v[i][k] += __ldcg(DA + 4 * (size_t)W + 4 * i + k);
-            }
-          if (Q == Pj) {
-#pragma unroll
-            for (int i = 0; i < BS; ++i) colbuf[bc_idx(BS * P) + i] = v[i][0];
-          } else if (P == Pj) {
-#pragma unroll
-            for (int k = 0; k < BS; ++k) colbuf[bc_idx(BS * Q) + k] = v[0][k];
-          }
-        }
-        bc_bar();
-      }
-    const int jend = phase == 0 ? jsplit : nsteps;
-#pragma unroll 1
-    for (int j0 = phase == 0 ? 0 : jsplit; j0 < jend; j0 += UN) {
-#pragma unroll
-      for (int u = 0; u < UN; ++u) {
-        const int ij = u % BS;
-        const int par = (u & 1) * BC_CSM, parn = ((u + 1) & 1) * BC_CSM, slot = u * BC_CSM;
-        bc_bar();
-        const double d = colbuf[par + pjp + u];            // 8 consecutive positions never straddle a padding gap
-        bad |= !(d > 0.0 && d <= 1.7976931348623157e308);
-        if (worker) {
-          const double invd = bc_rcp(d);
-          double cp[BS], tq[BS];
-#pragma unroll
-          for (int i = 0; i < BS; i += 2) {
-            const double2 x = *reinterpret_cast<const double2*>(sP + par + i);
-            const double2 y = *reinterpret_cast<const double2*>(sQ + par + i);
-            cp[i] = x.x; cp[i + 1] = x.y;
-            tq[i] = y.x * invd; tq[i + 1] = y.y * invd;
-          }
-          // rank-1 update
-#pragma unroll
-          for (int i = 0; i < BS; ++i)
-#pragma unroll
-            for (int k = 0; k < BS; ++k) v[i][k] = fma(-cp[i], tq[k], v[i][k]);
-          // the slots of position pj are free: they take row j + W (only their ~W/4 owners touch the ring)
-          if (Q == Pj) {
-#pragma unroll
-            for (int i = 0; i < BS; i += 2) {
-              const double2 z = *reinterpret_cast<const double2*>(sP + 2 * BC_CSM + slot + i);
-              v[i][ij] = z.x; v[i + 1][ij] = z.y;
-            }
-          }
-          if (P == Pj) {
-#pragma unroll
-            for (int k = 0; k < BS; k += 2) {
-              const double2 w = *reinterpret_cast<const double2*>(sQ + 2 * BC_CSM + slot + k);
-              v[ij][k] = w.x; v[ij][k + 1] = w.y;
-            }
-          }
-          // publish column j + 1
-          const int ijn = (ij + 1) % BS;
-          int Pjn = Pj;
-          if (ij == BS - 1) { Pjn = Pj + 1; if (Pjn == Wb) Pjn = 0; }
-          double* cbn = colbuf + parn;
-          if (Q == Pjn) {
-#pragma unroll
-            for (int i = 0; i < BS; i += 2) *reinterpret_cast<double2*>(cbn + bc_idx(BS * P) + i) = make_double2(v[i][ijn], v[i + 1][ijn]);
-          } else if (P == Pjn) {
-#pragma unroll
-            for (int k = 0; k < BS; k += 2) *reinterpret_cast<double2*>(cbn + bc_idx(BS * Q) + k) = make_double2(v[ijn][k], v[ijn][k + 1]);
-          }
-          if (ij == BS - 1) Pj = Pjn;
-        } else if (ij == BS - 1) {
-          if (++Pj == Wb) Pj = 0;
-        }
-      }
-      pj0 += UN;
-      if (pj0 == W) pj0 = 0;
-      pjp = bc_idx(pj0);
-    }
-    }
-  }
-  __syncthreads();
-  if (bad) s_fail = 1;
-  if (a.two && side == 1) {
-    // hand-over: what is left in the window (rows n1 .. n1 + W - 1 of the reversed matrix, zero on input)
-    // is the update of the middle block by this side's pivots; reversed row n1 + m is middle row W - 1 - m
-    if (worker) {
-      const int kw = npiv % W;
-      double* DA = a.D + (size_t)W * W;
-#pragma unroll
-      for (int i = 0; i < BS; ++i)
-#pragma unroll
-        for (int k = 0; k < BS; ++k) {
-          const int mk = W - 1 - (BS * Q + k - kw + W) % W;
-          if (P < Wb) {
-            const int mi = W - 1 - (BS * P + i - kw + W) % W;
-            a.D[(size_t)mi * W + mk] = v[i][k];
-            if (P != Q) a.D[(size_t)mk * W + mi] = v[i][k];
-          } else if (Q < Wb) { if (i < 4) DA[(size_t)i * W + mk] = v[i][k]; }
-          else if (i < 4 && k < 4) DA[4 * (size_t)W + 4 * i + k] = v[i][k];
-        }
-    }
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) bc_post(a.sync, a.epoch);
-  }
-  if (worker && tid == NT - 1) {
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int k = 0; k < 4; ++k) s_c4[4 * i + k] = v[i][k];
-  }
-  __syncthreads();
-  bc_tail<1>(a, sd, side, stage, s_fail, s_xI, s_c4);
-}
-
-// ------------------------------------------------------------------ block-6 form with look-ahead (k_band_chol6)
+// ------------------------------------------------------------------ block-6 Cholesky with look-ahead (k_band_chol6)
 //
-// The rank-1 kernel above pays ~450 cycles per pivot: ~65 instructions per lone worker warp and one CTA barrier
-// for 16 FMAs per thread.  The reduced camera system is made of 6 x 6 image blocks, so the natural unit is a
+// A scalar pivot per CTA barrier costs ~450 cycles (measured: ~65 instructions per lone worker warp and one barrier
+// for 16 FMAs per thread).  The reduced camera system is made of 6 x 6 image blocks, so the natural unit is a
 // BLOCK pivot: per step k one 6 x 6 diagonal block is factored, the 6-column panel below it solved and the
 // trailing window updated with a rank-6 product — one barrier per six pivots, and the two dependent chains
 // (factor + solve of the next panel | rank-6 update of the window) run side by side in different warps:
@@ -636,6 +366,10 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol(const BandCholArgs a) {
 constexpr int B6_PBS = 38;        // doubles per 6 x 6 panel block in shared memory (304 bytes: the blocks of eight
                                   // consecutive positions start in eight different groups of four banks)
 
+// Named barriers from role-specific loops: every participating thread executes the same NUMBER of barriers, from
+// different program counters.  One warp runs dependent scalar code at several cycles per instruction, so what a role
+// does per step is counted in instructions — all roles interleaved in one unrolled body, index arithmetic per pivot,
+// was measured several times slower per pivot.  Hence: per-role loops, no early exit.
 __device__ __forceinline__ void bc_gbar(int n) { asm volatile("bar.sync 1, %0;\n" ::"r"(n) : "memory"); }
 __device__ __forceinline__ void bc_pbar(int n) { asm volatile("bar.sync 2, %0;\n" ::"r"(n) : "memory"); }
 
@@ -1032,69 +766,44 @@ __global__ void __launch_bounds__(MAXT, 1) k_band_chol6(const BandCholArgs a) {
   if (bad) s_fail = 1;
   if (a.two && side == 1 && tid == 0) bc_post(a.sync, a.epoch);
   __syncthreads();
-  bc_tail<2>(a, sd, side, bc_smem, s_fail, s_xI, s_c4);
+  bc_tail(a, sd, side, bc_smem, s_fail, s_xI, s_c4);
 }
 
-// threads of the kernel for window W with BS x BS blocks
-inline int band_chol_threads(int W, int BS) {
-  const int Wb = W / BS, NT = (Wb + 1) * (Wb + 2) / 2;
-  return ((NT + 31) & ~31) + 32 * ((W + 4 + 31) / 32);
-}
-
+// shared memory of the back substitution's staging (bc_tail): two chunks of 32 rows of LSP doubles
 inline size_t band_chol_smem(int bw) {
   const int ms = 1 + (bw + 31) / 32, msv = ms <= 4 ? 4 : BC_MAXSLOT;
-  return sizeof(double) * ((size_t)(2 + BC_RING) * BC_CSM + 2 * 32 * (size_t)(32 * (msv + 1)));
-}
-
-// window for half bandwidth bw: the next multiple of 8 above bw (0 when it exceeds the register window)
-inline int band_chol_window(int bw) {
-  const int W = ((bw + 1 + 7) / 8) * 8;
-  return W <= BC_MAXW ? W : 0;
+  return sizeof(double) * (2 * 32 * (size_t)(32 * (msv + 1)));
 }
 
 // rows of Ab the kernel may touch (padding rows below the band part are identity rows)
 inline int band_chol_rows(int nb, int W) { return ((nb + 7) & ~7) + W + 8; }
 
-// How the pivot chain is cut.  Two-sided from 4 windows on (below that the hand-over costs more than
-// the shorter chain saves); PSFM_CHOL_ONE_SIDED forces the one-CTA form.
-// blk_span >= 0: the matrix is made of 6 x 6 blocks and blocks further apart than blk_span are zero (the reduced
-// camera system: blk_span = longest image span of a track); -1: only the scalar half bandwidth bw is known.
+// Plan of k_band_chol6, or W = 0 when the matrix has no block-6 plan (the caller takes the dense route): nb must be
+// a multiple of 6 of at least 3 blocks and the block window at most 25 blocks, unless it covers the whole matrix.
+// How the pivot chain is cut: two-sided from 4 windows on (below that the hand-over costs more than the shorter chain
+// saves); PSFM_CHOL_ONE_SIDED forces the one-CTA form.
+// blk_span >= 0: blocks further apart than blk_span are zero (the reduced camera system: blk_span = longest image
+// span of a track); -1: only the scalar half bandwidth bw is known.
 inline BandPlan band_chol_plan(int nb, int bw, int blk_span = -1) {
   BandPlan p{};
   p.nb = nb; p.bw = std::min(bw, nb - 1);
   static const bool one = getenv("PSFM_CHOL_ONE_SIDED") != nullptr;
-  static const bool rank1 = getenv("PSFM_CHOL_RANK1") != nullptr;
-  // window of the block-6 kernel, in blocks: every block at distance >= Wb from the pivot block must be zero
-  int Wb6 = blk_span >= 0 ? blk_span + 1 : (p.bw + 5) / 6 + 1;
-  if (nb % 6 == 0) Wb6 = std::max(3, std::min(Wb6, nb / 6));
-  if (!rank1 && nb % 6 == 0 && nb / 6 >= 3 && Wb6 <= 25 && 6 * Wb6 > p.bw) {
-    // block-6 form: W = 6 Wb, everything in units of image blocks
-    const int F = nb / 6, Wb = Wb6;
-    p.blk6 = 1;
-    p.W = 6 * Wb; p.RS = p.W + 4; p.nbp = nb;
-    p.two = (!one && F >= 4 * Wb) ? 1 : 0;
-    if (p.two) {
-      p.k0 = 6 * ((F - Wb) / 2);
-      p.n1 = p.nbp - p.W - p.k0;
-      p.nbs[0] = p.k0 + p.W; p.npiv[0] = p.k0 + p.W;
-      p.nbs[1] = p.n1 + p.W; p.npiv[1] = p.n1;
-      p.rows[0] = band_chol_rows(p.nbs[0], p.W); p.rows[1] = band_chol_rows(p.nbs[1], p.W);
-    } else {
-      p.nbs[0] = nb; p.npiv[0] = nb; p.rows[0] = band_chol_rows(nb, p.W);
-    }
-    return p;
-  }
-  p.W = band_chol_window(p.bw); p.RS = p.W + 4;
-  p.nbp = (nb + 7) & ~7;
-  p.two = (p.W > 0 && !one && p.nbp >= 4 * p.W) ? 1 : 0;
+  // window in blocks: every block at distance >= Wb from the pivot block must be zero
+  int Wb = blk_span >= 0 ? blk_span + 1 : (p.bw + 5) / 6 + 1;
+  if (nb % 6 != 0 || nb / 6 < 3) return p;
+  Wb = std::max(3, std::min(Wb, nb / 6));
+  if (Wb > 25 || 6 * Wb <= p.bw) return p;
+  const int F = nb / 6;
+  p.W = 6 * Wb; p.RS = p.W + 4;
+  p.two = (!one && F >= 4 * Wb) ? 1 : 0;
   if (p.two) {
-    p.k0 = (((p.nbp - p.W) / 2 + 7) / 8) * 8;
-    p.n1 = p.nbp - p.W - p.k0;
+    p.k0 = 6 * ((F - Wb) / 2);
+    p.n1 = nb - p.W - p.k0;
     p.nbs[0] = p.k0 + p.W; p.npiv[0] = p.k0 + p.W;
     p.nbs[1] = p.n1 + p.W; p.npiv[1] = p.n1;
     p.rows[0] = band_chol_rows(p.nbs[0], p.W); p.rows[1] = band_chol_rows(p.nbs[1], p.W);
   } else {
-    p.nbs[0] = nb; p.npiv[0] = nb; p.rows[0] = p.W ? band_chol_rows(nb, p.W) : 0;
+    p.nbs[0] = nb; p.npiv[0] = nb; p.rows[0] = band_chol_rows(nb, p.W);
   }
   return p;
 }
@@ -1126,8 +835,8 @@ struct BandWork {
       c.s[s].Ab = ab(s); c.s[s].C4 = C4.p + 16 * s; c.s[s].nb = pl.nbs[s]; c.s[s].npiv = pl.npiv[s];
       c.s[s].Lr = Lr.p + o * LS; c.s[s].La = La.p + 4 * o; c.s[s].dinv = dinv.p + o;
     }
-    c.two = pl.two; c.nbg = pl.nb; c.nbp = pl.nbp; c.k0 = pl.k0;
-    c.bw = pl.bw; c.W = pl.W; c.RS = pl.RS; c.ns = ns; c.blk6 = pl.blk6;
+    c.two = pl.two; c.nb = pl.nb; c.k0 = pl.k0;
+    c.bw = pl.bw; c.W = pl.W; c.RS = pl.RS; c.ns = ns;
     c.x = x; c.fail = fail; c.D = D.p; c.sync = sync.p; c.epoch = ++epoch;
     return c;
   }
@@ -1136,12 +845,11 @@ struct BandWork {
 // one launch: one CTA, or two for the two-sided form
 inline void band_chol_launch(const BandCholArgs& c, cudaStream_t st) {
   const int grid = c.two ? 2 : 1;
-  if (c.blk6) {
-    const int Wb = c.W / 6, nblk = (Wb + 1) * (Wb + 2) / 2;
-    const int np = (6 * (Wb + 1) + 31) & ~31;
-    const int ng4 = ((4 * nblk + 31) & ~31) + np, ng1 = ((nblk + 31) & ~31) + np;
-    const size_t fact = sizeof(double) * (7 * (size_t)(Wb + 1) * B6_PBS + 36 + 4 * 6 * (size_t)c.RS);
-    const size_t smem = std::max(fact, band_chol_smem(c.bw));
+  const int Wb = c.W / 6, nblk = (Wb + 1) * (Wb + 2) / 2;
+  const int np = (6 * (Wb + 1) + 31) & ~31;
+  const int ng4 = ((4 * nblk + 31) & ~31) + np, ng1 = ((nblk + 31) & ~31) + np;
+  const size_t fact = sizeof(double) * (7 * (size_t)(Wb + 1) * B6_PBS + 36 + 4 * 6 * (size_t)c.RS);
+  const size_t smem = std::max(fact, band_chol_smem(c.bw));
 #define PSFM_BC6_GO(MT, TRV, TCV)                                                                                      \
   do {                                                                                                             \
     static size_t attr = 0;                                                                                        \
@@ -1151,32 +859,15 @@ inline void band_chol_launch(const BandCholArgs& c, cudaStream_t st) {
     }                                                                                                              \
     k_band_chol6<MT, TRV, TCV><<<grid, MT, smem, st>>>(c);                                                               \
   } while (0)
-    // thin threads while the CTA has room for them (see k_band_chol6), else one fat thread per block; the threads
-    // after the workers and the panel group are the loader (>= 32)
-    const int ng2 = ((2 * nblk + 31) & ~31) + np;
-    if (ng4 + 32 <= 512) PSFM_BC6_GO(512, 3, 3);
-    else if (ng2 + 32 <= 384) PSFM_BC6_GO(384, 3, 6);
-    else if (ng1 + 64 <= 256) PSFM_BC6_GO(256, 6, 6);
-    else if (ng1 + 64 <= 512) PSFM_BC6_GO(512, 6, 6);
-    else PSFM_BC6_GO(640, 6, 6);
+  // thin threads while the CTA has room for them (see k_band_chol6), else one fat thread per block; the threads
+  // after the workers and the panel group are the loader (>= 32)
+  const int ng2 = ((2 * nblk + 31) & ~31) + np;
+  if (ng4 + 32 <= 512) PSFM_BC6_GO(512, 3, 3);
+  else if (ng2 + 32 <= 384) PSFM_BC6_GO(384, 3, 6);
+  else if (ng1 + 64 <= 256) PSFM_BC6_GO(256, 6, 6);
+  else if (ng1 + 64 <= 512) PSFM_BC6_GO(512, 6, 6);
+  else PSFM_BC6_GO(640, 6, 6);
 #undef PSFM_BC6_GO
-    PSFM_LAUNCH_CHECK();
-    return;
-  }
-  const int threads = band_chol_threads(c.W, 4);
-  const size_t smem = band_chol_smem(c.bw);
-#define PSFM_BC_GO(BSV, MT)                                                                                        \
-  do {                                                                                                             \
-    static size_t attr = 0;                                                                                        \
-    if (smem > attr) {                                                                                             \
-      PSFM_CUDA(cudaFuncSetAttribute(k_band_chol<BSV, MT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-      attr = smem;                                                                                                 \
-    }                                                                                                              \
-    k_band_chol<BSV, MT><<<grid, threads, smem, st>>>(c);                                                           \
-  } while (0)
-  if (threads <= 512) PSFM_BC_GO(4, 512);
-  else PSFM_BC_GO(4, 1024);
-#undef PSFM_BC_GO
   PSFM_LAUNCH_CHECK();
 }
 

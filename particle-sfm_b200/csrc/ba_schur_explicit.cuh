@@ -15,8 +15,8 @@
 //                    fused kernel's shared memory: the same per-image sums and the same pair
 //                    tasks into the same Sband, with W, W H~ per observation through HBM (AoS)
 //   reduced system   [per-image sums | Sband] is all-reduced, then either assembled into a
-//                    compact band matrix for k_band_chol (ba_band_chol.cuh) or, when the band is
-//                    too wide, into dense S (k_schur_assemble_*) for k_chol_blocked: cooperative
+//                    compact band matrix for k_band_chol6 (ba_band_chol.cuh) or, when the band is
+//                    too wide or there are fewer than 3 images, into dense S (k_schur_assemble_*) for k_chol_blocked: cooperative
 //                    blocked banded(+arrow) Cholesky, band = 6 * (longest image span of a track)
 // Everything accumulates with the UNSCALED factored Jacobian (see ba_kernels.cuh); the
 // scaling diag(s) is applied when the reduced system is assembled.

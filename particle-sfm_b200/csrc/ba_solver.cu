@@ -174,7 +174,7 @@ struct psfm_ba_solver {
   int ndense = 0;                       // tiles whose pair phase is the dense product
   // single-CTA sliding-window band Cholesky (ba_band_chol.cuh): compact band matrix, factor, scratch
   bool band_chol = false;
-  BandWork bwk;             // plan + buffers of k_band_chol
+  BandWork bwk;             // plan + buffers of k_band_chol6
   DBuf<PcgState> d_pcg;
   HostScalars* hs = nullptr;
   double* pin_state = nullptr;     // pinned staging of the state: pose (8F) | X (3P) | K (3C)
@@ -909,8 +909,8 @@ __global__ void k_point_span(const int* pt_ptr, const int* obs_img, int P, int* 
   if (e > b) atomicMax(span_max, obs_img[e - 1] - obs_img[b]);
 }
 
-// Both paths end in Sband: when the band is narrow enough for the register window of
-// k_band_chol, the reduced system never exists as a dense matrix.
+// Both paths end in Sband: when the band has a block-6 plan (at least 3 images, a block window of at most
+// 25 images) k_band_chol6 factors it and the reduced system never exists as a dense matrix; otherwise dense S.
 void setup_band_chol(psfm_ba_solver* S) {
   const BandPlan pl = band_chol_plan(6 * S->F, S->bw, S->span);
   S->band_chol = pl.W > 0;
@@ -1882,7 +1882,11 @@ extern "C" int psfm_ba_band_solve(const double* A, const double* b, int32_t nb, 
   bw = std::min(bw, nb - 1);
   const BandPlan pl = band_chol_plan(nb, bw);
   const int W = pl.W, RS = pl.RS, n = nb + 3;
-  if (W == 0) { set_error("psfm_ba_band_solve: band too wide for the register window"); return PSFM_ERR_UNSUPPORTED; }
+  if (W == 0) {
+    set_error("psfm_ba_band_solve: needs nb a multiple of 6 and at least 18, and a block window (bw + 5) / 6 + 1 of at "
+              "most 25 blocks unless it covers the whole matrix");
+    return PSFM_ERR_UNSUPPORTED;
+  }
   bw = pl.bw;
   // the layout k_band_assemble writes, from the dense input (both sides of the two-sided form)
   auto entry = [&](int R, int e) -> double {            // A[R][R - e], identity below nb
@@ -1904,9 +1908,9 @@ extern "C" int psfm_ba_band_solve(const double* A, const double* b, int32_t nb, 
     double* row = &Ab[(size_t)(pl.rows[0] + r) * RS];
     if (r >= pl.nbs[1]) { row[0] = 1.0; continue; }
     for (int k = 0; k <= std::min((int)bw, r); ++k)
-      if (!(r >= pl.n1 && r - k >= pl.n1)) row[k] = entry(pl.nbp - 1 - (r - k), k);
+      if (!(r >= pl.n1 && r - k >= pl.n1)) row[k] = entry(pl.nb - 1 - (r - k), k);
     if (r < pl.n1)
-      for (int a = 0; a < 4; ++a) row[W + a] = arrow(pl.nbp - 1 - r, a);
+      for (int a = 0; a < 4; ++a) row[W + a] = arrow(pl.nb - 1 - r, a);
   }
   for (int a = 0; a < 3; ++a) {
     for (int c = 0; c < 3; ++c) C4[4 * a + c] = A[(size_t)(nb + a) * n + nb + c];

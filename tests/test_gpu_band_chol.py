@@ -34,13 +34,20 @@ def _solve(A, b, nb, bw):
     return rc, x
 
 
-# (nb, bw): tiny window, window wider than the matrix, nb not a multiple of 4, the bench shape
-# (6 * 200 images, span 11/12), the 1024-thread instantiation, the widest supported window
-CASES = [(30, 9), (18, 17), (18, 40), (90, 59), (1200, 71), (1200, 77), (600, 127), (3000, 71), (700, 150), (100, 31), (1203, 95),
-         (64, 6), (41, 14), (500, 38),
-         # block-6 kernel (nb and bw + 1 multiples of 6): window = matrix, one-sided, two-sided, the 512-thread
-         # instantiation, the widest window (25 blocks), a window of 3 blocks, identity padding past the matrix
-         (36, 17), (36, 35), (900, 35), (1200, 95), (1200, 149), (150, 149), (2400, 23), (78, 17), (1200, 83)]
+# (nb, bw), grouped by the instantiation of the block-6 kernel they launch (threads, tile of a worker thread)
+CASES = [
+    # 512, 3 x 3: window of 3 blocks (also clamped up from bw = 5 on a two-sided matrix), window = matrix (bw clamped
+    # to nb - 1), one CTA, two CTAs, the two-sided threshold F = 4 Wb (162: one CTA, 168: two), identity padding rows
+    # past the matrix (nb not a multiple of 8), and the widest window of this instantiation (12 blocks: the bench's
+    # reduced system, 6 * 200 images with tracks spanning 11)
+    (30, 9), (18, 17), (18, 40), (36, 17), (36, 35), (78, 17), (90, 59), (900, 35), (2400, 23), (2400, 5),
+    (162, 35), (168, 35), (1206, 40), (1200, 65),
+    # 384, 3 x 6: two CTAs
+    (1200, 71), (1200, 77), (3000, 71),
+    # 512, 6 x 6: two CTAs, up to the widest window of this instantiation (22 blocks)
+    (1200, 83), (1200, 95), (1200, 125),
+    # 640, 6 x 6: window of 23 blocks, the widest window (25 blocks) as the whole matrix and on a long matrix (two CTAs)
+    (600, 127), (150, 149), (1200, 143)]
 
 
 @pytest.mark.parametrize("nb,bw", CASES)
@@ -62,48 +69,42 @@ def test_band_solve_inactive_arrow_and_failure(gpu):
     A[57, 57] = -1.0                    # not positive definite -> reported, no garbage accepted
     rc, _ = _solve(A, b, 120, 35)
     assert rc == -1
-    rc, _ = _solve(A, b, 120, 400)      # clamped to nb - 1 = 119 <= window limit: still solvable shape
+    rc, _ = _solve(A, b, 120, 400)      # clamped to nb - 1 = 119: a window of the whole matrix, still a solvable shape
     assert rc == -1
-    A2, b2 = _system(400, 300, seed=2)                # window would be 304 > 152
-    rc, _ = _solve(A2, b2, 400, 300)
-    assert rc == -4                     # PSFM_ERR_UNSUPPORTED: wider than the register window
+    # PSFM_ERR_UNSUPPORTED: nb not a multiple of 6 (400 with a window of 51 blocks, 100), a window of
+    # (149 + 5) / 6 + 1 = 26 blocks on a 200-block matrix
+    for nb, bw in ((400, 300), (100, 31), (1200, 149)):
+        A2, b2 = _system(nb, bw, seed=2)
+        rc, _ = _solve(A2, b2, nb, bw)
+        assert rc == -4, (nb, bw)
 
 
-@pytest.mark.parametrize("bad", [57, 199, 200, 215, 330, 399])
-def test_two_sided_form_reports_a_bad_pivot_wherever_it_is(gpu, bad):
-    """nb = 400, bw = 35: window 40, two CTAs (top-down 184 pivots, bottom-up 176, 40 in the middle).  A negative
-    diagonal on either side or in the middle must come back as an error, never as a hang or a silent solve."""
-    A, b = _system(400, 35, seed=3)
-    rc, x = _solve(A, b, 400, 35)
-    assert rc == 0
-    ref = np.linalg.solve(A, b)
-    assert np.abs(x - ref).max() <= 1e-11 * np.abs(ref).max()
-    A[bad, bad] = -1.0
-    rc, _ = _solve(A, b, 400, 35)
-    assert rc == -1
-
-
-def test_two_sided_and_one_sided_forms_agree(gpu, tmp_path):
-    """PSFM_CHOL_ONE_SIDED is read once per process: run the one-sided form in a child process."""
+def test_block6_forms_agree(gpu, tmp_path):
+    """Two-sided (default) vs one-sided (PSFM_CHOL_ONE_SIDED) on two long matrices: a different but fixed elimination
+    order, so the solutions agree to rounding and are not the same bits.  The switch is read once per process: each
+    form runs in a child process."""
     import os
     import subprocess
     import sys
     code = ("import numpy as np, sys; sys.path[:0] = [%r, %r]; from test_gpu_band_chol import _system, _solve;"
-            "A, b = _system(1203, 95, seed=9); rc, x = _solve(A, b, 1203, 95); assert rc == 0; np.save(sys.argv[1], x)")
+            "A, b = _system(%d, %d, seed=11); rc, x = _solve(A, b, %d, %d); assert rc == 0; np.save(sys.argv[1], x)")
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = {}
-    for name, env in (("two", {}), ("one", {"PSFM_CHOL_ONE_SIDED": "1"})):
-        path = str(tmp_path / f"_band_{name}.npy")
-        subprocess.run([sys.executable, "-c", code % (root, os.path.join(root, "tests")), path], check=True, env={**os.environ, **env}, cwd=root)
-        out[name] = np.load(path)
-    assert np.abs(out["two"] - out["one"]).max() <= 1e-12 * np.abs(out["one"]).max()
-    assert not np.array_equal(out["two"], out["one"])      # a different elimination order: not the same bits
+    for nb, bw in ((1200, 71), (1200, 95)):
+        out = {}
+        for name, env in (("two", {}), ("one", {"PSFM_CHOL_ONE_SIDED": "1"})):
+            path = str(tmp_path / f"_band_{nb}_{bw}_{name}.npy")
+            subprocess.run([sys.executable, "-c", code % (root, os.path.join(root, "tests"), nb, bw, nb, bw), path],
+                           check=True, env={**os.environ, **env}, cwd=root)
+            out[name] = np.load(path)
+        assert np.abs(out["two"] - out["one"]).max() <= 1e-12 * np.abs(out["one"]).max(), (nb, bw)
+        assert not np.array_equal(out["two"], out["one"]), (nb, bw)
 
 
 @pytest.mark.parametrize("bad", [0, 57, 281, 282, 299, 317, 318, 450, 599])
 def test_block6_two_sided_form_reports_a_bad_pivot_wherever_it_is(gpu, bad):
     """nb = 600, bw = 35: block-6 kernel, window of 6 image blocks, two CTAs (top-down 47 blocks, bottom-up 47, 6 in
-    the middle)."""
+    the middle).  A negative diagonal on either side or in the middle must come back as an error, never as a hang or
+    a silent solve."""
     A, b = _system(600, 35, seed=5)
     rc, x = _solve(A, b, 600, 35)
     assert rc == 0
@@ -112,22 +113,3 @@ def test_block6_two_sided_form_reports_a_bad_pivot_wherever_it_is(gpu, bad):
     A[bad, bad] = -1.0
     rc, _ = _solve(A, b, 600, 35)
     assert rc == -1
-
-
-def test_block6_forms_agree(gpu, tmp_path):
-    """Block-6 two-sided (default) vs block-6 one-sided vs the rank-1 kernel on the bench shape (child processes:
-    the switches are read once per process)."""
-    import os
-    import subprocess
-    import sys
-    code = ("import numpy as np, sys; sys.path[:0] = [%r, %r]; from test_gpu_band_chol import _system, _solve;"
-            "A, b = _system(1200, 71, seed=11); rc, x = _solve(A, b, 1200, 71); assert rc == 0; np.save(sys.argv[1], x)")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = {}
-    for name, env in (("b6two", {}), ("b6one", {"PSFM_CHOL_ONE_SIDED": "1"}), ("rank1", {"PSFM_CHOL_RANK1": "1"})):
-        path = str(tmp_path / f"_band_{name}.npy")
-        subprocess.run([sys.executable, "-c", code % (root, os.path.join(root, "tests")), path], check=True, env={**os.environ, **env}, cwd=root)
-        out[name] = np.load(path)
-    scale = np.abs(out["rank1"]).max()
-    assert np.abs(out["b6two"] - out["rank1"]).max() <= 1e-12 * scale
-    assert np.abs(out["b6one"] - out["rank1"]).max() <= 1e-12 * scale
