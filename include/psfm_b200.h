@@ -114,8 +114,9 @@ int psfm_traj_optimize(const double* uv12, const double* ref1, const double* ref
                        psfm_traj_summary* summary);
 
 /* Same, all six array arguments are DEVICE pointers (inputs already resident in HBM);
-   runs on `stream` (a cudaStream_t cast to void*, NULL = default stream) and
-   synchronises it before returning. */
+   runs on `stream` (a cudaStream_t cast to void*) and synchronises it before returning.
+   NULL = the library's own non-blocking HP1 stream, which does not wait for work on the
+   legacy default stream; pass cudaStreamLegacy for that. */
 int psfm_traj_optimize_device(const double* d_uv12, const double* d_ref1,
                               const double* d_ref2, const double* d_scale,
                               const float* d_flow12, int32_t n, int32_t w, int32_t h,
@@ -144,6 +145,46 @@ int psfm_tracker_step(const float* flow, const uint8_t* occ, int32_t h, int32_t 
    scale = (1 - occ02(x0)) * (|flow02(x0)| < upper_flow) */
 int psfm_tracker_buffer_inputs(const float* flow01, const float* flow02, const uint8_t* occ02, int32_t h, int32_t w,
                                const double* x0, int32_t n, double upper_flow, double* ref1, double* ref2, double* scale);
+
+/* ------------------------------------------------------------------------- */
+/* The whole tracker stage resident on the device: point_trajectory/             */
+/* track_optimize.py:24-54 from flow maps to the track set.  Maps are DEVICE       */
+/* pointers, [H][W][2] float32 flows and [H][W] uint8 (0/1) occlusion maps; the     */
+/* particles, their history and HP1's inputs never leave the device.  All work      */
+/* runs on `stream` (a cudaStream_t cast to void*, NULL = the legacy default       */
+/* stream; HP1 too).  Same results, bit for bit, as the per-op entry points above   */
+/* with psfm_traj_optimize as the optimiser.  Once a call on a handle has failed     */
+/* for a CUDA reason, every later call on it but psfm_tracker_destroy is refused.   */
+/* ------------------------------------------------------------------------- */
+typedef struct psfm_tracker psfm_tracker;
+/* num_frames = number of images = number of forward flows + 1 */
+int psfm_tracker_create(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, void* stream, psfm_tracker** out);
+/* One frame t (t = 0, 1, ... in call order) of track_optimize.py:31-50: seed (all grid points at t = 0, else the
+   re-seed mask of the previous frame in row-major order), step with flow = flows[t] and occ = occ_maps[t], extend
+   (survivors in active order, retired particles ranked in active order, re-seed mask of the survivors' next
+   positions), and from t = 1 on select the particles with 3 observations and build HP1's inputs from
+   flow_prev = flows[t-1], flow2_prev = flows_f2[t-1], occ2_prev = occ_maps_s2[t-1] (NULL at t = 0).
+   counts (may be NULL) [3]: survivors, seeds of the next frame, buffered particles.  When counts[2] > 0 the
+   buffered set must be optimised (psfm_tracker_optimize, or psfm_tracker_get_buffer + psfm_tracker_set_buffer)
+   before the next frame; `flow` must stay valid until then (it is HP1's flow12). */
+int psfm_tracker_advance(psfm_tracker* t, const float* flow, const uint8_t* occ, const float* flow_prev,
+                         const float* flow2_prev, const uint8_t* occ2_prev, int32_t* counts);
+/* HP1 on the buffered set (opts NULL = defaults), then the optimised x1, x2 written back into the history */
+int psfm_tracker_optimize(psfm_tracker* t, const psfm_traj_options* opts, psfm_traj_summary* summary);
+/* the buffered set to a host optimiser, in buffer order: uv12 [n][4], ref1 [n][2], ref2 [n][2], scale [n] (host) */
+int psfm_tracker_get_buffer(psfm_tracker* t, double* uv12, double* ref1, double* ref2, double* scale);
+/* its result, uv12 [n][4] (host), written back as psfm_tracker_optimize does */
+int psfm_tracker_set_buffer(psfm_tracker* t, const double* uv12);
+/* flow_check for one frame pair on DEVICE buffers, on `stream`, without synchronising: err (may be NULL), occ */
+int psfm_flow_check_device(const float* flow_f, const float* flow_b, int32_t h, int32_t w, float thres, float* err,
+                           uint8_t* occ, void* stream);
+/* clear_active, then the track set in full_trajs order: trajectory id = retire rank, observations in time order,
+   trajectories shorter than traj_min_len dropped (ids keep their unfiltered numbering) */
+int psfm_tracker_finish(psfm_tracker* t, int32_t traj_min_len, int64_t* num_trajs, int64_t* num_obs);
+/* host copies of the finished track set: ids [num_trajs], ptr [num_trajs + 1] (trajectory k owns observations
+   ptr[k] .. ptr[k + 1]), frame_ids [num_obs], xy [num_obs][2] */
+int psfm_tracker_result(psfm_tracker* t, int64_t* ids, int64_t* ptr, int32_t* frame_ids, double* xy);
+void psfm_tracker_destroy(psfm_tracker* t);
 
 /* ------------------------------------------------------------------------- */
 /* SURVEY.md 8(f) row f-4: the RANSAC-free steps that initialise HP2, batched (csrc/init_geometry.cu). */

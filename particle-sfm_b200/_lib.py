@@ -20,7 +20,9 @@ EXPORTS = [
     "psfm_ba_linear_step", "psfm_ba_band_solve", "psfm_measure_dfma", "psfm_ba_default_refine_options",
     "psfm_ba_filter_negative_depth", "psfm_ba_filter_points", "psfm_ba_normalize", "psfm_ba_num_observations",
     "psfm_ba_get_observation_mask", "psfm_ba_get_point_errors", "psfm_ba_iterative_refinement",
-    "psfm_grid_sample", "psfm_flow_check", "psfm_tracker_step", "psfm_tracker_buffer_inputs", "psfm_known_rotation_translations", "psfm_triangulate_tracks", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
+    "psfm_grid_sample", "psfm_flow_check", "psfm_tracker_step", "psfm_tracker_buffer_inputs",
+    "psfm_tracker_create", "psfm_tracker_advance", "psfm_tracker_optimize", "psfm_tracker_get_buffer", "psfm_tracker_set_buffer",
+    "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy", "psfm_known_rotation_translations", "psfm_triangulate_tracks", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
 
@@ -70,6 +72,17 @@ def lib():
     L.psfm_known_rotation_translations.argtypes = [dp, dp, ip, dp, dp, C.c_int32, dp, ip]
     L.psfm_triangulate_tracks.argtypes = [dp, dp, ip, C.c_int32, dp]
     i64p = C.POINTER(C.c_int64)
+    vp = C.c_void_p
+    L.psfm_tracker_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.POINTER(vp)]
+    L.psfm_tracker_advance.argtypes = [vp] * 6 + [ip]
+    L.psfm_tracker_optimize.argtypes = [vp, C.POINTER(_abi.TrajOptions), C.POINTER(_abi.TrajSummary)]
+    L.psfm_tracker_get_buffer.argtypes = [vp, dp, dp, dp, dp]
+    L.psfm_tracker_set_buffer.argtypes = [vp, dp]
+    L.psfm_flow_check_device.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_float, vp, vp, vp]
+    L.psfm_tracker_finish.argtypes = [vp, C.c_int32, i64p, i64p]
+    L.psfm_tracker_result.argtypes = [vp, i64p, i64p, ip, dp]
+    L.psfm_tracker_destroy.argtypes = [vp]
+    L.psfm_tracker_destroy.restype = None
     L.psfm_ba_default_refine_options.argtypes = [C.POINTER(_abi.BARefineOptions)]
     L.psfm_ba_default_refine_options.restype = None
     L.psfm_ba_filter_negative_depth.argtypes = [C.c_void_p, i64p]

@@ -19,9 +19,14 @@
 // an explicit round-to-nearest intrinsic, immune to -fmad.  torch.norm over the 2 flow channels is
 // sqrt(a*a + b*b) without fma.  The distance transform is only ever compared with the integer
 // sample_ratio: dist > r  <=>  no occupied pixel within squared distance r^2 — exact in integers.
+#include <thrust/iterator/transform_iterator.h>
+
+#include <algorithm>
+#include <cub/device/device_scan.cuh>
 #include <vector>
 
 #include "psfm_common.cuh"
+#include "traj_solver.cuh"
 
 namespace {
 
@@ -126,32 +131,177 @@ __global__ void k_buffer_inputs(const float* f01, const float* f02, const unsign
   scale[i] = (double)__fmul_rn(__fsub_rn(1.0f, o[0]), keep);
 }
 
+__device__ __forceinline__ void mark_occupied(const double* xy, int H, int W, unsigned char* occ) {
+  const long long x = (long long)xy[0], y = (long long)xy[1];      // astype(int64): truncation
+  if (x >= 0 && x < W && y >= 0 && y < H) occ[(size_t)y * W + x] = 1;
+}
+
 __global__ void k_occupancy(const double* xy, int n, int H, int W, unsigned char* occ) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const long long x = (long long)xy[2 * (size_t)i], y = (long long)xy[2 * (size_t)i + 1];      // astype(int64): truncation
-  if (x >= 0 && x < W && y >= 0 && y < H) occ[(size_t)y * W + x] = 1;
+  mark_occupied(xy + 2 * (size_t)i, H, W, occ);
 }
 
 // (distance_transform_edt(1 - occupied) > ratio)[::ratio, ::ratio]: a strided grid point is a new seed iff no
 // occupied pixel lies within squared distance ratio^2
-__global__ void k_reseed_mask(const unsigned char* occ, int H, int W, int ratio, int GH, int GW, unsigned char* mask) {
-  const int g = blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= GH * GW) return;
-  const int y = (g / GW) * ratio, x = (g % GW) * ratio;
+__device__ __forceinline__ bool occupied_near(const unsigned char* occ, int H, int W, int ratio, int y, int x) {
   const int r2 = ratio * ratio;
-  bool hit = false;
-  for (int dy = -ratio; dy <= ratio && !hit; ++dy) {
+  for (int dy = -ratio; dy <= ratio; ++dy) {
     const int yy = y + dy;
     if (yy < 0 || yy >= H) continue;
     for (int dx = -ratio; dx <= ratio; ++dx) {
       const int xx = x + dx;
       if (xx < 0 || xx >= W || dy * dy + dx * dx > r2) continue;
-      if (occ[(size_t)yy * W + xx]) { hit = true; break; }
+      if (occ[(size_t)yy * W + xx]) return true;
     }
   }
-  mask[g] = hit ? 0 : 1;
+  return false;
 }
+
+__global__ void k_reseed_mask(const unsigned char* occ, int H, int W, int ratio, int GH, int GW, unsigned char* mask) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= GH * GW) return;
+  mask[g] = occupied_near(occ, H, W, ratio, (g / GW) * ratio, (g % GW) * ratio) ? 0 : 1;
+}
+
+// ------------------------------------------------------------------ resident stage (psfm_tracker_*)
+//
+// The active list mirrors the reference's active_trajs: entry i is the particle in slot i of history[t]
+// (survivors first, then this frame's seeds), with its id, length and its slots one and two steps back.
+// Every compaction is an exclusive scan of 0/1 flags followed by a scatter, so it keeps the active order.
+
+// new_traj_all (trajectory.py:117-120): the grid points whose mask is set (all of them when mask == NULL),
+// in row-major order, appended after the `base` survivors of history[t] and of the active list
+__global__ void k_seed(const unsigned char* mask, const int* pos, int G, int GW, int ratio, int next_id, int base,
+                       int* hid, double* hxy, int* act_id, int* act_len, int* act_m1, int* act_m2) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= G || (mask && !mask[g])) return;
+  const int k = mask ? pos[g] : g;
+  const size_t i = (size_t)base + k;
+  hid[i] = next_id + k;
+  hxy[2 * i] = (double)((g % GW) * ratio);
+  hxy[2 * i + 1] = (double)((g / GW) * ratio);
+  act_id[i] = next_id + k; act_len[i] = 1; act_m1[i] = -1; act_m2[i] = -1;
+}
+
+// extend_all (trajectory.py:129-152): survivors move to the new active list and to history[t + 1] in active
+// order; the others retire, ranked in active order after the `retired` already retired ones
+__global__ void k_extend(int n, const unsigned char* flags, const int* pos, const double* next, const int* act_id,
+                         const int* act_len, const int* act_m1, int t, int retired, int* nid, int* nlen, int* nm1, int* nm2,
+                         int* hid_next, double* hxy_next, int* rank, int* rlen, int* rstart) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int p = pos[i], id = act_id[i], len = act_len[i];
+  if (flags[i]) {
+    nid[p] = id; nlen[p] = len + 1; nm1[p] = i; nm2[p] = act_m1[i];
+    hid_next[p] = id;
+    hxy_next[2 * (size_t)p] = next[2 * (size_t)i];
+    hxy_next[2 * (size_t)p + 1] = next[2 * (size_t)i + 1];
+  } else {
+    const int r = retired + (i - p);
+    rank[id] = r; rlen[r] = len; rstart[r] = t - len + 1;
+  }
+}
+
+// number of set flags, from the exclusive scan of them
+__global__ void k_total(const unsigned char* flags, const int* pos, int n, int* out) {
+  *out = n ? pos[n - 1] + (flags[n - 1] ? 1 : 0) : 0;
+}
+
+__global__ void k_occupancy_kept(const double* next, const unsigned char* flags, int n, int H, int W, unsigned char* occ) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !flags[i]) return;
+  mark_occupied(next + 2 * (size_t)i, H, W, occ);
+}
+
+// the re-seed mask of extend_all.  Without a survivor, the occupancy map scipy's distance_transform_edt
+// receives ([H, W, 1], 1 - occupied) has no zero; scipy 1.x then returns sqrt((y + 1)^2 + x^2) at (y, x, 0).
+__global__ void k_reseed_stage(const unsigned char* occ, int H, int W, int ratio, int GH, int GW, const int* num_survivors,
+                               unsigned char* mask) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= GH * GW) return;
+  const int y = (g / GW) * ratio, x = (g % GW) * ratio;
+  if (*num_survivors == 0) {
+    const long long d2 = (long long)(y + 1) * (y + 1) + (long long)x * x;
+    mask[g] = d2 > (long long)ratio * ratio ? 1 : 0;
+  } else {
+    mask[g] = occupied_near(occ, H, W, ratio, y, x) ? 0 : 1;
+  }
+}
+
+// optimize_buffer's selection (trajectory.py:165): the survivors with three observations, in active order
+__global__ void k_buffer_flags(const int* len, const int* num_survivors, int n, unsigned char* flags) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  flags[i] = (i < *num_survivors && len[i] >= 3) ? 1 : 0;
+}
+
+// x0 = history[t-1], uv12 = (history[t], history[t+1]) of the selected particles, and their active slot
+__global__ void k_buffer_gather(int n, const unsigned char* flags, const int* pos, const int* m1, const int* m2,
+                                const double* hxy_prev, const double* hxy_cur, const double* hxy_next, double* x0,
+                                double* uv12, int* slot) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !flags[i]) return;
+  const size_t b = pos[i], a = m2[i], c = m1[i];
+  x0[2 * b] = hxy_prev[2 * a]; x0[2 * b + 1] = hxy_prev[2 * a + 1];
+  uv12[4 * b] = hxy_cur[2 * c]; uv12[4 * b + 1] = hxy_cur[2 * c + 1];
+  uv12[4 * b + 2] = hxy_next[2 * (size_t)i]; uv12[4 * b + 3] = hxy_next[2 * (size_t)i + 1];
+  slot[b] = i;
+}
+
+// optimize_buffer's write-back (trajectory.py:190-194): optimised x1 into history[t], x2 into history[t+1]
+__global__ void k_writeback(int n, const double* out, const int* slot, const int* m1, double* hxy_cur, double* hxy_next) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= n) return;
+  const size_t j = slot[b], c = m1[j];
+  hxy_cur[2 * c] = out[4 * (size_t)b]; hxy_cur[2 * c + 1] = out[4 * (size_t)b + 1];
+  hxy_next[2 * j] = out[4 * (size_t)b + 2]; hxy_next[2 * j + 1] = out[4 * (size_t)b + 3];
+}
+
+// clear_active (trajectory.py:154-159): the particles still alive at time t retire in active order
+__global__ void k_clear_active(int n, const int* act_id, const int* act_len, int t, int retired, int* rank, int* rlen, int* rstart) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int r = retired + i, len = act_len[i];
+  rank[act_id[i]] = r; rlen[r] = len; rstart[r] = t - len + 1;
+}
+
+// main_connect_point_trajectories.py:57-60: keep the trajectories of at least min_len observations
+__global__ void k_keep(int T, const int* rlen, int min_len, unsigned char* keep, long long* klen) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= T) return;
+  const bool k = rlen[r] >= min_len;
+  keep[r] = k ? 1 : 0;
+  klen[r] = k ? rlen[r] : 0;
+}
+
+__global__ void k_emit_ids(int T, const unsigned char* keep, const int* kpos, const long long* off, const long long* klen,
+                           long long* ids, long long* ptr, long long* totals) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= T) return;
+  if (keep[r]) { ids[kpos[r]] = r; ptr[kpos[r]] = off[r]; }
+  if (r == T - 1) {
+    const long long nt = kpos[r] + (keep[r] ? 1 : 0), m = off[r] + klen[r];
+    ptr[nt] = m;
+    totals[0] = nt; totals[1] = m;
+  }
+}
+
+// every observation of time t goes to offset[rank] + (t - start[rank]): the track set in full_trajs order
+__global__ void k_emit_obs(int n, int t, const int* hid, const double* hxy, const int* rank, const unsigned char* keep,
+                           const long long* off, const int* rstart, int* frame_ids, double* xy) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int r = rank[hid[i]];
+  if (!keep[r]) return;
+  const size_t o = (size_t)(off[r] + (t - rstart[r]));
+  frame_ids[o] = t;
+  xy[2 * o] = hxy[2 * (size_t)i]; xy[2 * o + 1] = hxy[2 * (size_t)i + 1];
+}
+
+struct FlagToInt {
+  __host__ __device__ int operator()(unsigned char f) const { return f ? 1 : 0; }
+};
 
 int device_ok() {
   int n = 0;
@@ -251,4 +401,358 @@ extern "C" int psfm_tracker_buffer_inputs(const float* flow01, const float* flow
     PSFM_CUDA(cudaMemcpy(scale, sc.p, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost));
     return PSFM_OK;
   } catch (const CudaFail& f) { return f.code; }
+}
+
+// ------------------------------------------------------------------ resident stage: host side
+
+namespace {
+
+template <typename T>
+void swap_buf(DBuf<T>& a, DBuf<T>& b) {
+  std::swap(a.p, b.p); std::swap(a.n, b.n); std::swap(a.st, b.st); std::swap(a.async, b.async);
+}
+
+// capacity >= need, the first `keep` elements preserved; grows geometrically
+template <typename T>
+void grow(DBuf<T>& b, size_t need, size_t keep, cudaStream_t st) {
+  if (b.p && b.n >= need) return;
+  DBuf<T> nb;
+  nb.alloc(std::max(need, 2 * b.n), st);
+  if (keep) PSFM_CUDA(cudaMemcpyAsync(nb.p, b.p, keep * sizeof(T), cudaMemcpyDeviceToDevice, st));
+  swap_buf(b, nb);
+}
+
+}  // namespace
+
+struct psfm_tracker {
+  int h = 0, w = 0, ratio = 1, gh = 0, gw = 0, num_frames = 0;
+  cudaStream_t st = nullptr;
+  int t = 0;                      // frames advanced; the active particles live at time t
+  int n_active = 0;               // = history[t]'s survivors until the next seeding
+  int seeds = 0;                  // seeds of the next frame (set bits of `mask`)
+  int next_id = 0, retired = 0;
+  int n_buf = 0, buf_frame = -1;  // buffered set of frame buf_frame waiting for HP1 (n_buf > 0)
+  const float* flow12 = nullptr;  // flows[buf_frame] (the caller's map)
+  bool finished = false;
+  bool failed = false;            // a CUDA failure left the device state unknown: every later call is refused
+  long long res_trajs = 0, res_obs = 0;
+  std::vector<long long> hoff;    // history[s] starts at hoff[s]
+  std::vector<int> hcnt;          // particles alive at time s
+  DBuf<int> hid; DBuf<double> hxy;
+  DBuf<int> act_id[2], act_len[2], act_m1[2], act_m2[2];
+  int cur = 0;
+  DBuf<double> next; DBuf<unsigned char> flags, bflags; DBuf<int> pos, bpos;
+  DBuf<unsigned char> occ, mask; DBuf<int> mpos;
+  DBuf<int> rank, rlen, rstart;
+  DBuf<double> bx0, buv, bref1, bref2, bscale, bout; DBuf<int> bslot;
+  DBuf<unsigned char> keep; DBuf<int> kpos; DBuf<long long> klen, off, ids, ptr, totals;
+  DBuf<int> res_frames; DBuf<double> res_xy;
+  DBuf<unsigned char> tmp;        // CUB scratch
+  DBuf<int> d_counts;
+  int* h_counts = nullptr;        // pinned [3]
+  long long* h_totals = nullptr;  // pinned [2]
+
+  template <typename In, typename Out>
+  void scan(In in, Out out, int n) {
+    if (n == 0) return;
+    size_t bytes = 0;
+    PSFM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, in, out, n, st));
+    grow(tmp, bytes, 0, st);
+    PSFM_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, in, out, n, st));
+    PSFM_LAUNCH_CHECK();
+  }
+  void scan_flags(const unsigned char* f, int* out, int n) { scan(thrust::make_transform_iterator(f, FlagToInt()), out, n); }
+  void sync() { PSFM_CUDA(cudaStreamSynchronize(st)); }
+};
+
+namespace {
+
+int tracker_fail(const std::string& msg) {
+  set_error(msg);
+  return PSFM_ERR_INVALID;
+}
+
+// argument check shared by the calls on a handle: PSFM_OK or the error to return
+int tracker_usable(const psfm_tracker* T, bool args_ok, const char* fn) {
+  if (!T || !args_ok) return tracker_fail(std::string(fn) + ": null argument");
+  if (T->failed) return tracker_fail(std::string(fn) + ": an earlier call on this tracker failed; destroy it");
+  return PSFM_OK;
+}
+
+int tracker_broken(psfm_tracker* T, int code) {
+  T->failed = true;
+  return code;
+}
+
+}  // namespace
+
+extern "C" int psfm_flow_check_device(const float* d_flow_f, const float* d_flow_b, int32_t h, int32_t w, float thres, float* d_err,
+                                      uint8_t* d_occ, void* stream) {
+  if (!d_flow_f || !d_flow_b || !d_occ) return tracker_fail("psfm_flow_check_device: null argument");
+  if (h < 2 || w < 2) return tracker_fail("psfm_flow_check_device: bad sizes");
+  int rc = device_ok();
+  if (rc != PSFM_OK) return rc;
+  try {
+    const size_t hw = (size_t)h * w;
+    k_flow_check<<<grid_of(hw), 256, 0, (cudaStream_t)stream>>>(d_flow_f, d_flow_b, h, w, thres, d_err, d_occ);
+    PSFM_LAUNCH_CHECK();
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return f.code; }
+}
+
+extern "C" int psfm_tracker_create(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, void* stream, psfm_tracker** out) {
+  if (!out) return tracker_fail("psfm_tracker_create: null argument");
+  *out = nullptr;
+  if (h < 2 || w < 2 || sample_ratio < 1 || num_frames < 1) return tracker_fail("psfm_tracker_create: bad sizes");
+  int rc = device_ok();
+  if (rc != PSFM_OK) return rc;
+  psfm_tracker* T = new psfm_tracker;
+  try {
+    T->h = h; T->w = w; T->ratio = sample_ratio; T->num_frames = num_frames;
+    T->gh = (h + sample_ratio - 1) / sample_ratio; T->gw = (w + sample_ratio - 1) / sample_ratio;
+    T->st = (cudaStream_t)stream;
+    T->hoff.assign(1, 0);
+    T->hcnt.assign(1, 0);
+    const size_t G = (size_t)T->gh * T->gw;
+    T->occ.alloc((size_t)h * w, T->st);
+    T->mask.alloc(G, T->st);
+    T->mpos.alloc(G, T->st);
+    T->d_counts.alloc(3, T->st);
+    T->totals.alloc(2, T->st);
+    PSFM_CUDA(cudaMallocHost((void**)&T->h_counts, 3 * sizeof(int)));
+    PSFM_CUDA(cudaMallocHost((void**)&T->h_totals, 2 * sizeof(long long)));
+  } catch (const CudaFail& f) {
+    psfm_tracker_destroy(T);
+    return f.code;
+  }
+  *out = T;
+  return PSFM_OK;
+}
+
+extern "C" int psfm_tracker_advance(psfm_tracker* T, const float* d_flow, const uint8_t* d_occ, const float* d_flow_prev,
+                                    const float* d_flow2_prev, const uint8_t* d_occ2_prev, int32_t* counts) {
+  int rc = tracker_usable(T, d_flow && d_occ, "psfm_tracker_advance");
+  if (rc != PSFM_OK) return rc;
+  if (T->finished) return tracker_fail("psfm_tracker_advance: the track set was already assembled");
+  if (T->n_buf > 0) return tracker_fail("psfm_tracker_advance: the buffered set of the previous frame was not optimised");
+  if (T->t + 1 >= T->num_frames) return tracker_fail("psfm_tracker_advance: more frames than the tracker was created for");
+  if (T->t >= 1 && (!d_flow_prev || !d_flow2_prev || !d_occ2_prev))
+    return tracker_fail("psfm_tracker_advance: from frame 1 on, flows[t-1], flows_f2[t-1] and occ_maps_s2[t-1] are needed");
+  try {
+    cudaStream_t st = T->st;
+    const int t = T->t, G = T->gh * T->gw, H = T->h, W = T->w;
+    const int seeds = t == 0 ? G : T->seeds, base = T->n_active, n = base + seeds;
+    const long long h0 = T->hoff[t], h1 = h0 + n;
+    // capacities: history[t + 1] gets at most n entries; ids, ranks and the per-frame scratch grow with them
+    grow(T->hid, (size_t)(h1 + n), (size_t)(h0 + base), st);
+    grow(T->hxy, 2 * (size_t)(h1 + n), 2 * (size_t)(h0 + base), st);
+    const int c = T->cur, d = 1 - c;
+    grow(T->act_id[c], n, base, st); grow(T->act_len[c], n, base, st);
+    grow(T->act_m1[c], n, base, st); grow(T->act_m2[c], n, base, st);
+    grow(T->act_id[d], n, 0, st); grow(T->act_len[d], n, 0, st); grow(T->act_m1[d], n, 0, st); grow(T->act_m2[d], n, 0, st);
+    const size_t ids_now = (size_t)T->next_id + seeds;
+    grow(T->rank, ids_now, T->next_id, st); grow(T->rlen, ids_now, T->next_id, st); grow(T->rstart, ids_now, T->next_id, st);
+    grow(T->next, 2 * (size_t)n, 0, st); grow(T->flags, n, 0, st); grow(T->pos, n, 0, st);
+    grow(T->bflags, n, 0, st); grow(T->bpos, n, 0, st);
+    grow(T->bx0, 2 * (size_t)n, 0, st); grow(T->buv, 4 * (size_t)n, 0, st); grow(T->bslot, n, 0, st);
+    grow(T->bref1, 2 * (size_t)n, 0, st); grow(T->bref2, 2 * (size_t)n, 0, st); grow(T->bscale, n, 0, st);
+    grow(T->bout, 4 * (size_t)n, 0, st);
+    int* hid_t = T->hid.p + h0;
+    double* hxy_t = T->hxy.p + 2 * h0;
+    // 1. seed (new_traj_all)
+    if (seeds) {
+      k_seed<<<grid_of(G), 256, 0, st>>>(t == 0 ? nullptr : T->mask.p, T->mpos.p, G, T->gw, T->ratio, T->next_id, base, hid_t, hxy_t,
+                                         T->act_id[c].p, T->act_len[c].p, T->act_m1[c].p, T->act_m2[c].p);
+      PSFM_LAUNCH_CHECK();
+    }
+    // 2. step (step_forward) from history[t], which is in active order
+    if (n) {
+      k_tracker_step<<<grid_of(n), 256, 0, st>>>(d_flow, d_occ, H, W, hxy_t, n, T->next.p, T->flags.p);
+      PSFM_LAUNCH_CHECK();
+    }
+    // 3. extend (extend_all): stable compaction, retire ranks, then the re-seed mask of the survivors' next positions
+    T->scan_flags(T->flags.p, T->pos.p, n);
+    if (n) {
+      k_extend<<<grid_of(n), 256, 0, st>>>(n, T->flags.p, T->pos.p, T->next.p, T->act_id[c].p, T->act_len[c].p, T->act_m1[c].p, t,
+                                           T->retired, T->act_id[d].p, T->act_len[d].p, T->act_m1[d].p, T->act_m2[d].p,
+                                           T->hid.p + h1, T->hxy.p + 2 * h1, T->rank.p, T->rlen.p, T->rstart.p);
+      PSFM_LAUNCH_CHECK();
+    }
+    k_total<<<1, 1, 0, st>>>(T->flags.p, T->pos.p, n, T->d_counts.p);
+    PSFM_LAUNCH_CHECK();
+    PSFM_CUDA(cudaMemsetAsync(T->occ.p, 0, (size_t)H * W, st));
+    if (n) {
+      k_occupancy_kept<<<grid_of(n), 256, 0, st>>>(T->next.p, T->flags.p, n, H, W, T->occ.p);
+      PSFM_LAUNCH_CHECK();
+    }
+    k_reseed_stage<<<grid_of(G), 256, 0, st>>>(T->occ.p, H, W, T->ratio, T->gh, T->gw, T->d_counts.p, T->mask.p);
+    PSFM_LAUNCH_CHECK();
+    T->scan_flags(T->mask.p, T->mpos.p, G);
+    k_total<<<1, 1, 0, st>>>(T->mask.p, T->mpos.p, G, T->d_counts.p + 1);
+    PSFM_LAUNCH_CHECK();
+    // 4. buffer (optimize_buffer's selection and gather), from frame 1 on
+    if (t >= 1 && n) {
+      k_buffer_flags<<<grid_of(n), 256, 0, st>>>(T->act_len[d].p, T->d_counts.p, n, T->bflags.p);
+      PSFM_LAUNCH_CHECK();
+      T->scan_flags(T->bflags.p, T->bpos.p, n);
+      k_total<<<1, 1, 0, st>>>(T->bflags.p, T->bpos.p, n, T->d_counts.p + 2);
+      PSFM_LAUNCH_CHECK();
+      k_buffer_gather<<<grid_of(n), 256, 0, st>>>(n, T->bflags.p, T->bpos.p, T->act_m1[d].p, T->act_m2[d].p,
+                                                  T->hxy.p + 2 * T->hoff[t - 1], hxy_t, T->hxy.p + 2 * h1, T->bx0.p, T->buv.p,
+                                                  T->bslot.p);
+      PSFM_LAUNCH_CHECK();
+    } else {
+      PSFM_CUDA(cudaMemsetAsync(T->d_counts.p + 2, 0, sizeof(int), st));
+    }
+    PSFM_CUDA(cudaMemcpyAsync(T->h_counts, T->d_counts.p, 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    T->sync();
+    // the host-side state moves on only once the frame's device work has completed
+    const int survivors = T->h_counts[0];
+    T->hcnt[t] = n;
+    T->hoff.push_back(h1);
+    T->next_id += seeds;
+    T->retired += n - survivors;
+    T->n_active = survivors;
+    T->seeds = T->h_counts[1];
+    T->cur = d;
+    T->t = t + 1;
+    T->hcnt.push_back(survivors);
+    T->n_buf = T->h_counts[2];
+    T->buf_frame = t;
+    T->flow12 = d_flow;
+    if (T->n_buf > 0) {
+      k_buffer_inputs<<<grid_of(T->n_buf), 256, 0, st>>>(d_flow_prev, d_flow2_prev, d_occ2_prev, H, W, T->bx0.p, T->n_buf, 20.0,
+                                                          T->bref1.p, T->bref2.p, T->bscale.p);
+      PSFM_LAUNCH_CHECK();
+    }
+    if (counts) { counts[0] = survivors; counts[1] = T->seeds; counts[2] = T->n_buf; }
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+}
+
+namespace {
+
+int tracker_writeback(psfm_tracker* T) {
+  const int t = T->buf_frame;
+  k_writeback<<<grid_of(T->n_buf), 256, 0, T->st>>>(T->n_buf, T->bout.p, T->bslot.p, T->act_m1[T->cur].p, T->hxy.p + 2 * T->hoff[t],
+                                                     T->hxy.p + 2 * T->hoff[t + 1]);
+  PSFM_LAUNCH_CHECK();
+  T->n_buf = 0;
+  return PSFM_OK;
+}
+
+}  // namespace
+
+extern "C" int psfm_tracker_optimize(psfm_tracker* T, const psfm_traj_options* opts, psfm_traj_summary* summary) {
+  if (summary) memset(summary, 0, sizeof(*summary));
+  int rc = tracker_usable(T, true, "psfm_tracker_optimize");
+  if (rc != PSFM_OK) return rc;
+  if (T->n_buf <= 0) return tracker_fail("psfm_tracker_optimize: no buffered trajectory");
+  try {
+    // HP1 runs on the tracker's stream, after k_buffer_inputs.  NULL (the legacy default stream) is passed as
+    // cudaStreamLegacy: a NULL stream would make solve_device use the HP1 workspace's non-blocking stream, which
+    // is not ordered after the legacy stream's work.
+    rc = traj::solve_device(T->buv.p, T->bref1.p, T->bref2.p, T->bscale.p, T->flow12, T->n_buf, T->w, T->h, opts, T->bout.p,
+                            summary, T->st ? T->st : cudaStreamLegacy);
+    if (rc != PSFM_OK) return tracker_broken(T, rc);
+    return tracker_writeback(T);
+  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+}
+
+extern "C" int psfm_tracker_get_buffer(psfm_tracker* T, double* uv12, double* ref1, double* ref2, double* scale) {
+  int rc = tracker_usable(T, uv12 && ref1 && ref2 && scale, "psfm_tracker_get_buffer");
+  if (rc != PSFM_OK) return rc;
+  if (T->n_buf <= 0) return tracker_fail("psfm_tracker_get_buffer: no buffered trajectory");
+  try {
+    const size_t n = T->n_buf;
+    PSFM_CUDA(cudaMemcpyAsync(uv12, T->buv.p, 4 * n * sizeof(double), cudaMemcpyDeviceToHost, T->st));
+    PSFM_CUDA(cudaMemcpyAsync(ref1, T->bref1.p, 2 * n * sizeof(double), cudaMemcpyDeviceToHost, T->st));
+    PSFM_CUDA(cudaMemcpyAsync(ref2, T->bref2.p, 2 * n * sizeof(double), cudaMemcpyDeviceToHost, T->st));
+    PSFM_CUDA(cudaMemcpyAsync(scale, T->bscale.p, n * sizeof(double), cudaMemcpyDeviceToHost, T->st));
+    T->sync();
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+}
+
+extern "C" int psfm_tracker_set_buffer(psfm_tracker* T, const double* uv12) {
+  int rc = tracker_usable(T, uv12 != nullptr, "psfm_tracker_set_buffer");
+  if (rc != PSFM_OK) return rc;
+  if (T->n_buf <= 0) return tracker_fail("psfm_tracker_set_buffer: no buffered trajectory");
+  try {
+    PSFM_CUDA(cudaMemcpyAsync(T->bout.p, uv12, 4 * (size_t)T->n_buf * sizeof(double), cudaMemcpyHostToDevice, T->st));
+    rc = tracker_writeback(T);
+    T->sync();        // uv12 is the caller's (possibly pageable) memory
+    return rc;
+  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+}
+
+extern "C" int psfm_tracker_finish(psfm_tracker* T, int32_t traj_min_len, int64_t* num_trajs, int64_t* num_obs) {
+  int rc = tracker_usable(T, num_trajs && num_obs, "psfm_tracker_finish");
+  if (rc != PSFM_OK) return rc;
+  if (T->finished) return tracker_fail("psfm_tracker_finish: already finished");
+  if (T->n_buf > 0) return tracker_fail("psfm_tracker_finish: the buffered set of the last frame was not optimised");
+  try {
+    cudaStream_t st = T->st;
+    const int t = T->t;
+    if (T->n_active) {
+      k_clear_active<<<grid_of(T->n_active), 256, 0, st>>>(T->n_active, T->act_id[T->cur].p, T->act_len[T->cur].p, t, T->retired,
+                                                            T->rank.p, T->rlen.p, T->rstart.p);
+      PSFM_LAUNCH_CHECK();
+    }
+    T->retired += T->n_active;
+    T->n_active = 0;
+    const int NT = T->next_id;    // every id is retired now: ranks 0 .. NT-1
+    T->finished = true;
+    if (NT == 0) { *num_trajs = *num_obs = T->res_trajs = T->res_obs = 0; return PSFM_OK; }
+    grow(T->keep, NT, 0, st); grow(T->kpos, NT, 0, st); grow(T->klen, NT, 0, st); grow(T->off, NT, 0, st);
+    grow(T->ids, NT, 0, st); grow(T->ptr, (size_t)NT + 1, 0, st);
+    k_keep<<<grid_of(NT), 256, 0, st>>>(NT, T->rlen.p, traj_min_len, T->keep.p, T->klen.p);
+    PSFM_LAUNCH_CHECK();
+    T->scan_flags(T->keep.p, T->kpos.p, NT);
+    T->scan(T->klen.p, T->off.p, NT);
+    k_emit_ids<<<grid_of(NT), 256, 0, st>>>(NT, T->keep.p, T->kpos.p, T->off.p, T->klen.p, T->ids.p, T->ptr.p, T->totals.p);
+    PSFM_LAUNCH_CHECK();
+    PSFM_CUDA(cudaMemcpyAsync(T->h_totals, T->totals.p, 2 * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    T->sync();
+    T->res_trajs = T->h_totals[0];
+    T->res_obs = T->h_totals[1];
+    grow(T->res_frames, (size_t)T->res_obs, 0, st);
+    grow(T->res_xy, 2 * (size_t)T->res_obs, 0, st);
+    for (int s = 0; s <= t; ++s) {
+      const int n = T->hcnt[s];
+      if (!n) continue;
+      k_emit_obs<<<grid_of(n), 256, 0, st>>>(n, s, T->hid.p + T->hoff[s], T->hxy.p + 2 * T->hoff[s], T->rank.p, T->keep.p, T->off.p,
+                                             T->rstart.p, T->res_frames.p, T->res_xy.p);
+      PSFM_LAUNCH_CHECK();
+    }
+    T->sync();
+    *num_trajs = T->res_trajs;
+    *num_obs = T->res_obs;
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+}
+
+extern "C" int psfm_tracker_result(psfm_tracker* T, int64_t* ids, int64_t* ptr, int32_t* frame_ids, double* xy) {
+  int rc = tracker_usable(T, ids && ptr && frame_ids && xy, "psfm_tracker_result");
+  if (rc != PSFM_OK) return rc;
+  if (!T->finished) return tracker_fail("psfm_tracker_result: call psfm_tracker_finish first");
+  try {
+    const size_t nt = T->res_trajs, m = T->res_obs;
+    if (T->next_id == 0) { ptr[0] = 0; return PSFM_OK; }
+    PSFM_CUDA(cudaMemcpyAsync(ids, T->ids.p, nt * sizeof(int64_t), cudaMemcpyDeviceToHost, T->st));
+    PSFM_CUDA(cudaMemcpyAsync(ptr, T->ptr.p, (nt + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, T->st));
+    PSFM_CUDA(cudaMemcpyAsync(frame_ids, T->res_frames.p, m * sizeof(int32_t), cudaMemcpyDeviceToHost, T->st));
+    PSFM_CUDA(cudaMemcpyAsync(xy, T->res_xy.p, 2 * m * sizeof(double), cudaMemcpyDeviceToHost, T->st));
+    T->sync();
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+}
+
+extern "C" void psfm_tracker_destroy(psfm_tracker* T) {
+  if (!T) return;
+  cudaStreamSynchronize(T->st);
+  if (T->h_counts) cudaFreeHost(T->h_counts);
+  if (T->h_totals) cudaFreeHost(T->h_totals);
+  delete T;
+  cudaGetLastError();
 }

@@ -22,7 +22,7 @@
 #include <chrono>
 #include <mutex>
 
-#include "psfm_common.cuh"
+#include "traj_solver.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -564,6 +564,19 @@ static int launch_solve(Workspace& ws, const double* d_uv12, const double* d_ref
   return PSFM_OK;
 }
 
+int solve_device(const double* d_uv12, const double* d_ref1, const double* d_ref2, const double* d_scale,
+                 const float* d_flow12, int n, int w, int h, const psfm_traj_options* opts, double* d_out,
+                 psfm_traj_summary* summary, cudaStream_t stream) {
+  std::lock_guard<std::mutex> lock(g_ws.mu);
+  try {
+    g_ws.ensure((size_t)n, (size_t)(n + CH - 1) / CH);
+    return launch_solve(g_ws, d_uv12, d_ref1, d_ref2, d_scale, d_flow12, n, w, h, opts, d_out, summary,
+                        stream ? stream : g_ws.stream);
+  } catch (const CudaFail& f) {
+    return f.code;
+  }
+}
+
 }  // namespace traj
 }  // namespace psfm
 
@@ -601,15 +614,8 @@ extern "C" int psfm_traj_optimize_device(const double* d_uv12, const double* d_r
   if (n == 0) return PSFM_OK;
   int rc = traj_check_device();
   if (rc != PSFM_OK) return rc;
-  traj::Workspace& ws = traj::g_ws;
-  std::lock_guard<std::mutex> lock(ws.mu);
-  try {
-    ws.ensure((size_t)n, (size_t)(n + traj::CH - 1) / traj::CH);
-    cudaStream_t st = stream ? (cudaStream_t)stream : ws.stream;
-    return traj::launch_solve(ws, d_uv12, d_ref1, d_ref2, d_scale, d_flow12, n, w, h, opts, d_out_uv12, summary, st);
-  } catch (const CudaFail& f) {
-    return f.code;
-  }
+  return traj::solve_device(d_uv12, d_ref1, d_ref2, d_scale, d_flow12, n, w, h, opts, d_out_uv12, summary,
+                            (cudaStream_t)stream);
 }
 
 extern "C" int psfm_traj_optimize(const double* uv12, const double* ref1, const double* ref2, const double* scale,

@@ -206,6 +206,34 @@ def make_flow_triplet(height, width, seed=0, amplitude=6.0, noise=0.1):
     return f01n.astype(np.float32), f12n.astype(np.float32), f02.astype(np.float32), occ02
 
 
+def make_flow_sequence(n_frames, height, width, seed=0, amplitude=3.0, waves=4):
+    """The four flow lists main_connect_point_trajectories takes for n_frames images, as
+    tests/golden/make_tracker_golden.py builds them at any size: smooth forward flows fw [n-1],
+    crude backward flows fb, two-step flows f2 [n-2] = fw[i] composed with fw[i+1] plus noise, their
+    backward flows b2, and a block of extra motion moving across fw (not in fb) that the flow check
+    marks occluded, so that particles die and new ones are seeded.  f32 [H, W, 2] each."""
+    h, w = height, width
+    rng = np.random.default_rng(seed)
+    fw = [smooth_flow(h, w, rng, amplitude, waves).astype(np.float32) for _ in range(n_frames - 1)]
+    yy, xx = np.meshgrid(np.arange(h, dtype=np.float64), np.arange(w, dtype=np.float64), indexing="ij")
+
+    def compose(a, b):   # a then b
+        p = np.stack([xx + a[..., 0], yy + a[..., 1]], -1).reshape(-1, 2)
+        return (a + bilinear_zeros(b, p).reshape(h, w, 2)).astype(np.float32)
+
+    def backward(a):     # crude inverse: -a sampled at x - a
+        p = np.stack([xx - a[..., 0], yy - a[..., 1]], -1).reshape(-1, 2)
+        return (-bilinear_zeros(a, p).reshape(h, w, 2)).astype(np.float32)
+    fb = [backward(f) for f in fw]
+    f2 = [compose(fw[i], fw[i + 1]) + rng.normal(0, 0.05, (h, w, 2)).astype(np.float32) for i in range(n_frames - 2)]
+    b2 = [backward(f) for f in f2]
+    r0, r1 = (10 * h) // 36, (18 * h) // 36                  # the golden's rows 10:18 of 36
+    c0, dc = (8 * w) // 52, max(1, (4 * w) // 52)            # its columns 8+4i : 16+4i of 52
+    for i, f in enumerate(fw):
+        f[r0:r1, c0 + dc * i:2 * c0 + dc * i] += 6.0
+    return fw, fb, f2, b2
+
+
 def make_traj_inputs(num, height, width, seed=0, amplitude=6.0, upper_flow=20.0):
     """The argument tuple IncrementalTrajectorySet.optimize_buffer hands to
     particlesfm.optimize_location (point_trajectory/trajectory.py:161-186) for `num`

@@ -23,6 +23,9 @@ Semantics that decide the INTEGER TRACK CONNECTIVITY are kept bit-for-bit:
   * re-seeding: occupancy at (int(y), int(x)), Euclidean distance transform > ratio on the
     ratio-strided grid,
   * trajectory ids are the positions in the reference's `full_trajs` list (retire order).
+
+track_optimize_device / main_connect_point_trajectories_device run the same loop with every particle array
+resident on the GPU (csrc/tracker.cu, psfm_tracker_*) and return a TrackArrays; DESIGN.md §4.1.
 """
 import ctypes as _C
 
@@ -144,10 +147,9 @@ def flow_check(flows, flows_b, thres):
 class BatchedTrajectorySet:
     """SoA replacement of IncrementalTrajectorySet (buffer_size = 3)."""
 
-    def __init__(self, total_length, img_h, img_w, sample_ratio, optimize_fn, device=False):
+    def __init__(self, total_length, img_h, img_w, sample_ratio, optimize_fn):
         self.total_length, self.h, self.w, self.ratio = total_length, img_h, img_w, sample_ratio
         self.optimize_fn = optimize_fn
-        self.device = device            # True: sampling / survival / re-seeding on the GPU (csrc/tracker.cu)
         x, y = np.arange(0, img_w), np.arange(0, img_h)
         xx, yy = np.meshgrid(x, y)
         self.all_candidates = np.stack([xx, yy], -1)[::sample_ratio, ::sample_ratio, :]
@@ -190,7 +192,7 @@ class BatchedTrajectorySet:
         return self.xy_at[self.cur_time][self.act_i0]
 
     # -- extend_all (trajectory.py:129-152)
-    def extend_all(self, next_xys, next_time, flags, reseed_mask=None):
+    def extend_all(self, next_xys, next_time, flags):
         assert len(next_xys) == self.act_id.shape[0] == len(flags)
         keep = np.asarray(flags) != 0
         self.retired.append(self.act_id[~keep])
@@ -203,14 +205,11 @@ class BatchedTrajectorySet:
         self.act_im1 = self.act_i0[keep]
         self.act_i0 = np.arange(n, dtype=np.int64)
         self.cur_time = next_time
-        if reseed_mask is not None:          # computed on the device with the step (exact: squared integer distances)
-            sample_map = reseed_mask
-        else:
-            import scipy.ndimage
-            occupied = np.zeros((self.h, self.w, 1))
-            occupied[nx[:, 1].astype(np.int64), nx[:, 0].astype(np.int64)] = 1      # int() truncation
-            dist = scipy.ndimage.distance_transform_edt(1.0 - occupied)
-            sample_map = (dist > self.ratio)[::self.ratio, ::self.ratio, 0]
+        import scipy.ndimage
+        occupied = np.zeros((self.h, self.w, 1))
+        occupied[nx[:, 1].astype(np.int64), nx[:, 0].astype(np.int64)] = 1      # int() truncation
+        dist = scipy.ndimage.distance_transform_edt(1.0 - occupied)
+        sample_map = (dist > self.ratio)[::self.ratio, ::self.ratio, 0]
         self.sample_candidates = np.copy(self.all_candidates[sample_map])
 
     def clear_active(self):
@@ -229,15 +228,12 @@ class BatchedTrajectorySet:
         if sel.shape[0] == 0:
             raise ValueError("need at least one array to stack")     # np.stack([]) in the reference
         h, w = flow01_map.shape[0], flow01_map.shape[1]
-        if self.device:
-            ref1, ref2, scale = buffer_inputs_device(flow01_map, flow02_map, occ02_map, x0, upper_flow)
-        else:
-            flow01 = grid_sample(torch.from_numpy(flow01_map).permute(2, 0, 1).float(), x0)
-            flow02 = grid_sample(torch.from_numpy(flow02_map).permute(2, 0, 1).float(), x0)
-            occ02 = grid_sample(torch.from_numpy(occ02_map).unsqueeze(0).float(), x0)
-            scale = (1.0 - occ02) * (np.linalg.norm(flow02, axis=-1, keepdims=True) < upper_flow)
-            ref1 = x0 + flow01
-            ref2 = x0 + flow02
+        flow01 = grid_sample(torch.from_numpy(flow01_map).permute(2, 0, 1).float(), x0)
+        flow02 = grid_sample(torch.from_numpy(flow02_map).permute(2, 0, 1).float(), x0)
+        occ02 = grid_sample(torch.from_numpy(occ02_map).unsqueeze(0).float(), x0)
+        scale = (1.0 - occ02) * (np.linalg.norm(flow02, axis=-1, keepdims=True) < upper_flow)
+        ref1 = x0 + flow01
+        ref2 = x0 + flow02
         uv12 = np.concatenate([x1, x2], axis=1)
         new = self.optimize_fn(uv12, ref1, ref2, scale, flow12_map, uv12.shape[0], w, h)
         new = np.asarray(new, np.float64).reshape(-1, 2, 2)
@@ -266,6 +262,29 @@ class BatchedTrajectorySet:
         return out
 
 
+class TrackArrays:
+    """The track set in the reference's `full_trajs` order as four arrays: trajectory k has id ids[k] and owns
+    observations ptr[k] .. ptr[k + 1] of frame_ids / xy, in time order.
+        ids [T] int64, ptr [T + 1] int64, frame_ids [M] int32, xy [M, 2] float64"""
+
+    def __init__(self, ids, ptr, frame_ids, xy):
+        self.ids, self.ptr, self.frame_ids, self.xy = ids, ptr, frame_ids, xy
+
+    def lengths(self):
+        return np.diff(self.ptr)
+
+    def to_dict(self):
+        """{traj_id: {"frame_ids", "locations", "labels"}}, exactly what BatchedTrajectorySet.full_trajs returns."""
+        frames = self.frame_ids.tolist()
+        rows = list(self.xy.copy())             # one 1-D float64 array per location, none aliasing self.xy
+        ptr = self.ptr.tolist()
+        out = {}
+        for k, i in enumerate(self.ids.tolist()):
+            s, e = ptr[k], ptr[k + 1]
+            out[i] = {"frame_ids": frames[s:e], "locations": rows[s:e], "labels": [False] * (e - s)}
+        return out
+
+
 def _default_optimize():
     from . import traj
     return traj.optimize_location
@@ -275,23 +294,18 @@ def track_optimize(flows, flows_f2, occ_maps, occ_maps_s2, sample_ratio, optimiz
     """Sequentially track and optimise point trajectories (track_optimize.py:24-54).
     Returns {traj_id: {"frame_ids", "locations", "labels"}} with the reference's ids
     (= positions in its `full_trajs` list); `traj_min_len` applies the filter of
-    main_connect_point_trajectories.py:57-60.  device=True: the float32 sampling, the survival test and
-    the re-seeding run on the GPU (same bits, csrc/tracker.cu) instead of torch-CPU / scipy."""
+    main_connect_point_trajectories.py:57-60.  device=True: the whole stage runs resident on the GPU
+    (track_optimize_device, same bits)."""
+    if device:
+        return track_optimize_device(flows, flows_f2, occ_maps, occ_maps_s2, sample_ratio, optimize_fn, traj_min_len).to_dict()
     import torch
     optimize_fn = optimize_fn or _default_optimize()
     n_flows = len(flows)
     h, w = flows[0].shape[:2]
-    trajs = BatchedTrajectorySet(n_flows + 1, h, w, sample_ratio, optimize_fn, device=device)
+    trajs = BatchedTrajectorySet(n_flows + 1, h, w, sample_ratio, optimize_fn)
     for frame_id in range(n_flows):
         trajs.new_traj_all(frame_id, trajs.sample_candidates)
         cur_xys = trajs.get_cur_pos()
-        if device:
-            next_xys, flags, mask = tracker_step_device(flows[frame_id], occ_maps[frame_id], cur_xys, sample_ratio)
-            trajs.extend_all(next_xys, frame_id + 1, flags, mask)
-            if frame_id + 1 >= 2:
-                trajs.optimize_buffer(flows[frame_id - 1], flows[frame_id], flows_f2[frame_id - 1],
-                                      occ_maps_s2[frame_id - 1], frame_id + 1)
-            continue
         flow_sample = grid_sample(torch.from_numpy(flows[frame_id]).permute(2, 0, 1).float(), cur_xys)
         # step_forward (trajectory.py:45-62)
         occ = grid_sample(torch.from_numpy(occ_maps[frame_id]).unsqueeze(0).float(), cur_xys) > 0.1
@@ -310,8 +324,143 @@ def main_connect_point_trajectories(flows_f, flows_b, flows_f2, flows_b2, sample
                                     traj_min_len=3, optimize_fn=None, device=False):
     """In-memory equivalent of main_connect_point_trajectories.py:27-62 with
     skip_path_consistency=False: returns the dict a `particlesfm.TrajectorySet` is built
-    from (and np.save'd as track.npy)."""
-    fc = flow_check_device if device else flow_check
-    _, occ = fc(flows_f, flows_b, flow_check_thres)
-    _, occ2 = fc(flows_f2, flows_b2, flow_check_thres)
-    return track_optimize(flows_f, flows_f2, occ, occ2, sample_ratio, optimize_fn, traj_min_len, device=device)
+    from (and np.save'd as track.npy).  device=True: main_connect_point_trajectories_device(...).to_dict()."""
+    if device:
+        return main_connect_point_trajectories_device(flows_f, flows_b, flows_f2, flows_b2, sample_ratio, flow_check_thres,
+                                                      traj_min_len, optimize_fn).to_dict()
+    _, occ = flow_check(flows_f, flows_b, flow_check_thres)
+    _, occ2 = flow_check(flows_f2, flows_b2, flow_check_thres)
+    return track_optimize(flows_f, flows_f2, occ, occ2, sample_ratio, optimize_fn, traj_min_len)
+
+
+# ----------------------------------------------------------------------------- the stage resident on the GPU
+
+def _on_device(a, dtype):
+    """A map as a contiguous CUDA tensor of `dtype` (torch.float32 flows, torch.uint8 occlusion maps).  A numpy
+    array crosses the bus here, once; a CUDA tensor of the right type is used in place."""
+    import torch
+    if not isinstance(a, torch.Tensor):
+        a = np.ascontiguousarray(a)
+        a = torch.from_numpy(a.view(np.uint8) if a.dtype == np.bool_ else a)
+    if a.dtype == torch.bool and dtype == torch.uint8:
+        a = a.contiguous().view(torch.uint8)
+    return a.to(device="cuda", dtype=dtype).contiguous()
+
+
+def _on_host(a):
+    import torch
+    return a.cpu().numpy() if isinstance(a, torch.Tensor) else a
+
+
+class _ResidentTracker:
+    """A psfm_tracker handle (csrc/tracker.cu) on torch's current stream."""
+
+    def __init__(self, h, w, sample_ratio, num_frames):
+        from . import _lib
+        self.L, self.check = _lib.lib(), _lib.check
+        self.h, self.w = h, w
+        self.handle = _C.c_void_p()
+        self.stream = None
+        if self.L.psfm_device_count() > 0:      # without a device the library refuses below, before torch touches CUDA
+            import torch
+            self.stream = torch.cuda.current_stream().cuda_stream
+        self.check(self.L.psfm_tracker_create(h, w, sample_ratio, num_frames, self.stream, _C.byref(self.handle)),
+                   "psfm_tracker_create")
+
+    def close(self):
+        if self.handle:
+            self.L.psfm_tracker_destroy(self.handle)
+            self.handle = _C.c_void_p()
+
+    def flow_check(self, flow_f, flow_b, thres):
+        import torch
+        occ = torch.empty((self.h, self.w), dtype=torch.uint8, device=flow_f.device)
+        self.check(self.L.psfm_flow_check_device(flow_f.data_ptr(), flow_b.data_ptr(), self.h, self.w, float(thres), None,
+                                                 occ.data_ptr(), self.stream), "psfm_flow_check_device")
+        return occ
+
+    def step(self, flow, occ, flow_prev=None, flow2_prev=None, occ2_prev=None):
+        """new_traj_all + step_forward + extend_all (+ optimize_buffer's selection) -> number of buffered particles"""
+        ptr = lambda t: None if t is None else t.data_ptr()
+        counts = (_C.c_int32 * 3)()
+        self.check(self.L.psfm_tracker_advance(self.handle, flow.data_ptr(), occ.data_ptr(), ptr(flow_prev), ptr(flow2_prev),
+                                               ptr(occ2_prev), counts), "psfm_tracker_advance")
+        return counts[2]
+
+    def optimize_buffer(self, n, optimize_fn, flow12_map):
+        if n == 0:
+            raise ValueError("need at least one array to stack")     # np.stack([]) in the reference
+        if optimize_fn is None:
+            self.check(self.L.psfm_tracker_optimize(self.handle, None, None), "psfm_tracker_optimize")
+            return
+        from . import _lib
+        uv12, ref1, ref2, scale = np.empty((n, 4)), np.empty((n, 2)), np.empty((n, 2)), np.empty((n, 1))
+        self.check(self.L.psfm_tracker_get_buffer(self.handle, _lib.dptr(uv12), _lib.dptr(ref1), _lib.dptr(ref2),
+                                                  _lib.dptr(scale)), "psfm_tracker_get_buffer")
+        new = optimize_fn(uv12, ref1, ref2, scale, _on_host(flow12_map), n, self.w, self.h)
+        new = np.ascontiguousarray(np.asarray(new, np.float64).reshape(n, 4))
+        self.check(self.L.psfm_tracker_set_buffer(self.handle, _lib.dptr(new)), "psfm_tracker_set_buffer")
+
+    def finish(self, traj_min_len):
+        from . import _lib
+        nt, m = _C.c_int64(), _C.c_int64()
+        self.check(self.L.psfm_tracker_finish(self.handle, int(traj_min_len), _C.byref(nt), _C.byref(m)), "psfm_tracker_finish")
+        ids, ptr = np.empty(nt.value, np.int64), np.empty(nt.value + 1, np.int64)
+        frame_ids, xy = np.empty(m.value, np.int32), np.empty((m.value, 2), np.float64)
+        i64 = lambda a: a.ctypes.data_as(_C.POINTER(_C.c_int64))
+        self.check(self.L.psfm_tracker_result(self.handle, i64(ids), i64(ptr), frame_ids.ctypes.data_as(_C.POINTER(_C.c_int32)),
+                                              _lib.dptr(xy)), "psfm_tracker_result")
+        return TrackArrays(ids, ptr, frame_ids, xy)
+
+
+def track_optimize_device(flows, flows_f2, occ_maps, occ_maps_s2, sample_ratio, optimize_fn=None, traj_min_len=0):
+    """track_optimize (track_optimize.py:24-54) resident on the GPU -> TrackArrays, bit for bit the host path's
+    track set.  Maps are numpy arrays or CUDA tensors ([H, W, 2] float32 flows, [H, W] bool occlusion maps); each
+    crosses the bus at most once.  optimize_fn=None: HP1 on the device; otherwise it is called per frame with host
+    arrays, as optimize_buffer calls it: (uv12, ref1, ref2, scale, flow12_map, n, w, h)."""
+    n_flows = len(flows)
+    h, w = flows[0].shape[:2]
+    trk = _ResidentTracker(h, w, sample_ratio, n_flows + 1)
+    try:
+        import torch
+        prev = None
+        for frame_id in range(n_flows):
+            flow = _on_device(flows[frame_id], torch.float32)
+            occ = _on_device(occ_maps[frame_id], torch.uint8)
+            if frame_id + 1 >= 2:
+                n = trk.step(flow, occ, prev, _on_device(flows_f2[frame_id - 1], torch.float32),
+                             _on_device(occ_maps_s2[frame_id - 1], torch.uint8))
+                trk.optimize_buffer(n, optimize_fn, flows[frame_id])
+            else:
+                trk.step(flow, occ)
+            prev = flow
+        return trk.finish(traj_min_len)
+    finally:
+        trk.close()
+
+
+def main_connect_point_trajectories_device(flows_f, flows_b, flows_f2, flows_b2, sample_ratio=2, flow_check_thres=1.0,
+                                           traj_min_len=3, optimize_fn=None):
+    """main_connect_point_trajectories resident on the GPU -> TrackArrays: the flow check runs inside the loop on
+    the resident maps, and its occlusion maps never leave the device."""
+    n_flows = len(flows_f)
+    h, w = flows_f[0].shape[:2]
+    trk = _ResidentTracker(h, w, sample_ratio, n_flows + 1)
+    try:
+        import torch
+        f32 = torch.float32
+        prev = None
+        for frame_id in range(n_flows):
+            flow = _on_device(flows_f[frame_id], f32)
+            occ = trk.flow_check(flow, _on_device(flows_b[frame_id], f32), flow_check_thres)
+            if frame_id + 1 >= 2:
+                f2 = _on_device(flows_f2[frame_id - 1], f32)
+                occ2 = trk.flow_check(f2, _on_device(flows_b2[frame_id - 1], f32), flow_check_thres)
+                n = trk.step(flow, occ, prev, f2, occ2)
+                trk.optimize_buffer(n, optimize_fn, flows_f[frame_id])
+            else:
+                trk.step(flow, occ)
+            prev = flow
+        return trk.finish(traj_min_len)
+    finally:
+        trk.close()
