@@ -187,6 +187,30 @@ int psfm_tracker_result(psfm_tracker* t, int64_t* ids, int64_t* ptr, int32_t* fr
 void psfm_tracker_destroy(psfm_tracker* t);
 
 /* ------------------------------------------------------------------------- */
+/* SURVEY.md 8(f) row f-2: track set -> COLMAP keypoints and matches          */
+/* (sfm/matches_from_flow.py:51-118, csrc/handoff.cu).  Host buffers in, host   */
+/* buffers out; the result stays on the device until it is fetched.  Bit for   */
+/* bit what handoff.traj_to_matches returns.                                    */
+/* ------------------------------------------------------------------------- */
+typedef struct psfm_matches psfm_matches;
+/* The kept samples of num_trajs trajectories in the reference's visiting order: trajectory t owns samples
+   traj_ptr[t] .. traj_ptr[t + 1] (traj_ptr[0] = 0, non-decreasing, at most 2^31 - 1 samples), frame_ids [..]
+   and xy [..][2] per sample.  Every sample becomes a keypoint of its frame (keypoint index = number of earlier
+   samples of that frame); a trajectory of n samples matches sample j with every k != j when n <= sample_k,
+   otherwise with the targets s * (n / sample_k), s < sample_k, other than j.  Matches are grouped by ordered
+   image pair (a, b), in visiting order inside a pair; pairs are listed by a, then by first appearance.
+   num_pairs / num_matches receive the result's sizes.  A frame id outside [0, num_images) is PSFM_ERR_INVALID. */
+int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, const int64_t* frame_ids, const double* xy,
+                        int32_t num_images, int32_t sample_k, psfm_matches** out, int64_t* num_pairs,
+                        int64_t* num_matches);
+/* host copies of the result: keypoint_ptr [num_images + 1] (image i owns keypoints keypoint_ptr[i] ..
+   keypoint_ptr[i + 1]), keypoints [traj_ptr[num_trajs]][2], pair_images [num_pairs][2], pair_ptr [num_pairs + 1]
+   (pair p owns matches pair_ptr[p] .. pair_ptr[p + 1]), matches [num_matches][2] (keypoint in a, keypoint in b) */
+int psfm_matches_result(const psfm_matches* m, int64_t* keypoint_ptr, double* keypoints, int64_t* pair_images,
+                        int64_t* pair_ptr, int64_t* matches);
+void psfm_matches_destroy(psfm_matches* m);
+
+/* ------------------------------------------------------------------------- */
 /* SURVEY.md 8(f) row f-4: the RANSAC-free steps that initialise HP2, batched (csrc/init_geometry.cu). */
 /* Host buffers in, host buffers out.                                          */
 /* ------------------------------------------------------------------------- */

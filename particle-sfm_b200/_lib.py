@@ -22,7 +22,8 @@ EXPORTS = [
     "psfm_ba_get_observation_mask", "psfm_ba_get_point_errors", "psfm_ba_iterative_refinement",
     "psfm_grid_sample", "psfm_flow_check", "psfm_tracker_step", "psfm_tracker_buffer_inputs",
     "psfm_tracker_create", "psfm_tracker_advance", "psfm_tracker_optimize", "psfm_tracker_get_buffer", "psfm_tracker_set_buffer",
-    "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy", "psfm_known_rotation_translations", "psfm_triangulate_tracks", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
+    "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy",
+    "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy", "psfm_known_rotation_translations", "psfm_triangulate_tracks", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
 
@@ -83,6 +84,10 @@ def lib():
     L.psfm_tracker_result.argtypes = [vp, i64p, i64p, ip, dp]
     L.psfm_tracker_destroy.argtypes = [vp]
     L.psfm_tracker_destroy.restype = None
+    L.psfm_matches_create.argtypes = [i64p, C.c_int64, i64p, dp, C.c_int32, C.c_int32, C.POINTER(vp), i64p, i64p]
+    L.psfm_matches_result.argtypes = [vp, i64p, dp, i64p, i64p, i64p]
+    L.psfm_matches_destroy.argtypes = [vp]
+    L.psfm_matches_destroy.restype = None
     L.psfm_ba_default_refine_options.argtypes = [C.POINTER(_abi.BARefineOptions)]
     L.psfm_ba_default_refine_options.restype = None
     L.psfm_ba_filter_negative_depth.argtypes = [C.c_void_p, i64p]

@@ -28,6 +28,7 @@ UNITS = [
     ("common.cu", []),
     ("microbench.cu", []),
     ("tracker.cu", []),
+    ("handoff.cu", []),
     ("init_geometry.cu", []),
     ("dist.cu", []),
     ("ba_solver.cu", []),

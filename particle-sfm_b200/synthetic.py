@@ -253,3 +253,26 @@ def make_traj_inputs(num, height, width, seed=0, amplitude=6.0, upper_flow=20.0)
     scale = scale.astype(np.float32).astype(np.float64)
     uv12 = np.concatenate([x1, x2], -1)
     return uv12, x0 + fl01, x0 + fl02, scale, f12
+
+
+def make_track_arrays(num_trajs, num_frames, num_obs, seed=0, min_len=3, width=1024, height=436):
+    """A seeded tracker.TrackArrays shaped like the tracker's output, with exactly `num_obs` observations:
+    contiguous frame windows, geometric lengths clipped to [min_len, num_frames], then lengthened or shortened one
+    observation at a time on random trajectories until the total matches."""
+    from .tracker import TrackArrays
+    if not min_len * num_trajs <= num_obs <= num_frames * num_trajs:
+        raise ValueError("num_obs is out of reach of num_trajs trajectories of min_len .. num_frames observations")
+    rng = np.random.default_rng(seed)
+    lens = np.clip(rng.geometric(num_trajs / num_obs, num_trajs), min_len, num_frames).astype(np.int64)
+    diff = num_obs - int(lens.sum())
+    while diff:
+        step = 1 if diff > 0 else -1
+        cand = np.nonzero(lens < num_frames if step > 0 else lens > min_len)[0]
+        pick = rng.choice(cand, min(abs(diff), cand.shape[0]), replace=False)
+        lens[pick] += step
+        diff -= step * pick.shape[0]
+    start = (rng.random(num_trajs) * (num_frames - lens + 1)).astype(np.int64)
+    ptr = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    frames = (np.arange(num_obs) - np.repeat(ptr[:-1], lens) + np.repeat(start, lens)).astype(np.int32)
+    xy = rng.random((num_obs, 2)) * np.array([width - 1, height - 1], np.float64)
+    return TrackArrays(np.arange(num_trajs, dtype=np.int64), ptr, frames, xy)
