@@ -229,6 +229,29 @@ int psfm_known_rotation_translations(const double* points1, const double* points
    normalised image points (:492-493), track t owns the range track_ptr[t] .. track_ptr[t + 1]; xyz: [num_tracks][3] */
 int psfm_triangulate_tracks(const double* proj_matrices, const double* points, const int32_t* track_ptr,
                             int32_t num_tracks, double* xyz);
+/* TwoViewGeometry::EstimateRelativePose (estimators/two_view_geometry.cc:172-239) of num_pairs verified image pairs
+   at once, the step gcolmap's DatabaseCache::Load runs as one ThreadPool task per pair (base/database_cache.cc:206-228)
+   (csrc/two_view.cu).  Images: keypoint_ptr [num_images + 1] (image f owns keypoints keypoint_ptr[f] ..
+   keypoint_ptr[f + 1]), keypoints [..][2] float32 as stored in the database (COLMAP origin), image_camera
+   [num_images] into cameras [num_cameras][3] SIMPLE_PINHOLE (f, cx, cy).  Pairs: pair_images [num_pairs][2] image
+   indices (image 1, image 2), config, E / F / H [num_pairs][9] row-major, inlier_ptr [num_pairs + 1] (pair p owns
+   inlier_matches [inlier_ptr[p] .. inlier_ptr[p + 1]][2]: keypoint in image 1, keypoint in image 2).
+   Per pair: CALIBRATED (2) and UNCALIBRATED (3, E = K2' F K1) decompose E, PLANAR (4), PANORAMIC (5) and
+   PLANAR_OR_PANORAMIC (6) decompose H; the candidate with the most correspondences triangulated in front of both
+   cameras (CheckCheirality) gives qvec (w, x, y, z), tvec, num_points3D and tri_angle = the median triangulation
+   angle of its points (0 without any); PLANAR_OR_PANORAMIC becomes PANORAMIC (tri_angle 0) when |t| = 0, else
+   PLANAR.  estimated = 1 for those configs; any other config passes through (estimated 0, config unchanged, zero
+   outputs).  Two results the reference leaves undefined are defined here: the four essential candidates are ordered
+   (R1, t), (R2, t), (R1, -t), (R2, -t) with t's largest-magnitude component positive and trace R1 >= trace R2, and
+   a homography of which no candidate keeps a point (a pure rotation: R = the normalised H, t = 0) gives candidate 0
+   with tri_angle 0.  An image, camera or keypoint index out of range is PSFM_ERR_INVALID before anything runs.
+   With no pair nothing is launched; with no inlier match only the per-pair kernels run. */
+int psfm_two_view_relative_poses(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
+                                 const int32_t* image_camera, const double* cameras, int32_t num_cameras,
+                                 int64_t num_pairs, const int32_t* pair_images, const int32_t* config,
+                                 const double* E, const double* F, const double* H, const int64_t* inlier_ptr,
+                                 const uint32_t* inlier_matches, double* qvec, double* tvec, double* tri_angle,
+                                 int32_t* config_out, int64_t* num_points3D, uint8_t* estimated);
 
 /* ------------------------------------------------------------------------- */
 /* HP2 — global bundle adjustment                                             */

@@ -23,7 +23,8 @@ EXPORTS = [
     "psfm_grid_sample", "psfm_flow_check", "psfm_tracker_step", "psfm_tracker_buffer_inputs",
     "psfm_tracker_create", "psfm_tracker_advance", "psfm_tracker_optimize", "psfm_tracker_get_buffer", "psfm_tracker_set_buffer",
     "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy",
-    "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy", "psfm_known_rotation_translations", "psfm_triangulate_tracks", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
+    "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy", "psfm_known_rotation_translations", "psfm_triangulate_tracks",
+    "psfm_two_view_relative_poses", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
 
@@ -73,6 +74,8 @@ def lib():
     L.psfm_known_rotation_translations.argtypes = [dp, dp, ip, dp, dp, C.c_int32, dp, ip]
     L.psfm_triangulate_tracks.argtypes = [dp, dp, ip, C.c_int32, dp]
     i64p = C.POINTER(C.c_int64)
+    L.psfm_two_view_relative_poses.argtypes = [C.c_int32, i64p, fp, ip, dp, C.c_int32, C.c_int64, ip, ip, dp, dp, dp, i64p,
+                                               C.POINTER(C.c_uint32), dp, dp, dp, ip, i64p, C.POINTER(C.c_uint8)]
     vp = C.c_void_p
     L.psfm_tracker_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.POINTER(vp)]
     L.psfm_tracker_advance.argtypes = [vp] * 6 + [ip]

@@ -30,6 +30,7 @@ UNITS = [
     ("tracker.cu", []),
     ("handoff.cu", []),
     ("init_geometry.cu", []),
+    ("two_view.cu", []),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

@@ -276,3 +276,63 @@ def make_track_arrays(num_trajs, num_frames, num_obs, seed=0, min_len=3, width=1
     frames = (np.arange(num_obs) - np.repeat(ptr[:-1], lens) + np.repeat(start, lens)).astype(np.int32)
     xy = rng.random((num_obs, 2)) * np.array([width - 1, height - 1], np.float64)
     return TrackArrays(np.arange(num_trajs, dtype=np.int64), ptr, frames, xy)
+
+
+def make_two_view_scene(num_trajs, num_frames, num_obs, seed=0, focal=500.0, width=1024, height=436, step=0.02):
+    """Static points seen by a camera that moves `step` per frame along x with a slow yaw: a tracker.TrackArrays with
+    make_track_arrays' counts whose locations are the points' exact projections, minus the 0.5 that
+    import_keypoints_matches adds back.  Every point lies 2 .. 40 in front of the camera at its first frame, so that
+    between adjacent frames it is 100 .. 2000 baselines away: it straddles CheckCheirality's max_depth.
+    Returns (tracks, qvec [F][4], tvec [F][3] world-to-camera, camera (f, cx, cy))."""
+    tracks = make_track_arrays(num_trajs, num_frames, num_obs, seed=seed, width=width, height=height)
+    rng = np.random.default_rng(seed + 1)
+    f = np.arange(num_frames, dtype=np.float64)
+    R = axis_angle_to_rotmat(np.stack([0.001 * f, 0.004 * f, np.zeros_like(f)], axis=1))
+    centres = np.stack([step * f, 0.1 * step * np.sin(f), np.zeros_like(f)], axis=1)
+    tvec = -np.einsum("fij,fj->fi", R, centres)
+    cam = np.array([focal, width / 2.0, height / 2.0])
+    first = tracks.frame_ids[tracks.ptr[:-1]]
+    px = rng.random((num_trajs, 2)) * np.array([width, height])
+    depth = 2.0 + 38.0 * rng.random(num_trajs)
+    Xc = np.stack([(px[:, 0] - cam[1]) / focal * depth, (px[:, 1] - cam[2]) / focal * depth, depth], axis=1)
+    Xw = np.einsum("nji,nj->ni", R[first], Xc - tvec[first])
+    X = np.repeat(Xw, np.diff(tracks.ptr), axis=0)
+    fr = tracks.frame_ids
+    Xcam = np.einsum("nij,nj->ni", R[fr], X) + tvec[fr]
+    tracks.xy = focal * Xcam[:, :2] / Xcam[:, 2:] + cam[1:] - 0.5
+    return tracks, rotmat_to_qvec(R), tvec, cam
+
+
+def relative_essential(qvec, tvec, a, b):
+    """E = [t]x R of the relative pose from image a to image b (world-to-camera poses)."""
+    Ra, Rb = qvec_to_rotmat(qvec[a]), qvec_to_rotmat(qvec[b])
+    Rr = Rb @ Ra.T
+    t = tvec[b] - Rr @ tvec[a]
+    tx = np.array([[0.0, -t[2], t[1]], [t[2], 0.0, -t[0]], [-t[1], t[0], 0.0]])
+    return tx @ Rr
+
+
+def two_view_inputs(rows, image_ids, qvec, tvec, camera):
+    """The arguments of init_geometry.estimate_relative_poses for handoff.DatabaseRows of one SIMPLE_PINHOLE camera:
+    images in image_id order, pairs in row order, config CALIBRATED with E from the poses (qvec / tvec indexed by the
+    position of the image in `image_ids`, a list of database ids); F = H = I."""
+    order = np.argsort(image_ids)
+    index = {int(image_ids[k]): r for r, k in enumerate(order)}
+    kp = dict(rows.keypoints)
+    kps = [kp[int(image_ids[k])] for k in order]
+    from .handoff import pair_id_to_image_ids
+    R = len(rows.matches)
+    pair_images = np.zeros((R, 2), np.int32)
+    E = np.zeros((R, 3, 3))
+    for p, (pid, _) in enumerate(rows.matches):
+        a, b = (index[int(i)] for i in pair_id_to_image_ids(pid))
+        pair_images[p] = a, b
+        E[p] = relative_essential(qvec, tvec, order[a], order[b])
+    counts = np.array([m.shape[0] for _, m in rows.matches], np.int64)
+    eye = np.broadcast_to(np.eye(3), (R, 3, 3))
+    return dict(keypoint_ptr=np.concatenate([[0], np.cumsum([k.shape[0] for k in kps])]).astype(np.int64),
+                keypoints=np.concatenate(kps) if kps else np.zeros((0, 2), np.float32),
+                image_camera=np.zeros(len(image_ids), np.int32), cameras=np.asarray(camera, np.float64).reshape(1, 3),
+                pair_images=pair_images, config=np.full(R, 2, np.int32), E=E, F=eye, H=eye,
+                inlier_ptr=np.concatenate([[0], np.cumsum(counts)]).astype(np.int64),
+                inlier_matches=np.concatenate([m for _, m in rows.matches]) if R else np.zeros((0, 2), np.uint32))
