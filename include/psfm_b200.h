@@ -36,6 +36,8 @@ typedef enum {
   PSFM_OK = 0,
   PSFM_ZERO_RESIDUALS = 1,      /* HP2: problem has no residual (reference returns false,
                                    bundle_adjustment.cc:268-271) */
+  PSFM_NO_ROTATIONS = 2,        /* psfm_estimate_global_rotations: no posed pair, or a factorisation failed
+                                   (reference returns false, robust_rotation_estimator.cc:101-109, 315-317) */
   PSFM_ERR_INVALID = -1,        /* bad argument / inconsistent sizes */
   PSFM_ERR_NO_DEVICE = -2,      /* no CUDA device: the product has no CPU path */
   PSFM_ERR_CUDA = -3,           /* CUDA runtime error; see psfm_last_error() */
@@ -252,6 +254,60 @@ int psfm_two_view_relative_poses(int32_t num_images, const int64_t* keypoint_ptr
                                  const double* E, const double* F, const double* H, const int64_t* inlier_ptr,
                                  const uint32_t* inlier_matches, double* qvec, double* tvec, double* tri_angle,
                                  int32_t* config_out, int64_t* num_points3D, uint8_t* estimated);
+
+/* RobustRotationEstimator::Options (global/robust_rotation_estimator.h:61-89); NULL gives these defaults, which are
+   what sfm/main_sfm.py runs.  Check() (robust_rotation_estimator.cc:54-62): every field > 0. */
+typedef struct {
+  int32_t max_num_l1_iterations;            /* 5: L1 rounds (at most PSFM_ROTATION_MAX_L1_ROUNDS here) */
+  double l1_step_convergence_threshold;     /* 0.001 */
+  int32_t max_num_irls_iterations;          /* 100 */
+  double irls_step_convergence_threshold;   /* 0.001 */
+  double irls_loss_parameter_sigma;         /* DegToRad(5.0) */
+  double rotation_filter_max_degrees;       /* 5.0 */
+} psfm_rotation_options;
+
+/* The ADMM cap doubles every L1 round from 5 (robust_rotation_estimator.cc:164, 179): 16 rounds end at 163,840
+   iterations, and the reference's int cap overflows past 28. */
+#define PSFM_ROTATION_MAX_L1_ROUNDS 16
+
+typedef struct {
+  int32_t num_l1_rounds;                               /* L1Solver::Solve calls */
+  int32_t admm_iterations[PSFM_ROTATION_MAX_L1_ROUNDS]; /* ADMM iterations of each round (0 past the last) */
+  int32_t num_irls_iterations;
+  double l1_final_step;                                /* ComputeAverageStepSize after the last L1 round */
+  double irls_final_step;                              /* ... after the last IRLS iteration */
+  int32_t gauge_image;                                 /* image index held at the identity (-1: none) */
+  int32_t num_images_connected, num_pairs_connected;   /* after the first RemoveDisconnectedViewPairs */
+  int32_t num_images_kept, num_pairs_kept;             /* after the rotation filter and the second one */
+  int64_t num_launches;                                /* kernels this call launched */
+  double host_ms, device_ms;                           /* graph work on the host, device loop (wall, synchronised) */
+} psfm_rotation_summary;
+
+void psfm_rotation_default_options(psfm_rotation_options* opts);
+
+/* EstimateGlobalRotations (global/robust_rotation_estimator.cc:310-331), the first step of
+   GlobalMapper's reconstruction (controllers/global_mapper.cc:136-184, sfm/global_mapper.cc:89-92)
+   (csrc/rotation_averaging.cu).  Pairs: pair_images [num_pairs][2] image indices (image 1, image 2), qvec
+   [num_pairs][4] (w, x, y, z) the relative rotation 2_R_1 (world-to-camera orientations: R2 = R12 R1),
+   num_correspondences [num_pairs], has_pose [num_pairs] (NULL: all 1).  A pair takes part when has_pose is set and
+   its qvec is finite (AllPairs(only_with_pose), base/correspondence_graph.cc:92-100, 148-150).  Steps:
+   RemoveDisconnectedViewPairs (global/filter_util.cc:382-431), OrientationsFromMaximumSpanningTree
+   (global/orientation_util.cc:102-178), RobustRotationEstimator::EstimateRotations (L1 regression by ADMM, then
+   IRLS, robust_rotation_estimator.cc:80-250), FilterViewPairsFromOrientation (filter_util.cc:271-325) and
+   RemoveDisconnectedViewPairs again.  Defined here where the reference follows hash order: among equally large
+   components the one holding the smallest image index is kept; the gauge image and spanning-tree root is the
+   smallest image index of the component (identity orientation); spanning-tree ties go by (-num_correspondences,
+   image 1, image 2).
+   Out: orientations [num_images][4] (w, x, y, z; zero without one), has_orientation [num_images] (the images of the
+   kept component, as the reference keeps them even when the second pruning leaves them no pair), pair_kept
+   [num_pairs], summary (nullable).  PSFM_ERR_INVALID before anything runs for an image index out of range, a pair of
+   an image with itself, an unordered pair listed twice, or options that fail Check(); PSFM_ERR_UNSUPPORTED for more
+   than 8192 images in the kept component (the dense factor) or more than PSFM_ROTATION_MAX_L1_ROUNDS L1 rounds;
+   PSFM_NO_ROTATIONS, with nothing launched, when no posed pair exists. */
+int psfm_estimate_global_rotations(int32_t num_images, int64_t num_pairs, const int32_t* pair_images,
+                                   const double* qvec, const int32_t* num_correspondences, const uint8_t* has_pose,
+                                   const psfm_rotation_options* opts, double* orientations, uint8_t* has_orientation,
+                                   uint8_t* pair_kept, psfm_rotation_summary* summary);
 
 /* ------------------------------------------------------------------------- */
 /* HP2 — global bundle adjustment                                             */

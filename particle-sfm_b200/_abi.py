@@ -252,3 +252,36 @@ class BAProblem:
         s.tvec_constant_mask = _ptr(self.tvec_constant_mask, C.c_uint8)
         s.camera_constant = _ptr(self.camera_constant, C.c_uint8)
         return s
+
+
+ROTATION_MAX_L1_ROUNDS = 16   # PSFM_ROTATION_MAX_L1_ROUNDS
+NO_ROTATIONS = 2              # PSFM_NO_ROTATIONS
+
+
+class RotationOptions(C.Structure):
+    _fields_ = [
+        ("max_num_l1_iterations", C.c_int32),
+        ("l1_step_convergence_threshold", C.c_double),
+        ("max_num_irls_iterations", C.c_int32),
+        ("irls_step_convergence_threshold", C.c_double),
+        ("irls_loss_parameter_sigma", C.c_double),
+        ("rotation_filter_max_degrees", C.c_double),
+    ]
+
+
+class RotationSummary(C.Structure):
+    _fields_ = [
+        ("num_l1_rounds", C.c_int32),
+        ("admm_iterations", C.c_int32 * ROTATION_MAX_L1_ROUNDS),
+        ("num_irls_iterations", C.c_int32),
+        ("l1_final_step", C.c_double),
+        ("irls_final_step", C.c_double),
+        ("gauge_image", C.c_int32),
+        ("num_images_connected", C.c_int32),
+        ("num_pairs_connected", C.c_int32),
+        ("num_images_kept", C.c_int32),
+        ("num_pairs_kept", C.c_int32),
+        ("num_launches", C.c_int64),
+        ("host_ms", C.c_double),
+        ("device_ms", C.c_double),
+    ]

@@ -31,6 +31,7 @@ UNITS = [
     ("handoff.cu", []),
     ("init_geometry.cu", []),
     ("two_view.cu", []),
+    ("rotation_averaging.cu", []),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

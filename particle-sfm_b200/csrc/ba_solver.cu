@@ -22,6 +22,7 @@
 #include "ba_band_chol.cuh"
 #include "ba_refine.cuh"
 #include "dist.cuh"
+#include "dense_chol.cuh"
 
 namespace psfm {
 namespace ba {
@@ -1067,6 +1068,23 @@ void ensure_pairs(psfm_ba_solver* S) {
   tm.mark("tile pair tasks (explicit Schur)");
 }
 
+// co-resident CTAs k_chol_blocked may use on the current device (one per SM), cached per device
+int chol_grid_limit() {
+  int dev = 0;
+  PSFM_CUDA(cudaGetDevice(&dev));
+  static std::mutex mu;
+  static std::vector<int> grid_limit_by_dev;
+  std::lock_guard<std::mutex> lk(mu);
+  if ((int)grid_limit_by_dev.size() <= dev) grid_limit_by_dev.resize(dev + 1, 0);
+  if (grid_limit_by_dev[dev] == 0) {
+    int sms = 0, per_sm = 0;
+    PSFM_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PSFM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_chol_blocked, 256, 0));
+    grid_limit_by_dev[dev] = std::max(1, sms * std::min(per_sm, 1));
+  }
+  return grid_limit_by_dev[dev];
+}
+
 // blocked band(+arrow) Cholesky of d_S (rhs carried as the extra row) -> d_x; d_cholfail[0] = 1 on a
 // bad pivot (read back with the step scalars at the end of compute_step: no host sync here)
 void launch_cholesky(psfm_ba_solver* S) {
@@ -1074,22 +1092,7 @@ void launch_cholesky(psfm_ba_solver* S) {
   const int nbnd = 6 * S->F;
   const int bw = std::min(S->bw, nbnd);
   {
-    int dev = 0;
-    PSFM_CUDA(cudaGetDevice(&dev));
-    static std::mutex mu;
-    static std::vector<int> grid_limit_by_dev;
-    int grid_limit = 0;
-    {
-      std::lock_guard<std::mutex> lk(mu);
-      if ((int)grid_limit_by_dev.size() <= dev) grid_limit_by_dev.resize(dev + 1, 0);
-      if (grid_limit_by_dev[dev] == 0) {
-        int sms = 0, per_sm = 0;
-        PSFM_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-        PSFM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_chol_blocked, 256, 0));
-        grid_limit_by_dev[dev] = std::max(1, sms * std::min(per_sm, 1));
-      }
-      grid_limit = grid_limit_by_dev[dev];
-    }
+    const int grid_limit = chol_grid_limit();
     CholArgs ca;
     ca.A = S->d_S.p; ca.ns = S->NS; ca.lda = S->NS + 1; ca.nb = nbnd; ca.bw = bw + 1; ca.x = S->d_x.p; ca.fail = S->d_cholfail.p;
     if (S->d_cholbar.n == 0) S->d_cholbar.alloc(1, st);
@@ -1971,4 +1974,19 @@ extern "C" int psfm_ba_linear_step(psfm_ba_solver* S, const psfm_ba_options* opt
   } catch (const CudaFail& f) {
     return f.code;
   }
+}
+
+// dense_chol.cuh: k_chol_blocked on a whole dense system, launched the way launch_cholesky launches it for dense S
+// (nb = ns, a band as wide as the matrix: every row below a panel is a band row, the rhs row is the only arrow row)
+void psfm::dense_cholesky_launch(double* A, int ns, double* x, int* fail, unsigned int* bar, double* Lp, double* Ld,
+                                 cudaStream_t st) {
+  CholArgs ca;
+  ca.A = A; ca.ns = ns; ca.lda = ns + 1; ca.nb = ns; ca.bw = ns; ca.x = x; ca.fail = fail; ca.bar = bar;
+  ca.Lp = Lp; ca.Ld = Ld; ca.rmax = dense_chol_rmax(ns);
+  PSFM_CUDA(cudaMemsetAsync(bar, 0, sizeof(unsigned int), st));
+  void* kargs[] = {(void*)&ca};
+  const int tiles = (ns + 1 + CB - 1) / CB;
+  const int grid = std::max(1, std::min(chol_grid_limit(), tiles * (tiles + 1) / 2));
+  PSFM_CUDA(cudaLaunchCooperativeKernel((void*)k_chol_blocked, dim3(grid), dim3(256), kargs, 0, st));
+  PSFM_LAUNCH_CHECK();
 }

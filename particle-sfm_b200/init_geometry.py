@@ -10,13 +10,16 @@ Names and argument meaning follow the reference:
   (sfm/incremental_triangulator.cc:463-548), every track in one launch;
 * `estimate_relative_poses(...)` — TwoViewGeometry::EstimateRelativePose (estimators/two_view_geometry.cc:172-239)
   of every verified pair in one call, instead of the ThreadPool loop of DatabaseCache::Load
-  (base/database_cache.cc:206-228); its inputs are what `handoff.read_two_view_geometries` reads from a database.
+  (base/database_cache.cc:206-228); its inputs are what `handoff.read_two_view_geometries` reads from a database;
+* `estimate_global_rotations(...)` — EstimateGlobalRotations (global/robust_rotation_estimator.cc:310-331), the
+  first step of the global mapper: pair relative rotations in, one orientation per image out, which
+  `batch_optimize_relative_position_with_known_rotation` takes as its rotations.
 There is no CPU fallback: the library raises without a CUDA device."""
 import ctypes as C
 
 import numpy as np
 
-from . import _lib
+from . import _abi, _lib
 
 
 def _ptr(sizes):
@@ -110,3 +113,64 @@ def estimate_relative_poses(keypoint_ptr, keypoints, image_camera, cameras, pair
         out.estimated.ctypes.data_as(C.POINTER(C.c_uint8))), "psfm_two_view_relative_poses")
     out.estimated = out.estimated.astype(bool)
     return out
+
+
+class RobustRotationEstimatorOptions:
+    """RobustRotationEstimator::Options (global/robust_rotation_estimator.h:61-89) with the reference's names and
+    defaults, which are what sfm/main_sfm.py runs."""
+
+    def __init__(self, max_num_l1_iterations=5, l1_step_convergence_threshold=0.001, max_num_irls_iterations=100,
+                 irls_step_convergence_threshold=0.001, irls_loss_parameter_sigma=np.deg2rad(5.0),
+                 rotation_filter_max_degrees=5.0):
+        self.max_num_l1_iterations = max_num_l1_iterations
+        self.l1_step_convergence_threshold = l1_step_convergence_threshold
+        self.max_num_irls_iterations = max_num_irls_iterations
+        self.irls_step_convergence_threshold = irls_step_convergence_threshold
+        self.irls_loss_parameter_sigma = irls_loss_parameter_sigma
+        self.rotation_filter_max_degrees = rotation_filter_max_degrees
+
+    def to_struct(self):
+        return _abi.RotationOptions(*(getattr(self, n) for n, _ in _abi.RotationOptions._fields_))
+
+
+class GlobalRotations:
+    """orientations [F][4] (w, x, y, z world-to-camera; zero where has_orientation is False), has_orientation [F]
+    bool, pair_kept [R] bool, success (False where the reference returns false: no posed pair, or a failed
+    factorisation), summary (dict of psfm_rotation_summary; admm_iterations trimmed to num_l1_rounds)."""
+
+    def __init__(self, orientations, has_orientation, pair_kept, success, summary):
+        self.orientations, self.has_orientation, self.pair_kept = orientations, has_orientation, pair_kept
+        self.success, self.summary = success, summary
+
+
+def estimate_global_rotations(num_images, pair_images, qvec, num_correspondences, has_pose=None, options=None):
+    """pair_images [R][2] image indices (image 1, image 2; images ordered by id), qvec [R][4] relative rotations 2_R_1
+    (w, x, y, z), num_correspondences [R], has_pose [R] (None: every pair), options RobustRotationEstimatorOptions
+    (None: the defaults).  Returns GlobalRotations (psfm_estimate_global_rotations, csrc/rotation_averaging.cu).
+    From `RelativePoses`: has_pose = poses.estimated, num_correspondences = np.diff(inlier_ptr)."""
+    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
+    R = pairs.shape[0]
+    q = np.ascontiguousarray(qvec, np.float64).reshape(-1, 4)
+    nc = np.ascontiguousarray(num_correspondences, np.int32)
+    if q.shape[0] != R or nc.shape != (R,):
+        raise ValueError("pair_images, qvec and num_correspondences must describe the same pairs")
+    hp = None
+    if has_pose is not None:
+        hp = np.ascontiguousarray(has_pose, np.uint8)
+        if hp.shape != (R,):
+            raise ValueError("has_pose must have one entry per pair")
+    opts = (options or RobustRotationEstimatorOptions()).to_struct()
+    F = int(num_images)
+    orientations = np.zeros((F, 4))
+    has_orientation = np.zeros(F, np.uint8)
+    pair_kept = np.zeros(R, np.uint8)
+    s = _abi.RotationSummary()
+    u8 = C.POINTER(C.c_uint8)
+    i32 = C.POINTER(C.c_int32)
+    rc = _lib.check(_lib.lib().psfm_estimate_global_rotations(
+        F, R, pairs.ctypes.data_as(i32), _lib.dptr(q), nc.ctypes.data_as(i32),
+        hp.ctypes.data_as(u8) if hp is not None else None, C.byref(opts), _lib.dptr(orientations),
+        has_orientation.ctypes.data_as(u8), pair_kept.ctypes.data_as(u8), C.byref(s)), "psfm_estimate_global_rotations")
+    summary = {n: getattr(s, n) for n, _ in _abi.RotationSummary._fields_}
+    summary["admm_iterations"] = list(s.admm_iterations)[:s.num_l1_rounds]
+    return GlobalRotations(orientations, has_orientation.astype(bool), pair_kept.astype(bool), rc == 0, summary)

@@ -336,3 +336,66 @@ def two_view_inputs(rows, image_ids, qvec, tvec, camera):
                 pair_images=pair_images, config=np.full(R, 2, np.int32), E=E, F=eye, H=eye,
                 inlier_ptr=np.concatenate([[0], np.cumsum(counts)]).astype(np.int64),
                 inlier_matches=np.concatenate([m for _, m in rows.matches]) if R else np.zeros((0, 2), np.uint32))
+
+
+# ----------------------------------------------------------------------------- view graphs for rotation averaging
+
+def _quat_mul(a, b):
+    w1, x1, y1, z1 = np.moveaxis(a, -1, 0)
+    w2, x2, y2, z2 = np.moveaxis(b, -1, 0)
+    return np.stack([w1 * w2 - x1 * x2 - y1 * y2 - z1 * z2, w1 * x2 + x1 * w2 + y1 * z2 - z1 * y2,
+                     w1 * y2 - x1 * z2 + y1 * w2 + z1 * x2, w1 * z2 + x1 * y2 - y1 * x2 + z1 * w2], -1)
+
+
+def _axis_angle_quat(v):
+    th = np.linalg.norm(v, axis=-1, keepdims=True)
+    k = np.divide(v, th, out=np.zeros_like(v), where=th > 0)
+    return np.concatenate([np.cos(0.5 * th), k * np.sin(0.5 * th)], -1)
+
+
+def make_view_graph(num_images, graph="complete", band=10, noise_deg=0.0, outlier_fraction=0.0, seed=0,
+                    num_isolated=0, unposed_fraction=0.0, max_angle_deg=30.0):
+    """A seeded view graph for rotation averaging.  Ground truth: world-to-camera orientations within max_angle_deg of
+    the identity.  graph: "complete", "banded" (pairs up to `band` frames apart, a video) or "two_components" (images
+    split 2 : 1, the larger half first, each half complete).  The last num_isolated images get no pair.  Each pair's
+    2_R_1 = R2 R1^-1 is perturbed by a rotation of N(0, noise_deg) degrees about a random axis; an outlier_fraction of
+    the pairs get a uniformly random rotation instead; an unposed_fraction get has_pose = 0.  num_correspondences is
+    100 + 10 * (max(0, band - |a - b|) // 5): few distinct values, so many ties on purpose.
+    Returns dict(num_images, pair_images [R][2], qvec [R][4], num_correspondences [R], has_pose [R], truth [F][4],
+    outlier [R] bool)."""
+    rng = np.random.default_rng(seed)
+    F = num_images
+    axis = rng.normal(size=(F, 3))
+    axis /= np.linalg.norm(axis, axis=1, keepdims=True)
+    truth = _axis_angle_quat(axis * np.deg2rad(max_angle_deg) * rng.random((F, 1)))
+    active = F - num_isolated
+    if graph == "complete":
+        groups = [range(active)]
+    elif graph == "banded":
+        groups = None
+    elif graph == "two_components":
+        cut = (2 * active) // 3
+        groups = [range(cut), range(cut, active)]
+    else:
+        raise ValueError("graph must be complete, banded or two_components")
+    if groups is None:
+        pairs = [(a, b) for a in range(active) for b in range(a + 1, min(active, a + band + 1))]
+    else:
+        pairs = [(a, b) for g in groups for a in g for b in g if a < b]
+    pairs = np.array(pairs, np.int32).reshape(-1, 2)
+    R = pairs.shape[0]
+    inv1 = truth[pairs[:, 0]] * np.array([1.0, -1.0, -1.0, -1.0])
+    rel = _quat_mul(truth[pairs[:, 1]], inv1)
+    if noise_deg > 0:
+        ax = rng.normal(size=(R, 3))
+        ax /= np.linalg.norm(ax, axis=1, keepdims=True)
+        rel = _quat_mul(_axis_angle_quat(ax * np.deg2rad(noise_deg) * rng.normal(size=(R, 1))), rel)
+    outlier = rng.random(R) < outlier_fraction
+    if outlier.any():
+        q = rng.normal(size=(int(outlier.sum()), 4))
+        rel[outlier] = q / np.linalg.norm(q, axis=1, keepdims=True)
+    gap = np.abs(pairs[:, 1] - pairs[:, 0])
+    num_corr = (100 + 10 * (np.maximum(0, band - gap) // 5)).astype(np.int32)
+    has_pose = (rng.random(R) >= unposed_fraction).astype(np.uint8)
+    return dict(num_images=F, pair_images=pairs, qvec=rel, num_correspondences=num_corr, has_pose=has_pose,
+                truth=truth, outlier=outlier)
