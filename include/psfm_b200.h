@@ -309,6 +309,76 @@ int psfm_estimate_global_rotations(int32_t num_images, int64_t num_pairs, const 
                                    const psfm_rotation_options* opts, double* orientations, uint8_t* has_orientation,
                                    uint8_t* pair_kept, psfm_rotation_summary* summary);
 
+/* GlobalMapper::OptimizePairwiseTranslations (sfm/global_mapper.cc:106-109 -> BatchOptimizeRelativePositionWithKnownRotation,
+   global/known_rotation_util.cc:195-229): every used pair's translation direction re-estimated from all of its inlier
+   matches under the image orientations, with psfm_known_rotation_translations' kernel (csrc/init_geometry.cu), the
+   keypoints gathered and normalised (SIMPLE_PINHOLE ImageToWorld) on the device.  Images and pairs as
+   psfm_two_view_relative_poses takes them; orientations [num_images][4] (w, x, y, z world-to-camera, normally
+   psfm_estimate_global_rotations' output), pair_used [num_pairs] (NULL: every pair; normally its pair_kept).
+   Out: tvec [num_pairs][3] unit relative positions, iterations [num_pairs] IRLS iterations; an unused pair gets zeros.
+   The result is bit-identical to psfm_known_rotation_translations on points normalised as (x - cx) / f in double.
+   PSFM_ERR_INVALID before anything runs for an image, camera or keypoint index out of range, or a used pair whose
+   image has a zero or non-finite orientation. */
+int psfm_optimize_pairwise_translations(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
+                                        const int32_t* image_camera, const double* cameras, int32_t num_cameras,
+                                        int64_t num_pairs, const int32_t* pair_images, const int64_t* inlier_ptr,
+                                        const uint32_t* inlier_matches, const double* orientations,
+                                        const uint8_t* pair_used, double* tvec, int32_t* iterations);
+
+/* theia::ConstrainedL1Solver::Options, which LeastUnsquaredDeviationPositionEstimator constructs with its defaults
+   (global/least_unsquared_deviation_position_estimator.cc:161); NULL gives these defaults.  They are recalled, not
+   vendored (csrc/position_recalled.cuh).  Check(): max_num_iterations > 0, rho > 0, 0 < alpha < 2, both tolerances
+   > 0, all finite.  The reference LUD options max_num_iterations, max_num_reweighted_iterations and
+   convergence_criterion never reach the solver there, so they are not mirrored. */
+typedef struct {
+  int32_t max_num_iterations;   /* 1000 */
+  double rho;                   /* 10.0 */
+  double alpha;                 /* 1.2 (over-relaxation) */
+  double absolute_tolerance;    /* 1e-4 */
+  double relative_tolerance;    /* 1e-2 */
+} psfm_lud_options;
+
+typedef struct {
+  int32_t gauge_image;               /* image index fixed at the origin */
+  int32_t num_views;                 /* images of the used pairs */
+  int32_t num_pairs_used;
+  int32_t admm_iterations;           /* ConstrainedL1Solver iterations run */
+  int32_t admm_iterations_queued;    /* iterations launched (in chunks of 32 behind the done flag) */
+  int32_t converged;                 /* 1: the stopping test passed; 0: max_num_iterations ran out */
+  double primal_residual, primal_tolerance;   /* |A~x - z - b~| and its bound, last iteration */
+  double dual_residual, dual_tolerance;       /* |rho A~'(z - z_old)| and its bound, last iteration */
+  int64_t num_launches;              /* kernels this call launched: 4 + 4 * admm_iterations_queued */
+  double host_ms;                    /* validation and graph work on the host */
+  double build_ms, factor_ms, inverse_ms;     /* building S, factoring it, inverting it (CUDA events) */
+  double admm_ms;                    /* the ADMM loop with its control reads (wall, synchronised) */
+} psfm_position_summary;
+
+void psfm_lud_default_options(psfm_lud_options* opts);
+
+/* GlobalMapper::EstimatePositions (sfm/global_mapper.cc:111-132) with the default method "lud"
+   (LeastUnsquaredDeviationPositionEstimator, use_scale_constraints = false, no 1DSfM filter), then the positions'
+   part of RegisterAllImages (:140-160), in one call (csrc/position_estimation.cu).  Pairs: pair_images
+   [num_pairs][2] (image 1, image 2), pair_tvec [num_pairs][3] the relative translation (psfm_optimize_pairwise_translations),
+   pair_used [num_pairs] (NULL: every pair).  Images: orientations [num_images][4] (w, x, y, z world-to-camera),
+   has_orientation [num_images] (NULL: all 1).  Solves min sum_k |c1 - c2 - s_k R2' t_k|_1 subject to s_k >= 1 by
+   ADMM (theia::ConstrainedL1Solver), with the positions' normal equations reduced to a 3 x 3-block graph Laplacian
+   that is factored and inverted once.
+   Out: positions [num_images][3] (camera centres), has_position [num_images] (the images of the used pairs), image_tvec
+   [num_images][3] = -QuaternionRotatePoint(q, c) (zero without a position), scales [num_pairs] (0 for unused pairs), summary
+   (nullable).  Defined here where the reference follows hash order: the gauge is the smallest image index among the
+   views, fixed at the origin (any other choice moves every position by one common vector).
+   PSFM_ERR_INVALID before anything runs for: no used pair; an image index out of range, a pair of an image with
+   itself, an unordered pair listed twice; a used pair touching an image without an orientation; a non-finite
+   orientation or pair tvec; used pairs that do not form one connected graph (S singular); options that fail Check().
+   PSFM_ERR_UNSUPPORTED before anything runs for 3 (V - 1) > 8190 (more than 2731 views: the dense factor's bound).
+   PSFM_ERR_NO_DEVICE without a device (there is no CPU path); PSFM_ERR_INVALID after the launches when S is not
+   numerically positive definite. */
+int psfm_estimate_global_positions(int32_t num_images, int64_t num_pairs, const int32_t* pair_images,
+                                   const double* pair_tvec, const double* orientations, const uint8_t* has_orientation,
+                                   const uint8_t* pair_used, const psfm_lud_options* opts, double* positions,
+                                   uint8_t* has_position, double* image_tvec, double* scales,
+                                   psfm_position_summary* summary);
+
 /* ------------------------------------------------------------------------- */
 /* HP2 — global bundle adjustment                                             */
 /* ------------------------------------------------------------------------- */

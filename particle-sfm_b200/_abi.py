@@ -285,3 +285,35 @@ class RotationSummary(C.Structure):
         ("host_ms", C.c_double),
         ("device_ms", C.c_double),
     ]
+
+
+class LudOptions(C.Structure):
+    """psfm_lud_options: theia::ConstrainedL1Solver::Options."""
+    _fields_ = [
+        ("max_num_iterations", C.c_int32),
+        ("rho", C.c_double),
+        ("alpha", C.c_double),
+        ("absolute_tolerance", C.c_double),
+        ("relative_tolerance", C.c_double),
+    ]
+
+
+class PositionSummary(C.Structure):
+    _fields_ = [
+        ("gauge_image", C.c_int32),
+        ("num_views", C.c_int32),
+        ("num_pairs_used", C.c_int32),
+        ("admm_iterations", C.c_int32),
+        ("admm_iterations_queued", C.c_int32),
+        ("converged", C.c_int32),
+        ("primal_residual", C.c_double),
+        ("primal_tolerance", C.c_double),
+        ("dual_residual", C.c_double),
+        ("dual_tolerance", C.c_double),
+        ("num_launches", C.c_int64),
+        ("host_ms", C.c_double),
+        ("build_ms", C.c_double),
+        ("factor_ms", C.c_double),
+        ("inverse_ms", C.c_double),
+        ("admm_ms", C.c_double),
+    ]

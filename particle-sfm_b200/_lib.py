@@ -24,7 +24,8 @@ EXPORTS = [
     "psfm_tracker_create", "psfm_tracker_advance", "psfm_tracker_optimize", "psfm_tracker_get_buffer", "psfm_tracker_set_buffer",
     "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy",
     "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy", "psfm_known_rotation_translations", "psfm_triangulate_tracks",
-    "psfm_two_view_relative_poses", "psfm_rotation_default_options", "psfm_estimate_global_rotations", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
+    "psfm_two_view_relative_poses", "psfm_rotation_default_options", "psfm_estimate_global_rotations",
+    "psfm_optimize_pairwise_translations", "psfm_lud_default_options", "psfm_estimate_global_positions", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
 
@@ -81,6 +82,13 @@ def lib():
     L.psfm_estimate_global_rotations.argtypes = [C.c_int32, C.c_int64, ip, dp, ip, C.POINTER(C.c_uint8),
                                                  C.POINTER(_abi.RotationOptions), dp, C.POINTER(C.c_uint8),
                                                  C.POINTER(C.c_uint8), C.POINTER(_abi.RotationSummary)]
+    L.psfm_optimize_pairwise_translations.argtypes = [C.c_int32, i64p, fp, ip, dp, C.c_int32, C.c_int64, ip, i64p,
+                                                      C.POINTER(C.c_uint32), dp, C.POINTER(C.c_uint8), dp, ip]
+    L.psfm_lud_default_options.argtypes = [C.POINTER(_abi.LudOptions)]
+    L.psfm_lud_default_options.restype = None
+    L.psfm_estimate_global_positions.argtypes = [C.c_int32, C.c_int64, ip, dp, dp, C.POINTER(C.c_uint8),
+                                                 C.POINTER(C.c_uint8), C.POINTER(_abi.LudOptions), dp,
+                                                 C.POINTER(C.c_uint8), dp, dp, C.POINTER(_abi.PositionSummary)]
     vp = C.c_void_p
     L.psfm_tracker_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.POINTER(vp)]
     L.psfm_tracker_advance.argtypes = [vp] * 6 + [ip]

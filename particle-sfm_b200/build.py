@@ -32,6 +32,7 @@ UNITS = [
     ("init_geometry.cu", []),
     ("two_view.cu", []),
     ("rotation_averaging.cu", []),
+    ("position_estimation.cu", []),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

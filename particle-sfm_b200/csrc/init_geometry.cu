@@ -6,6 +6,9 @@
 //       C diag(1/w) C' with w_i = max(|t' c_i|, 1e-7) — <= 100 iterations, stop after 10 consecutive iterations
 //       whose cost change is <= 1e-5 (:116-176), sign by the cheirality majority (:85-101, :181-189; COLMAP
 //       CheckCheirality / TriangulatePoint / CalculateDepth).  The reference runs one ThreadPool task per pair.
+//       Two callers of one kernel, templated on its point loader: psfm_known_rotation_translations (normalised
+//       points from the caller) and psfm_optimize_pairwise_translations (GlobalMapper::OptimizePairwiseTranslations,
+//       sfm/global_mapper.cc:106-109: the database arrays, keypoints gathered and normalised on the device).
 //   multi-view DLT of a track   COLMAP TriangulateMultiViewPoint, the estimator behind
 //       IncrementalTriangulator::Create (sfm/incremental_triangulator.cc:463-548): smallest eigenvector of
 //       sum (P - x x' P)' (P - x x' P).
@@ -13,6 +16,7 @@
 // solves the 3 x 3 eigenproblem redundantly — no broadcast), one thread per track.  Eigenvectors by cyclic Jacobi
 // rotations in fp64 (the reference uses Eigen's JacobiSVD / SelfAdjointEigenSolver: same vector up to sign and
 // rounding; parity tolerance in tests/test_gpu_init.py).
+#include <cmath>
 #include <vector>
 
 #include "psfm_common.cuh"
@@ -116,12 +120,56 @@ __device__ __forceinline__ void constraint(const double* R1, const double* R2, d
   c[2] = R2[6] * k0 + R2[7] * k1 + R2[8] * k2;
 }
 
-__global__ void __launch_bounds__(128) k_known_rotation(const double2* __restrict__ p1, const double2* __restrict__ p2,
-                                                        const int* __restrict__ pair_ptr, const double* __restrict__ q1,
+// Point loaders of k_known_rotation: pair p's correspondence range and its normalised points.
+// PointArrays: normalised points given by the caller (psfm_known_rotation_translations).
+struct PointArrays {
+  const double2* __restrict__ p1;
+  const double2* __restrict__ p2;
+  const int* __restrict__ ptr;
+  __device__ __forceinline__ void range(int p, long long& e0, long long& e1) const { e0 = ptr[p]; e1 = ptr[p + 1]; }
+  __device__ __forceinline__ void load(int, long long i, double& x1, double& y1, double& x2, double& y2) const {
+    const double2 a = p1[i], b = p2[i];
+    x1 = a.x; y1 = a.y; x2 = b.x; y2 = b.y;
+  }
+};
+
+// MatchGather: the database arrays of psfm_two_view_relative_poses; both keypoints gathered through the match's
+// indices and normalised (SIMPLE_PINHOLE ImageToWorld) with two_view.cu's expression.  An unused pair has an empty
+// range.
+struct MatchGather {
+  const long long* __restrict__ iptr;
+  const uint2* __restrict__ matches;
+  const int* __restrict__ pair_images;
+  const long long* __restrict__ kp_ptr;
+  const float2* __restrict__ kps;
+  const int* __restrict__ image_camera;
+  const double* __restrict__ cameras;
+  const unsigned char* __restrict__ used;     // may be null: every pair
+  __device__ __forceinline__ void range(int p, long long& e0, long long& e1) const {
+    e0 = iptr[p];
+    e1 = (used && !used[p]) ? e0 : iptr[p + 1];
+  }
+  __device__ __forceinline__ void load(int p, long long i, double& x1, double& y1, double& x2, double& y2) const {
+    const uint2 m = matches[i];
+    const int a = pair_images[2 * p], b = pair_images[2 * p + 1];
+    const float2 pa = kps[kp_ptr[a] + m.x], pb = kps[kp_ptr[b] + m.y];
+    const double* ka = cameras + 3 * image_camera[a];
+    const double* kb = cameras + 3 * image_camera[b];
+    x1 = ((double)pa.x - ka[1]) / ka[0];
+    y1 = ((double)pa.y - ka[2]) / ka[0];
+    x2 = ((double)pb.x - kb[1]) / kb[0];
+    y2 = ((double)pb.y - kb[2]) / kb[0];
+  }
+};
+
+template <class Points>
+__global__ void __launch_bounds__(128) k_known_rotation(const Points pts, const double* __restrict__ q1,
                                                         const double* __restrict__ q2, double* __restrict__ tvec, int* __restrict__ iters) {
   __shared__ double sbuf[7 * 32];
   const int pair = blockIdx.x, tid = threadIdx.x;
-  const int e0 = pair_ptr[pair], e1 = pair_ptr[pair + 1], n = e1 - e0;
+  long long e0, e1;
+  pts.range(pair, e0, e1);
+  const long long n = e1 - e0;
   double R1[9], R2[9];
   quat_to_rot(q1 + 4 * (size_t)pair, R1);
   quat_to_rot(q2 + 4 * (size_t)pair, R2);
@@ -139,10 +187,11 @@ __global__ void __launch_bounds__(128) k_known_rotation(const double2* __restric
   double newpos[3] = {0.0, 0.0, 0.0};
   for (int it = 0; it <= 100; ++it) {
     double acc[7] = {0, 0, 0, 0, 0, 0, 0};
-    for (int i = e0 + tid; i < e1; i += 128) {
-      const double2 a = p1[i], b = p2[i];
+    for (long long i = e0 + tid; i < e1; i += 128) {
+      double ax, ay, bx, by;
+      pts.load(pair, i, ax, ay, bx, by);
       double c[3];
-      constraint(R1, R2, a.x, a.y, b.x, b.y, c);
+      constraint(R1, R2, ax, ay, bx, by, c);
       double w = first ? 1.0 : fabs(newpos[0] * c[0] + newpos[1] * c[1] + newpos[2] * c[2]);
       acc[6] += w;                                  // cost of newpos (unclamped)
       w = w < 1e-7 ? 1e-7 : w;
@@ -177,13 +226,14 @@ __global__ void __launch_bounds__(128) k_known_rotation(const double2* __restric
   const double max_depth = 1000.0 * sqrt(rt0 * rt0 + rt1 * rt1 + rt2 * rt2);
   const double eps = 2.220446049250313e-16;
   double cnt[1] = {0.0};
-  for (int i = e0 + tid; i < e1; i += 128) {
-    const double2 a = p1[i], b = p2[i];
+  for (long long i = e0 + tid; i < e1; i += 128) {
+    double ax, ay, bx, by;
+    pts.load(pair, i, ax, ay, bx, by);
     // DLT rows: x1 P1[2] - P1[0], y1 P1[2] - P1[1], x2 P2[2] - P2[0], y2 P2[2] - P2[1]
-    double Am[4][4] = {{-1.0, 0.0, a.x, 0.0},
-                       {0.0, -1.0, a.y, 0.0},
-                       {b.x * R[6] - R[0], b.x * R[7] - R[1], b.x * R[8] - R[2], b.x * pos[2] - pos[0]},
-                       {b.y * R[6] - R[3], b.y * R[7] - R[4], b.y * R[8] - R[5], b.y * pos[2] - pos[1]}};
+    double Am[4][4] = {{-1.0, 0.0, ax, 0.0},
+                       {0.0, -1.0, ay, 0.0},
+                       {bx * R[6] - R[0], bx * R[7] - R[1], bx * R[8] - R[2], bx * pos[2] - pos[0]},
+                       {by * R[6] - R[3], by * R[7] - R[4], by * R[8] - R[5], by * pos[2] - pos[1]}};
     double G[4][4];
 #pragma unroll
     for (int r = 0; r < 4; ++r)
@@ -268,8 +318,8 @@ extern "C" int psfm_known_rotation_translations(const double* points1, const dou
     dt.alloc(3 * (size_t)num_pairs); dp.alloc((size_t)num_pairs + 1); di.alloc((size_t)num_pairs);
     d1.upload(points1, 2 * m, nullptr); d2.upload(points2, 2 * m, nullptr);
     dq1.upload(qvec1, dq1.n, nullptr); dq2.upload(qvec2, dq2.n, nullptr); dp.upload(pair_ptr, dp.n, nullptr);
-    k_known_rotation<<<num_pairs, 128>>>(reinterpret_cast<const double2*>(d1.p), reinterpret_cast<const double2*>(d2.p), dp.p, dq1.p,
-                                         dq2.p, dt.p, di.p);
+    const PointArrays pts{reinterpret_cast<const double2*>(d1.p), reinterpret_cast<const double2*>(d2.p), dp.p};
+    k_known_rotation<<<num_pairs, 128>>>(pts, dq1.p, dq2.p, dt.p, di.p);
     PSFM_LAUNCH_CHECK();
     PSFM_CUDA(cudaMemcpy(tvec, dt.p, sizeof(double) * dt.n, cudaMemcpyDeviceToHost));
     if (iterations) PSFM_CUDA(cudaMemcpy(iterations, di.p, sizeof(int) * di.n, cudaMemcpyDeviceToHost));
@@ -295,6 +345,88 @@ extern "C" int psfm_triangulate_tracks(const double* proj_matrices, const double
     k_triangulate_tracks<<<(num_tracks + 127) / 128, 128>>>(dP.p, reinterpret_cast<const double2*>(dx.p), dp.p, num_tracks, dX.p);
     PSFM_LAUNCH_CHECK();
     PSFM_CUDA(cudaMemcpy(xyz, dX.p, sizeof(double) * dX.n, cudaMemcpyDeviceToHost));
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return f.code; }
+}
+
+namespace {
+int pairwise_fail(const std::string& msg) {
+  set_error("psfm_optimize_pairwise_translations: " + msg);
+  return PSFM_ERR_INVALID;
+}
+}  // namespace
+
+extern "C" int psfm_optimize_pairwise_translations(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
+                                                   const int32_t* image_camera, const double* cameras, int32_t num_cameras,
+                                                   int64_t num_pairs, const int32_t* pair_images, const int64_t* inlier_ptr,
+                                                   const uint32_t* inlier_matches, const double* orientations,
+                                                   const uint8_t* pair_used, double* tvec, int32_t* iterations) {
+  if (num_images < 0 || num_cameras < 0 || num_pairs < 0) return pairwise_fail("negative size");
+  if (num_pairs > 0x7fffffffLL) return pairwise_fail("more than 2^31 - 1 pairs");
+  if (num_pairs > 0 && (!keypoint_ptr || !image_camera || !cameras || !pair_images || !inlier_ptr || !orientations ||
+                        !tvec || !iterations))
+    return pairwise_fail("null argument");
+  const int R = (int)num_pairs;
+  if (R > 0) {
+    if (keypoint_ptr[0] != 0) return pairwise_fail("keypoint_ptr[0] must be 0");
+    for (int32_t f = 0; f < num_images; ++f)
+      if (keypoint_ptr[f + 1] < keypoint_ptr[f]) return pairwise_fail("keypoint_ptr must be non-decreasing");
+    for (int32_t f = 0; f < num_images; ++f)
+      if (image_camera[f] < 0 || image_camera[f] >= num_cameras) return pairwise_fail("a camera index is outside [0, num_cameras)");
+    if (inlier_ptr[0] != 0) return pairwise_fail("inlier_ptr[0] must be 0");
+    for (int p = 0; p < R; ++p) {
+      if (inlier_ptr[p + 1] < inlier_ptr[p]) return pairwise_fail("inlier_ptr must be non-decreasing");
+      for (int k = 0; k < 2; ++k)
+        if (pair_images[2 * p + k] < 0 || pair_images[2 * p + k] >= num_images)
+          return pairwise_fail("an image index is outside [0, num_images)");
+    }
+    for (int p = 0; p < R; ++p) {
+      if (pair_used && !pair_used[p]) continue;
+      for (int k = 0; k < 2; ++k) {
+        const double* q = orientations + 4 * (size_t)pair_images[2 * p + k];
+        const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+        if (!(std::isfinite(n2) && n2 > 0.0)) return pairwise_fail("a used pair's image has a zero or non-finite orientation");
+      }
+    }
+    if (inlier_ptr[R] > 0 && (!inlier_matches || (keypoint_ptr[num_images] > 0 && !keypoints)))
+      return pairwise_fail("null argument");
+    if (!keypoints_in_range(R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches))
+      return pairwise_fail("a keypoint index is outside its image's keypoints");
+  }
+  int rc = init_device_ok();
+  if (rc != PSFM_OK) return rc;
+  if (R == 0) return PSFM_OK;
+  const long long N = inlier_ptr[R], K = keypoint_ptr[num_images];
+  // the kernel reads one quaternion pair per pair: gathered here from the image orientations
+  std::vector<double> q1(4 * (size_t)R), q2(4 * (size_t)R);
+  for (int p = 0; p < R; ++p)
+    for (int k = 0; k < 4; ++k) {
+      q1[4 * (size_t)p + k] = orientations[4 * (size_t)pair_images[2 * p] + k];
+      q2[4 * (size_t)p + k] = orientations[4 * (size_t)pair_images[2 * p + 1] + k];
+    }
+  try {
+    DBuf<double> d_q1, d_q2, d_t, d_cams;
+    DBuf<int> d_it, d_pairs, d_cam;
+    DBuf<long long> d_iptr, d_kp_ptr;
+    DBuf<uint2> d_m;
+    DBuf<float2> d_kps;
+    DBuf<unsigned char> d_used;
+    d_q1.alloc(4 * (size_t)R); d_q2.alloc(4 * (size_t)R); d_t.alloc(3 * (size_t)R); d_it.alloc(R);
+    d_pairs.alloc(2 * (size_t)R); d_cam.alloc(num_images); d_cams.alloc(3 * (size_t)num_cameras);
+    d_iptr.alloc((size_t)R + 1); d_kp_ptr.alloc((size_t)num_images + 1); d_m.alloc(N); d_kps.alloc(K);
+    d_q1.upload(q1.data(), q1.size(), nullptr); d_q2.upload(q2.data(), q2.size(), nullptr);
+    d_pairs.upload(pair_images, 2 * (size_t)R, nullptr); d_cam.upload(image_camera, num_images, nullptr);
+    d_cams.upload(cameras, 3 * (size_t)num_cameras, nullptr);
+    d_iptr.upload(reinterpret_cast<const long long*>(inlier_ptr), (size_t)R + 1, nullptr);
+    d_kp_ptr.upload(reinterpret_cast<const long long*>(keypoint_ptr), (size_t)num_images + 1, nullptr);
+    d_m.upload(reinterpret_cast<const uint2*>(inlier_matches), N, nullptr);
+    d_kps.upload(reinterpret_cast<const float2*>(keypoints), K, nullptr);
+    if (pair_used) { d_used.alloc(R); d_used.upload(pair_used, R, nullptr); }
+    const MatchGather pts{d_iptr.p, d_m.p, d_pairs.p, d_kp_ptr.p, d_kps.p, d_cam.p, d_cams.p, pair_used ? d_used.p : nullptr};
+    k_known_rotation<<<R, 128>>>(pts, d_q1.p, d_q2.p, d_t.p, d_it.p);
+    PSFM_LAUNCH_CHECK();
+    PSFM_CUDA(cudaMemcpy(tvec, d_t.p, sizeof(double) * 3 * (size_t)R, cudaMemcpyDeviceToHost));
+    PSFM_CUDA(cudaMemcpy(iterations, d_it.p, sizeof(int) * (size_t)R, cudaMemcpyDeviceToHost));
     return PSFM_OK;
   } catch (const CudaFail& f) { return f.code; }
 }

@@ -14,6 +14,9 @@
 namespace psfm {
 
 void set_error(const std::string& msg);
+// every inlier match's keypoint indices inside its images' keypoint ranges (two_view.cu; host, multi-threaded)
+bool keypoints_in_range(int64_t num_pairs, const int32_t* pair_images, const int64_t* keypoint_ptr,
+                        const int64_t* inlier_ptr, const uint32_t* inlier_matches);
 extern std::atomic<long long> g_launch_count;
 
 struct CudaFail {

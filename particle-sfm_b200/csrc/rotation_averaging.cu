@@ -30,12 +30,14 @@
 
 #include "dense_chol.cuh"
 #include "psfm_common.cuh"
+#include "quat.cuh"
 #include "rotation_recalled.cuh"
 
 namespace {
 
 using namespace psfm;
 using namespace psfm::rot;
+using namespace psfm::quat;
 
 constexpr int kMaxComponentImages = 8192;   // dense factor + its panels: 2 x 8191^2 doubles, about 1.1 GB
 constexpr int kIrlsChunk = 8;               // IRLS iterations queued between two reads of the done flag
@@ -45,44 +47,6 @@ struct Ctl {
   int admm_done, admm_count, irls_done, irls_count, failed;
   double avg_step;
 };
-
-// ---- COLMAP / Ceres quaternion helpers (w, x, y, z) --------------------------------------------------------------
-struct Quat {
-  double w, x, y, z;
-};
-
-__host__ __device__ inline Quat qmul(const Quat& a, const Quat& b) {     // a (x) b, Eigen's Hamilton product
-  return {a.w * b.w - a.x * b.x - a.y * b.y - a.z * b.z, a.w * b.x + a.x * b.w + a.y * b.z - a.z * b.y,
-          a.w * b.y - a.x * b.z + a.y * b.w + a.z * b.x, a.w * b.z + a.x * b.y - a.y * b.x + a.z * b.w};
-}
-__host__ __device__ inline Quat qnormalize(const Quat& q) {               // NormalizeQuaternion
-  const double n = sqrt(q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z);
-  if (n == 0.0) return {1.0, 0.0, 0.0, 0.0};
-  return {q.w / n, q.x / n, q.y / n, q.z / n};
-}
-__host__ __device__ inline Quat qconcat(const Quat& q1, const Quat& q2) {   // ConcatenateQuaternions: q2 (x) q1
-  return qnormalize(qmul(qnormalize(q2), qnormalize(q1)));
-}
-__host__ __device__ inline Quat qinv(const Quat& q) { return {q.w, -q.x, -q.y, -q.z}; }   // InvertQuaternion
-__host__ __device__ inline Quat aa_to_quat(double a0, double a1, double a2) {          // ceres::AngleAxisToQuaternion
-  const double t2 = a0 * a0 + a1 * a1 + a2 * a2;
-  if (t2 > 0.0) {
-    const double t = sqrt(t2), h = 0.5 * t, k = sin(h) / t;
-    return {cos(h), a0 * k, a1 * k, a2 * k};
-  }
-  return {1.0, 0.5 * a0, 0.5 * a1, 0.5 * a2};
-}
-__host__ __device__ inline void quat_to_aa(const Quat& q, double* a) {                 // ceres::QuaternionToAngleAxis
-  const double s2 = q.x * q.x + q.y * q.y + q.z * q.z;
-  double k = 2.0;
-  if (s2 > 0.0) {
-    const double s = sqrt(s2), c = q.w;
-    const double two_theta = 2.0 * (c < 0.0 ? atan2(-s, -c) : atan2(s, c));
-    k = two_theta / s;
-  }
-  a[0] = q.x * k; a[1] = q.y * k; a[2] = q.z * k;
-}
-__device__ inline Quat load_q(const double* q) { return {q[0], q[1], q[2], q[3]}; }
 
 // QuaternionToRotationMatrix (normalised, Eigen's toRotationMatrix) and RotationMatrixToQuaternion (Eigen's
 // Quaterniond(Matrix3d)): the chaining along the spanning tree (ComputeOrientation) works on matrices

@@ -531,8 +531,10 @@ void sort_pairs(cub::DoubleBuffer<K>& keys, cub::DoubleBuffer<V>& vals, long lon
   PSFM_LAUNCH_CHECK();
 }
 
+}  // namespace
+
 // every match's keypoint indices inside its images' keypoint ranges (host, split over threads: up to 10^9 indices)
-bool keypoints_in_range(int64_t R, const int32_t* pair_images, const int64_t* kp_ptr, const int64_t* iptr, const uint32_t* m) {
+bool psfm::keypoints_in_range(int64_t R, const int32_t* pair_images, const int64_t* kp_ptr, const int64_t* iptr, const uint32_t* m) {
   const unsigned nt = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
   std::vector<char> ok(nt, 1);
   std::vector<std::thread> th;
@@ -561,8 +563,6 @@ bool keypoints_in_range(int64_t R, const int32_t* pair_images, const int64_t* kp
   for (auto& t : th) t.join();
   return std::all_of(ok.begin(), ok.end(), [](char c) { return c != 0; });
 }
-
-}  // namespace
 
 extern "C" int psfm_two_view_relative_poses(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
                                             const int32_t* image_camera, const double* cameras, int32_t num_cameras,

@@ -13,7 +13,11 @@ Names and argument meaning follow the reference:
   (base/database_cache.cc:206-228); its inputs are what `handoff.read_two_view_geometries` reads from a database;
 * `estimate_global_rotations(...)` — EstimateGlobalRotations (global/robust_rotation_estimator.cc:310-331), the
   first step of the global mapper: pair relative rotations in, one orientation per image out, which
-  `batch_optimize_relative_position_with_known_rotation` takes as its rotations.
+  `batch_optimize_relative_position_with_known_rotation` takes as its rotations;
+* `optimize_pairwise_translations(...)` — GlobalMapper::OptimizePairwiseTranslations (sfm/global_mapper.cc:106-109):
+  the known-rotation translations of every kept pair, straight from the database arrays;
+* `estimate_global_positions(...)` — GlobalMapper::EstimatePositions (sfm/global_mapper.cc:111-132) with the default
+  method "lud" and the pose update of RegisterAllImages: camera centres and image tvecs.
 There is no CPU fallback: the library raises without a CUDA device."""
 import ctypes as C
 
@@ -174,3 +178,110 @@ def estimate_global_rotations(num_images, pair_images, qvec, num_correspondences
     summary = {n: getattr(s, n) for n, _ in _abi.RotationSummary._fields_}
     summary["admm_iterations"] = list(s.admm_iterations)[:s.num_l1_rounds]
     return GlobalRotations(orientations, has_orientation.astype(bool), pair_kept.astype(bool), rc == 0, summary)
+
+
+def optimize_pairwise_translations(keypoint_ptr, keypoints, image_camera, cameras, pair_images, inlier_ptr, inlier_matches,
+                                   orientations, pair_used=None, return_iterations=False):
+    """GlobalMapper::OptimizePairwiseTranslations (sfm/global_mapper.cc:106-109): every used pair's translation
+    direction re-estimated from all of its inlier matches under the image orientations (OptimizeRelativePositionWith
+    KnownRotation per pair, known_rotation_util.cc:195-229).  Images and pairs as `estimate_relative_poses` takes them
+    (keypoints normalised on the device with the SIMPLE_PINHOLE camera, (x - cx) / f); orientations [F][4] (w, x, y, z
+    world-to-camera, `GlobalRotations.orientations`), pair_used [R] (None: every pair; normally
+    `GlobalRotations.pair_kept`).  Returns tvec [R][3] (zeros for unused pairs), and the IRLS iterations [R] with
+    return_iterations (psfm_optimize_pairwise_translations, csrc/init_geometry.cu)."""
+    kp_ptr = np.ascontiguousarray(keypoint_ptr, np.int64)
+    kps = np.ascontiguousarray(keypoints, np.float32).reshape(-1, 2)
+    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    cams = np.ascontiguousarray(cameras, np.float64).reshape(-1, 3)
+    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
+    R = pairs.shape[0]
+    iptr = np.ascontiguousarray(inlier_ptr, np.int64)
+    m = np.ascontiguousarray(inlier_matches, np.uint32).reshape(-1, 2)
+    q = np.ascontiguousarray(orientations, np.float64).reshape(-1, 4)
+    num_images = kp_ptr.shape[0] - 1
+    if iptr.shape[0] != R + 1 or cam_of.shape[0] != num_images or q.shape[0] != num_images:
+        raise ValueError("pair_images and inlier_ptr must describe the same pairs, image_camera and orientations the same images")
+    if iptr[-1] != m.shape[0] or kp_ptr[-1] != kps.shape[0]:
+        raise ValueError("inlier_ptr / keypoint_ptr must end at the number of matches / keypoints")
+    used = None
+    if pair_used is not None:
+        used = np.ascontiguousarray(pair_used, np.uint8)
+        if used.shape != (R,):
+            raise ValueError("pair_used must have one entry per pair")
+    tvec, its = np.zeros((R, 3)), np.zeros(R, np.int32)
+    i32, i64 = C.POINTER(C.c_int32), C.POINTER(C.c_int64)
+    _lib.check(_lib.lib().psfm_optimize_pairwise_translations(
+        num_images, kp_ptr.ctypes.data_as(i64), kps.ctypes.data_as(C.POINTER(C.c_float)), cam_of.ctypes.data_as(i32),
+        _lib.dptr(cams), cams.shape[0], R, pairs.ctypes.data_as(i32), iptr.ctypes.data_as(i64),
+        m.ctypes.data_as(C.POINTER(C.c_uint32)), _lib.dptr(q), used.ctypes.data_as(C.POINTER(C.c_uint8)) if used is not None else None,
+        _lib.dptr(tvec), its.ctypes.data_as(i32)), "psfm_optimize_pairwise_translations")
+    return (tvec, its) if return_iterations else tvec
+
+
+class ConstrainedL1SolverOptions:
+    """theia::ConstrainedL1Solver::Options, which the reference's LUD estimator constructs with its defaults
+    (least_unsquared_deviation_position_estimator.cc:161).  A field left None takes the library's default
+    (psfm_lud_default_options; the defaults are recalled, not vendored: csrc/position_recalled.cuh)."""
+
+    def __init__(self, max_num_iterations=None, rho=None, alpha=None, absolute_tolerance=None, relative_tolerance=None):
+        self.max_num_iterations = max_num_iterations
+        self.rho = rho
+        self.alpha = alpha
+        self.absolute_tolerance = absolute_tolerance
+        self.relative_tolerance = relative_tolerance
+
+    def to_struct(self):
+        o = _abi.LudOptions()
+        _lib.lib().psfm_lud_default_options(C.byref(o))
+        for n, _ in _abi.LudOptions._fields_:
+            if getattr(self, n) is not None:
+                setattr(o, n, getattr(self, n))
+        return o
+
+
+class GlobalPositions:
+    """positions [F][3] camera centres (zero where has_position is False), has_position [F] bool (the images of the
+    used pairs), image_tvec [F][3] = -R c (RegisterAllImages), scales [R] (0 for unused pairs), summary (dict of
+    psfm_position_summary)."""
+
+    def __init__(self, positions, has_position, image_tvec, scales, summary):
+        self.positions, self.has_position, self.image_tvec = positions, has_position, image_tvec
+        self.scales, self.summary = scales, summary
+
+
+def estimate_global_positions(num_images, pair_images, tvec, orientations, has_orientation=None, pair_used=None,
+                              options=None):
+    """GlobalMapper::EstimatePositions (sfm/global_mapper.cc:111-132) with the default method "lud", then the pose
+    update of RegisterAllImages (:140-160).  pair_images [R][2] (image 1, image 2), tvec [R][3] pair translation
+    directions (`optimize_pairwise_translations`), orientations [F][4] (w, x, y, z world-to-camera), has_orientation [F]
+    (None: every image), pair_used [R] (None: every pair), options ConstrainedL1SolverOptions (None: the defaults).
+    The gauge is the smallest image index of the used pairs, at the origin.  Returns GlobalPositions
+    (psfm_estimate_global_positions, csrc/position_estimation.cu)."""
+    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
+    R = pairs.shape[0]
+    t = np.ascontiguousarray(tvec, np.float64).reshape(-1, 3)
+    q = np.ascontiguousarray(orientations, np.float64).reshape(-1, 4)
+    F = int(num_images)
+    if t.shape[0] != R or q.shape[0] != F:
+        raise ValueError("pair_images and tvec must describe the same pairs, orientations num_images images")
+    u8 = C.POINTER(C.c_uint8)
+    masks = []
+    for name, mask, size in (("has_orientation", has_orientation, F), ("pair_used", pair_used, R)):
+        if mask is None:
+            masks.append(None)
+            continue
+        a = np.ascontiguousarray(mask, np.uint8)
+        if a.shape != (size,):
+            raise ValueError("%s must have one entry per %s" % (name, "image" if size == F else "pair"))
+        masks.append(a)
+    opts = (options or ConstrainedL1SolverOptions()).to_struct()
+    out = GlobalPositions(np.zeros((F, 3)), np.zeros(F, np.uint8), np.zeros((F, 3)), np.zeros(R), None)
+    s = _abi.PositionSummary()
+    _lib.check(_lib.lib().psfm_estimate_global_positions(
+        F, R, pairs.ctypes.data_as(C.POINTER(C.c_int32)), _lib.dptr(t), _lib.dptr(q),
+        *(m.ctypes.data_as(u8) if m is not None else None for m in masks), C.byref(opts), _lib.dptr(out.positions),
+        out.has_position.ctypes.data_as(u8), _lib.dptr(out.image_tvec), _lib.dptr(out.scales), C.byref(s)),
+        "psfm_estimate_global_positions")
+    out.has_position = out.has_position.astype(bool)
+    out.summary = {n: getattr(s, n) for n, _ in _abi.PositionSummary._fields_}
+    return out

@@ -278,17 +278,26 @@ def make_track_arrays(num_trajs, num_frames, num_obs, seed=0, min_len=3, width=1
     return TrackArrays(np.arange(num_trajs, dtype=np.int64), ptr, frames, xy)
 
 
-def make_two_view_scene(num_trajs, num_frames, num_obs, seed=0, focal=500.0, width=1024, height=436, step=0.02):
+def make_two_view_scene(num_trajs, num_frames, num_obs, seed=0, focal=500.0, width=1024, height=436, step=0.02,
+                        path="line"):
     """Static points seen by a camera that moves `step` per frame along x with a slow yaw: a tracker.TrackArrays with
     make_track_arrays' counts whose locations are the points' exact projections, minus the 0.5 that
     import_keypoints_matches adds back.  Every point lies 2 .. 40 in front of the camera at its first frame, so that
     between adjacent frames it is 100 .. 2000 baselines away: it straddles CheckCheirality's max_depth.
+    path="helix" (opt-in) moves the camera on a helix about the x axis instead (x = step f, y and z on a circle of
+    radius 4 step at 0.6 rad per frame): the centres are not near-collinear, which the global position estimation
+    needs to be well conditioned.  The default path="line" is unchanged.
     Returns (tracks, qvec [F][4], tvec [F][3] world-to-camera, camera (f, cx, cy))."""
     tracks = make_track_arrays(num_trajs, num_frames, num_obs, seed=seed, width=width, height=height)
     rng = np.random.default_rng(seed + 1)
     f = np.arange(num_frames, dtype=np.float64)
     R = axis_angle_to_rotmat(np.stack([0.001 * f, 0.004 * f, np.zeros_like(f)], axis=1))
-    centres = np.stack([step * f, 0.1 * step * np.sin(f), np.zeros_like(f)], axis=1)
+    if path == "line":
+        centres = np.stack([step * f, 0.1 * step * np.sin(f), np.zeros_like(f)], axis=1)
+    elif path == "helix":
+        centres = step * np.stack([f, 4.0 * np.sin(0.6 * f), 4.0 * (1.0 - np.cos(0.6 * f))], axis=1)
+    else:
+        raise ValueError("path must be line or helix")
     tvec = -np.einsum("fij,fj->fi", R, centres)
     cam = np.array([focal, width / 2.0, height / 2.0])
     first = tracks.frame_ids[tracks.ptr[:-1]]
@@ -354,15 +363,20 @@ def _axis_angle_quat(v):
 
 
 def make_view_graph(num_images, graph="complete", band=10, noise_deg=0.0, outlier_fraction=0.0, seed=0,
-                    num_isolated=0, unposed_fraction=0.0, max_angle_deg=30.0):
+                    num_isolated=0, unposed_fraction=0.0, max_angle_deg=30.0, direction_noise_deg=0.0,
+                    direction_outlier_fraction=0.0):
     """A seeded view graph for rotation averaging.  Ground truth: world-to-camera orientations within max_angle_deg of
     the identity.  graph: "complete", "banded" (pairs up to `band` frames apart, a video) or "two_components" (images
     split 2 : 1, the larger half first, each half complete).  The last num_isolated images get no pair.  Each pair's
     2_R_1 = R2 R1^-1 is perturbed by a rotation of N(0, noise_deg) degrees about a random axis; an outlier_fraction of
     the pairs get a uniformly random rotation instead; an unposed_fraction get has_pose = 0.  num_correspondences is
     100 + 10 * (max(0, band - |a - b|) // 5): few distinct values, so many ties on purpose.
+    Camera centres and pair translation directions come from a second generator, so every other key of a seed is
+    the same with or without them: centres uniform in [-10, 10]^3, each pair's unit tvec = R2 (c1 - c2) / |c1 - c2|
+    (the world-to-camera relative translation of the true poses), each component perturbed by N(0, direction_noise_deg)
+    degrees and renormalised; a direction_outlier_fraction of the pairs get a uniformly random direction instead.
     Returns dict(num_images, pair_images [R][2], qvec [R][4], num_correspondences [R], has_pose [R], truth [F][4],
-    outlier [R] bool)."""
+    outlier [R] bool, centres [F][3], tvec [R][3], direction_outlier [R] bool)."""
     rng = np.random.default_rng(seed)
     F = num_images
     axis = rng.normal(size=(F, 3))
@@ -397,5 +411,16 @@ def make_view_graph(num_images, graph="complete", band=10, noise_deg=0.0, outlie
     gap = np.abs(pairs[:, 1] - pairs[:, 0])
     num_corr = (100 + 10 * (np.maximum(0, band - gap) // 5)).astype(np.int32)
     has_pose = (rng.random(R) >= unposed_fraction).astype(np.uint8)
+    rng2 = np.random.default_rng([seed, 2])
+    centres = rng2.uniform(-10.0, 10.0, (F, 3))
+    t = np.einsum("rij,rj->ri", qvec_to_rotmat(truth[pairs[:, 1]]), centres[pairs[:, 0]] - centres[pairs[:, 1]])
+    t /= np.linalg.norm(t, axis=1, keepdims=True)
+    if direction_noise_deg > 0:
+        t = t + np.deg2rad(direction_noise_deg) * rng2.normal(size=(R, 3))
+        t /= np.linalg.norm(t, axis=1, keepdims=True)
+    direction_outlier = rng2.random(R) < direction_outlier_fraction
+    if direction_outlier.any():
+        d = rng2.normal(size=(int(direction_outlier.sum()), 3))
+        t[direction_outlier] = d / np.linalg.norm(d, axis=1, keepdims=True)
     return dict(num_images=F, pair_images=pairs, qvec=rel, num_correspondences=num_corr, has_pose=has_pose,
-                truth=truth, outlier=outlier)
+                truth=truth, outlier=outlier, centres=centres, tvec=t, direction_outlier=direction_outlier)
