@@ -379,6 +379,68 @@ int psfm_estimate_global_positions(int32_t num_images, int64_t num_pairs, const 
                                    uint8_t* has_position, double* image_tvec, double* scales,
                                    psfm_position_summary* summary);
 
+/* IncrementalTriangulator::Options (sfm/incremental_triangulator.h:46-89): the fields TriangulateImage reads; NULL
+   gives these defaults (the bogus-camera thresholds are gcolmap's overrides, controllers/global_mapper.cc:73-79, equal
+   to the defaults).  Check() (incremental_triangulator.cc:40-53): max_transitivity >= 0, both angle errors > 0,
+   min_angle > 0; both focal ratios > 0, max_extra_param >= 0, all finite. */
+typedef struct {
+  int32_t max_transitivity;           /* 1 (only 1 is supported) */
+  double create_max_angle_error;      /* 2.0 degrees */
+  double continue_max_angle_error;    /* 2.0 degrees */
+  double min_angle;                   /* 1.5 degrees */
+  int32_t ignore_two_view_tracks;     /* 1 */
+  double min_focal_length_ratio;      /* 0.1 */
+  double max_focal_length_ratio;      /* 10.0 */
+  double max_extra_param;             /* 1.0 (SIMPLE_PINHOLE has no extra parameter) */
+} psfm_triangulator_options;
+
+typedef struct {
+  int64_t num_components;             /* connected components of the graph over registered, non-bogus images */
+  int64_t largest_component;          /* observations in the largest one */
+  int64_t num_points3D;               /* points created (Create) */
+  int64_t num_continued;              /* observations attached to an existing point (Continue) */
+  int64_t num_ransac_trials;          /* samples drawn by every EstimateTriangulation */
+  int64_t num_local_estimates;        /* multi-view DLTs of the local optimisation */
+  int64_t num_launches;               /* kernels this call launched (fixed per call) */
+  double host_ms;                     /* validation and per-image tables on the host */
+  double graph_ms, components_ms, replay_ms, assembly_ms;   /* CUDA events per phase */
+} psfm_triangulation_summary;
+
+void psfm_triangulator_default_options(psfm_triangulator_options* opts);
+
+typedef struct psfm_triangulation psfm_triangulation;
+/* GlobalMapper::TriangulateAllPoints (sfm/global_mapper.cc:232-247): IncrementalTriangulator::TriangulateImage
+   (sfm/incremental_triangulator.cc:61-119) of every registered image in index order, every Point2D in index order:
+   Find, Continue, Create with EstimateTriangulation (LO-RANSAC over CombinationSampler) (csrc/triangulation.cu).
+   Images and pairs as psfm_optimize_pairwise_translations takes them, images in ascending image_id; camera_size
+   [num_cameras][2] (width, height); pair_used [num_pairs] (NULL: every pair) is the database cache's pair set (at
+   least min_num_matches inliers, config not UNDEFINED), which the correspondence graph holds whole; orientations
+   [num_images][4] (w, x, y, z) and image_tvec [num_images][3] world-to-camera, registered [num_images].
+   The correspondence graph is built as CorrespondenceGraph::AddCorrespondences builds it (a match is dropped when
+   either point already has an accepted correspondence into the other image).  Defined here where the reference follows
+   hash order: the pairs enter the graph in the order of these arrays (pair_id order from a database).  Angular errors
+   are evaluated as atan2(|r1 x r2|, r1 . r2), the reference's acos of the normalised dot product without its loss of
+   accuracy near zero.
+   Runs everything; num_points3D and num_track_elements receive the result's sizes, psfm_triangulation_result copies
+   it.  PSFM_ERR_INVALID before any launch for: an image, camera or keypoint index out of range, a pair of an image
+   with itself, an unordered pair listed twice, a registered image with a non-finite pose, a camera size <= 0, options
+   that fail Check().  PSFM_ERR_UNSUPPORTED for max_transitivity != 1 or 2^31 - 1 keypoints or more.
+   PSFM_ERR_NO_DEVICE without a device. */
+int psfm_triangulation_create(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
+                              const int32_t* image_camera, const double* cameras, int32_t num_cameras,
+                              const int32_t* camera_size, int64_t num_pairs, const int32_t* pair_images,
+                              const int64_t* inlier_ptr, const uint32_t* inlier_matches, const uint8_t* pair_used,
+                              const double* orientations, const double* image_tvec, const uint8_t* registered,
+                              const psfm_triangulator_options* opts, psfm_triangulation** out, int64_t* num_points3D,
+                              int64_t* num_track_elements);
+/* Points in the reference's AddPoint3D order (ids 1, 2, ... are rows 0, 1, ...): xyz [P][3], track_ptr [P + 1], track
+   elements [E] (track_image, track_point2D) in the reference's element order (Create's inliers in list order, then
+   Continue's appends), point3D_of_keypoint [K] (row of the keypoint's point, -1 without one), summary (nullable).
+   Any output pointer may be NULL. */
+int psfm_triangulation_result(const psfm_triangulation* h, double* xyz, int64_t* track_ptr, int32_t* track_image,
+                              int32_t* track_point2D, int64_t* point3D_of_keypoint, psfm_triangulation_summary* summary);
+void psfm_triangulation_destroy(psfm_triangulation* h);
+
 /* ------------------------------------------------------------------------- */
 /* HP2 — global bundle adjustment                                             */
 /* ------------------------------------------------------------------------- */

@@ -317,3 +317,34 @@ class PositionSummary(C.Structure):
         ("inverse_ms", C.c_double),
         ("admm_ms", C.c_double),
     ]
+
+
+class TriangulatorOptions(C.Structure):
+    """psfm_triangulator_options: the fields of IncrementalTriangulator::Options that TriangulateImage reads."""
+    _fields_ = [
+        ("max_transitivity", C.c_int32),
+        ("create_max_angle_error", C.c_double),
+        ("continue_max_angle_error", C.c_double),
+        ("min_angle", C.c_double),
+        ("ignore_two_view_tracks", C.c_int32),
+        ("min_focal_length_ratio", C.c_double),
+        ("max_focal_length_ratio", C.c_double),
+        ("max_extra_param", C.c_double),
+    ]
+
+
+class TriangulationSummary(C.Structure):
+    _fields_ = [
+        ("num_components", C.c_int64),
+        ("largest_component", C.c_int64),
+        ("num_points3D", C.c_int64),
+        ("num_continued", C.c_int64),
+        ("num_ransac_trials", C.c_int64),
+        ("num_local_estimates", C.c_int64),
+        ("num_launches", C.c_int64),
+        ("host_ms", C.c_double),
+        ("graph_ms", C.c_double),
+        ("components_ms", C.c_double),
+        ("replay_ms", C.c_double),
+        ("assembly_ms", C.c_double),
+    ]

@@ -25,7 +25,9 @@ EXPORTS = [
     "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy",
     "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy", "psfm_known_rotation_translations", "psfm_triangulate_tracks",
     "psfm_two_view_relative_poses", "psfm_rotation_default_options", "psfm_estimate_global_rotations",
-    "psfm_optimize_pairwise_translations", "psfm_lud_default_options", "psfm_estimate_global_positions", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
+    "psfm_optimize_pairwise_translations", "psfm_lud_default_options", "psfm_estimate_global_positions",
+    "psfm_triangulator_default_options", "psfm_triangulation_create", "psfm_triangulation_result",
+    "psfm_triangulation_destroy", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
 
@@ -90,6 +92,14 @@ def lib():
                                                  C.POINTER(C.c_uint8), C.POINTER(_abi.LudOptions), dp,
                                                  C.POINTER(C.c_uint8), dp, dp, C.POINTER(_abi.PositionSummary)]
     vp = C.c_void_p
+    L.psfm_triangulator_default_options.argtypes = [C.POINTER(_abi.TriangulatorOptions)]
+    L.psfm_triangulator_default_options.restype = None
+    L.psfm_triangulation_create.argtypes = [C.c_int32, i64p, fp, ip, dp, C.c_int32, ip, C.c_int64, ip, i64p,
+                                            C.POINTER(C.c_uint32), C.POINTER(C.c_uint8), dp, dp, C.POINTER(C.c_uint8),
+                                            C.POINTER(_abi.TriangulatorOptions), C.POINTER(vp), i64p, i64p]
+    L.psfm_triangulation_result.argtypes = [vp, dp, i64p, ip, ip, i64p, C.POINTER(_abi.TriangulationSummary)]
+    L.psfm_triangulation_destroy.argtypes = [vp]
+    L.psfm_triangulation_destroy.restype = None
     L.psfm_tracker_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.POINTER(vp)]
     L.psfm_tracker_advance.argtypes = [vp] * 6 + [ip]
     L.psfm_tracker_optimize.argtypes = [vp, C.POINTER(_abi.TrajOptions), C.POINTER(_abi.TrajSummary)]

@@ -33,6 +33,7 @@ UNITS = [
     ("two_view.cu", []),
     ("rotation_averaging.cu", []),
     ("position_estimation.cu", []),
+    ("triangulation.cu", []),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

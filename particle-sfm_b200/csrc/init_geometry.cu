@@ -19,6 +19,7 @@
 #include <cmath>
 #include <vector>
 
+#include "dlt.cuh"
 #include "psfm_common.cuh"
 
 namespace {
@@ -32,63 +33,6 @@ __device__ __forceinline__ void quat_to_rot(const double* q, double* R) {
   R[0] = 1 - 2 * (y * y + z * z); R[1] = 2 * (x * y - w * z); R[2] = 2 * (x * z + w * y);
   R[3] = 2 * (x * y + w * z); R[4] = 1 - 2 * (x * x + z * z); R[5] = 2 * (y * z - w * x);
   R[6] = 2 * (x * z - w * y); R[7] = 2 * (y * z + w * x); R[8] = 1 - 2 * (x * x + y * y);
-}
-
-// eigenvector of the smallest eigenvalue of a symmetric N x N matrix (full storage, destroyed): cyclic Jacobi
-template <int N>
-__device__ __forceinline__ void smallest_eigenvector(double (&A)[N][N], double (&v)[N]) {
-  double V[N][N];
-#pragma unroll
-  for (int i = 0; i < N; ++i)
-#pragma unroll
-    for (int j = 0; j < N; ++j) V[i][j] = i == j ? 1.0 : 0.0;
-  for (int sweep = 0; sweep < 30; ++sweep) {
-    double off = 0.0, dia = 0.0;
-#pragma unroll
-    for (int i = 0; i < N; ++i) {
-      dia += A[i][i] * A[i][i];
-#pragma unroll
-      for (int j = i + 1; j < N; ++j) off += A[i][j] * A[i][j];
-    }
-    if (!(off > 1e-34 * dia)) break;
-#pragma unroll
-    for (int p = 0; p < N - 1; ++p)
-#pragma unroll
-      for (int q = p + 1; q < N; ++q) {
-        const double apq = A[p][q];
-        if (apq == 0.0) continue;
-        const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
-        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-#pragma unroll
-        for (int k = 0; k < N; ++k) {       // A <- A J (columns p, q)
-          const double akp = A[k][p], akq = A[k][q];
-          A[k][p] = c * akp - s * akq; A[k][q] = s * akp + c * akq;
-        }
-#pragma unroll
-        for (int k = 0; k < N; ++k) {       // A <- J' A (rows p, q)
-          const double apk = A[p][k], aqk = A[q][k];
-          A[p][k] = c * apk - s * aqk; A[q][k] = s * apk + c * aqk;
-        }
-#pragma unroll
-        for (int k = 0; k < N; ++k) {
-          const double vkp = V[k][p], vkq = V[k][q];
-          V[k][p] = c * vkp - s * vkq; V[k][q] = s * vkp + c * vkq;
-        }
-      }
-  }
-  int best = 0;
-#pragma unroll
-  for (int i = 1; i < N; ++i)
-    if (A[i][i] < A[best][best]) best = i;
-#pragma unroll
-  for (int i = 0; i < N; ++i) {
-    double x = V[i][0];
-#pragma unroll
-    for (int j = 1; j < N; ++j)
-      if (j == best) x = V[i][j];
-    v[i] = x;
-  }
 }
 
 // fixed-order block sum of NV values (blockDim.x = 128): result in every thread
@@ -267,21 +211,8 @@ __global__ void __launch_bounds__(128) k_triangulate_tracks(const double* __rest
 #pragma unroll
     for (int c = 0; c < 4; ++c) A[r][c] = 0.0;
   for (int i = track_ptr[t]; i < track_ptr[t + 1]; ++i) {
-    const double* P = proj + 12 * (size_t)i;
     const double2 p = xy[i];
-    const double inv = 1.0 / sqrt(p.x * p.x + p.y * p.y + 1.0);
-    const double r[3] = {p.x * inv, p.y * inv, inv};
-    double T[3][4];
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      const double d = r[0] * P[c] + r[1] * P[4 + c] + r[2] * P[8 + c];
-#pragma unroll
-      for (int k = 0; k < 3; ++k) T[k][c] = P[4 * k + c] - r[k] * d;
-    }
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int b = 0; b < 4; ++b) A[a][b] += T[0][a] * T[0][b] + T[1][a] * T[1][b] + T[2][a] * T[2][b];
+    multi_view_accumulate(proj + 12 * (size_t)i, p.x, p.y, A);
   }
   double v[4];
   smallest_eigenvector<4>(A, v);

@@ -33,6 +33,7 @@
 #include <thread>
 #include <vector>
 
+#include "dlt.cuh"
 #include "psfm_common.cuh"
 
 namespace {
@@ -43,72 +44,13 @@ typedef unsigned long long u64;
 constexpr int kCand = 4;
 constexpr int kCandStride = 16;          // doubles per candidate: R[9], t[3], max_depth, |R(:, 2)|, 2 unused
 constexpr double kEps = 2.220446049250313e-16;
-constexpr double kJacobiTol = 1e-15;     // columns p, q count as orthogonal when |a_p . a_q| <= tol |a_p| |a_q|
-
-// one-sided (Hestenes) Jacobi: A <- A V with mutually orthogonal columns, V orthogonal; column j of A then has the
-// norm of a singular value and V(:, j) is its right singular vector.  Working on A, not A'A, keeps the relative
-// accuracy of the small singular values.
-template <int N>
-__device__ __forceinline__ void one_sided_jacobi(double (&A)[N][N], double (&V)[N][N]) {
-#pragma unroll
-  for (int i = 0; i < N; ++i)
-#pragma unroll
-    for (int j = 0; j < N; ++j) V[i][j] = i == j ? 1.0 : 0.0;
-  for (int sweep = 0; sweep < 40; ++sweep) {
-    bool rotated = false;
-#pragma unroll
-    for (int p = 0; p < N - 1; ++p)
-#pragma unroll
-      for (int q = p + 1; q < N; ++q) {
-        double alpha = 0.0, beta = 0.0, gamma = 0.0;
-#pragma unroll
-        for (int k = 0; k < N; ++k) {
-          alpha += A[k][p] * A[k][p];
-          beta += A[k][q] * A[k][q];
-          gamma += A[k][p] * A[k][q];
-        }
-        if (!(fabs(gamma) > kJacobiTol * sqrt(alpha * beta))) continue;
-        rotated = true;
-        const double zeta = (beta - alpha) / (2.0 * gamma);
-        const double t = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
-        const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
-#pragma unroll
-        for (int k = 0; k < N; ++k) {
-          const double ap = A[k][p], aq = A[k][q];
-          A[k][p] = c * ap - s * aq; A[k][q] = s * ap + c * aq;
-          const double vp = V[k][p], vq = V[k][q];
-          V[k][p] = c * vp - s * vq; V[k][q] = s * vp + c * vq;
-        }
-      }
-    if (!rotated) break;
-  }
-}
-
 // TriangulatePoint with P1 = [I|0], P2 = [R|t] (c = R[9], t[3]), hnormalized
 __device__ __forceinline__ void triangulate(const double* c, double x1, double y1, double x2, double y2, double* X) {
   double A[4][4] = {{-1.0, 0.0, x1, 0.0},
                     {0.0, -1.0, y1, 0.0},
                     {x2 * c[6] - c[0], x2 * c[7] - c[1], x2 * c[8] - c[2], x2 * c[11] - c[9]},
                     {y2 * c[6] - c[3], y2 * c[7] - c[4], y2 * c[8] - c[5], y2 * c[11] - c[10]}};
-  double V[4][4];
-  one_sided_jacobi<4>(A, V);
-  int best = 0;
-  double bn = A[0][0] * A[0][0] + A[1][0] * A[1][0] + A[2][0] * A[2][0] + A[3][0] * A[3][0];
-#pragma unroll
-  for (int j = 1; j < 4; ++j) {
-    const double nj = A[0][j] * A[0][j] + A[1][j] * A[1][j] + A[2][j] * A[2][j] + A[3][j] * A[3][j];
-    if (nj < bn) { bn = nj; best = j; }
-  }
-  double v[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    double x = V[i][0];
-#pragma unroll
-    for (int j = 1; j < 4; ++j)
-      if (j == best) x = V[i][j];
-    v[i] = x;
-  }
-  X[0] = v[0] / v[3]; X[1] = v[1] / v[3]; X[2] = v[2] / v[3];
+  dlt_point_4x4(A, X);
 }
 
 // CheckCheirality's two CalculateDepth tests of one correspondence
@@ -448,18 +390,12 @@ __global__ void k_choose(int R, const int* __restrict__ config, const double* __
   estimated[p] = nc > 0;
 }
 
-// CalculateTriangulationAngle(0, -R' t, X), law-of-cosines form
+// CalculateTriangulationAngle(0, -R' t, X)
 __device__ __forceinline__ double triangulation_angle(const double* cd, const double* X) {
-  const double c0 = -(cd[0] * cd[9] + cd[3] * cd[10] + cd[6] * cd[11]), c1 = -(cd[1] * cd[9] + cd[4] * cd[10] + cd[7] * cd[11]),
-               c2 = -(cd[2] * cd[9] + cd[5] * cd[10] + cd[8] * cd[11]);
-  const double b2 = c0 * c0 + c1 * c1 + c2 * c2;
-  const double r1 = X[0] * X[0] + X[1] * X[1] + X[2] * X[2];
-  const double d0 = X[0] - c0, d1 = X[1] - c1, d2 = X[2] - c2;
-  const double r2 = d0 * d0 + d1 * d1 + d2 * d2;
-  const double den = 2.0 * sqrt(r1 * r2);
-  if (den == 0.0) return 0.0;
-  const double a = fabs(acos((r1 + r2 - b2) / den)), b = M_PI - a;
-  return b < a ? b : a;                        // std::min: a NaN angle stays NaN
+  const double o[3] = {0.0, 0.0, 0.0};
+  const double c[3] = {-(cd[0] * cd[9] + cd[3] * cd[10] + cd[6] * cd[11]), -(cd[1] * cd[9] + cd[4] * cd[10] + cd[7] * cd[11]),
+                       -(cd[2] * cd[9] + cd[5] * cd[10] + cd[8] * cd[11])};
+  return psfm::triangulation_angle(o, c, X);
 }
 
 __global__ void __launch_bounds__(256) k_angles(long long N, const long long* __restrict__ iptr, int R,

@@ -17,7 +17,9 @@ Names and argument meaning follow the reference:
 * `optimize_pairwise_translations(...)` — GlobalMapper::OptimizePairwiseTranslations (sfm/global_mapper.cc:106-109):
   the known-rotation translations of every kept pair, straight from the database arrays;
 * `estimate_global_positions(...)` — GlobalMapper::EstimatePositions (sfm/global_mapper.cc:111-132) with the default
-  method "lud" and the pose update of RegisterAllImages: camera centres and image tvecs.
+  method "lud" and the pose update of RegisterAllImages: camera centres and image tvecs;
+* `triangulate_all_points(...)` — GlobalMapper::TriangulateAllPoints (sfm/global_mapper.cc:232-247): the 3D points and
+  tracks of every registered image, and `Triangulation.to_reconstruction` the ba.Reconstruction the global BA takes.
 There is no CPU fallback: the library raises without a CUDA device."""
 import ctypes as C
 
@@ -285,3 +287,124 @@ def estimate_global_positions(num_images, pair_images, tvec, orientations, has_o
     out.has_position = out.has_position.astype(bool)
     out.summary = {n: getattr(s, n) for n, _ in _abi.PositionSummary._fields_}
     return out
+
+
+class IncrementalTriangulatorOptions:
+    """IncrementalTriangulator::Options (sfm/incremental_triangulator.h:46-89): the fields TriangulateImage reads, with
+    the reference's names.  A field left None takes the library's default (psfm_triangulator_default_options)."""
+
+    def __init__(self, max_transitivity=None, create_max_angle_error=None, continue_max_angle_error=None, min_angle=None,
+                 ignore_two_view_tracks=None, min_focal_length_ratio=None, max_focal_length_ratio=None,
+                 max_extra_param=None):
+        self.max_transitivity = max_transitivity
+        self.create_max_angle_error = create_max_angle_error
+        self.continue_max_angle_error = continue_max_angle_error
+        self.min_angle = min_angle
+        self.ignore_two_view_tracks = ignore_two_view_tracks
+        self.min_focal_length_ratio = min_focal_length_ratio
+        self.max_focal_length_ratio = max_focal_length_ratio
+        self.max_extra_param = max_extra_param
+
+    def to_struct(self):
+        o = _abi.TriangulatorOptions()
+        _lib.lib().psfm_triangulator_default_options(C.byref(o))
+        for n, _ in _abi.TriangulatorOptions._fields_:
+            if getattr(self, n) is not None:
+                setattr(o, n, int(getattr(self, n)) if n == "ignore_two_view_tracks" else getattr(self, n))
+        return o
+
+
+class Triangulation:
+    """Points in the reference's AddPoint3D order (point id = row + 1): xyz [P][3], track_ptr [P + 1], track_image /
+    track_point2D [E] (image index, keypoint index in that image) in the reference's track order, point3D_of_keypoint [K]
+    (row, -1 without a point), summary (dict of psfm_triangulation_summary).  The poses and cameras it was computed
+    with are kept for `to_reconstruction`."""
+
+    def __init__(self, xyz, track_ptr, track_image, track_point2D, point3D_of_keypoint, summary, inputs):
+        self.xyz, self.track_ptr = xyz, track_ptr
+        self.track_image, self.track_point2D = track_image, track_point2D
+        self.point3D_of_keypoint, self.summary = point3D_of_keypoint, summary
+        self._inputs = inputs
+
+    def to_reconstruction(self, image_ids, image_names, camera_ids):
+        """The ba.Reconstruction that ba.iterative_global_refinement and colmap_io.write_model take: SIMPLE_PINHOLE
+        cameras (camera_ids [C]), the registered images (image_ids [F], image_names [F]) with every keypoint as a Point2D
+        (point3D_ids -1 where untriangulated), points 1 .. P with their tracks; reg_image_ids in ascending id order."""
+        from . import ba
+        kp_ptr, kps, cam_of, cams, size, q, t, reg = self._inputs
+        cameras = {int(camera_ids[c]): ba.Camera(int(camera_ids[c]), 0, int(size[c, 0]), int(size[c, 1]), cams[c].copy())
+                   for c in range(len(cams))}
+        images = {}
+        for f in np.nonzero(reg)[0]:
+            lo, hi = int(kp_ptr[f]), int(kp_ptr[f + 1])
+            p3 = self.point3D_of_keypoint[lo:hi]
+            images[int(image_ids[f])] = ba.Image(int(image_ids[f]), q[f].copy(), t[f].copy(), int(camera_ids[cam_of[f]]),
+                                                 str(image_names[f]), kps[lo:hi].astype(np.float64),
+                                                 np.where(p3 >= 0, p3 + 1, -1).astype(np.int64))
+        ids = np.asarray(image_ids, np.int64)
+        points = {}
+        for p in range(self.xyz.shape[0]):
+            a, b = self.track_ptr[p], self.track_ptr[p + 1]
+            points[p + 1] = ba.Point3D(p + 1, self.xyz[p].copy(), np.zeros(3, np.uint8), 0.0,
+                                       ids[self.track_image[a:b]], self.track_point2D[a:b].astype(np.int64))
+        return ba.Reconstruction(cameras, images, points, reg_image_ids=sorted(images))
+
+
+def triangulate_all_points(keypoint_ptr, keypoints, image_camera, cameras, pair_images, inlier_ptr, inlier_matches,
+                           camera_size, orientations, image_tvec, registered, pair_used=None, options=None):
+    """GlobalMapper::TriangulateAllPoints (sfm/global_mapper.cc:232-247): TriangulateImage of every registered image in
+    index order (Find, Continue, Create with LO-RANSAC).  Images and pairs as `optimize_pairwise_translations` takes
+    them (images in ascending image_id), camera_size [C][2] (width, height), orientations [F][4] and image_tvec [F][3]
+    (`estimate_global_rotations` / `estimate_global_positions`), registered [F], pair_used [R] (None: every pair; the
+    database cache's pairs, not the rotation stage's pair_kept), options IncrementalTriangulatorOptions.  The pairs
+    enter the correspondence graph in array order.  Returns Triangulation (psfm_triangulation_create,
+    csrc/triangulation.cu)."""
+    kp_ptr = np.ascontiguousarray(keypoint_ptr, np.int64)
+    kps = np.ascontiguousarray(keypoints, np.float32).reshape(-1, 2)
+    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    cams = np.ascontiguousarray(cameras, np.float64).reshape(-1, 3)
+    size = np.ascontiguousarray(camera_size, np.int32).reshape(-1, 2)
+    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
+    R = pairs.shape[0]
+    iptr = np.ascontiguousarray(inlier_ptr, np.int64)
+    m = np.ascontiguousarray(inlier_matches, np.uint32).reshape(-1, 2)
+    q = np.ascontiguousarray(orientations, np.float64).reshape(-1, 4)
+    t = np.ascontiguousarray(image_tvec, np.float64).reshape(-1, 3)
+    reg = np.ascontiguousarray(registered, np.uint8)
+    F = kp_ptr.shape[0] - 1
+    if iptr.shape[0] != R + 1 or cam_of.shape[0] != F or q.shape[0] != F or t.shape[0] != F or reg.shape != (F,):
+        raise ValueError("pair_images and inlier_ptr must describe the same pairs; image_camera, orientations, image_tvec "
+                         "and registered the same images")
+    if size.shape[0] != cams.shape[0]:
+        raise ValueError("camera_size must have one (width, height) per camera")
+    if iptr[-1] != m.shape[0] or kp_ptr[-1] != kps.shape[0]:
+        raise ValueError("inlier_ptr / keypoint_ptr must end at the number of matches / keypoints")
+    used = None
+    if pair_used is not None:
+        used = np.ascontiguousarray(pair_used, np.uint8)
+        if used.shape != (R,):
+            raise ValueError("pair_used must have one entry per pair")
+    opts = (options or IncrementalTriangulatorOptions()).to_struct()
+    L = _lib.lib()
+    i32, i64, u8 = C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_uint8)
+    h = C.c_void_p()
+    P, E = C.c_int64(), C.c_int64()
+    _lib.check(L.psfm_triangulation_create(
+        F, kp_ptr.ctypes.data_as(i64), kps.ctypes.data_as(C.POINTER(C.c_float)), cam_of.ctypes.data_as(i32),
+        _lib.dptr(cams), cams.shape[0], size.ctypes.data_as(i32), R, pairs.ctypes.data_as(i32), iptr.ctypes.data_as(i64),
+        m.ctypes.data_as(C.POINTER(C.c_uint32)), used.ctypes.data_as(u8) if used is not None else None, _lib.dptr(q),
+        _lib.dptr(t), reg.ctypes.data_as(u8), C.byref(opts), C.byref(h), C.byref(P), C.byref(E)),
+        "psfm_triangulation_create")
+    try:
+        xyz, track_ptr = np.zeros((P.value, 3)), np.zeros(P.value + 1, np.int64)
+        track_image, track_point2D = np.zeros(E.value, np.int32), np.zeros(E.value, np.int32)
+        p3 = np.zeros(kps.shape[0], np.int64)
+        s = _abi.TriangulationSummary()
+        _lib.check(L.psfm_triangulation_result(h, _lib.dptr(xyz), track_ptr.ctypes.data_as(i64), track_image.ctypes.data_as(i32),
+                                               track_point2D.ctypes.data_as(i32), p3.ctypes.data_as(i64), C.byref(s)),
+                   "psfm_triangulation_result")
+    finally:
+        L.psfm_triangulation_destroy(h)
+    summary = {n: getattr(s, n) for n, _ in _abi.TriangulationSummary._fields_}
+    return Triangulation(xyz, track_ptr, track_image, track_point2D, p3, summary,
+                         (kp_ptr, kps, cam_of, cams, size, q, t, reg.astype(bool)))

@@ -312,6 +312,20 @@ def make_two_view_scene(num_trajs, num_frames, num_obs, seed=0, focal=500.0, wid
     return tracks, rotmat_to_qvec(R), tvec, cam
 
 
+def corrupt_keypoints(keypoints, fraction, seed=0, shift_px=(20.0, 60.0), noise_px=0.0):
+    """Observation outliers for triangulation fixtures: a copy of keypoints [K][2] where a seeded `fraction` of them is
+    moved by shift_px[0] .. shift_px[1] pixels in a random direction, and every keypoint gets Gaussian noise of
+    noise_px.  Returns (keypoints, corrupted index array)."""
+    rng = np.random.default_rng(seed)
+    out = np.array(keypoints, np.float64).reshape(-1, 2)
+    out += noise_px * rng.standard_normal(out.shape)
+    idx = np.nonzero(rng.random(out.shape[0]) < fraction)[0]
+    ang = rng.random(idx.shape[0]) * 2.0 * np.pi
+    r = shift_px[0] + (shift_px[1] - shift_px[0]) * rng.random(idx.shape[0])
+    out[idx] += np.stack([r * np.cos(ang), r * np.sin(ang)], 1)
+    return out.astype(np.asarray(keypoints).dtype), idx
+
+
 def relative_essential(qvec, tvec, a, b):
     """E = [t]x R of the relative pose from image a to image b (world-to-camera poses)."""
     Ra, Rb = qvec_to_rotmat(qvec[a]), qvec_to_rotmat(qvec[b])
