@@ -323,8 +323,8 @@ __device__ __forceinline__ void dense_pairs_mma(const double* __restrict__ zf, c
 }
 
 // One tile of the fused Schur kernel; shared memory holds the staged inputs (see linearize_tile).
-// rep is the tile's index.
-template <int TILE, bool ROT>
+// rep is the tile's index.  DENSE_ONLY: every tile of the launch is dense (the pair loop is not compiled).
+template <int TILE, bool ROT, bool DENSE_ONLY = false>
 __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs& a, TileSmem<TILE>& sm, const TileInfo& ti,
                                                 const bool act, const int ls, const int lp, const double a00, const double a02,
                                                 const double a12, const int rep, const int t0, const int nt) {
@@ -347,7 +347,7 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
   const bool valid_f = lane_task(tid, tq_f, par_f);
   int2 rg_f = make_int2(0, 0);
   int slot_f = 0;
-  if (valid_f) { rg_f = __ldg(a.task_rng + t0 + tq_f); slot_f = __ldg(a.task_slot + t0 + tq_f); }
+  if (!DENSE_ONLY && valid_f) { rg_f = __ldg(a.task_rng + t0 + tq_f); slot_f = __ldg(a.task_slot + t0 + tq_f); }
   double* sv = sm.sv + tid;
 #pragma unroll
   for (int k = 0; k < NVX2; ++k) sv[k * PSFM_SVS] = 0.0;
@@ -409,7 +409,7 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
     const double pw1 = jg[1][0] * gg[0] + jg[1][1] * gg[1] + jg[1][2] * gg[2];
 #pragma unroll
     for (int r = (ROT ? 0 : 3); r < 6; ++r) sv[(21 + r) * PSFM_SVS] = -(jc[0][r] * pw0 + jc[1][r] * pw1);   // -(W w^)
-    if (mode == TILE_PAIRS_LOOP) {
+    if (!DENSE_ONLY && mode == TILE_PAIRS_LOOP) {
       rec[0] = a00; rec[1] = a02; rec[2] = a12;
 #pragma unroll
       for (int m = 0; m < 2; ++m) {   // Q = JG G'
@@ -435,7 +435,7 @@ __device__ __forceinline__ void schur_tile_body(const TileCtx& tc, const StArgs&
   }
   __syncthreads();
   double* band = a.Sband + (size_t)(rep & a.nrep_mask) * a.band_stride;
-  if (mode != TILE_PAIRS_LOOP) {
+  if (DENSE_ONLY || mode != TILE_PAIRS_LOOP) {
     // the reduction rows are dead: stage Z there
     double* zf = sm.sv;
     const int KB2 = dense_z_kb2(ti.np), zrows = 16 * dense_z_rb(ti.ns), zcols = 8 * KB2;
@@ -608,9 +608,8 @@ __global__ void __launch_bounds__(TILE, (TILE == 256 ? 2 : 1)) k_schur_tile(cons
 
 // persistent, pipelined form (ba_tile_pipe.cuh): the inputs of the next tile are in flight
 // (cp.async) while this tile's pair tasks run
-template <int TILE, bool ROT>
-__global__ void __launch_bounds__(TILE, (TILE == 256 ? 2 : 1)) k_schur_tile_p(const TileCtx tc, const PipeSrc ps, const StArgs a) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
+template <int TILE, bool ROT, bool DENSE_ONLY>
+__device__ __forceinline__ void schur_tile_pipe(const TileCtx& tc, const PipeSrc& ps, const StArgs& a, unsigned char* smem_raw) {
   __shared__ __align__(16) int4 hdr_ring[4][2];
   __shared__ __align__(8) unsigned long long bars[2];
   const int cns = tc.cap_ns, cnp = tc.cap_np;
@@ -626,9 +625,24 @@ __global__ void __launch_bounds__(TILE, (TILE == 256 ? 2 : 1)) k_schur_tile_p(co
     int ls = 0, lp = 0;
     double a00 = 0, a02 = 0, a12 = 0;
     if (act) { ls = s.lseg[tid]; lp = s.lpt[tid]; a00 = s.a0[tid]; a02 = s.a1[tid]; a12 = s.a2[tid]; }
-    const int t0 = __ldg(a.tile_task + tile), nt = __ldg(a.tile_task + tile + 1) - t0;
-    schur_tile_body<TILE, ROT>(tc, a, sm, ti, act, ls, lp, a00, a02, a12, tile, t0, nt);
+    int t0 = 0, nt = 0;
+    if (!DENSE_ONLY) { t0 = __ldg(a.tile_task + tile); nt = __ldg(a.tile_task + tile + 1) - t0; }
+    schur_tile_body<TILE, ROT, DENSE_ONLY>(tc, a, sm, ti, act, ls, lp, a00, a02, a12, tile, t0, nt);
   });
+}
+
+template <int TILE, bool ROT>
+__global__ void __launch_bounds__(TILE, (TILE == 256 ? 2 : 1)) k_schur_tile_p(const TileCtx tc, const PipeSrc ps, const StArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  schur_tile_pipe<TILE, ROT, false>(tc, ps, a, smem_raw);
+}
+
+// the same kernel when every tile of the problem is dense (k_tile_pairs_mode): without the pair loop's code ptxas
+// keeps the dense phase in registers (k_schur_tile_p spills in it)
+template <int TILE, bool ROT>
+__global__ void __launch_bounds__(TILE, (TILE == 256 ? 2 : 1)) k_schur_dense_p(const TileCtx tc, const PipeSrc ps, const StArgs a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  schur_tile_pipe<TILE, ROT, true>(tc, ps, a, smem_raw);
 }
 
 template <int TILE>

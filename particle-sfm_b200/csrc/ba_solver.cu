@@ -1157,7 +1157,8 @@ void do_explicit_solve(psfm_ba_solver* S, const RunCfg& c, double radius) {
     if (pipe_ok(S, pipe_smem) && !getenv("PSFM_NO_PIPE_SCHUR")) {
       PipeSrc ps = pipe_src(S);
       ps.obs_a = S->d_a.p; ps.p6 = S->d_gf.p; ps.p3a = S->d_gv.p; ps.p3b = S->d_gu.p;
-      PSFM_PIPE_LAUNCH(k_schur_tile_p, pipe_smem, S, c.rot, ps, w);
+      if (S->ndense == S->T) PSFM_PIPE_LAUNCH(k_schur_dense_p, pipe_smem, S, c.rot, ps, w);
+      else PSFM_PIPE_LAUNCH(k_schur_tile_p, pipe_smem, S, c.rot, ps, w);
     } else {
       PSFM_TILE_LAUNCH(k_schur_tile, NVX2, 15, S, c.rot, w);
     }
