@@ -441,6 +441,68 @@ int psfm_triangulation_result(const psfm_triangulation* h, double* xyz, int64_t*
                               int32_t* track_point2D, int64_t* point3D_of_keypoint, psfm_triangulation_summary* summary);
 void psfm_triangulation_destroy(psfm_triangulation* h);
 
+/* TwoViewGeometry::Options with its RANSACOptions, as `colmap matches_importer --match_type pairs` takes them; NULL
+   gives what sfm/import_feature_matches.py:106-117 runs.  Check(): max_error > 0, confidence, min_inlier_ratio,
+   watermark_min_inlier_ratio and watermark_border_size in [0, 1], 0 <= min_num_trials <= max_num_trials,
+   min_num_inliers >= 0, dyn_num_trials_multiplier > 0, max_H_inlier_ratio >= 0, all finite. */
+typedef struct {
+  double max_error;                    /* 4.0 px */
+  double confidence;                   /* 0.999 */
+  int32_t max_num_trials;              /* 20000 */
+  int32_t min_num_trials;              /* 0 */
+  double min_inlier_ratio;             /* 0.1 */
+  int32_t min_num_inliers;             /* 15 */
+  double dyn_num_trials_multiplier;    /* 3.0 */
+  double max_H_inlier_ratio;           /* 0.8 */
+  int32_t detect_watermark;            /* 1 */
+  double watermark_min_inlier_ratio;   /* 0.7 */
+  double watermark_border_size;        /* 0.1 */
+  uint64_t random_seed;                /* 0 */
+} psfm_verification_options;
+
+/* per estimator kind: [0] F, [1] H, [2] the watermark translation */
+typedef struct {
+  int64_t num_trials[3];               /* samples the sequential LORANSAC loop draws */
+  int64_t num_trials_scored[3];        /* samples the device scored (the same: trials run in sequential order) */
+  int64_t num_local_rounds[3];         /* local-optimisation rounds */
+  int64_t num_config[8];               /* pairs per config (UNDEFINED 0 .. WATERMARK 7) */
+  int64_t num_launches;                /* kernels this call launched: 3 with pairs, 0 without */
+  double host_ms;                      /* validation on the host */
+  double gather_ms, ransac_ms, compact_ms;   /* CUDA events per phase */
+} psfm_verification_summary;
+
+void psfm_verification_default_options(psfm_verification_options* opts);
+
+/* The geometric verification of `colmap matches_importer --match_type pairs` (TwoViewGeometryVerifier ->
+   TwoViewGeometry::EstimateUncalibrated) of every image pair at once (csrc/verification.cu): raw matches in, the rows of
+   the two_view_geometries table out.  Images as psfm_two_view_relative_poses takes them, camera_size [num_cameras][2]
+   (width, height), prior_focal_length [num_cameras] (NULL: none).  Pairs in database orientation: pair_images
+   [num_pairs][2] (image 1 = the smaller image_id), match_ptr [num_pairs + 1], matches [M][2] (point2D_idx1,
+   point2D_idx2).
+   Per pair: fewer than min_num_inliers raw matches gives config UNDEFINED (0), no inliers and zero F / H.  Otherwise
+   LORANSAC of the seven-point F (eight-point local step, squared Sampson error) and of the normalised-DLT H (squared
+   transfer error), both against max_error^2: DEGENERATE (1) when neither succeeded or both have fewer than
+   min_num_inliers inliers, else PLANAR_OR_PANORAMIC (6) when H inliers / F inliers > max_H_inlier_ratio, else
+   UNCALIBRATED (3); the inlier matches are F's inliers in match order; with detect_watermark, WATERMARK (7) when
+   DetectWatermark finds them translated in the border strip.  E is zero.
+   Defined here, the same way in oracle/verification_oracle.py: each trial's sample comes from a SplitMix64 stream keyed
+   by (random_seed, pair, kind, trial) (kind 0 F, 1 H, 2 watermark); the seven-point models are ordered by (F00, F01, ...)
+   after F22 = 1; stored F and H have unit Frobenius norm with the largest-magnitude entry positive.
+   Out: config [num_pairs], F / E / H [num_pairs][9] row-major, inlier_ptr [num_pairs + 1], inlier_matches (room for
+   match_ptr[num_pairs] rows; inlier_ptr gives what was written), pair_trials [num_pairs][3] the samples drawn per kind
+   (may be NULL), summary (may be NULL).
+   PSFM_ERR_INVALID before any launch for an image, camera or keypoint index out of range, a pair of an image with
+   itself, an unordered pair listed twice, a camera size <= 0, or options that fail Check().  PSFM_ERR_UNSUPPORTED for a
+   pair whose two cameras both have a prior focal length (EstimateCalibrated) or a pair of 2^31 matches or more.
+   PSFM_ERR_NO_DEVICE without a device.  With no pair nothing is launched. */
+int psfm_verify_two_view_geometries(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
+                                    const int32_t* image_camera, int32_t num_cameras, const int32_t* camera_size,
+                                    const uint8_t* prior_focal_length, int64_t num_pairs, const int32_t* pair_images,
+                                    const int64_t* match_ptr, const uint32_t* matches,
+                                    const psfm_verification_options* opts, int32_t* config, double* F, double* E,
+                                    double* H, int64_t* inlier_ptr, uint32_t* inlier_matches, int32_t* pair_trials,
+                                    psfm_verification_summary* summary);
+
 /* ------------------------------------------------------------------------- */
 /* HP2 — global bundle adjustment                                             */
 /* ------------------------------------------------------------------------- */

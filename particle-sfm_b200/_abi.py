@@ -348,3 +348,35 @@ class TriangulationSummary(C.Structure):
         ("replay_ms", C.c_double),
         ("assembly_ms", C.c_double),
     ]
+
+
+class VerificationOptions(C.Structure):
+    """psfm_verification_options: TwoViewGeometry::Options with its RANSACOptions."""
+    _fields_ = [
+        ("max_error", C.c_double),
+        ("confidence", C.c_double),
+        ("max_num_trials", C.c_int32),
+        ("min_num_trials", C.c_int32),
+        ("min_inlier_ratio", C.c_double),
+        ("min_num_inliers", C.c_int32),
+        ("dyn_num_trials_multiplier", C.c_double),
+        ("max_H_inlier_ratio", C.c_double),
+        ("detect_watermark", C.c_int32),
+        ("watermark_min_inlier_ratio", C.c_double),
+        ("watermark_border_size", C.c_double),
+        ("random_seed", C.c_uint64),
+    ]
+
+
+class VerificationSummary(C.Structure):
+    _fields_ = [
+        ("num_trials", C.c_int64 * 3),
+        ("num_trials_scored", C.c_int64 * 3),
+        ("num_local_rounds", C.c_int64 * 3),
+        ("num_config", C.c_int64 * 8),
+        ("num_launches", C.c_int64),
+        ("host_ms", C.c_double),
+        ("gather_ms", C.c_double),
+        ("ransac_ms", C.c_double),
+        ("compact_ms", C.c_double),
+    ]

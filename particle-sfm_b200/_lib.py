@@ -27,7 +27,8 @@ EXPORTS = [
     "psfm_two_view_relative_poses", "psfm_rotation_default_options", "psfm_estimate_global_rotations",
     "psfm_optimize_pairwise_translations", "psfm_lud_default_options", "psfm_estimate_global_positions",
     "psfm_triangulator_default_options", "psfm_triangulation_create", "psfm_triangulation_result",
-    "psfm_triangulation_destroy", "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
+    "psfm_triangulation_destroy", "psfm_verification_default_options", "psfm_verify_two_view_geometries",
+    "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
 
@@ -100,6 +101,12 @@ def lib():
     L.psfm_triangulation_result.argtypes = [vp, dp, i64p, ip, ip, i64p, C.POINTER(_abi.TriangulationSummary)]
     L.psfm_triangulation_destroy.argtypes = [vp]
     L.psfm_triangulation_destroy.restype = None
+    L.psfm_verification_default_options.argtypes = [C.POINTER(_abi.VerificationOptions)]
+    L.psfm_verification_default_options.restype = None
+    u32p = C.POINTER(C.c_uint32)
+    L.psfm_verify_two_view_geometries.argtypes = [C.c_int32, i64p, fp, ip, C.c_int32, ip, C.POINTER(C.c_uint8), C.c_int64,
+                                                  ip, i64p, u32p, C.POINTER(_abi.VerificationOptions), ip, dp, dp, dp,
+                                                  i64p, u32p, ip, C.POINTER(_abi.VerificationSummary)]
     L.psfm_tracker_create.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.POINTER(vp)]
     L.psfm_tracker_advance.argtypes = [vp] * 6 + [ip]
     L.psfm_tracker_optimize.argtypes = [vp, C.POINTER(_abi.TrajOptions), C.POINTER(_abi.TrajSummary)]

@@ -34,6 +34,7 @@ UNITS = [
     ("rotation_averaging.cu", []),
     ("position_estimation.cu", []),
     ("triangulation.cu", []),
+    ("verification.cu", []),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

@@ -127,6 +127,45 @@ __device__ __forceinline__ void smallest_eigenvector(double (&A)[N][N], double (
   }
 }
 
+// smallest_eigenvector's cyclic Jacobi with A (n x n row-major, destroyed) and the workspace V (n x n) in memory, for a
+// caller that cannot hold 2 n^2 doubles in registers (the 9 x 9 normal matrices of verification.cu)
+__device__ inline void smallest_eigenvector_mem(double* A, double* V, int n, double* v) {
+  for (int i = 0; i < n; ++i)
+    for (int j = 0; j < n; ++j) V[i * n + j] = i == j ? 1.0 : 0.0;
+  for (int sweep = 0; sweep < 30; ++sweep) {
+    double off = 0.0, dia = 0.0;
+    for (int i = 0; i < n; ++i) {
+      dia += A[i * n + i] * A[i * n + i];
+      for (int j = i + 1; j < n; ++j) off += A[i * n + j] * A[i * n + j];
+    }
+    if (!(off > 1e-34 * dia)) break;
+    for (int p = 0; p < n - 1; ++p)
+      for (int q = p + 1; q < n; ++q) {
+        const double apq = A[p * n + q];
+        if (apq == 0.0) continue;
+        const double theta = (A[q * n + q] - A[p * n + p]) / (2.0 * apq);
+        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < n; ++k) {
+          const double akp = A[k * n + p], akq = A[k * n + q];
+          A[k * n + p] = c * akp - s * akq; A[k * n + q] = s * akp + c * akq;
+        }
+        for (int k = 0; k < n; ++k) {
+          const double apk = A[p * n + k], aqk = A[q * n + k];
+          A[p * n + k] = c * apk - s * aqk; A[q * n + k] = s * apk + c * aqk;
+        }
+        for (int k = 0; k < n; ++k) {
+          const double vkp = V[k * n + p], vkq = V[k * n + q];
+          V[k * n + p] = c * vkp - s * vkq; V[k * n + q] = s * vkp + c * vkq;
+        }
+      }
+  }
+  int best = 0;
+  for (int i = 1; i < n; ++i)
+    if (A[i * n + i] < A[best * n + best]) best = i;
+  for (int i = 0; i < n; ++i) v[i] = V[i * n + best];
+}
+
 // TriangulateMultiViewPoint's accumulation of one view: A += (P - r r' P)' (P - r r' P), r = (x, y, 1) / |(x, y, 1)|,
 // P row-major 3 x 4
 __device__ __forceinline__ void multi_view_accumulate(const double* P, double x, double y, double (&A)[4][4]) {

@@ -8,6 +8,9 @@ Names and argument meaning follow the reference:
   one launch instead of one ThreadPool task per pair;
 * `triangulate_multi_view_points(tracks)` — the multi-view DLT behind IncrementalTriangulator::Create
   (sfm/incremental_triangulator.cc:463-548), every track in one launch;
+* `verify_two_view_geometries(...)` — the geometric verification of `colmap matches_importer --match_type pairs`
+  (TwoViewGeometryVerifier -> TwoViewGeometry::EstimateUncalibrated) of every pair in one call: raw matches in, config,
+  F, H and inlier matches out, which `TwoViewVerification.to_two_view_geometries` hands to the next step;
 * `estimate_relative_poses(...)` — TwoViewGeometry::EstimateRelativePose (estimators/two_view_geometry.cc:172-239)
   of every verified pair in one call, instead of the ThreadPool loop of DatabaseCache::Load
   (base/database_cache.cc:206-228); its inputs are what `handoff.read_two_view_geometries` reads from a database;
@@ -408,3 +411,105 @@ def triangulate_all_points(keypoint_ptr, keypoints, image_camera, cameras, pair_
     summary = {n: getattr(s, n) for n, _ in _abi.TriangulationSummary._fields_}
     return Triangulation(xyz, track_ptr, track_image, track_point2D, p3, summary,
                          (kp_ptr, kps, cam_of, cams, size, q, t, reg.astype(bool)))
+
+
+class TwoViewVerificationOptions:
+    """TwoViewGeometry::Options with its RANSACOptions, the reference's names.  A field left None takes the library's
+    default (psfm_verification_default_options: what sfm/import_feature_matches.py:106-117 runs)."""
+
+    def __init__(self, max_error=None, confidence=None, max_num_trials=None, min_num_trials=None, min_inlier_ratio=None,
+                 min_num_inliers=None, dyn_num_trials_multiplier=None, max_H_inlier_ratio=None, detect_watermark=None,
+                 watermark_min_inlier_ratio=None, watermark_border_size=None, random_seed=None):
+        self.max_error = max_error
+        self.confidence = confidence
+        self.max_num_trials = max_num_trials
+        self.min_num_trials = min_num_trials
+        self.min_inlier_ratio = min_inlier_ratio
+        self.min_num_inliers = min_num_inliers
+        self.dyn_num_trials_multiplier = dyn_num_trials_multiplier
+        self.max_H_inlier_ratio = max_H_inlier_ratio
+        self.detect_watermark = detect_watermark
+        self.watermark_min_inlier_ratio = watermark_min_inlier_ratio
+        self.watermark_border_size = watermark_border_size
+        self.random_seed = random_seed
+
+    def to_struct(self):
+        o = _abi.VerificationOptions()
+        _lib.lib().psfm_verification_default_options(C.byref(o))
+        for n, _ in _abi.VerificationOptions._fields_:
+            if getattr(self, n) is not None:
+                setattr(o, n, int(getattr(self, n)) if n == "detect_watermark" else getattr(self, n))
+        return o
+
+
+class TwoViewVerification:
+    """Per pair (in the order of the input): config [R] (UNDEFINED 0, DEGENERATE 1, UNCALIBRATED 3,
+    PLANAR_OR_PANORAMIC 6, WATERMARK 7), F / E / H [R][3][3] (unit Frobenius norm, largest-magnitude entry positive; E
+    zero), inlier_ptr [R + 1], inlier_matches [N][2] uint32 (F's inliers in match order), trials [R][3] (samples drawn
+    for F, H and the watermark test), summary (dict of psfm_verification_summary)."""
+
+    def __init__(self, config, F, E, H, inlier_ptr, inlier_matches, trials, summary):
+        self.config, self.F, self.E, self.H = config, F, E, H
+        self.inlier_ptr, self.inlier_matches = inlier_ptr, inlier_matches
+        self.trials, self.summary = trials, summary
+
+    def two_view_rows(self, pair_ids):
+        """The two_view_geometries rows (pair_id, inlier matches, config, F, E, H) of every pair, which
+        handoff.write_colmap_database stores as `colmap matches_importer` would."""
+        return [(int(pid), np.ascontiguousarray(self.inlier_matches[self.inlier_ptr[p]:self.inlier_ptr[p + 1]]),
+                 int(self.config[p]), self.F[p], self.E[p], self.H[p]) for p, pid in enumerate(pair_ids)]
+
+    def to_two_view_geometries(self, tables):
+        """The handoff.TwoViewGeometries that read_two_view_geometries returns once two_view_rows(tables.pair_ids) are
+        written beside `tables` (a handoff.MatchTables): relative_pose_inputs() and triangulate_all_points then run
+        without SQLite."""
+        from .handoff import TwoViewGeometries
+        return TwoViewGeometries(
+            image_ids=tables.image_ids, keypoint_ptr=tables.keypoint_ptr, keypoints=tables.keypoints,
+            camera_ids=tables.camera_ids, cameras=tables.cameras, image_camera=tables.image_camera,
+            pair_ids=tables.pair_ids, pair_images=tables.pair_images, camera_size=tables.camera_size,
+            image_names=list(tables.image_names), config=self.config.copy(), F=self.F.copy(), E=self.E.copy(),
+            H=self.H.copy(), inlier_ptr=self.inlier_ptr.copy(), inlier_matches=self.inlier_matches.copy())
+
+
+def verify_two_view_geometries(keypoint_ptr, keypoints, image_camera, camera_size, pair_images, match_ptr, matches,
+                               prior_focal_length=None, options=None):
+    """The geometric verification of `colmap matches_importer --match_type pairs` (TwoViewGeometryVerifier ->
+    EstimateUncalibrated) of every pair at once: keypoint_ptr [F + 1], keypoints [K][2] (as stored in the database),
+    image_camera [F], camera_size [C][2] (width, height), pair_images [R][2] (image 1 = the smaller image_id),
+    match_ptr [R + 1], matches [M][2] (point2D_idx1, point2D_idx2), prior_focal_length [C] (None: no camera has one),
+    options TwoViewVerificationOptions.  handoff.MatchTables.verification_inputs() gives these arguments.  Returns
+    TwoViewVerification (psfm_verify_two_view_geometries, csrc/verification.cu)."""
+    kp_ptr = np.ascontiguousarray(keypoint_ptr, np.int64)
+    kps = np.ascontiguousarray(keypoints, np.float32).reshape(-1, 2)
+    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    size = np.ascontiguousarray(camera_size, np.int32).reshape(-1, 2)
+    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
+    R = pairs.shape[0]
+    mptr = np.ascontiguousarray(match_ptr, np.int64)
+    m = np.ascontiguousarray(matches, np.uint32).reshape(-1, 2)
+    F = kp_ptr.shape[0] - 1
+    if mptr.shape[0] != R + 1 or cam_of.shape[0] != F:
+        raise ValueError("pair_images and match_ptr must describe the same pairs, image_camera the images")
+    if mptr[-1] != m.shape[0] or kp_ptr[-1] != kps.shape[0]:
+        raise ValueError("match_ptr / keypoint_ptr must end at the number of matches / keypoints")
+    prior = None
+    if prior_focal_length is not None:
+        prior = np.ascontiguousarray(prior_focal_length, np.uint8)
+        if prior.shape != (size.shape[0],):
+            raise ValueError("prior_focal_length must have one entry per camera")
+    opts = (options or TwoViewVerificationOptions()).to_struct()
+    config, Fm, Em, Hm = np.zeros(R, np.int32), np.zeros((R, 3, 3)), np.zeros((R, 3, 3)), np.zeros((R, 3, 3))
+    iptr, out = np.zeros(R + 1, np.int64), np.zeros((m.shape[0], 2), np.uint32)
+    trials = np.zeros((R, 3), np.int32)
+    s = _abi.VerificationSummary()
+    i32, i64, u32 = C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_uint32)
+    _lib.check(_lib.lib().psfm_verify_two_view_geometries(
+        F, kp_ptr.ctypes.data_as(i64), kps.ctypes.data_as(C.POINTER(C.c_float)), cam_of.ctypes.data_as(i32),
+        size.shape[0], size.ctypes.data_as(i32), prior.ctypes.data_as(C.POINTER(C.c_uint8)) if prior is not None else None,
+        R, pairs.ctypes.data_as(i32), mptr.ctypes.data_as(i64), m.ctypes.data_as(u32), C.byref(opts),
+        config.ctypes.data_as(i32), _lib.dptr(Fm), _lib.dptr(Em), _lib.dptr(Hm), iptr.ctypes.data_as(i64),
+        out.ctypes.data_as(u32), trials.ctypes.data_as(i32), C.byref(s)), "psfm_verify_two_view_geometries")
+    summary = {n: (list(getattr(s, n)) if n.startswith(("num_trials", "num_local", "num_config")) else getattr(s, n))
+               for n, _ in _abi.VerificationSummary._fields_}
+    return TwoViewVerification(config, Fm, Em, Hm, iptr, np.ascontiguousarray(out[:iptr[-1]]), trials, summary)
