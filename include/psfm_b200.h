@@ -713,6 +713,41 @@ int psfm_ba_get_point_errors(psfm_ba_solver* s, double* error);
 int psfm_ba_iterative_refinement(psfm_ba_solver* s, const psfm_ba_options* opts, const psfm_ba_refine_options* ropts,
                                  psfm_ba_refine_report* report);
 
+/* ------------------------------------------------------------------------- */
+/* Triangulation -> bundle adjustment -> model, on the device (DESIGN.md §4.9) */
+/* ------------------------------------------------------------------------- */
+/* The resident problem of a triangulation (psfm_triangulation_create) without its keypoints or point3D_of_keypoint
+   leaving the device: the problem ba.flatten builds from Triangulation.to_reconstruction with every registered image
+   in the config.  Problem images are the registered images in ascending index, problem cameras the cameras they use
+   in ascending index, problem points the triangulation's rows; observations are every keypoint of a registered image
+   with a point, images first, keypoints in index order.
+     qvec [F][4], tvec [F][3]          poses of the triangulation's F images (rows of unregistered images are ignored)
+     cam_params [C][3]                 f, cx, cy of its C cameras
+     pose_constant, tvec_constant_mask [F], camera_constant [C]: as in psfm_ba_problem, indexed like the triangulation;
+                                       may be NULL
+   num_images, num_cameras, num_observations (may be NULL) receive the problem's sizes.  PSFM_ERR_INVALID for a NULL
+   argument or no registered image, PSFM_ERR_UNSUPPORTED with a multi-GPU communicator.  The triangulation may be
+   destroyed once this returns. */
+int psfm_ba_create_from_triangulation(const psfm_triangulation* tri, const double* qvec, const double* tvec,
+                                      const double* cam_params, const uint8_t* pose_constant,
+                                      const uint8_t* tvec_constant_mask, const uint8_t* camera_constant,
+                                      psfm_ba_solver** out, int32_t* num_images, int32_t* num_cameras,
+                                      int64_t* num_observations);
+/* The refined model of a solver made by psfm_ba_create_from_triangulation, in the triangulation's layout:
+     qvec [F][4], tvec [F][3], cam_params [C][3]: the problem's rows are written, the others left as they are
+     xyz [P][3]                        every row (a point no observation keeps holds its triangulated position)
+     track_ptr [P + 1]                 a point whose observations were all filtered has length 0
+     track_image, track_point2D        room for num_observations elements; track_ptr[P] are written: (image index,
+                                       point2D_idx) of the alive observations, by point, images ascending within a track
+     point3D_of_keypoint [K]           point row of every alive observation's keypoint, -1 elsewhere
+   Point errors come from psfm_ba_get_point_errors. */
+int psfm_ba_get_model(psfm_ba_solver* s, double* qvec, double* tvec, double* cam_params, double* xyz, int64_t* track_ptr,
+                      int32_t* track_image, int32_t* track_point2D, int64_t* point3D_of_keypoint);
+/* The observations the solver was created with, in order (any output may be NULL): obs_image [M], obs_point [M],
+   obs_xy [M][2], point2D_idx [M] (a solver made by psfm_ba_create_from_triangulation only). */
+int psfm_ba_get_observations(psfm_ba_solver* s, int32_t* obs_image, int32_t* obs_point, double* obs_xy,
+                             int32_t* point2D_idx);
+
 /* Measured fp64 roof of the current device (bench.py's roofline denominator for the kernels
    that are bounded by the fp64 FMA pipe rather than by HBM): sustained fused multiply-adds
    per second over the whole chip, and the latency in SM cycles of one dependent DFMA. */

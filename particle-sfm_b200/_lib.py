@@ -20,6 +20,7 @@ EXPORTS = [
     "psfm_ba_linear_step", "psfm_ba_band_solve", "psfm_measure_dfma", "psfm_ba_default_refine_options",
     "psfm_ba_filter_negative_depth", "psfm_ba_filter_points", "psfm_ba_normalize", "psfm_ba_num_observations",
     "psfm_ba_get_observation_mask", "psfm_ba_get_point_errors", "psfm_ba_iterative_refinement",
+    "psfm_ba_create_from_triangulation", "psfm_ba_get_model", "psfm_ba_get_observations",
     "psfm_grid_sample", "psfm_flow_check", "psfm_tracker_step", "psfm_tracker_buffer_inputs",
     "psfm_tracker_create", "psfm_tracker_advance", "psfm_tracker_optimize", "psfm_tracker_get_buffer", "psfm_tracker_set_buffer",
     "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy",
@@ -34,7 +35,11 @@ EXPORTS = [
 
 
 class PsfmError(RuntimeError):
-    pass
+    """code: the library's negative status (_abi.PSFM_ERR_*) when a call returned one, else None."""
+
+    def __init__(self, message, code=None):
+        super().__init__(message)
+        self.code = code
 
 
 def lib():
@@ -131,6 +136,9 @@ def lib():
     L.psfm_ba_get_point_errors.argtypes = [C.c_void_p, dp]
     L.psfm_ba_iterative_refinement.argtypes = [C.c_void_p, C.POINTER(_abi.BAOptions), C.POINTER(_abi.BARefineOptions),
                                                C.POINTER(_abi.BARefineReport)]
+    L.psfm_ba_create_from_triangulation.argtypes = [vp, dp, dp, dp, u8p, u8p, u8p, C.POINTER(vp), ip, ip, i64p]
+    L.psfm_ba_get_model.argtypes = [vp, dp, dp, dp, dp, i64p, ip, ip, i64p]
+    L.psfm_ba_get_observations.argtypes = [vp, ip, ip, dp, ip]
     L.psfm_ba_band_solve.argtypes = [dp, dp, C.c_int32, C.c_int32, dp]
     L.psfm_dist_get_unique_id.argtypes = [C.POINTER(C.c_uint8)]
     L.psfm_dist_init.argtypes = [C.POINTER(C.c_uint8), C.c_int32, C.c_int32]
@@ -142,7 +150,7 @@ def lib():
 def check(rc, what):
     if rc < 0:
         msg = lib().psfm_last_error().decode("utf-8", "replace")
-        raise PsfmError(f"{what} failed with status {rc}: {msg}")
+        raise PsfmError(f"{what} failed with status {rc}: {msg}", rc)
     return rc
 
 

@@ -625,3 +625,93 @@ def iterative_global_refinement(reconstruction, force_update_rotation, ba_refine
     scatter(problem, maps, reconstruction)
     apply_observation_mask(problem, maps, reconstruction, alive, err)
     return rep
+
+
+# ----------------------------------------------------------------------------- triangulation -> BA -> model on the device
+
+class TriangulationModel:
+    """What psfm_ba_get_model returns, in the triangulation's layout (image / camera index, point row = point id - 1):
+    qvec [F][4], tvec [F][3], cam_params [C][3], xyz [P][3], track_ptr [P + 1] (length 0: a deleted point),
+    track_image / track_point2D [E], point3D_of_keypoint [K] (row, -1), error [P] (Point3D::Error, 0 where no point
+    filter set it)."""
+
+    def __init__(self, **arrays):
+        self.__dict__.update(arrays)
+
+
+class TriangulationSolver:
+    """The resident problem of an init_geometry.ResidentTriangulation (psfm_ba_create_from_triangulation): the problem
+    `flatten` builds from Triangulation.to_reconstruction with every registered image in the config, built on the
+    device.  qvec [F][4], tvec [F][3] and cam_params [C][3] are indexed like the triangulation's inputs; the masks too
+    (None: nothing constant).  The refinement loop and its filters act on it as on a ResidentSolver; get_model()
+    compacts the surviving observations into tracks on the device.  num_images / num_cameras / num_observations are the
+    problem's sizes as created; num_alive() counts the observations still in the problem."""
+
+    def __init__(self, triangulation, qvec, tvec, cam_params, pose_constant=None, tvec_constant_mask=None,
+                 camera_constant=None):
+        self._h = C.c_void_p()
+        self._q = np.ascontiguousarray(qvec, np.float64).reshape(-1, 4)
+        self._t = np.ascontiguousarray(tvec, np.float64).reshape(-1, 3)
+        self._k = np.ascontiguousarray(cam_params, np.float64).reshape(-1, 3)
+        u8 = C.POINTER(C.c_uint8)
+        masks = [None if m is None else np.ascontiguousarray(m, np.uint8) for m in (pose_constant, tvec_constant_mask, camera_constant)]
+        for m, n in zip(masks, (len(self._q), len(self._q), len(self._k))):
+            if m is not None and m.shape != (n,):
+                raise ValueError("pose_constant / tvec_constant_mask need one entry per image, camera_constant per camera")
+        if len(self._t) != len(self._q):
+            raise ValueError("qvec and tvec must describe the same images")
+        F, Cn, M = C.c_int32(), C.c_int32(), C.c_int64()
+        _lib.check(_lib.lib().psfm_ba_create_from_triangulation(
+            triangulation.handle, _lib.dptr(self._q), _lib.dptr(self._t), _lib.dptr(self._k),
+            *(m.ctypes.data_as(u8) if m is not None else None for m in masks), C.byref(self._h), C.byref(F), C.byref(Cn),
+            C.byref(M)), "psfm_ba_create_from_triangulation")
+        self.num_images, self.num_cameras, self.num_observations = F.value, Cn.value, M.value
+        self.num_points = triangulation.num_points3D
+
+    # the entry points that only need the handle are ResidentSolver's
+    filter_negative_depth = ResidentSolver.filter_negative_depth
+    filter_points = ResidentSolver.filter_points
+    normalize = ResidentSolver.normalize
+    iterative_refinement = ResidentSolver.iterative_refinement
+    num_alive = ResidentSolver.num_observations
+    close = ResidentSolver.close
+    __del__ = ResidentSolver.__del__
+
+    def observation_mask(self):
+        """alive [num_observations] bool over the observations the problem was created with."""
+        m = np.zeros(self.num_observations, np.uint8)
+        _lib.check(_lib.lib().psfm_ba_get_observation_mask(self._h, m.ctypes.data_as(C.POINTER(C.c_uint8))),
+                   "psfm_ba_get_observation_mask")
+        return m.astype(bool)
+
+    def observations(self):
+        """The observations the problem was built with: obs_image [M] (problem image = rank among the registered
+        images), obs_point [M] (point row), obs_xy [M][2], point2D_idx [M]."""
+        M = self.num_observations
+        img, pt, p2d, xy = np.zeros(M, np.int32), np.zeros(M, np.int32), np.zeros(M, np.int32), np.zeros((M, 2))
+        ip = C.POINTER(C.c_int32)
+        _lib.check(_lib.lib().psfm_ba_get_observations(self._h, img.ctypes.data_as(ip), pt.ctypes.data_as(ip), _lib.dptr(xy),
+                                                       p2d.ctypes.data_as(ip)), "psfm_ba_get_observations")
+        return img, pt, xy, p2d
+
+    def point_errors(self):
+        e = np.zeros(self.num_points)
+        _lib.check(_lib.lib().psfm_ba_get_point_errors(self._h, _lib.dptr(e)), "psfm_ba_get_point_errors")
+        return e
+
+    def get_model(self, num_keypoints):
+        """TriangulationModel of the solver's current state; num_keypoints: the triangulation's K."""
+        P, M = self.num_points, self.num_observations
+        q, t, k = self._q.copy(), self._t.copy(), self._k.copy()
+        xyz, track_ptr = np.zeros((P, 3)), np.zeros(P + 1, np.int64)
+        ti, tp = np.zeros(M, np.int32), np.zeros(M, np.int32)
+        p3 = np.zeros(int(num_keypoints), np.int64)
+        ip, i64 = C.POINTER(C.c_int32), C.POINTER(C.c_int64)
+        _lib.check(_lib.lib().psfm_ba_get_model(self._h, _lib.dptr(q), _lib.dptr(t), _lib.dptr(k), _lib.dptr(xyz),
+                                                track_ptr.ctypes.data_as(i64), ti.ctypes.data_as(ip), tp.ctypes.data_as(ip),
+                                                p3.ctypes.data_as(i64)), "psfm_ba_get_model")
+        E = int(track_ptr[-1])
+        err = self.point_errors()
+        return TriangulationModel(qvec=q, tvec=t, cam_params=k, xyz=xyz, track_ptr=track_ptr, track_image=ti[:E].copy(),
+                                  track_point2D=tp[:E].copy(), point3D_of_keypoint=p3,
+                                  error=np.where(np.isnan(err), 0.0, err))

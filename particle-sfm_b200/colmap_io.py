@@ -138,3 +138,61 @@ def write_model(reconstruction, path):
     write_cameras_bin(reconstruction.cameras, os.path.join(path, "cameras.bin"))
     write_images_bin(reconstruction.images, os.path.join(path, "images.bin"))
     write_points3D_bin(reconstruction.points3D, os.path.join(path, "points3D.bin"))
+
+
+_PT_CHUNK = 1 << 16
+_PT_HDR = np.dtype([("id", "<i8"), ("xyz", "<f8", 3), ("rgb", "u1", 3), ("error", "<f8"), ("len", "<u8")])   # 51 bytes
+
+
+def write_model_arrays(path, camera_ids, camera_size, cam_params, image_ids, image_names, image_camera, qvec, tvec,
+                       keypoint_ptr, keypoints, point3D_ids, point_ids, xyz, error, track_ptr, track_image_ids,
+                       track_point2D, camera_model=0):
+    """cameras.bin, images.bin and points3D.bin from flat arrays, byte for byte what write_model writes for the
+    equivalent Reconstruction (cameras, images and points in array order, rgb 0).
+      cameras   camera_ids [C], camera_size [C][2] (width, height), cam_params [C][k] of `camera_model`
+      images    the images to write: image_ids [F], image_names [F], image_camera [F] (index into the cameras),
+                qvec [F][4], tvec [F][3], keypoint_ptr [F + 1] over keypoints [K][2] and point3D_ids [K] (-1: none)
+      points    point_ids [P], xyz [P][3], error [P], track_ptr [P + 1] over track_image_ids / track_point2D [E]
+    The per-observation and per-track-element bytes are laid out with numpy, without a loop over them."""
+    os.makedirs(path, exist_ok=True)
+    cam_params = np.asarray(cam_params, "<f8").reshape(len(camera_ids), -1)
+    with open(os.path.join(path, "cameras.bin"), "wb") as f:
+        f.write(struct.pack("<Q", len(camera_ids)))
+        for c in range(len(camera_ids)):
+            f.write(struct.pack("<iiQQ", int(camera_ids[c]), int(camera_model), int(camera_size[c][0]), int(camera_size[c][1])))
+            f.write(cam_params[c].tobytes())
+    kp_ptr = np.asarray(keypoint_ptr, np.int64)
+    obs = np.empty(kp_ptr[-1], _P2D)
+    kps = np.asarray(keypoints).reshape(-1, 2)
+    obs["x"], obs["y"], obs["id"] = kps[:, 0], kps[:, 1], point3D_ids
+    obs = obs.view(np.uint8).reshape(-1)
+    q, t = np.asarray(qvec, "<f8").reshape(-1, 4), np.asarray(tvec, "<f8").reshape(-1, 3)
+    with open(os.path.join(path, "images.bin"), "wb") as f:
+        f.write(struct.pack("<Q", len(image_ids)))
+        cam_ids = np.asarray(camera_ids)[np.asarray(image_camera, np.int64)] if len(image_ids) else []
+        for i in range(len(image_ids)):
+            lo, hi = int(kp_ptr[i]), int(kp_ptr[i + 1])
+            f.write(struct.pack("<i", int(image_ids[i])) + q[i].tobytes() + t[i].tobytes() + struct.pack("<i", int(cam_ids[i]))
+                    + image_names[i].encode("utf-8") + b"\x00" + struct.pack("<Q", hi - lo))
+            f.write(obs[24 * lo:24 * hi].tobytes())
+    P = len(point_ids)
+    tp = np.asarray(track_ptr, np.int64)
+    xyz = np.asarray(xyz).reshape(-1, 3)
+    with open(os.path.join(path, "points3D.bin"), "wb") as f:
+        f.write(struct.pack("<Q", P))
+        # points in chunks, so that the byte-placement indices stay bounded (8 B per output byte of one chunk: about
+        # 27 MB for the chunk's headers plus 64 B per track element) whatever the model's size
+        for a in range(0, P, _PT_CHUNK):
+            b = min(P, a + _PT_CHUNK)
+            lo, hi = int(tp[a]), int(tp[b])
+            hdr = np.zeros(b - a, _PT_HDR)
+            hdr["id"], hdr["xyz"], hdr["error"], hdr["len"] = point_ids[a:b], xyz[a:b], error[a:b], np.diff(tp[a:b + 1])
+            trk = np.empty(hi - lo, _TRK)
+            trk["image_id"], trk["point2D_idx"] = track_image_ids[lo:hi], track_point2D[lo:hi]
+            # within the chunk, point p's header starts at 51 p + 8 (track_ptr[p] - lo); element e at 51 (p + 1) + 8 e
+            out = np.empty(51 * (b - a) + 8 * (hi - lo), np.uint8)
+            h0 = 51 * np.arange(b - a, dtype=np.int64) + 8 * (tp[a:b] - lo)
+            out[(h0[:, None] + np.arange(51)).reshape(-1)] = hdr.view(np.uint8)
+            e0 = 51 * (np.repeat(np.arange(b - a, dtype=np.int64), np.diff(tp[a:b + 1])) + 1) + 8 * np.arange(hi - lo, dtype=np.int64)
+            out[(e0[:, None] + np.arange(8)).reshape(-1)] = trk.view(np.uint8)
+            f.write(out.tobytes())

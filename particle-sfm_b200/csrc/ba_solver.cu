@@ -23,6 +23,7 @@
 #include "ba_refine.cuh"
 #include "dist.cuh"
 #include "dense_chol.cuh"
+#include "triangulation_handle.cuh"
 
 namespace psfm {
 namespace ba {
@@ -122,6 +123,15 @@ struct psfm_ba_solver {
   DBuf<unsigned char> d_alive;
   DBuf<double> d_pt_error;       // [P_total] Point3D::Error of the last point filter (NaN: not set)
   DBuf<unsigned long long> d_count;
+  // a solver made by psfm_ba_create_from_triangulation: each problem image's and camera's index in the triangulation's
+  // arrays, each problem image's first keypoint, each observation's keypoint and the triangulation's points (the state
+  // of the points no observation keeps); psfm_ba_get_model writes the model back in the triangulation's layout
+  bool from_triangulation = false;
+  long long K_total = 0;
+  std::vector<int> img_map, cam_map;
+  std::vector<double> xyz0;
+  DBuf<int> d_in_kp, d_img_map;
+  DBuf<long long> d_img_kp0;
   // host structure / config
   std::vector<int> pt_orig;      // internal point -> caller's point id
   std::vector<int> obs_orig;     // sorted observation -> caller's observation index
@@ -240,21 +250,36 @@ double reduce_over_ranks(cudaStream_t st, double v, void (*op)(double*, size_t, 
   return h;
 }
 
-// Configuration and the caller's observations -> device (once per solver).
-int upload_problem(psfm_ba_solver* S, const psfm_ba_problem* pb) {
-  const int F = pb->num_images, Pt = pb->num_points, M = pb->num_observations, C = pb->num_cameras;
+// Sizes, cameras of the images and the config (host); the caller fills pose_constant / tvec_mask / camera_constant.
+int configure_problem(psfm_ba_solver* S, int F, int Pt, int M, int C, const int32_t* image_camera) {
   if (F <= 0 || C <= 0 || Pt < 0 || M < 0) { set_error("psfm_ba_create: bad sizes"); return PSFM_ERR_INVALID; }
   S->F = F; S->P_total = Pt; S->M = M; S->M0 = M; S->num_alive = M; S->C = C; S->NS = 6 * F + 3 * C; S->NB = 2 * F + C;
-  S->image_camera.assign(pb->image_camera, pb->image_camera + F);
+  S->image_camera.assign(image_camera, image_camera + F);
   for (int i = 0; i < F; ++i)
     if (S->image_camera[i] < 0 || S->image_camera[i] >= C) { set_error("image_camera out of range"); return PSFM_ERR_INVALID; }
   S->pose_constant.assign(F, 0); S->tvec_mask.assign(F, 0); S->camera_constant.assign(C, 0);
+  return PSFM_OK;
+}
+
+// The device side of the configuration and the alive mask, once the observations are on their way.
+void upload_config(psfm_ba_solver* S) {
+  cudaStream_t st = S->stream;
+  S->d_img_cam.alloc(S->F, st); S->d_img_cam.upload(S->image_camera.data(), S->F, st);
+  S->d_alive.alloc(S->M0, st);
+  PSFM_CUDA(cudaMemsetAsync(S->d_alive.p, 1, (size_t)(S->M0 ? S->M0 : 1), st));
+  S->d_count.alloc(1, st);
+}
+
+// Configuration and the caller's observations -> device (once per solver).
+int upload_problem(psfm_ba_solver* S, const psfm_ba_problem* pb) {
+  const int F = pb->num_images, M = pb->num_observations, C = pb->num_cameras;
+  const int rc = configure_problem(S, F, pb->num_points, M, C, pb->image_camera);
+  if (rc != PSFM_OK) return rc;
   if (pb->pose_constant) S->pose_constant.assign(pb->pose_constant, pb->pose_constant + F);
   if (pb->tvec_constant_mask) S->tvec_mask.assign(pb->tvec_constant_mask, pb->tvec_constant_mask + F);
   if (pb->camera_constant) S->camera_constant.assign(pb->camera_constant, pb->camera_constant + C);
   cudaStream_t st = S->stream;
-  S->d_img_cam.alloc(F, st); S->d_img_cam.upload(S->image_camera.data(), F, st);
-  S->d_in_img.alloc(M, st); S->d_in_pt.alloc(M, st); S->d_in_xy.alloc(M, st); S->d_alive.alloc(M, st);
+  S->d_in_img.alloc(M, st); S->d_in_pt.alloc(M, st); S->d_in_xy.alloc(M, st);
   S->d_in_img.upload(pb->obs_image, M, st); S->d_in_pt.upload(pb->obs_point, M, st);
   // the coordinates (half of the bytes) follow on the copy queue: counting, ordering and sorting need the
   // indices only, k_st_gather waits for ev_xy
@@ -262,8 +287,50 @@ int upload_problem(psfm_ba_solver* S, const psfm_ba_problem* pb) {
   PSFM_CUDA(cudaStreamWaitEvent(S->sh.copy, S->sh.ev_idx, 0));
   S->d_in_xy.upload(reinterpret_cast<const double2*>(pb->obs_xy), M, S->sh.copy);
   PSFM_CUDA(cudaEventRecord(S->sh.ev_xy, S->sh.copy));
-  PSFM_CUDA(cudaMemsetAsync(S->d_alive.p, 1, (size_t)(M ? M : 1), st));
-  S->d_count.alloc(1, st);
+  upload_config(S);
+  return PSFM_OK;
+}
+
+// The observations of a triangulation's registered images, built on the device (psfm_ba_create_from_triangulation).
+// Problem images are the registered images in ascending index, problem cameras the cameras they use in ascending
+// index: the layout ba.flatten gives Triangulation.to_reconstruction.
+int upload_triangulation(psfm_ba_solver* S, const psfm_triangulation* T, const uint8_t* pose_constant,
+                         const uint8_t* tvec_constant_mask, const uint8_t* camera_constant) {
+  std::vector<int> rank(T->F, -1), cam_rank(T->C, -1), image_camera;
+  for (int f = 0; f < T->F; ++f)
+    if (T->registered[f]) {
+      rank[f] = (int)S->img_map.size();
+      S->img_map.push_back(f);
+      cam_rank[T->image_camera[f]] = 0;
+    }
+  for (int c = 0; c < T->C; ++c)
+    if (cam_rank[c] == 0) { cam_rank[c] = (int)S->cam_map.size(); S->cam_map.push_back(c); }
+  for (int f : S->img_map) image_camera.push_back(cam_rank[T->image_camera[f]]);
+  const int F = (int)S->img_map.size(), C = (int)S->cam_map.size();
+  if (F == 0) { set_error("psfm_ba_create_from_triangulation: no registered image"); return PSFM_ERR_INVALID; }
+  if (T->P > 0x7fffffffLL) { set_error("psfm_ba_create_from_triangulation: 2^31 points or more"); return PSFM_ERR_UNSUPPORTED; }
+  cudaStream_t st = S->stream;
+  const long long M = triangulation_observations(T, rank.data(), st, S->d_in_img, S->d_in_pt, S->d_in_xy, S->d_in_kp);
+  const int rc = configure_problem(S, F, (int)T->P, (int)M, C, image_camera.data());
+  if (rc != PSFM_OK) return rc;
+  std::vector<long long> kp0(F);
+  for (int k = 0; k < F; ++k) {
+    const int f = S->img_map[k];
+    kp0[k] = T->h_kp_ptr[f];
+    if (pose_constant) S->pose_constant[k] = pose_constant[f];
+    if (tvec_constant_mask) S->tvec_mask[k] = tvec_constant_mask[f];
+  }
+  if (camera_constant)
+    for (int k = 0; k < C; ++k) S->camera_constant[k] = camera_constant[S->cam_map[k]];
+  S->from_triangulation = true;
+  S->K_total = T->K;
+  S->d_img_map.alloc(F, st); S->d_img_map.upload(S->img_map.data(), F, st);
+  S->d_img_kp0.alloc(F, st); S->d_img_kp0.upload(kp0.data(), F, st);
+  S->xyz0.resize(3 * (size_t)T->P);
+  if (T->P) PSFM_CUDA(cudaMemcpyAsync(S->xyz0.data(), T->xyz.p, sizeof(double) * S->xyz0.size(), cudaMemcpyDeviceToHost, st));
+  PSFM_CUDA(cudaEventRecord(S->sh.ev_xy, st));
+  upload_config(S);
+  PSFM_CUDA(cudaStreamSynchronize(st));
   return PSFM_OK;
 }
 
@@ -1519,6 +1586,34 @@ extern "C" void psfm_ba_global_options(psfm_ba_options* o) {
   o->loss_function_type = PSFM_LOSS_SOFT_L1;
 }
 
+namespace {
+
+void open_streams(psfm_ba_solver* S) {
+  PSFM_CUDA(cudaStreamCreateWithFlags(&S->sh.s, cudaStreamNonBlocking));
+  PSFM_CUDA(cudaStreamCreateWithFlags(&S->sh.copy, cudaStreamNonBlocking));
+  PSFM_CUDA(cudaEventCreateWithFlags(&S->sh.ev_idx, cudaEventDisableTiming));
+  PSFM_CUDA(cudaEventCreateWithFlags(&S->sh.ev_xy, cudaEventDisableTiming));
+  S->stream = S->sh.s;
+}
+
+// What both create entry points run once the observations are on the device: the structure, the state (qvec [F][4],
+// tvec [F][3], cam_params [C][3] in the problem's layout, xyz [P_total][3]) and the work buffers.
+int finish_create(psfm_ba_solver* S, const double* qvec, const double* tvec, const double* cam_params, const double* xyz) {
+  const int rc = build_structure(S);
+  if (rc != PSFM_OK) return rc;
+  S->h_qvec.assign(qvec, qvec + 4 * (size_t)S->F);
+  S->h_tvec.assign(tvec, tvec + 3 * (size_t)S->F);
+  S->h_K.assign(cam_params, cam_params + 3 * (size_t)S->C);
+  PhaseTimer tm;
+  alloc_work(S);
+  gather_points(S, xyz);
+  PSFM_CUDA(cudaStreamSynchronize(S->stream));
+  tm.mark("allocate work buffers");
+  return PSFM_OK;
+}
+
+}  // namespace
+
 extern "C" int psfm_ba_create(const psfm_ba_problem* pb, psfm_ba_solver** out) {
   if (!pb || !out) { set_error("psfm_ba_create: null argument"); return PSFM_ERR_INVALID; }
   *out = nullptr;
@@ -1526,28 +1621,193 @@ extern "C" int psfm_ba_create(const psfm_ba_problem* pb, psfm_ba_solver** out) {
   if (rc != PSFM_OK) return rc;
   psfm_ba_solver* S = new psfm_ba_solver();
   try {
-    PSFM_CUDA(cudaStreamCreateWithFlags(&S->sh.s, cudaStreamNonBlocking));
-    PSFM_CUDA(cudaStreamCreateWithFlags(&S->sh.copy, cudaStreamNonBlocking));
-    PSFM_CUDA(cudaEventCreateWithFlags(&S->sh.ev_idx, cudaEventDisableTiming));
-    PSFM_CUDA(cudaEventCreateWithFlags(&S->sh.ev_xy, cudaEventDisableTiming));
-    S->stream = S->sh.s;
+    open_streams(S);
     rc = upload_problem(S, pb);
-    if (rc == PSFM_OK) rc = build_structure(S);
+    if (rc == PSFM_OK) rc = finish_create(S, pb->qvec, pb->tvec, pb->cam_params, pb->xyz);
     if (rc != PSFM_OK) { delete S; return rc; }
-    S->h_qvec.assign(pb->qvec, pb->qvec + 4 * (size_t)S->F);
-    S->h_tvec.assign(pb->tvec, pb->tvec + 3 * (size_t)S->F);
-    S->h_K.assign(pb->cam_params, pb->cam_params + 3 * (size_t)S->C);
-    PhaseTimer tm;
-    alloc_work(S);
-    gather_points(S, pb->xyz);
-    PSFM_CUDA(cudaStreamSynchronize(S->stream));
-    tm.mark("allocate work buffers");
   } catch (const CudaFail& f) {
     delete S;
     return f.code;
   }
   *out = S;
   return PSFM_OK;
+}
+
+extern "C" int psfm_ba_create_from_triangulation(const psfm_triangulation* tri, const double* qvec, const double* tvec,
+                                                 const double* cam_params, const uint8_t* pose_constant,
+                                                 const uint8_t* tvec_constant_mask, const uint8_t* camera_constant,
+                                                 psfm_ba_solver** out, int32_t* num_images, int32_t* num_cameras,
+                                                 int64_t* num_observations) {
+  if (!tri || !qvec || !tvec || !cam_params || !out) {
+    set_error("psfm_ba_create_from_triangulation: null argument");
+    return PSFM_ERR_INVALID;
+  }
+  *out = nullptr;
+  int rc = check_device();
+  if (rc != PSFM_OK) return rc;
+  if (dist::world_size() > 1) {
+    set_error("psfm_ba_create_from_triangulation: a sharded problem is not supported");
+    return PSFM_ERR_UNSUPPORTED;
+  }
+  psfm_ba_solver* S = new psfm_ba_solver();
+  try {
+    open_streams(S);
+    rc = upload_triangulation(S, tri, pose_constant, tvec_constant_mask, camera_constant);
+    if (rc == PSFM_OK) {
+      std::vector<double> q(4 * (size_t)S->F), t(3 * (size_t)S->F), k(3 * (size_t)S->C);
+      for (int i = 0; i < S->F; ++i) {
+        const int f = S->img_map[i];
+        std::copy(qvec + 4 * (size_t)f, qvec + 4 * (size_t)f + 4, q.begin() + 4 * (size_t)i);
+        std::copy(tvec + 3 * (size_t)f, tvec + 3 * (size_t)f + 3, t.begin() + 3 * (size_t)i);
+      }
+      for (int i = 0; i < S->C; ++i)
+        std::copy(cam_params + 3 * (size_t)S->cam_map[i], cam_params + 3 * (size_t)S->cam_map[i] + 3, k.begin() + 3 * (size_t)i);
+      rc = finish_create(S, q.data(), t.data(), k.data(), S->xyz0.data());
+    }
+    if (rc != PSFM_OK) { delete S; return rc; }
+  } catch (const CudaFail& f) {
+    delete S;
+    return f.code;
+  }
+  if (num_images) *num_images = S->F;
+  if (num_cameras) *num_cameras = S->C;
+  if (num_observations) *num_observations = S->M0;
+  *out = S;
+  return PSFM_OK;
+}
+
+namespace {
+
+// key of every caller observation: its point while alive, P_total (sorts last) once filtered
+__global__ void k_model_keys(int M, int P, const unsigned char* __restrict__ alive, const int* __restrict__ pt,
+                             unsigned* __restrict__ key, int* __restrict__ val) {
+  const int m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  key[m] = alive[m] ? (unsigned)pt[m] : (unsigned)P;
+  val[m] = m;
+}
+
+// track_ptr by binary search over the sorted keys (track_ptr[P] = the number of alive observations); track elements
+// (triangulation image index, point2D_idx) and point3D_of_keypoint of the alive observations
+__global__ void k_model_tracks(int P, int M, const unsigned* __restrict__ key, const int* __restrict__ obs,
+                               const int* __restrict__ in_img, const int* __restrict__ in_kp,
+                               const int* __restrict__ img_map, const long long* __restrict__ img_kp0,
+                               long long* __restrict__ track_ptr, int* __restrict__ track_image,
+                               int* __restrict__ track_p2d, long long* __restrict__ kp_point) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i <= P) {
+    int lo = 0, hi = M;
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      if (key[mid] < (unsigned)i) lo = mid + 1;
+      else hi = mid;
+    }
+    track_ptr[i] = lo;
+  }
+  if (i < M && key[i] < (unsigned)P) {
+    const int m = obs[i], f = in_img[m], k = in_kp[m];
+    track_image[i] = img_map[f];
+    track_p2d[i] = (int)(k - img_kp0[f]);
+    kp_point[k] = key[i];
+  }
+}
+
+}  // namespace
+
+extern "C" int psfm_ba_get_model(psfm_ba_solver* S, double* qvec, double* tvec, double* cam_params, double* xyz,
+                                 int64_t* track_ptr, int32_t* track_image, int32_t* track_point2D,
+                                 int64_t* point3D_of_keypoint) {
+  if (!S || !qvec || !tvec || !cam_params || !xyz || !track_ptr || !track_image || !track_point2D || !point3D_of_keypoint) {
+    set_error("psfm_ba_get_model: null argument");
+    return PSFM_ERR_INVALID;
+  }
+  int rc = check_device();
+  if (rc != PSFM_OK) return rc;
+  if (!S->from_triangulation) {
+    set_error("psfm_ba_get_model: the solver was not made by psfm_ba_create_from_triangulation");
+    return PSFM_ERR_INVALID;
+  }
+  try {
+    cudaStream_t st = S->stream;
+    const int M = S->M0, P = S->P_total;
+    DBuf<unsigned> k0, k1;
+    DBuf<int> v0, v1;
+    DBuf<long long> d_ptr, d_kp;
+    DBuf<int> d_img, d_p2d;
+    k0.alloc(M, st); k1.alloc(M, st); v0.alloc(M, st); v1.alloc(M, st);
+    d_ptr.alloc((size_t)P + 1, st); d_kp.alloc(S->K_total, st); d_img.alloc(M, st); d_p2d.alloc(M, st);
+    if (S->K_total) PSFM_CUDA(cudaMemsetAsync(d_kp.p, 0xff, sizeof(long long) * (size_t)S->K_total, st));   // -1
+    if (M) {
+      k_model_keys<<<grid_for(M), 256, 0, st>>>(M, P, S->d_alive.p, S->d_in_pt.p, k0.p, v0.p);
+      PSFM_LAUNCH_CHECK();
+      int bits = 1;
+      while (bits < 32 && ((unsigned long long)P >> bits)) ++bits;
+      cub::DoubleBuffer<unsigned> keys(k0.p, k1.p);
+      cub::DoubleBuffer<int> vals(v0.p, v1.p);
+      size_t bytes = 0;
+      PSFM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys, vals, M, 0, bits, st));
+      DBuf<unsigned char> tmp;
+      tmp.alloc(bytes, st);
+      PSFM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, keys, vals, M, 0, bits, st));
+      PSFM_LAUNCH_CHECK();
+      k_model_tracks<<<grid_for(std::max(P + 1, M)), 256, 0, st>>>(P, M, keys.Current(), vals.Current(), S->d_in_img.p,
+                                                                   S->d_in_kp.p, S->d_img_map.p, S->d_img_kp0.p, d_ptr.p,
+                                                                   d_img.p, d_p2d.p, d_kp.p);
+      PSFM_LAUNCH_CHECK();
+    } else {
+      PSFM_CUDA(cudaMemsetAsync(d_ptr.p, 0, sizeof(long long) * ((size_t)P + 1), st));
+    }
+    d2h_sync(st, track_ptr, reinterpret_cast<const int64_t*>(d_ptr.p), (size_t)P + 1);
+    const long long E = track_ptr[P];
+    if (E) {
+      PSFM_CUDA(cudaMemcpyAsync(track_image, d_img.p, sizeof(int32_t) * (size_t)E, cudaMemcpyDeviceToHost, st));
+      PSFM_CUDA(cudaMemcpyAsync(track_point2D, d_p2d.p, sizeof(int32_t) * (size_t)E, cudaMemcpyDeviceToHost, st));
+    }
+    if (S->K_total)
+      PSFM_CUDA(cudaMemcpyAsync(point3D_of_keypoint, d_kp.p, sizeof(int64_t) * (size_t)S->K_total, cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaStreamSynchronize(st));
+  } catch (const CudaFail& f) { return f.code; }
+  for (int i = 0; i < S->F; ++i) {
+    const int f = S->img_map[i];
+    std::copy(S->h_qvec.begin() + 4 * (size_t)i, S->h_qvec.begin() + 4 * (size_t)i + 4, qvec + 4 * (size_t)f);
+    std::copy(S->h_tvec.begin() + 3 * (size_t)i, S->h_tvec.begin() + 3 * (size_t)i + 3, tvec + 3 * (size_t)f);
+  }
+  for (int i = 0; i < S->C; ++i)
+    std::copy(S->h_K.begin() + 3 * (size_t)i, S->h_K.begin() + 3 * (size_t)i + 3, cam_params + 3 * (size_t)S->cam_map[i]);
+  std::copy(S->xyz0.begin(), S->xyz0.end(), xyz);
+  scatter_points(S, xyz);
+  return PSFM_OK;
+}
+
+extern "C" int psfm_ba_get_observations(psfm_ba_solver* S, int32_t* obs_image, int32_t* obs_point, double* obs_xy,
+                                        int32_t* point2D_idx) {
+  if (!S) { set_error("psfm_ba_get_observations: null argument"); return PSFM_ERR_INVALID; }
+  const int rc = check_device();
+  if (rc != PSFM_OK) return rc;
+  if (point2D_idx && !S->from_triangulation) {
+    set_error("psfm_ba_get_observations: point2D_idx needs a solver made by psfm_ba_create_from_triangulation");
+    return PSFM_ERR_INVALID;
+  }
+  try {
+    cudaStream_t st = S->stream;
+    const size_t M = (size_t)S->M0;
+    PSFM_CUDA(cudaStreamWaitEvent(st, S->sh.ev_xy, 0));
+    std::vector<int> kp(point2D_idx ? M : 0), img(M);
+    if (M) {
+      PSFM_CUDA(cudaMemcpyAsync(img.data(), S->d_in_img.p, sizeof(int) * M, cudaMemcpyDeviceToHost, st));
+      if (obs_point) PSFM_CUDA(cudaMemcpyAsync(obs_point, S->d_in_pt.p, sizeof(int) * M, cudaMemcpyDeviceToHost, st));
+      if (obs_xy) PSFM_CUDA(cudaMemcpyAsync(obs_xy, S->d_in_xy.p, sizeof(double2) * M, cudaMemcpyDeviceToHost, st));
+      if (point2D_idx) PSFM_CUDA(cudaMemcpyAsync(kp.data(), S->d_in_kp.p, sizeof(int) * M, cudaMemcpyDeviceToHost, st));
+    }
+    PSFM_CUDA(cudaStreamSynchronize(st));
+    if (obs_image) std::copy(img.begin(), img.end(), obs_image);
+    if (point2D_idx) {
+      std::vector<long long> kp0(S->F);
+      PSFM_CUDA(cudaMemcpy(kp0.data(), S->d_img_kp0.p, sizeof(long long) * (size_t)S->F, cudaMemcpyDeviceToHost));
+      for (size_t m = 0; m < M; ++m) point2D_idx[m] = (int32_t)(kp[m] - kp0[img[m]]);
+    }
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return f.code; }
 }
 
 extern "C" int psfm_ba_set_state(psfm_ba_solver* S, const double* qvec, const double* tvec, const double* xyz,

@@ -27,7 +27,8 @@
 //               elements by point -> k_tracks -> k_kp_points
 // The launch count is fixed per call; no floating-point atomics (integer counters only): two calls are bit-identical.
 // Memory: the sort holds 24 bytes per directed entry (48 per match) with the matches (8) beside it; from the replay on,
-// 8 bytes per match (the neighbour lists) and about 70 bytes per keypoint stay resident.
+// 8 bytes per match (the neighbour lists) and about 70 bytes per keypoint stay resident.  The handle keeps 20 bytes per
+// keypoint (keypoint, image, point row) for psfm_ba_create_from_triangulation beside the points and tracks.
 #include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
@@ -39,6 +40,7 @@
 #include "dlt.cuh"
 #include "psfm_common.cuh"
 #include "quat.cuh"
+#include "triangulation_handle.cuh"
 #include "triangulation_recalled.cuh"
 
 namespace {
@@ -635,13 +637,59 @@ int bits_for(unsigned long long v) {
 
 }  // namespace
 
-struct psfm_triangulation {
-  long long P = 0, E = 0, K = 0;
-  psfm_triangulation_summary summary;
-  DBuf<double> xyz;
-  DBuf<long long> track_ptr, kp_points;
-  DBuf<int> track_image, track_p2d;
-};
+// ---- hand-off to the bundle adjustment (psfm_ba_create_from_triangulation) ------------------------------------------
+namespace {
+
+// flag[k] = 1 when keypoint k lies in a registered image and has a point; flag[K] stays 0 for the scan's total
+__global__ void k_obs_flag(long long K, const long long* __restrict__ kp_points, const int* __restrict__ img_of,
+                           const int* __restrict__ rank, int* __restrict__ flag) {
+  const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  flag[k] = (kp_points[k] >= 0 && rank[img_of[k]] >= 0) ? 1 : 0;
+}
+
+__global__ void k_obs_scatter(long long K, const int* __restrict__ flag, const int* __restrict__ pos,
+                              const long long* __restrict__ kp_points, const int* __restrict__ img_of,
+                              const int* __restrict__ rank, const float2* __restrict__ kps, int* __restrict__ obs_image,
+                              int* __restrict__ obs_point, double2* __restrict__ obs_xy, int* __restrict__ obs_kp) {
+  const long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (k >= K || !flag[k]) return;
+  const int m = pos[k];
+  const float2 x = kps[k];
+  obs_image[m] = rank[img_of[k]];
+  obs_point[m] = (int)kp_points[k];
+  obs_xy[m] = make_double2((double)x.x, (double)x.y);
+  obs_kp[m] = (int)k;
+}
+
+}  // namespace
+
+long long psfm::triangulation_observations(const psfm_triangulation* h, const int* image_rank, cudaStream_t st,
+                                           DBuf<int>& obs_image, DBuf<int>& obs_point, DBuf<double2>& obs_xy,
+                                           DBuf<int>& obs_kp) {
+  const long long K = h->K;
+  DBuf<int> rank, flag, pos;
+  rank.alloc(h->F, st); flag.alloc(K + 1, st); pos.alloc(K + 1, st);
+  rank.upload(image_rank, h->F, st);
+  flag.zero(st);
+  if (K) { k_obs_flag<<<grid_of(K), 256, 0, st>>>(K, h->kp_points.p, h->img_of.p, rank.p, flag.p); PSFM_LAUNCH_CHECK(); }
+  size_t bytes = 0;
+  PSFM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, flag.p, pos.p, K + 1, st));
+  DBuf<unsigned char> tmp;
+  tmp.alloc(bytes, st);
+  PSFM_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, flag.p, pos.p, K + 1, st));
+  PSFM_LAUNCH_CHECK();
+  int M = 0;
+  PSFM_CUDA(cudaMemcpyAsync(&M, pos.p + K, sizeof(int), cudaMemcpyDeviceToHost, st));
+  PSFM_CUDA(cudaStreamSynchronize(st));
+  obs_image.alloc(M, st); obs_point.alloc(M, st); obs_xy.alloc(M, st); obs_kp.alloc(M, st);
+  if (K) {
+    k_obs_scatter<<<grid_of(K), 256, 0, st>>>(K, flag.p, pos.p, h->kp_points.p, h->img_of.p, rank.p, h->kps.p, obs_image.p,
+                                              obs_point.p, obs_xy.p, obs_kp.p);
+    PSFM_LAUNCH_CHECK();
+  }
+  return M;
+}
 
 extern "C" void psfm_triangulator_default_options(psfm_triangulator_options* o) {
   if (!o) return;
@@ -758,9 +806,16 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
       cudaEvent_t* e;
       ~EvFree() { for (int i = 0; i < 5; ++i) cudaEventDestroy(e[i]); }
     } ev_free{ev};
-    DBuf<long long> d_kp_ptr, d_iptr, d_list_ptr;
-    DBuf<float2> d_kps;
-    DBuf<int> d_cam_of, d_img_of, d_pt_of, d_parent, d_deg, d_first, d_nbr;
+    // the keypoints, their images and keypoint_ptr stay with the handle for psfm_ba_create_from_triangulation
+    DBuf<long long>& d_kp_ptr = h->kp_ptr;
+    DBuf<float2>& d_kps = h->kps;
+    DBuf<int>& d_img_of = h->img_of;
+    h->F = F; h->C = num_cameras;
+    h->h_kp_ptr.assign(keypoint_ptr, keypoint_ptr + F + 1);
+    h->image_camera.assign(image_camera, image_camera + F);
+    h->registered.assign(registered, registered + F);
+    DBuf<long long> d_iptr, d_list_ptr;
+    DBuf<int> d_cam_of, d_pt_of, d_parent, d_deg, d_first, d_nbr;
     DBuf<int2> d_pairs;
     DBuf<uint2> d_m;
     DBuf<double> d_cams, d_img;
