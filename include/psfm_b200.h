@@ -763,6 +763,22 @@ int psfm_measure_dfma(double* dfma_per_second, double* dependent_latency_cycles)
    nb / 6 does too. */
 int psfm_ba_band_solve(const double* A, const double* b, int32_t nb, int32_t bw, double* x);
 
+/* Test entries of the blocked dense Cholesky (k_chol_blocked, csrc/ba_schur_explicit.cuh) and of the two solvers that
+   reuse its factor.  A is [n][n] row-major and symmetric; only its lower triangle is read.  Each returns PSFM_OK,
+   PSFM_ERR_INVALID on a bad argument or when a pivot is not positive (psfm_last_error says which), PSFM_ERR_NO_DEVICE
+   without a device; argument checks come first.
+   psfm_blocked_cholesky_solve: x [ns] = A^-1 b, ns = n, with the bundle adjustment's dense-S launch.  The first nb
+     rows form a band, A[i][j] == 0 for i - j > bw there (CholArgs::bw); rows nb .. ns - 1 are dense (the arrow).
+     nb = bw = ns is a dense matrix and goes through dense_cholesky_launch.  max_ctas > 0 caps the cooperative grid,
+     0 keeps the solver's grid.
+   psfm_laplacian_solve: X [n][3] = A^-1 B for three interleaved right-hand sides B [n][3], the rotation averaging's
+     factor-then-k_trsv.
+   psfm_spd_inverse: X = A^-1 by the position estimation's k_pos_inverse; column j at X + j n. */
+int psfm_blocked_cholesky_solve(const double* A, const double* b, int32_t ns, int32_t nb, int32_t bw, int32_t max_ctas,
+                                double* x);
+int psfm_laplacian_solve(const double* A, const double* B, int32_t n, double* X);
+int psfm_spd_inverse(const double* A, int32_t n, double* X);
+
 /* ------------------------------------------------------------------------- */
 /* Multi-GPU (HP2): points sharded across ranks, one all-reduce of the         */
 /* camera-side vector per PCG step (SURVEY.md §8e).                            */

@@ -29,6 +29,7 @@ EXPORTS = [
     "psfm_optimize_pairwise_translations", "psfm_lud_default_options", "psfm_estimate_global_positions",
     "psfm_triangulator_default_options", "psfm_triangulation_create", "psfm_triangulation_result",
     "psfm_triangulation_destroy", "psfm_verification_default_options", "psfm_verify_two_view_geometries",
+    "psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse",
     "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
@@ -140,6 +141,9 @@ def lib():
     L.psfm_ba_get_model.argtypes = [vp, dp, dp, dp, dp, i64p, ip, ip, i64p]
     L.psfm_ba_get_observations.argtypes = [vp, ip, ip, dp, ip]
     L.psfm_ba_band_solve.argtypes = [dp, dp, C.c_int32, C.c_int32, dp]
+    L.psfm_blocked_cholesky_solve.argtypes = [dp, dp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, dp]
+    L.psfm_laplacian_solve.argtypes = [dp, dp, C.c_int32, dp]
+    L.psfm_spd_inverse.argtypes = [dp, C.c_int32, dp]
     L.psfm_dist_get_unique_id.argtypes = [C.POINTER(C.c_uint8)]
     L.psfm_dist_init.argtypes = [C.POINTER(C.c_uint8), C.c_int32, C.c_int32]
     L.psfm_dist_finalize.restype = None

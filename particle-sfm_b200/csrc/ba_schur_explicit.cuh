@@ -879,8 +879,11 @@ __device__ __noinline__ bool chol_diag_warp(const double* __restrict__ A, int ld
   for (int j = 0; j < CB; ++j) {
     const double d = __shfl_sync(0xffffffffu, arow[j], j);
     if (!(d > 0.0) || isinf(d)) bad = true;
-    const double idj = rsqrt(d);
-    if (lane == j) { arow[j] = d * idj; myinv = idj; }
+    // L_jj = sqrt(d) correctly rounded and its reciprocal, as LAPACK's potf2 scales a column: d * rsqrt(d) is not
+    // correctly rounded and disagrees with the reciprocal it scales by, which cost up to 9x LAPACK's forward error
+    // on ill-conditioned Laplacians (tests/test_gpu_dense_chol.py)
+    const double ljj = sqrt(d), idj = 1.0 / ljj;
+    if (lane == j) { arow[j] = ljj; myinv = idj; }
     else if (lane > j) arow[j] = arow[j] * idj;
     const double lr = arow[j];
 #pragma unroll

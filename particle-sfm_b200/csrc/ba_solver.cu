@@ -1152,6 +1152,22 @@ int chol_grid_limit() {
   return grid_limit_by_dev[dev];
 }
 
+// rows of Lp that k_chol_blocked fills per panel for ns unknowns whose first nb rows have band width bw
+// (CholArgs::bw): the band rows, the arrow rows and the rhs row, plus one row of slack
+int chol_blocked_rmax(int ns, int nb, int bw) { return std::min(bw, nb) + (ns + 1 - nb) + 1; }
+
+// one cooperative launch of k_chol_blocked on ca (ca.bar zeroed before): one CTA per trailing tile pair of the first
+// panel up to one per SM, so few CTAs when the band is narrow (cheaper grid barriers) and all SMs for a dense system.
+// max_ctas > 0 caps the grid further (tests: the result must not depend on it).
+void launch_chol_blocked(const CholArgs& ca, cudaStream_t st, int max_ctas = 0) {
+  const int tiles = (std::min(ca.bw + 1, ca.nb) + (ca.ns + 1 - ca.nb) + CB - 1) / CB;
+  int grid = std::max(1, std::min(chol_grid_limit(), tiles * (tiles + 1) / 2));
+  if (max_ctas > 0) grid = std::min(grid, max_ctas);
+  void* kargs[] = {(void*)&ca};
+  PSFM_CUDA(cudaLaunchCooperativeKernel((void*)k_chol_blocked, dim3(grid), dim3(256), kargs, 0, st));
+  PSFM_LAUNCH_CHECK();
+}
+
 // blocked band(+arrow) Cholesky of d_S (rhs carried as the extra row) -> d_x; d_cholfail[0] = 1 on a
 // bad pivot (read back with the step scalars at the end of compute_step: no host sync here)
 void launch_cholesky(psfm_ba_solver* S) {
@@ -1159,7 +1175,6 @@ void launch_cholesky(psfm_ba_solver* S) {
   const int nbnd = 6 * S->F;
   const int bw = std::min(S->bw, nbnd);
   {
-    const int grid_limit = chol_grid_limit();
     CholArgs ca;
     ca.A = S->d_S.p; ca.ns = S->NS; ca.lda = S->NS + 1; ca.nb = nbnd; ca.bw = bw + 1; ca.x = S->d_x.p; ca.fail = S->d_cholfail.p;
     if (S->d_cholbar.n == 0) S->d_cholbar.alloc(1, st);
@@ -1167,17 +1182,12 @@ void launch_cholesky(psfm_ba_solver* S) {
     ca.bar = S->d_cholbar.p;
     {
       const int npanel = (S->NS + CB - 1) / CB;
-      const int rmax = std::min(bw + 1, nbnd) + (S->NS + 1 - nbnd) + 1;
+      const int rmax = chol_blocked_rmax(ca.ns, ca.nb, ca.bw);
       if (S->d_cholLp.n < (size_t)npanel * rmax * CB) S->d_cholLp.alloc((size_t)npanel * rmax * CB, st);
       if (S->d_cholLd.n < (size_t)npanel * CB * CB) S->d_cholLd.alloc((size_t)npanel * CB * CB, st);
       ca.Lp = S->d_cholLp.p; ca.Ld = S->d_cholLd.p; ca.rmax = rmax;
     }
-    void* kargs[] = {(void*)&ca};
-    // few CTAs when the band is narrow (cheaper grid barriers), all SMs for a dense system
-    const int tiles = (std::min(bw + 2, nbnd) + (S->NS + 1 - nbnd) + CB - 1) / CB;
-    const int grid = std::max(1, std::min(grid_limit, tiles * (tiles + 1) / 2));
-    PSFM_CUDA(cudaLaunchCooperativeKernel((void*)k_chol_blocked, dim3(grid), dim3(256), kargs, 0, st));
-    PSFM_LAUNCH_CHECK();
+    launch_chol_blocked(ca, st);
   }
   { cudaEvent_t e = S->events.get(); PSFM_CUDA(cudaEventRecord(e, st)); S->ev_chol.back().second = e; }
 }
@@ -2240,14 +2250,56 @@ extern "C" int psfm_ba_linear_step(psfm_ba_solver* S, const psfm_ba_options* opt
 // dense_chol.cuh: k_chol_blocked on a whole dense system, launched the way launch_cholesky launches it for dense S
 // (nb = ns, a band as wide as the matrix: every row below a panel is a band row, the rhs row is the only arrow row)
 void psfm::dense_cholesky_launch(double* A, int ns, double* x, int* fail, unsigned int* bar, double* Lp, double* Ld,
-                                 cudaStream_t st) {
+                                 cudaStream_t st, int max_ctas) {
   CholArgs ca;
   ca.A = A; ca.ns = ns; ca.lda = ns + 1; ca.nb = ns; ca.bw = ns; ca.x = x; ca.fail = fail; ca.bar = bar;
   ca.Lp = Lp; ca.Ld = Ld; ca.rmax = dense_chol_rmax(ns);
   PSFM_CUDA(cudaMemsetAsync(bar, 0, sizeof(unsigned int), st));
-  void* kargs[] = {(void*)&ca};
-  const int tiles = (ns + 1 + CB - 1) / CB;
-  const int grid = std::max(1, std::min(chol_grid_limit(), tiles * (tiles + 1) / 2));
-  PSFM_CUDA(cudaLaunchCooperativeKernel((void*)k_chol_blocked, dim3(grid), dim3(256), kargs, 0, st));
-  PSFM_LAUNCH_CHECK();
+  launch_chol_blocked(ca, st, max_ctas);
+}
+
+// test entry: k_chol_blocked and its back substitution on one band(+arrow) system, through the launch the solver uses
+// (dense_cholesky_launch when the band covers the whole matrix)
+extern "C" int psfm_blocked_cholesky_solve(const double* A, const double* b, int32_t ns, int32_t nb, int32_t bw,
+                                           int32_t max_ctas, double* x) {
+  if (!A || !b || !x) { set_error("psfm_blocked_cholesky_solve: null argument"); return PSFM_ERR_INVALID; }
+  if (ns < 1 || ns > 32767 || nb < 1 || nb > ns || bw < 0 || max_ctas < 0) {
+    set_error("psfm_blocked_cholesky_solve: needs 1 <= nb <= ns <= 32767, bw >= 0 and max_ctas >= 0");
+    return PSFM_ERR_INVALID;
+  }
+  int rc = check_device();
+  if (rc != PSFM_OK) return rc;
+  bw = std::min(bw, nb);             // the kernel's band ends at row nb whatever bw says
+  try {
+    cudaStream_t st = nullptr;
+    const int lda = ns + 1, npanel = dense_chol_panels(ns);
+    const bool dense = nb == ns && bw == ns;
+    const int rmax = dense ? dense_chol_rmax(ns) : chol_blocked_rmax(ns, nb, bw);
+    DBuf<double> dA, dx, dLp, dLd;
+    DBuf<int> dfail;
+    DBuf<unsigned int> dbar;
+    dA.alloc((size_t)lda * lda); dx.alloc(ns); dLp.alloc((size_t)npanel * rmax * CB); dLd.alloc((size_t)npanel * CB * CB);
+    dfail.alloc(1); dbar.alloc(1);
+    dA.zero(st); dfail.zero(st);
+    // A's rows at leading dimension ns + 1, b as row ns
+    PSFM_CUDA(cudaMemcpy2DAsync(dA.p, sizeof(double) * lda, A, sizeof(double) * ns, sizeof(double) * ns, ns,
+                                cudaMemcpyHostToDevice, st));
+    PSFM_CUDA(cudaMemcpyAsync(dA.p + (size_t)ns * lda, b, sizeof(double) * ns, cudaMemcpyHostToDevice, st));
+    if (dense) {
+      dense_cholesky_launch(dA.p, ns, dx.p, dfail.p, dbar.p, dLp.p, dLd.p, st, max_ctas);
+    } else {
+      CholArgs ca;
+      ca.A = dA.p; ca.ns = ns; ca.lda = lda; ca.nb = nb; ca.bw = bw; ca.x = dx.p; ca.fail = dfail.p; ca.bar = dbar.p;
+      ca.Lp = dLp.p; ca.Ld = dLd.p; ca.rmax = rmax;
+      dbar.zero(st);
+      launch_chol_blocked(ca, st, max_ctas);
+    }
+    int fail = 0;
+    PSFM_CUDA(cudaMemcpy(&fail, dfail.p, sizeof(int), cudaMemcpyDeviceToHost));
+    if (fail) { set_error("psfm_blocked_cholesky_solve: matrix is not positive definite"); return PSFM_ERR_INVALID; }
+    PSFM_CUDA(cudaMemcpy(x, dx.p, sizeof(double) * ns, cudaMemcpyDeviceToHost));
+    return PSFM_OK;
+  } catch (const CudaFail& f) {
+    return f.code;
+  }
 }

@@ -18,8 +18,9 @@ __host__ __device__ inline int dense_chol_panels(int ns) { return (ns + kDenseCh
 //   L[i][c0 + k] = Ld[(p * 32 + (i - c0)) * 32 + k]          for c0 <= i < c1   (Ld: [panels][32][32], lower)
 //   L[i][c0 + k] = Lp[(p * rmax + (i - c1)) * 32 + k]        for c1 <= i < ns   (Lp: [panels][rmax][32])
 // Ld and Lp hold dense_chol_panels(ns) * 32 * 32 and dense_chol_panels(ns) * dense_chol_rmax(ns) * 32 doubles.
-// One cooperative launch on stream st, counted by launch_count().
+// One cooperative launch on stream st, counted by launch_count().  max_ctas > 0 caps its grid (tests only: the result
+// does not depend on the grid).
 void dense_cholesky_launch(double* A, int ns, double* x, int* fail, unsigned int* bar, double* Lp, double* Ld,
-                           cudaStream_t st);
+                           cudaStream_t st, int max_ctas = 0);
 
 }  // namespace psfm

@@ -536,3 +536,40 @@ extern "C" int psfm_estimate_global_positions(int32_t num_images, int64_t num_pa
   }
   return finish(PSFM_OK);
 }
+
+// test entry: the stage's explicit inverse of one SPD matrix, dense_cholesky_launch then k_pos_inverse, failure through
+// Ctl.failed
+extern "C" int psfm_spd_inverse(const double* A, int32_t n, double* X) {
+  if (!A || !X) { set_error("psfm_spd_inverse: null argument"); return PSFM_ERR_INVALID; }
+  if (n < 1 || n > kMaxUnknowns) {
+    set_error("psfm_spd_inverse: needs 1 <= n <= 8190 (the stage's bound)");
+    return PSFM_ERR_INVALID;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    set_error("psfm_spd_inverse: no CUDA device available (this library has no CPU path)");
+    return PSFM_ERR_NO_DEVICE;
+  }
+  try {
+    const int lda = n + 1, np = dense_chol_panels(n), rmax = dense_chol_rmax(n);
+    DBuf<double> d_S, d_xc, d_Lp, d_Ld, d_X;
+    DBuf<int> d_fail;
+    DBuf<unsigned int> d_bar;
+    DBuf<Ctl> d_ctl;
+    d_S.alloc((size_t)lda * lda); d_xc.alloc(n); d_Lp.alloc((size_t)np * rmax * kDenseCholBlock);
+    d_Ld.alloc((size_t)np * kDenseCholBlock * kDenseCholBlock); d_X.alloc((size_t)n * n);
+    d_fail.alloc(1); d_bar.alloc(1); d_ctl.alloc(1);
+    d_S.zero(nullptr); d_ctl.zero(nullptr);
+    PSFM_CUDA(cudaMemcpy2DAsync(d_S.p, sizeof(double) * lda, A, sizeof(double) * n, sizeof(double) * n, n,
+                                cudaMemcpyHostToDevice, nullptr));
+    dense_cholesky_launch(d_S.p, n, d_xc.p, d_fail.p, d_bar.p, d_Lp.p, d_Ld.p, nullptr);
+    k_pos_inverse<<<(n + kInvCols - 1) / kInvCols, 256>>>(n, d_Ld.p, d_Lp.p, d_X.p, d_fail.p, d_ctl.p);
+    PSFM_LAUNCH_CHECK();
+    Ctl h;
+    PSFM_CUDA(cudaMemcpy(&h, d_ctl.p, sizeof(Ctl), cudaMemcpyDeviceToHost));
+    if (h.failed) { set_error("psfm_spd_inverse: matrix is not positive definite"); return PSFM_ERR_INVALID; }
+    PSFM_CUDA(cudaMemcpy(X, d_X.p, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost));
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return f.code; }
+}

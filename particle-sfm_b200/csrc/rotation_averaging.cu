@@ -629,3 +629,40 @@ extern "C" int psfm_estimate_global_rotations(int32_t num_images, int64_t num_pa
   sm.device_ms = ms(t1, t2);
   return finish(PSFM_OK);
 }
+
+// test entry: the stage's x update on one SPD matrix, dense_cholesky_launch then k_trsv, failure through Ctl.failed
+extern "C" int psfm_laplacian_solve(const double* A, const double* B, int32_t n, double* X) {
+  if (!A || !B || !X) { set_error("psfm_laplacian_solve: null argument"); return PSFM_ERR_INVALID; }
+  if (n < 1 || n > kMaxComponentImages - 1) {
+    set_error("psfm_laplacian_solve: needs 1 <= n <= 8191 (the stage's bound)");
+    return PSFM_ERR_INVALID;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
+    cudaGetLastError();
+    set_error("psfm_laplacian_solve: no CUDA device available (this library has no CPU path)");
+    return PSFM_ERR_NO_DEVICE;
+  }
+  try {
+    const int lda = n + 1, np = dense_chol_panels(n), rmax = dense_chol_rmax(n);
+    DBuf<double> d_A, d_b, d_x, d_xc, d_Lp, d_Ld;
+    DBuf<int> d_fail, d_skip;
+    DBuf<unsigned int> d_bar;
+    DBuf<Ctl> d_ctl;
+    d_A.alloc((size_t)lda * lda); d_b.alloc(3 * (size_t)n); d_x.alloc(3 * (size_t)n); d_xc.alloc(n);
+    d_Lp.alloc((size_t)np * rmax * kDenseCholBlock); d_Ld.alloc((size_t)np * kDenseCholBlock * kDenseCholBlock);
+    d_fail.alloc(1); d_skip.alloc(1); d_bar.alloc(1); d_ctl.alloc(1);
+    d_A.zero(nullptr); d_skip.zero(nullptr); d_ctl.zero(nullptr);
+    PSFM_CUDA(cudaMemcpy2DAsync(d_A.p, sizeof(double) * lda, A, sizeof(double) * n, sizeof(double) * n, n,
+                                cudaMemcpyHostToDevice, nullptr));
+    d_b.upload(B, 3 * (size_t)n, nullptr);
+    dense_cholesky_launch(d_A.p, n, d_xc.p, d_fail.p, d_bar.p, d_Lp.p, d_Ld.p, nullptr);
+    k_trsv<<<1, 1024>>>(n, d_Ld.p, d_Lp.p, d_b.p, d_x.p, d_fail.p, d_ctl.p, d_skip.p);
+    PSFM_LAUNCH_CHECK();
+    Ctl h;
+    PSFM_CUDA(cudaMemcpy(&h, d_ctl.p, sizeof(Ctl), cudaMemcpyDeviceToHost));
+    if (h.failed) { set_error("psfm_laplacian_solve: matrix is not positive definite"); return PSFM_ERR_INVALID; }
+    PSFM_CUDA(cudaMemcpy(X, d_x.p, sizeof(double) * 3 * (size_t)n, cudaMemcpyDeviceToHost));
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return f.code; }
+}

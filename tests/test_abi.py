@@ -65,6 +65,69 @@ def test_no_cpu_fallback():
         ba.solve_problem(prob, o)
 
 
+def _dense_chol_entries(A, b, ns, nb, bw, max_ctas, only=None):
+    """The three dense-Cholesky test entries (those named in `only`, default all) on the same arguments: (name,
+    status, psfm_last_error).  The outputs are sized for A; a call with a larger ns must be refused before it reads
+    or writes anything."""
+    L = _lib.lib()
+    m = max(A.shape[0] if A is not None else ns, 1)
+    x, X3, Xi = np.zeros(m), np.zeros((m, 3)), np.zeros((m, m))
+    B = None if b is None else np.ascontiguousarray(np.repeat(b[:, None], 3, axis=1))
+    out = []
+    for name, call in (
+            ("psfm_blocked_cholesky_solve",
+             lambda: L.psfm_blocked_cholesky_solve(_lib.dptr(A), _lib.dptr(b), ns, nb, bw, max_ctas, _lib.dptr(x))),
+            ("psfm_laplacian_solve", lambda: L.psfm_laplacian_solve(_lib.dptr(A), _lib.dptr(B), ns, _lib.dptr(X3))),
+            ("psfm_spd_inverse", lambda: L.psfm_spd_inverse(_lib.dptr(A), ns, _lib.dptr(Xi)))):
+        if only is None or name in only:
+            rc = call()
+            out.append((name, rc, L.psfm_last_error().decode()))
+    return out
+
+
+# (change to the good arguments A = I4, b = 1, ns = nb = bw = 4, max_ctas = 0; the entries that must refuse it)
+DENSE_CHOL_BAD = {
+    "null_A": (dict(A=None), {"psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse"}),
+    "null_b": (dict(b=None), {"psfm_blocked_cholesky_solve", "psfm_laplacian_solve"}),
+    "n0": (dict(ns=0, nb=0), {"psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse"}),
+    "nb0": (dict(nb=0), {"psfm_blocked_cholesky_solve"}),
+    "nb_above_ns": (dict(nb=5), {"psfm_blocked_cholesky_solve"}),
+    "bw_negative": (dict(bw=-1), {"psfm_blocked_cholesky_solve"}),
+    "max_ctas_negative": (dict(max_ctas=-1), {"psfm_blocked_cholesky_solve"}),
+    # above the position stage's 8,190 unknowns, the rotation stage's 8,191, and the solver entry's 32,767
+    "n8191": (dict(ns=8191, nb=8191, bw=8191), {"psfm_spd_inverse"}),
+    "n8192": (dict(ns=8192, nb=8192, bw=8192), {"psfm_laplacian_solve", "psfm_spd_inverse"}),
+    "n32768": (dict(ns=32768, nb=32768, bw=32768),
+               {"psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse"}),
+}
+
+
+@pytest.mark.parametrize("case", list(DENSE_CHOL_BAD))
+def test_dense_chol_entries_check_arguments_before_the_device(case):
+    """Bad arguments are PSFM_ERR_INVALID, named in psfm_last_error, on any machine and before any launch."""
+    args = dict(A=np.eye(4), b=np.ones(4), ns=4, nb=4, bw=4, max_ctas=0)
+    change, refused = DENSE_CHOL_BAD[case]
+    args.update(change)
+    n0 = _lib.lib().psfm_launch_count()
+    too_large = case in ("n8191", "n8192", "n32768")       # only the entries that must refuse the size are called
+    for name, rc, msg in _dense_chol_entries(**args, only=refused if too_large else None):
+        if name in refused:
+            assert rc == _abi.PSFM_ERR_INVALID and msg.startswith(name + ":"), (name, rc, msg)
+        else:
+            assert rc in (_abi.PSFM_OK, _abi.PSFM_ERR_NO_DEVICE), (name, rc, msg)
+    if _lib.lib().psfm_device_count() == 0:
+        assert _lib.lib().psfm_launch_count() == n0
+
+
+@pytest.mark.skipif(_lib.lib().psfm_device_count() > 0, reason="needs a machine WITHOUT a GPU")
+def test_no_cpu_fallback_of_the_dense_chol_entries():
+    for name, rc, msg in _dense_chol_entries(np.eye(4), np.ones(4), 4, 4, 4, 0):
+        assert rc == _abi.PSFM_ERR_NO_DEVICE and "no CUDA device" in msg, (name, rc, msg)
+    for name, rc, msg in _dense_chol_entries(np.eye(40), np.ones(40), 40, 37, 5, 2):      # the band route too
+        if name == "psfm_blocked_cholesky_solve":
+            assert rc == _abi.PSFM_ERR_NO_DEVICE, (rc, msg)
+
+
 @pytest.mark.skipif(_lib.lib().psfm_device_count() > 0, reason="needs a machine WITHOUT a GPU")
 def test_no_cpu_fallback_of_the_initialisation_ops():
     """SURVEY.md 8(f) f-4 ops: host-side argument checks come first, then the library refuses without a device."""

@@ -17,6 +17,10 @@ FIXTURES = {
     "complete_200": dict(num_images=200, direction_noise_deg=1.0, direction_outlier_fraction=0.1, seed=5),
     "unused_pairs": dict(num_images=40, graph="banded", band=6, direction_noise_deg=0.5, seed=4),
     "outliers_stops_mid_chunk": dict(num_images=30, direction_noise_deg=1.0, direction_outlier_fraction=0.2, seed=1),
+    # long videos: S of 2,997 unknowns, and of 8,190 at the accepted bound of 2,731 views.  Seed 2 keeps every stopping
+    # test at least 1e-2 relative away from its bound at both sizes.
+    "banded_1000": dict(num_images=1000, graph="banded", band=10, direction_noise_deg=0.5, seed=2),
+    "banded_2731": dict(num_images=2731, graph="banded", band=10, direction_noise_deg=0.5, seed=2),
 }
 # With the default options only two_images passes the stopping test (at its first iteration); these options make it
 # fire at iteration 702, 30 iterations into a chunk of 32, so the test decides the count and the done flag must stop

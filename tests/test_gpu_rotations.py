@@ -16,6 +16,10 @@ FIXTURES = {
                            seed=4),
     "two_images": dict(num_images=2, noise_deg=0.3, seed=3),
     "complete_200": dict(num_images=200, noise_deg=1.0, outlier_fraction=0.1, seed=5),
+    # long videos: dense Laplacians of 999 and 1,999 unknowns (k_chol_blocked's pair loop wraps the grid).  Seed 2
+    # keeps every pair's residual at least 1e-2 rad away from the 5 degree filter threshold at both sizes.
+    "banded_1000": dict(num_images=1000, graph="banded", band=10, noise_deg=0.5, seed=2),
+    "banded_2000": dict(num_images=2000, graph="banded", band=10, noise_deg=0.5, seed=2),
 }
 
 
