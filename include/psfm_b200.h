@@ -748,6 +748,47 @@ int psfm_ba_get_model(psfm_ba_solver* s, double* qvec, double* tvec, double* cam
 int psfm_ba_get_observations(psfm_ba_solver* s, int32_t* obs_image, int32_t* obs_point, double* obs_xy,
                              int32_t* point2D_idx);
 
+/* ------------------------------------------------------------------------- */
+/* The model -> sparse depth maps and their display images                   */
+/* (sfm/convert.py:43-96, csrc/convert.cu).  Host buffers in, host buffers out. */
+/* ------------------------------------------------------------------------- */
+typedef struct psfm_convert psfm_convert;
+typedef struct {
+  int32_t num_batches;       /* batches of images the memory budget allowed */
+  int32_t pad;
+  double upload_ms;          /* create: the model's upload (CUDA events) */
+  double kernel_ms;          /* create: the counting pass; result: every batch's kernels, summed */
+  double d2h_ms;             /* result: every batch's device-to-pinned copies, summed (they overlap the next batch) */
+  double alloc_ms;           /* host wall time of the allocations: create, the model's buffers and the counting slot;
+                                result, the two batch slots with their pinned buffers (its first call only) */
+  double host_copy_ms;       /* result: host wall time of the copies from the pinned buffers to the caller's */
+} psfm_convert_summary;
+/* Uploads a model and counts each image's valid pixels (depth > 0 after the last keypoint in keypoint order has
+   claimed every pixel).
+     cameras     camera_size [num_cameras][2] (width, height), each > 0 and at most 2^31 - 1 pixels
+     images      qvec [F][4] (not renormalised), tvec [F][3], image_camera [F], keypoint_ptr [F + 1] over
+                 keypoints [K][2] and point_row [K] (row of xyz, -1: no point), K < 2^31
+     points      xyz [num_points][3]
+     gray_lut    [256] grey level of each colormap entry; a NaN display value is black
+     memory_budget  bytes of device memory for the two batch slots (16 B per pixel, 32 B per keypoint each); a batch
+                 holds at least one image and at most 65,535
+   valid_count [F] receives each image's valid pixels, batch_ptr [F + 1] the batches (batch j holds images
+   batch_ptr[j] .. batch_ptr[j + 1], summary->num_batches of them); summary may be NULL.  PSFM_ERR_INVALID before any launch for a
+   bad camera size, a camera index or point row out of range, or a bad keypoint_ptr; PSFM_ERR_NO_DEVICE without a
+   device. */
+int psfm_convert_create(int32_t num_cameras, const int32_t* camera_size, int32_t num_images, const double* qvec,
+                        const double* tvec, const int32_t* image_camera, const int64_t* keypoint_ptr,
+                        const double* keypoints, const int32_t* point_row, int64_t num_points, const double* xyz,
+                        const uint8_t* gray_lut, int64_t memory_budget, psfm_convert** out, int64_t* valid_count,
+                        int32_t* batch_ptr, psfm_convert_summary* summary);
+/* The maps of the images of batches first_batch .. first_batch + num_batches - 1, images in order, each row-major
+   h x w: depth [sum w h] float64, rgba [sum w h][4].  Batch j runs while batch j - 1's maps are copied out.
+   PSFM_ERR_INVALID before any launch for a batch out of range or when one of the images has no valid pixel (its
+   percentiles do not exist).  The first call allocates the pinned staging buffers the handle keeps. */
+int psfm_convert_result(psfm_convert* c, int32_t first_batch, int32_t num_batches, double* depth, uint8_t* rgba,
+                        psfm_convert_summary* summary);
+void psfm_convert_destroy(psfm_convert* c);
+
 /* Measured fp64 roof of the current device (bench.py's roofline denominator for the kernels
    that are bounded by the fp64 FMA pipe rather than by HBM): sustained fused multiply-adds
    per second over the whole chip, and the latency in SM cycles of one dependent DFMA. */

@@ -380,3 +380,16 @@ class VerificationSummary(C.Structure):
         ("ransac_ms", C.c_double),
         ("compact_ms", C.c_double),
     ]
+
+
+class ConvertSummary(C.Structure):
+    """psfm_convert_summary: batches and CUDA-event times of psfm_convert_create / psfm_convert_result."""
+    _fields_ = [
+        ("num_batches", C.c_int32),
+        ("pad", C.c_int32),
+        ("upload_ms", C.c_double),
+        ("kernel_ms", C.c_double),
+        ("d2h_ms", C.c_double),
+        ("alloc_ms", C.c_double),
+        ("host_copy_ms", C.c_double),
+    ]

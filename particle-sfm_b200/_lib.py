@@ -30,6 +30,7 @@ EXPORTS = [
     "psfm_triangulator_default_options", "psfm_triangulation_create", "psfm_triangulation_result",
     "psfm_triangulation_destroy", "psfm_verification_default_options", "psfm_verify_two_view_geometries",
     "psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse",
+    "psfm_convert_create", "psfm_convert_result", "psfm_convert_destroy",
     "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
@@ -144,6 +145,11 @@ def lib():
     L.psfm_blocked_cholesky_solve.argtypes = [dp, dp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, dp]
     L.psfm_laplacian_solve.argtypes = [dp, dp, C.c_int32, dp]
     L.psfm_spd_inverse.argtypes = [dp, C.c_int32, dp]
+    L.psfm_convert_create.argtypes = [C.c_int32, ip, C.c_int32, dp, dp, ip, i64p, dp, ip, C.c_int64, dp, u8p, C.c_int64,
+                                      C.POINTER(vp), i64p, ip, C.POINTER(_abi.ConvertSummary)]
+    L.psfm_convert_result.argtypes = [vp, C.c_int32, C.c_int32, dp, u8p, C.POINTER(_abi.ConvertSummary)]
+    L.psfm_convert_destroy.argtypes = [vp]
+    L.psfm_convert_destroy.restype = None
     L.psfm_dist_get_unique_id.argtypes = [C.POINTER(C.c_uint8)]
     L.psfm_dist_init.argtypes = [C.POINTER(C.c_uint8), C.c_int32, C.c_int32]
     L.psfm_dist_finalize.restype = None

@@ -23,7 +23,8 @@ ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", CXX]
 
 # (source, extra flags).  traj_solver.cu: -fmad=false so that its iterates are
-# bit-identical to the oracle compiled with -ffp-contract=off (DESIGN.md §4).
+# bit-identical to the oracle compiled with -ffp-contract=off (DESIGN.md §4).  convert.cu: the same, so that its
+# depths and percentiles equal the numpy restatement's (DESIGN.md §4.10).
 UNITS = [
     ("common.cu", []),
     ("microbench.cu", []),
@@ -35,6 +36,7 @@ UNITS = [
     ("position_estimation.cu", []),
     ("triangulation.cu", []),
     ("verification.cu", []),
+    ("convert.cu", ["-fmad=false"]),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

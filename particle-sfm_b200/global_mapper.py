@@ -17,6 +17,8 @@ GlobalMapperController::Reconstruct (reference controllers/global_mapper.cc:136-
     10  refinement pass B           the same resident solver, rotations and focal length
     11  model                       psfm_ba_get_model
     12  write                       colmap_io.write_model_arrays -> OUT/0/{cameras,images,points3D}.bin
+    13  convert (convert_path set)  convert.save_depth_pose_arrays on the same arrays -> CONVERT/{depths,poses,
+                                    intrinsics}, what sfm/convert.py writes from the model (DESIGN.md §4.10)
 
 The model differs from gcolmap's by exactly the steps this library does not run: CompleteAndMergeTracks and
 Retriangulate inside the refinement loop, FilterImages after it, and the colour extraction (points are written with
@@ -31,7 +33,7 @@ import time
 
 import numpy as np
 
-from . import _abi, _lib, ba, colmap_io, handoff, init_geometry
+from . import _abi, _lib, ba, colmap_io, convert, handoff, init_geometry
 
 NOT_RUN = ("CompleteAndMergeTracks", "Retriangulate", "FilterImages", "ExtractColors")
 
@@ -150,9 +152,13 @@ def poses_and_points(g, used, o, report):
     return used, rot, pos, tri
 
 
-def global_mapper(database_path, output_path, options=None):
+def global_mapper(database_path, output_path, options=None, convert_path=None):
     """Run the mapper on `database_path` and write OUT/0/{cameras,images,points3D}.bin under `output_path`.  Returns
-    a MapperReport; a failed rotation or position stage writes nothing and is not an exception."""
+    a MapperReport; a failed rotation or position stage writes nothing and is not an exception.  With convert_path,
+    the model's depth maps, poses and intrinsics are then written there from the arrays in memory (stage `convert`),
+    as convert.write_depth_pose_from_colmap_format would write them from OUT/0.  OUT/0 is written first: a registered
+    image with no pixel of positive depth leaves it in place, writes nothing under convert_path and raises the
+    conversion's IndexError instead of returning a report."""
     o = options or GlobalMapperOptions()
     report = MapperReport()
     t0 = time.perf_counter()
@@ -192,8 +198,13 @@ def global_mapper(database_path, output_path, options=None):
         S.close()
     t0 = time.perf_counter()
     out = os.path.join(output_path, "0")
-    write_model(out, g, pos.has_position, model)
+    arrays = model_arrays(g, pos.has_position, model)
+    colmap_io.write_model_arrays(out, *arrays)
     report.add("write", t0, {"points": int((np.diff(model.track_ptr) > 0).sum()), "observations": int(model.track_ptr[-1])})
+    if convert_path is not None:
+        t0 = time.perf_counter()
+        c = convert.save_depth_pose_arrays(convert_path, *arrays)
+        report.add("convert", t0, {"images": c.images, "batches": c.num_batches})
     report.success, report.output = True, out
     return report
 
@@ -201,14 +212,19 @@ def global_mapper(database_path, output_path, options=None):
 def write_model(path, g, registered, model):
     """OUT/0 of a TriangulationModel: every camera, the registered images with all their keypoints, the points that
     kept an observation (id = row + 1)."""
+    colmap_io.write_model_arrays(path, *model_arrays(g, registered, model))
+
+
+def model_arrays(g, registered, model):
+    """The positional arguments of colmap_io.write_model_arrays after its path, for write_model."""
     reg = np.nonzero(registered)[0]
     sizes = np.diff(g.keypoint_ptr)
     sel = np.repeat(np.asarray(registered, bool), sizes)        # the keypoints of the registered images
     p3 = model.point3D_of_keypoint[sel]
     alive = np.nonzero(np.diff(model.track_ptr) > 0)[0]
     # a deleted point has an empty track, so the elements of the kept points are all of them, in order
-    colmap_io.write_model_arrays(
-        path, g.camera_ids, g.camera_size, model.cam_params, g.image_ids[reg], [g.image_names[f] for f in reg],
+    return (
+        g.camera_ids, g.camera_size, model.cam_params, g.image_ids[reg], [g.image_names[f] for f in reg],
         g.image_camera[reg], model.qvec[reg], model.tvec[reg], np.concatenate([[0], np.cumsum(sizes[reg])]),
         np.asarray(g.keypoints, np.float64)[sel], np.where(p3 >= 0, p3 + 1, -1), alive + 1, model.xyz[alive],
         model.error[alive], np.concatenate([[0], model.track_ptr[alive + 1]]), np.asarray(g.image_ids)[model.track_image],
