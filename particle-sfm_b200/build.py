@@ -27,6 +27,7 @@ COMMON = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", CXX
 # depths and percentiles equal the numpy restatement's (DESIGN.md §4.10).
 UNITS = [
     ("common.cu", []),
+    ("pair_inputs.cu", []),
     ("microbench.cu", []),
     ("tracker.cu", []),
     ("handoff.cu", []),

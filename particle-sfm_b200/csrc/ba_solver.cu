@@ -23,6 +23,7 @@
 #include "ba_refine.cuh"
 #include "dist.cuh"
 #include "dense_chol.cuh"
+#include "radix_sort.cuh"
 #include "triangulation_handle.cuh"
 
 namespace psfm {
@@ -237,7 +238,6 @@ void d2h_sync(cudaStream_t st, T* dst, const T* src, size_t n) {
   PSFM_CUDA(cudaStreamSynchronize(st));
 }
 
-inline unsigned grid_for(size_t n, int block = 256) { return (unsigned)((n + block - 1) / block); }
 
 // a host scalar reduced over the ranks with op (dist::allreduce_max | dist::allreduce_sum); v itself on one rank
 double reduce_over_ranks(cudaStream_t st, double v, void (*op)(double*, size_t, cudaStream_t)) {
@@ -356,7 +356,7 @@ int build_structure(psfm_ba_solver* S) {
     // stream compaction of the alive observations (index select + gather)
     DBuf<int> iota, nsel;
     iota.alloc(S->M0, st); sel.alloc(S->M0, st); nsel.alloc(1, st);
-    k_st_iota<<<grid_for(S->M0), 256, 0, st>>>(iota.p, S->M0); PSFM_LAUNCH_CHECK();
+    k_st_iota<<<grid_of(S->M0), 256, 0, st>>>(iota.p, S->M0); PSFM_LAUNCH_CHECK();
     size_t need = 0;
     cub::DeviceSelect::Flagged(nullptr, need, iota.p, S->d_alive.p, sel.p, nsel.p, S->M0, st);
     DBuf<unsigned char> t2; t2.alloc(need + 256, st);
@@ -366,22 +366,22 @@ int build_structure(psfm_ba_solver* S) {
     PSFM_CUDA(cudaStreamSynchronize(st));
     M = h_n;
     c_img.alloc(M, st); c_pt.alloc(M, st); c_xy.alloc(M, st);
-    if (M) { k_gather_alive<<<grid_for(M), 256, 0, st>>>(sel.p, M, S->d_in_img.p, S->d_in_pt.p, S->d_in_xy.p, c_img.p, c_pt.p, c_xy.p); PSFM_LAUNCH_CHECK(); }
+    if (M) { k_gather_alive<<<grid_of(M), 256, 0, st>>>(sel.p, M, S->d_in_img.p, S->d_in_pt.p, S->d_in_xy.p, c_img.p, c_pt.p, c_xy.p); PSFM_LAUNCH_CHECK(); }
     in_img_p = c_img.p; in_pt_p = c_pt.p; in_xy_p = c_xy.p;
     S->num_alive = M;
   }
   S->M = M;
   cnt.alloc(Pt, st); min_img.alloc(Pt, st); has_obs.alloc(F, st); bad.alloc(1, st);
   has_obs.zero(st); bad.zero(st);
-  if (Pt) { k_st_init<<<grid_for(Pt), 256, 0, st>>>(cnt.p, min_img.p, Pt, F); PSFM_LAUNCH_CHECK(); }
-  if (M) { k_st_count<<<grid_for(M), 256, 0, st>>>(in_img_p, in_pt_p, M, F, Pt, cnt.p, min_img.p, has_obs.p, bad.p); PSFM_LAUNCH_CHECK(); }
+  if (Pt) { k_st_init<<<grid_of(Pt), 256, 0, st>>>(cnt.p, min_img.p, Pt, F); PSFM_LAUNCH_CHECK(); }
+  if (M) { k_st_count<<<grid_of(M), 256, 0, st>>>(in_img_p, in_pt_p, M, F, Pt, cnt.p, min_img.p, has_obs.p, bad.p); PSFM_LAUNCH_CHECK(); }
   // internal point order: observed points by (first image, id); unobserved (key F) last
   order.alloc(Pt, st); keys32.alloc(Pt, st); keys32_out.alloc(Pt, st); idx.alloc(std::max(Pt, M), st); idx_out.alloc(std::max(Pt, M), st);
   pt_new.alloc(Pt, st); cnt_sorted.alloc((size_t)Pt + 1, st);
   int fbits = 1; while ((1 << fbits) <= F) ++fbits;
   size_t tmp_bytes = 0, need = 0;
   if (Pt) {
-    k_st_iota<<<grid_for(Pt), 256, 0, st>>>(idx.p, Pt); PSFM_LAUNCH_CHECK();
+    k_st_iota<<<grid_of(Pt), 256, 0, st>>>(idx.p, Pt); PSFM_LAUNCH_CHECK();
     cub::DeviceRadixSort::SortPairs(nullptr, need, min_img.p, keys32_out.p, idx.p, order.p, Pt, 0, fbits, st);
     tmp_bytes = std::max(tmp_bytes, need);
     cub::DeviceScan::ExclusiveSum(nullptr, need, cnt_sorted.p, cnt_sorted.p, Pt + 1, st);
@@ -398,7 +398,7 @@ int build_structure(psfm_ba_solver* S) {
   if (Pt) {
     need = tmp_bytes + 256;
     cub::DeviceRadixSort::SortPairs(tmp.p, need, min_img.p, keys32_out.p, idx.p, order.p, Pt, 0, fbits, st);
-    k_st_rank<<<grid_for(Pt), 256, 0, st>>>(order.p, cnt.p, Pt, pt_new.p, cnt_sorted.p); PSFM_LAUNCH_CHECK();
+    k_st_rank<<<grid_of(Pt), 256, 0, st>>>(order.p, cnt.p, Pt, pt_new.p, cnt_sorted.p); PSFM_LAUNCH_CHECK();
   }
   PSFM_CUDA(cudaMemsetAsync(cnt_sorted.p + Pt, 0, sizeof(int), st));
   // host needs: validity, observed flags, point order, counts
@@ -418,13 +418,13 @@ int build_structure(psfm_ba_solver* S) {
   // the device while the host packs the tiles below (radix sort is stable => ties keep input order)
   S->d_obs_img.alloc(M, st); S->d_obs_pt.alloc(M, st); S->d_obs_xy.alloc(M, st); S->d_obs_orig.alloc(M, st);
   if (M) {
-    k_st_keys<<<grid_for(M), 256, 0, st>>>(in_img_p, in_pt_p, pt_new.p, M, keys.p, idx.p); PSFM_LAUNCH_CHECK();
+    k_st_keys<<<grid_of(M), 256, 0, st>>>(in_img_p, in_pt_p, pt_new.p, M, keys.p, idx.p); PSFM_LAUNCH_CHECK();
     need = tmp_bytes + 256;
     cub::DeviceRadixSort::SortPairs(tmp.p, need, keys.p, keys_out.p, idx.p, S->d_obs_orig.p, M, 0, 32 + pbits, st);
     PSFM_CUDA(cudaStreamWaitEvent(st, S->sh.ev_xy, 0));
-    k_st_gather<<<grid_for(M), 256, 0, st>>>(keys_out.p, S->d_obs_orig.p, in_xy_p, M, S->d_obs_img.p, S->d_obs_pt.p, S->d_obs_xy.p);
+    k_st_gather<<<grid_of(M), 256, 0, st>>>(keys_out.p, S->d_obs_orig.p, in_xy_p, M, S->d_obs_img.p, S->d_obs_pt.p, S->d_obs_xy.p);
     PSFM_LAUNCH_CHECK();
-    if (sel.n) { k_compose_index<<<grid_for(M), 256, 0, st>>>(S->d_obs_orig.p, sel.p, M); PSFM_LAUNCH_CHECK(); }   // -> caller's index
+    if (sel.n) { k_compose_index<<<grid_of(M), 256, 0, st>>>(S->d_obs_orig.p, sel.p, M); PSFM_LAUNCH_CHECK(); }   // -> caller's index
   }
   for (int i = 0; i < F; ++i) if (h_has[i]) { S->img_has_obs[i] = 1; S->cam_has_obs[S->image_camera[i]] = 1; }
   int P = 0, maxL = 0;
@@ -502,11 +502,11 @@ int build_structure(psfm_ba_solver* S) {
   if (S->pipe) {
     S->d_tile_hdr.alloc(2 * (size_t)T, st); S->d_pstart_rel.alloc((size_t)P + 1, st);
     S->d_cseg_off32.alloc((size_t)S->nseg + 1, st); S->d_seg_pose.alloc(PSFM_SPS * (size_t)S->nseg + 2, st); S->d_seg_pose.zero(st);
-    k_pipe_headers<<<grid_for(T), 256, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_cseg_ptr.p, T, S->d_tile_hdr.p);
+    k_pipe_headers<<<grid_of(T), 256, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_cseg_ptr.p, T, S->d_tile_hdr.p);
     PSFM_LAUNCH_CHECK();
     k_pipe_pstart<<<T, 128, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_pt_ptr.p, T, S->d_pstart_rel.p);
     PSFM_LAUNCH_CHECK();
-    k_pipe_off32<<<grid_for(S->nseg), 256, 0, st>>>(S->d_cseg_off.p, S->nseg, S->d_cseg_off32.p);
+    k_pipe_off32<<<grid_of(S->nseg), 256, 0, st>>>(S->d_cseg_off.p, S->nseg, S->d_cseg_off32.p);
     PSFM_LAUNCH_CHECK();
   }
   PSFM_CUDA(cudaStreamSynchronize(st));
@@ -758,7 +758,7 @@ void do_linearize(psfm_ba_solver* S, const RunCfg& c, bool timed) {
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   const size_t pipe_smem = S->tile == 256 ? pipe_smem_linearize<256>(S->cap_ns, S->cap_np) : pipe_smem_linearize<512>(S->cap_ns, S->cap_np);
   if (pipe_ok(S, pipe_smem)) {
-    k_seg_pose<<<grid_for(12 * (size_t)S->nseg), 256, 0, S->stream>>>(S->d_cseg_img.p, S->d_pose16.p, S->nseg, S->d_seg_pose.p);
+    k_seg_pose<<<grid_of(12 * (size_t)S->nseg), 256, 0, S->stream>>>(S->d_cseg_img.p, S->d_pose16.p, S->nseg, S->d_seg_pose.p);
     PSFM_LAUNCH_CHECK();
   }
   if (timed) { e0 = S->events.get(); e1 = S->events.get(); PSFM_CUDA(cudaEventRecord(e0, S->stream)); }
@@ -1001,9 +1001,9 @@ void ensure_pairs(psfm_ba_solver* S) {
   cnt.alloc((size_t)M + 1, st); span.alloc(1, st); span.zero(st);
   PSFM_CUDA(cudaMemsetAsync(cnt.p + M, 0, sizeof(int), st));
   if (M) {   // a rank of a sharded problem may own no observation at all
-    k_pair_count<<<grid_for(M), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_pt.p, S->d_obs_img.p, M, cnt.p);
+    k_pair_count<<<grid_of(M), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_pt.p, S->d_obs_img.p, M, cnt.p);
     PSFM_LAUNCH_CHECK();
-    k_point_span<<<grid_for(S->P), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_img.p, S->P, span.p);
+    k_point_span<<<grid_of(S->P), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_img.p, S->P, span.p);
     PSFM_LAUNCH_CHECK();
   }
   // exclusive scan of the per-observation entry counts (64-bit total)
@@ -1067,7 +1067,7 @@ void ensure_pairs(psfm_ba_solver* S) {
   DBuf<unsigned long long> k64, k64_out, uk64;
   DBuf<unsigned int> v32;
   k64.alloc(NPr, st); k64_out.alloc(NPr, st); v32.alloc(NPr, st); S->d_tentries.alloc(NPr, st);
-  k_pair_fill_tile<<<grid_for(M), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_pt.p, S->d_obs_img.p, ptr32.p, M,
+  k_pair_fill_tile<<<grid_of(M), 256, 0, st>>>(S->d_pt_ptr.p, S->d_obs_pt.p, S->d_obs_img.p, ptr32.p, M,
                                                  S->d_tile_start.p, T, fb, k64.p, v32.p);
   PSFM_LAUNCH_CHECK();
   {
@@ -1075,7 +1075,7 @@ void ensure_pairs(psfm_ba_solver* S) {
     // sort of each tile's ~1.6 k entries by their image pair (the low 2 fb bits) — one pass through shared
     // memory per tile instead of four passes of a global 64-bit radix sort over 39 M pairs
     DBuf<int> seg; seg.alloc((size_t)T + 1, st);
-    k_tile_entry_offsets<<<grid_for((size_t)T + 1), 256, 0, st>>>(S->d_tile_start.p, ptr32.p, T, seg.p); PSFM_LAUNCH_CHECK();
+    k_tile_entry_offsets<<<grid_of((size_t)T + 1), 256, 0, st>>>(S->d_tile_start.p, ptr32.p, T, seg.p); PSFM_LAUNCH_CHECK();
     size_t need = 0;
     cub::DeviceSegmentedRadixSort::SortPairs(nullptr, need, k64.p, k64_out.p, v32.p, S->d_tentries.p, (int)NPr, T, seg.p, seg.p + 1, 0, 2 * fb, st);
     DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
@@ -1101,10 +1101,10 @@ void ensure_pairs(psfm_ba_solver* S) {
     cub::DeviceScan::ExclusiveSum(nullptr, need, ucount.p, beg.p, nr, st);
     DBuf<unsigned char> tmp; tmp.alloc(need + 256, st);
     cub::DeviceScan::ExclusiveSum(tmp.p, need, ucount.p, beg.p, nr, st);
-    k_pair_tasks<<<grid_for(nr), 256, 0, st>>>(uk64.p, ucount.p, beg.p, nr, fb, S->span, S->d_task_slot.p, S->d_task_rng.p);
+    k_pair_tasks<<<grid_of(nr), 256, 0, st>>>(uk64.p, ucount.p, beg.p, nr, fb, S->span, S->d_task_slot.p, S->d_task_rng.p);
     PSFM_LAUNCH_CHECK();
   }
-  k_tile_tasks<<<grid_for((size_t)T + 1), 256, 0, st>>>(uk64.p, nr, fb, T, S->d_tile_task.p);
+  k_tile_tasks<<<grid_of((size_t)T + 1), 256, 0, st>>>(uk64.p, nr, fb, T, S->d_tile_task.p);
   PSFM_LAUNCH_CHECK();
   {
     // PSFM_SCHUR_PAIRS=loop keeps every tile on the pair loop (measurement and tests); by default every
@@ -1115,7 +1115,7 @@ void ensure_pairs(psfm_ba_solver* S) {
     DBuf<int> nd; nd.alloc(1, st); nd.zero(st);
     S->d_tile_pairs.alloc((size_t)std::max(T, 1), st);
     if (T > 0) {
-      k_tile_pairs_mode<<<grid_for(T), 256, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_cseg_ptr.p, S->d_obs_pt.p,
+      k_tile_pairs_mode<<<grid_of(T), 256, 0, st>>>(S->d_tile_start.p, S->d_tile_pt.p, S->d_cseg_ptr.p, S->d_obs_pt.p,
                                                      S->d_obs_img.p, T, zcap, allow, S->d_tile_pairs.p, nd.p);
       PSFM_LAUNCH_CHECK();
     }
@@ -1205,7 +1205,7 @@ void launch_band_cholesky(psfm_ba_solver* S) {
   b.scale_c = S->d_scale_c.p; b.Dc2 = S->d_Dc2.p; b.rhs = S->d_rhs.p; b.active = S->d_active.p;
   b.F = S->F; b.span = S->span; b.pl = pl;
   b.Ab = S->bwk.ab(0); b.Ab1 = S->bwk.ab(1); b.C4 = S->bwk.C4.p; b.fail = S->d_cholfail.p;
-  k_band_assemble<<<grid_for((size_t)(pl.rows[0] + pl.rows[1]) * pl.RS), 256, 0, st>>>(b);
+  k_band_assemble<<<grid_of((size_t)(pl.rows[0] + pl.rows[1]) * pl.RS), 256, 0, st>>>(b);
   PSFM_LAUNCH_CHECK();
   band_chol_launch(S->bwk.args(S->d_x.p, S->NS, S->d_cholfail.p), st);
   { cudaEvent_t e = S->events.get(); PSFM_CUDA(cudaEventRecord(e, st)); S->ev_chol.back().second = e; }
@@ -1256,7 +1256,7 @@ void do_explicit_solve(psfm_ba_solver* S, const RunCfg& c, double radius) {
     mark(S->ev_pairs, false);
   }
   mark(S->ev_chol, true);
-  k_fold_replicas2<<<grid_for(nx + S->band_n), 256, 0, st>>>(S->d_xband.p, S->d_xcamrep.p, nx, NREP, S->d_bandrep.p, S->band_n, S->band_nrep);
+  k_fold_replicas2<<<grid_of(nx + S->band_n), 256, 0, st>>>(S->d_xband.p, S->d_xcamrep.p, nx, NREP, S->d_bandrep.p, S->band_n, S->band_nrep);
   PSFM_LAUNCH_CHECK();
   dist::allreduce_sum(S->d_xband.p, S->d_xband.n, st);
   // the unfused path's rhs correction is already in d_rhs (do_reduced_setup); rows 21.. of its sums are zero
@@ -1265,16 +1265,16 @@ void do_explicit_solve(psfm_ba_solver* S, const RunCfg& c, double radius) {
   S->d_S.zero(st);
   BandAsmArgs ba_;
   ba_.Sband = S->d_xband.p + nx; ba_.scale_c = S->d_scale_c.p; ba_.F = S->F; ba_.span = S->span; ba_.lda = S->NS + 1; ba_.S = S->d_S.p;
-  k_schur_assemble_band<<<grid_for(S->band_n), 256, 0, st>>>(ba_); PSFM_LAUNCH_CHECK();
+  k_schur_assemble_band<<<grid_of(S->band_n), 256, 0, st>>>(ba_); PSFM_LAUNCH_CHECK();
   AsmArgs a;
   a.lin_cam = S->d_lin.p; a.lin_intr = S->d_lin.p + (size_t)S->F * NVL;
   a.prep_intr = S->d_prep.p + (size_t)S->F * NVL; a.xcam = S->d_xband.p; a.xstride = NVX2;
   a.scale_c = S->d_scale_c.p; a.Dc2 = S->d_Dc2.p; a.active = S->d_active.p;
   a.rhs = S->d_rhs.p;
   a.F = S->F; a.C = S->C; a.NS = S->NS; a.lda = S->NS + 1; a.S = S->d_S.p;
-  k_schur_assemble_local<<<grid_for(S->F, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
-  k_schur_assemble_global<<<grid_for(S->F + S->C, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
-  k_schur_assemble_finish<<<grid_for(S->NS, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
+  k_schur_assemble_local<<<grid_of(S->F, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
+  k_schur_assemble_global<<<grid_of(S->F + S->C, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
+  k_schur_assemble_finish<<<grid_of(S->NS, 128), 128, 0, st>>>(a); PSFM_LAUNCH_CHECK();
   launch_cholesky(S);
 }
 
@@ -1534,16 +1534,6 @@ int run_impl(psfm_ba_solver* S, const psfm_ba_options* opts, psfm_ba_summary* ou
   return PSFM_OK;
 }
 
-int check_device() {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    set_error("no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
-  return PSFM_OK;
-}
-
 }  // namespace
 
 // ---------------------------------------------------------------- C ABI
@@ -1627,7 +1617,7 @@ int finish_create(psfm_ba_solver* S, const double* qvec, const double* tvec, con
 extern "C" int psfm_ba_create(const psfm_ba_problem* pb, psfm_ba_solver** out) {
   if (!pb || !out) { set_error("psfm_ba_create: null argument"); return PSFM_ERR_INVALID; }
   *out = nullptr;
-  int rc = check_device();
+  int rc = require_device("psfm_ba_create");
   if (rc != PSFM_OK) return rc;
   psfm_ba_solver* S = new psfm_ba_solver();
   try {
@@ -1653,7 +1643,7 @@ extern "C" int psfm_ba_create_from_triangulation(const psfm_triangulation* tri, 
     return PSFM_ERR_INVALID;
   }
   *out = nullptr;
-  int rc = check_device();
+  int rc = require_device("psfm_ba_create_from_triangulation");
   if (rc != PSFM_OK) return rc;
   if (dist::world_size() > 1) {
     set_error("psfm_ba_create_from_triangulation: a sharded problem is not supported");
@@ -1731,7 +1721,7 @@ extern "C" int psfm_ba_get_model(psfm_ba_solver* S, double* qvec, double* tvec, 
     set_error("psfm_ba_get_model: null argument");
     return PSFM_ERR_INVALID;
   }
-  int rc = check_device();
+  int rc = require_device("psfm_ba_get_model");
   if (rc != PSFM_OK) return rc;
   if (!S->from_triangulation) {
     set_error("psfm_ba_get_model: the solver was not made by psfm_ba_create_from_triangulation");
@@ -1748,19 +1738,12 @@ extern "C" int psfm_ba_get_model(psfm_ba_solver* S, double* qvec, double* tvec, 
     d_ptr.alloc((size_t)P + 1, st); d_kp.alloc(S->K_total, st); d_img.alloc(M, st); d_p2d.alloc(M, st);
     if (S->K_total) PSFM_CUDA(cudaMemsetAsync(d_kp.p, 0xff, sizeof(long long) * (size_t)S->K_total, st));   // -1
     if (M) {
-      k_model_keys<<<grid_for(M), 256, 0, st>>>(M, P, S->d_alive.p, S->d_in_pt.p, k0.p, v0.p);
+      k_model_keys<<<grid_of(M), 256, 0, st>>>(M, P, S->d_alive.p, S->d_in_pt.p, k0.p, v0.p);
       PSFM_LAUNCH_CHECK();
-      int bits = 1;
-      while (bits < 32 && ((unsigned long long)P >> bits)) ++bits;
       cub::DoubleBuffer<unsigned> keys(k0.p, k1.p);
       cub::DoubleBuffer<int> vals(v0.p, v1.p);
-      size_t bytes = 0;
-      PSFM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys, vals, M, 0, bits, st));
-      DBuf<unsigned char> tmp;
-      tmp.alloc(bytes, st);
-      PSFM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, keys, vals, M, 0, bits, st));
-      PSFM_LAUNCH_CHECK();
-      k_model_tracks<<<grid_for(std::max(P + 1, M)), 256, 0, st>>>(P, M, keys.Current(), vals.Current(), S->d_in_img.p,
+      sort_pairs(keys, vals, M, key_bits((unsigned long long)P), st);
+      k_model_tracks<<<grid_of(std::max(P + 1, M)), 256, 0, st>>>(P, M, keys.Current(), vals.Current(), S->d_in_img.p,
                                                                    S->d_in_kp.p, S->d_img_map.p, S->d_img_kp0.p, d_ptr.p,
                                                                    d_img.p, d_p2d.p, d_kp.p);
       PSFM_LAUNCH_CHECK();
@@ -1792,7 +1775,7 @@ extern "C" int psfm_ba_get_model(psfm_ba_solver* S, double* qvec, double* tvec, 
 extern "C" int psfm_ba_get_observations(psfm_ba_solver* S, int32_t* obs_image, int32_t* obs_point, double* obs_xy,
                                         int32_t* point2D_idx) {
   if (!S) { set_error("psfm_ba_get_observations: null argument"); return PSFM_ERR_INVALID; }
-  const int rc = check_device();
+  const int rc = require_device("psfm_ba_get_observations");
   if (rc != PSFM_OK) return rc;
   if (point2D_idx && !S->from_triangulation) {
     set_error("psfm_ba_get_observations: point2D_idx needs a solver made by psfm_ba_create_from_triangulation");
@@ -1859,8 +1842,10 @@ extern "C" int psfm_ba_solve(psfm_ba_problem* pb, const psfm_ba_options* opts, p
     if (summary) memset(summary, 0, sizeof(*summary));
     return PSFM_ZERO_RESIDUALS;
   }
+  int rc = require_device("psfm_ba_solve");
+  if (rc != PSFM_OK) return rc;
   psfm_ba_solver* S = nullptr;
-  int rc = psfm_ba_create(pb, &S);
+  rc = psfm_ba_create(pb, &S);
   if (rc != PSFM_OK) return rc;
   rc = psfm_ba_run(S, opts, summary);
   if (rc == PSFM_OK) psfm_ba_get_state(S, pb->qvec, pb->tvec, pb->xyz, pb->cam_params);
@@ -1947,7 +1932,7 @@ long long filter_negative_depth_impl(psfm_ba_solver* S) {
   upload_state(S);
   S->d_count.zero(S->stream);
   if (S->P) {
-    k_filter_negative_depth<<<grid_for(S->P, 128), 128, 0, S->stream>>>(filter_ctx(S));
+    k_filter_negative_depth<<<grid_of(S->P, 128), 128, 0, S->stream>>>(filter_ctx(S));
     PSFM_LAUNCH_CHECK();
   }
   const long long n = read_filter_count(S);
@@ -1961,20 +1946,20 @@ long long filter_points_impl(psfm_ba_solver* S, double max_reproj_error, double 
   cudaStream_t st = S->stream;
   if (S->d_pt_error.n != (size_t)S->P_total) {
     S->d_pt_error.alloc(S->P_total, st);
-    if (S->P_total) { k_fill<<<grid_for(S->P_total), 256, 0, st>>>(S->d_pt_error.p, nan(""), (size_t)S->P_total); PSFM_LAUNCH_CHECK(); }
+    if (S->P_total) { k_fill<<<grid_of(S->P_total), 256, 0, st>>>(S->d_pt_error.p, nan(""), (size_t)S->P_total); PSFM_LAUNCH_CHECK(); }
   }
   DBuf<double> centres;
   DBuf<int> pt_orig;
   centres.alloc(3 * (size_t)S->F, st);
   pt_orig.alloc(S->P, st);
   pt_orig.upload(S->pt_orig.data(), S->P, st);
-  k_proj_centres<<<grid_for(S->F, 128), 128, 0, st>>>(S->d_pose[S->cur].p, S->F, centres.p);
+  k_proj_centres<<<grid_of(S->F, 128), 128, 0, st>>>(S->d_pose[S->cur].p, S->F, centres.p);
   PSFM_LAUNCH_CHECK();
   S->d_count.zero(st);
   if (S->P) {
     FilterCtx c = filter_ctx(S);
     c.pt_orig = pt_orig.p;
-    k_filter_points<<<grid_for(S->P, 128), 128, 0, st>>>(c, centres.p, max_reproj_error * max_reproj_error,
+    k_filter_points<<<grid_of(S->P, 128), 128, 0, st>>>(c, centres.p, max_reproj_error * max_reproj_error,
                                                         min_tri_angle_deg * 0.017453292519943295, S->d_pt_error.p);
     PSFM_LAUNCH_CHECK();
   }
@@ -2151,7 +2136,7 @@ extern "C" int psfm_ba_iterative_refinement(psfm_ba_solver* S, const psfm_ba_opt
 
 extern "C" int psfm_ba_band_solve(const double* A, const double* b, int32_t nb, int32_t bw, double* x) {
   if (!A || !b || !x || nb < 1 || bw < 0) return PSFM_ERR_INVALID;
-  int rc = check_device();
+  int rc = require_device("psfm_ba_band_solve");
   if (rc != PSFM_OK) return rc;
   bw = std::min(bw, nb - 1);
   const BandPlan pl = band_chol_plan(nb, bw);
@@ -2267,7 +2252,7 @@ extern "C" int psfm_blocked_cholesky_solve(const double* A, const double* b, int
     set_error("psfm_blocked_cholesky_solve: needs 1 <= nb <= ns <= 32767, bw >= 0 and max_ctas >= 0");
     return PSFM_ERR_INVALID;
   }
-  int rc = check_device();
+  int rc = require_device("psfm_blocked_cholesky_solve");
   if (rc != PSFM_OK) return rc;
   bw = std::min(bw, nb);             // the kernel's band ends at row nb whatever bw says
   try {

@@ -5,6 +5,18 @@ namespace psfm {
 static thread_local std::string g_error;
 std::atomic<long long> g_launch_count{0};
 void set_error(const std::string& msg) { g_error = msg; }
+int fail(const char* entry, int code, const std::string& msg) {
+  set_error(std::string(entry) + ": " + msg);
+  return code;
+}
+int require_device(const char* entry) {
+  int n = 0;
+  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
+    cudaGetLastError();
+    return fail(entry, PSFM_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU path)");
+  }
+  return PSFM_OK;
+}
 void keep_pool_memory() {
   static bool done = false;
   if (done) return;

@@ -30,6 +30,7 @@
 #include <climits>
 #include <vector>
 
+#include "pair_inputs.h"
 #include "psfm_common.cuh"
 
 namespace {
@@ -173,23 +174,8 @@ struct Slot {
   }
 };
 
-struct Event {
-  cudaEvent_t e = nullptr;
-  Event() { PSFM_CUDA(cudaEventCreate(&e)); }
-  Event(const Event&) = delete;
-  Event& operator=(const Event&) = delete;
-  ~Event() {
-    if (e) cudaEventDestroy(e);
-  }
-};
-
 double host_ms_since(std::chrono::steady_clock::time_point t0) {
   return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-}
-
-int convert_fail(const std::string& msg) {
-  set_error(msg);
-  return PSFM_ERR_INVALID;
 }
 
 inline unsigned blocks_for(long long n) { return (unsigned)std::max<long long>(1, std::min<long long>((n + 255) / 256, 64)); }
@@ -268,35 +254,30 @@ extern "C" int psfm_convert_create(int32_t num_cameras, const int32_t* camera_si
                                    const double* keypoints, const int32_t* point_row, int64_t num_points,
                                    const double* xyz, const uint8_t* gray_lut, int64_t memory_budget, psfm_convert** out,
                                    int64_t* valid_count, int32_t* batch_ptr, psfm_convert_summary* summary) {
+  const char* entry = "psfm_convert_create";
   if (!out || !camera_size || !image_camera || !keypoint_ptr || !gray_lut || !valid_count || !batch_ptr ||
       (num_images > 0 && (!qvec || !tvec)))
-    return convert_fail("psfm_convert_create: null argument");
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
   *out = nullptr;
   if (num_cameras < 0 || num_images < 0 || num_points < 0 || memory_budget <= 0)
-    return convert_fail("psfm_convert_create: num_cameras, num_images, num_points must be >= 0 and memory_budget > 0");
+    return fail(entry, PSFM_ERR_INVALID, "num_cameras, num_images, num_points must be >= 0 and memory_budget > 0");
   for (int c = 0; c < num_cameras; ++c)
     if (camera_size[2 * c] <= 0 || camera_size[2 * c + 1] <= 0 ||
         (long long)camera_size[2 * c] * camera_size[2 * c + 1] > 0x7fffffffLL)
-      return convert_fail("psfm_convert_create: camera " + std::to_string(c) + " has a bad size (camera size)");
-  if (keypoint_ptr[0] != 0) return convert_fail("psfm_convert_create: keypoint_ptr[0] must be 0");
-  for (int i = 0; i < num_images; ++i) {
+      return fail(entry, PSFM_ERR_INVALID, "camera " + std::to_string(c) + " has a bad size (camera size)");
+  int rc = check_keypoint_ptr(entry, num_images, keypoint_ptr);
+  if (rc != PSFM_OK) return rc;
+  for (int i = 0; i < num_images; ++i)
     if (image_camera[i] < 0 || image_camera[i] >= num_cameras)
-      return convert_fail("psfm_convert_create: image " + std::to_string(i) + " has a camera index out of range (camera index)");
-    if (keypoint_ptr[i + 1] < keypoint_ptr[i]) return convert_fail("psfm_convert_create: keypoint_ptr must be non-decreasing");
-  }
+      return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(i) + " has a camera index out of range (camera index)");
   const long long K = keypoint_ptr[num_images];
-  if (K > 0x7fffffffLL) return convert_fail("psfm_convert_create: more than 2^31 - 1 keypoints");
-  if (K > 0 && (!keypoints || !point_row)) return convert_fail("psfm_convert_create: null argument");
-  if (num_points > 0 && !xyz) return convert_fail("psfm_convert_create: null argument");
+  if (K > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 keypoints");
+  if (K > 0 && (!keypoints || !point_row)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  if (num_points > 0 && !xyz) return fail(entry, PSFM_ERR_INVALID, "null argument");
   for (long long k = 0; k < K; ++k)
     if (point_row[k] < -1 || point_row[k] >= num_points)
-      return convert_fail("psfm_convert_create: keypoint " + std::to_string(k) + " has a point row out of range (point row)");
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error("no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
+      return fail(entry, PSFM_ERR_INVALID, "keypoint " + std::to_string(k) + " has a point row out of range (point row)");
+  if ((rc = require_device(entry)) != PSFM_OK) return rc;
   psfm_convert* H = new psfm_convert;
   H->F = num_images;
   H->K = K;
@@ -382,16 +363,17 @@ extern "C" int psfm_convert_create(int32_t num_cameras, const int32_t* camera_si
 
 extern "C" int psfm_convert_result(psfm_convert* H, int32_t first_batch, int32_t num_batches, double* depth,
                                    uint8_t* rgba, psfm_convert_summary* summary) {
-  if (!H) return convert_fail("psfm_convert_result: null argument");
+  const char* entry = "psfm_convert_result";
+  if (!H) return fail(entry, PSFM_ERR_INVALID, "null argument");
   const int nb = (int)H->batches.size();
   if (first_batch < 0 || num_batches < 0 || first_batch > nb || num_batches > nb - first_batch)
-    return convert_fail("psfm_convert_result: batches out of range");
-  if (num_batches > 0 && (!depth || !rgba)) return convert_fail("psfm_convert_result: null argument");
+    return fail(entry, PSFM_ERR_INVALID, "batches out of range");
+  if (num_batches > 0 && (!depth || !rgba)) return fail(entry, PSFM_ERR_INVALID, "null argument");
   const int j0 = first_batch, j1 = first_batch + num_batches;
   for (int j = j0; j < j1; ++j)
     for (int i = H->batches[j].first; i < H->batches[j].first + H->batches[j].count; ++i)
       if (H->valid[i] == 0)
-        return convert_fail("psfm_convert_result: image " + std::to_string(i) + " has no valid pixel (no percentile)");
+        return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(i) + " has no valid pixel (no percentile)");
   try {
     Slot* slots = H->slots;
     const auto t_alloc = std::chrono::steady_clock::now();

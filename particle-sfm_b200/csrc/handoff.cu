@@ -14,7 +14,6 @@
 //   7. k_scatter      each record to pair_ptr[rank of its run] + its place in the run, as (kp[src], kp[dst])
 // Memory: 32 bytes per record during the sort (keys and values, double-buffered), 24 bytes per record in the
 // scatter (sorted values and the int64 output), about 80 bytes per sample besides.
-#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
@@ -22,6 +21,7 @@
 #include <vector>
 
 #include "psfm_common.cuh"
+#include "radix_sort.cuh"
 
 namespace {
 
@@ -148,41 +148,6 @@ __global__ void k_scatter(long long M, const long long* run_start, int R, const 
   }
 }
 
-int handoff_device_ok() {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    set_error("no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
-  return PSFM_OK;
-}
-
-int handoff_fail(const std::string& msg) {
-  set_error(msg);
-  return PSFM_ERR_INVALID;
-}
-
-inline unsigned grid_of(long long n) { return (unsigned)((n + 255) / 256); }
-inline unsigned grid_stride_of(long long n) { return (unsigned)std::min<long long>((n + 255) / 256, 132 * 16); }
-
-// number of bits the radix sorts look at for keys in [0, max_key]
-inline int key_bits(u64 max_key) {
-  int b = 1;
-  while (b < 64 && (max_key >> b)) ++b;
-  return b;
-}
-
-template <typename K, typename V, typename NumT>
-void sort_pairs(cub::DoubleBuffer<K>& keys, cub::DoubleBuffer<V>& vals, NumT n, int end_bit) {
-  size_t bytes = 0;
-  PSFM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys, vals, n, 0, end_bit, nullptr));
-  DBuf<unsigned char> tmp;
-  tmp.alloc(bytes);
-  PSFM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, keys, vals, n, 0, end_bit, nullptr));
-  PSFM_LAUNCH_CHECK();
-}
-
 // of two buffers, free the one a CUB double buffer does not currently point at
 template <typename T>
 void release_other(DBuf<T>& a, DBuf<T>& b, const T* current) {
@@ -204,17 +169,18 @@ struct psfm_matches {
 extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, const int64_t* frame_ids, const double* xy,
                                    int32_t num_images, int32_t sample_k, psfm_matches** out, int64_t* num_pairs,
                                    int64_t* num_matches) {
-  if (!out || !num_pairs || !num_matches || !traj_ptr) return handoff_fail("psfm_matches_create: null argument");
+  const char* entry = "psfm_matches_create";
+  if (!out || !num_pairs || !num_matches || !traj_ptr) return fail(entry, PSFM_ERR_INVALID, "null argument");
   *out = nullptr;
   if (num_trajs < 0 || num_images < 0 || sample_k < 1)
-    return handoff_fail("psfm_matches_create: num_trajs and num_images must be >= 0, sample_k >= 1");
-  if (traj_ptr[0] != 0) return handoff_fail("psfm_matches_create: traj_ptr[0] must be 0");
+    return fail(entry, PSFM_ERR_INVALID, "num_trajs and num_images must be >= 0, sample_k >= 1");
+  if (traj_ptr[0] != 0) return fail(entry, PSFM_ERR_INVALID, "traj_ptr[0] must be 0");
   for (int64_t t = 0; t < num_trajs; ++t)
-    if (traj_ptr[t + 1] < traj_ptr[t]) return handoff_fail("psfm_matches_create: traj_ptr must be non-decreasing");
+    if (traj_ptr[t + 1] < traj_ptr[t]) return fail(entry, PSFM_ERR_INVALID, "traj_ptr must be non-decreasing");
   const long long N = traj_ptr[num_trajs];
-  if (N > 0x7fffffffLL) return handoff_fail("psfm_matches_create: more than 2^31 - 1 samples");
-  if (N > 0 && (!frame_ids || !xy)) return handoff_fail("psfm_matches_create: null argument");
-  int rc = handoff_device_ok();
+  if (N > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 samples");
+  if (N > 0 && (!frame_ids || !xy)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  int rc = require_device(entry);
   if (rc != PSFM_OK) return rc;
   psfm_matches* H = new psfm_matches;
   H->num_images = num_images;
@@ -256,7 +222,7 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
     PSFM_CUDA(cudaMemcpy(&M, off.p + N, sizeof(long long), cudaMemcpyDeviceToHost));
     if (h_bad) {
       delete H;
-      return handoff_fail("psfm_matches_create: a frame id is outside [0, num_images)");
+      return fail(entry, PSFM_ERR_INVALID, "a frame id is outside [0, num_images)");
     }
     // keypoints: stable sort of the samples by frame
     cub::DoubleBuffer<int> fk(f32a.p, f32b.p), fv(ida.p, idb.p);
@@ -356,7 +322,7 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
 extern "C" int psfm_matches_result(const psfm_matches* H, int64_t* keypoint_ptr, double* keypoints, int64_t* pair_images,
                                    int64_t* pair_ptr, int64_t* matches) {
   if (!H || !keypoint_ptr || !pair_ptr || (H->num_obs && !keypoints) || (H->num_matches && (!pair_images || !matches)))
-    return handoff_fail("psfm_matches_result: null argument");
+    return fail("psfm_matches_result", PSFM_ERR_INVALID, "null argument");
   try {
     std::copy(H->kstart.begin(), H->kstart.end(), keypoint_ptr);
     std::copy(H->pair_ptr.begin(), H->pair_ptr.end(), pair_ptr);

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "dlt.cuh"
+#include "pair_inputs.h"
 #include "psfm_common.cuh"
 
 namespace {
@@ -219,23 +220,13 @@ __global__ void __launch_bounds__(128) k_triangulate_tracks(const double* __rest
   xyz[3 * (size_t)t] = v[0] / v[3]; xyz[3 * (size_t)t + 1] = v[1] / v[3]; xyz[3 * (size_t)t + 2] = v[2] / v[3];
 }
 
-int init_device_ok() {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    set_error("no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
-  return PSFM_OK;
-}
-
 }  // namespace
 
 extern "C" int psfm_known_rotation_translations(const double* points1, const double* points2, const int32_t* pair_ptr,
                                                 const double* qvec1, const double* qvec2, int32_t num_pairs, double* tvec,
                                                 int32_t* iterations) {
   if (num_pairs < 0 || (num_pairs > 0 && (!pair_ptr || !qvec1 || !qvec2 || !tvec))) return PSFM_ERR_INVALID;
-  int rc = init_device_ok();
+  int rc = require_device("psfm_known_rotation_translations");
   if (rc != PSFM_OK) return rc;
   if (num_pairs == 0) return PSFM_OK;
   const size_t m = (size_t)pair_ptr[num_pairs];
@@ -261,7 +252,7 @@ extern "C" int psfm_known_rotation_translations(const double* points1, const dou
 extern "C" int psfm_triangulate_tracks(const double* proj_matrices, const double* points, const int32_t* track_ptr,
                                        int32_t num_tracks, double* xyz) {
   if (num_tracks < 0 || (num_tracks > 0 && (!track_ptr || !xyz))) return PSFM_ERR_INVALID;
-  int rc = init_device_ok();
+  int rc = require_device("psfm_triangulate_tracks");
   if (rc != PSFM_OK) return rc;
   if (num_tracks == 0) return PSFM_OK;
   const size_t m = (size_t)track_ptr[num_tracks];
@@ -280,52 +271,38 @@ extern "C" int psfm_triangulate_tracks(const double* proj_matrices, const double
   } catch (const CudaFail& f) { return f.code; }
 }
 
-namespace {
-int pairwise_fail(const std::string& msg) {
-  set_error("psfm_optimize_pairwise_translations: " + msg);
-  return PSFM_ERR_INVALID;
-}
-}  // namespace
-
 extern "C" int psfm_optimize_pairwise_translations(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
                                                    const int32_t* image_camera, const double* cameras, int32_t num_cameras,
                                                    int64_t num_pairs, const int32_t* pair_images, const int64_t* inlier_ptr,
                                                    const uint32_t* inlier_matches, const double* orientations,
                                                    const uint8_t* pair_used, double* tvec, int32_t* iterations) {
-  if (num_images < 0 || num_cameras < 0 || num_pairs < 0) return pairwise_fail("negative size");
-  if (num_pairs > 0x7fffffffLL) return pairwise_fail("more than 2^31 - 1 pairs");
+  const char* entry = "psfm_optimize_pairwise_translations";
+  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+  if (rc != PSFM_OK) return rc;
   if (num_pairs > 0 && (!keypoint_ptr || !image_camera || !cameras || !pair_images || !inlier_ptr || !orientations ||
                         !tvec || !iterations))
-    return pairwise_fail("null argument");
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
   const int R = (int)num_pairs;
   if (R > 0) {
-    if (keypoint_ptr[0] != 0) return pairwise_fail("keypoint_ptr[0] must be 0");
-    for (int32_t f = 0; f < num_images; ++f)
-      if (keypoint_ptr[f + 1] < keypoint_ptr[f]) return pairwise_fail("keypoint_ptr must be non-decreasing");
-    for (int32_t f = 0; f < num_images; ++f)
-      if (image_camera[f] < 0 || image_camera[f] >= num_cameras) return pairwise_fail("a camera index is outside [0, num_cameras)");
-    if (inlier_ptr[0] != 0) return pairwise_fail("inlier_ptr[0] must be 0");
-    for (int p = 0; p < R; ++p) {
-      if (inlier_ptr[p + 1] < inlier_ptr[p]) return pairwise_fail("inlier_ptr must be non-decreasing");
-      for (int k = 0; k < 2; ++k)
-        if (pair_images[2 * p + k] < 0 || pair_images[2 * p + k] >= num_images)
-          return pairwise_fail("an image index is outside [0, num_images)");
-    }
+    // no check_distinct_pairs: this stage accepts self pairs and repeated pairs
+    if ((rc = check_keypoint_ptr(entry, num_images, keypoint_ptr)) != PSFM_OK) return rc;
+    if ((rc = check_image_cameras(entry, num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
+    if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
+    if ((rc = check_pair_images(entry, R, pair_images, num_images)) != PSFM_OK) return rc;
     for (int p = 0; p < R; ++p) {
       if (pair_used && !pair_used[p]) continue;
       for (int k = 0; k < 2; ++k) {
         const double* q = orientations + 4 * (size_t)pair_images[2 * p + k];
         const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-        if (!(std::isfinite(n2) && n2 > 0.0)) return pairwise_fail("a used pair's image has a zero or non-finite orientation");
+        if (!(std::isfinite(n2) && n2 > 0.0))
+          return fail(entry, PSFM_ERR_INVALID, "a used pair's image has a zero or non-finite orientation");
       }
     }
     if (inlier_ptr[R] > 0 && (!inlier_matches || (keypoint_ptr[num_images] > 0 && !keypoints)))
-      return pairwise_fail("null argument");
-    if (!keypoints_in_range(R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches))
-      return pairwise_fail("a keypoint index is outside its image's keypoints");
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
   }
-  int rc = init_device_ok();
-  if (rc != PSFM_OK) return rc;
+  if ((rc = require_device(entry)) != PSFM_OK) return rc;
   if (R == 0) return PSFM_OK;
   const long long N = inlier_ptr[R], K = keypoint_ptr[num_images];
   // the kernel reads one quaternion pair per pair: gathered here from the image orientations

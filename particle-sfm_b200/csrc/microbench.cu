@@ -42,12 +42,8 @@ __global__ void k_fp64_latency(long long* cycles, double* sink, int n, double se
 // dependent_latency_cycles: SM cycles from one DFMA to the next dependent one.
 extern "C" int psfm_measure_dfma(double* dfma_per_second, double* dependent_latency_cycles) {
   using namespace psfm;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    set_error("no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
+  const int rc = require_device("psfm_measure_dfma");
+  if (rc != PSFM_OK) return rc;
   try {
     int dev = 0, sms = 0;
     PSFM_CUDA(cudaGetDevice(&dev));

@@ -34,6 +34,7 @@
 #include <vector>
 
 #include "dense_chol.cuh"
+#include "pair_inputs.h"
 #include "position_recalled.cuh"
 #include "psfm_common.cuh"
 #include "quat.cuh"
@@ -320,13 +321,6 @@ __global__ void __launch_bounds__(1024) k_pos_check(int R, int nv, const double*
 }
 
 // ---- host ----------------------------------------------------------------------------------------------------------
-int pos_fail(int code, const std::string& msg) {
-  set_error("psfm_estimate_global_positions: " + msg);
-  return code;
-}
-
-inline unsigned grid_of(long long n) { return (unsigned)std::max<long long>(1, (n + 255) / 256); }
-
 int find_root(std::vector<int>& parent, int v) {
   while (parent[v] != v) v = parent[v] = parent[parent[v]];
   return v;
@@ -350,34 +344,26 @@ extern "C" int psfm_estimate_global_positions(int32_t num_images, int64_t num_pa
                                               double* image_tvec, double* scales, psfm_position_summary* summary) {
   const auto t0 = std::chrono::steady_clock::now();
   const long long launches0 = g_launch_count.load();
-  if (num_images < 0 || num_pairs < 0) return pos_fail(PSFM_ERR_INVALID, "negative size");
-  if (num_pairs > 0x7fffffffLL) return pos_fail(PSFM_ERR_INVALID, "more than 2^31 - 1 pairs");
+  const char* entry = "psfm_estimate_global_positions";
+  int rc = check_sizes(entry, num_images, 0, num_pairs);
+  if (rc != PSFM_OK) return rc;
   if ((num_pairs > 0 && (!pair_images || !pair_tvec || !scales)) ||
       (num_images > 0 && (!orientations || !positions || !has_position || !image_tvec)))
-    return pos_fail(PSFM_ERR_INVALID, "null argument");
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
   psfm_lud_options o;
   psfm_lud_default_options(&o);
   if (opts) o = *opts;
   if (!(o.max_num_iterations > 0 && o.rho > 0.0 && o.alpha > 0.0 && o.alpha < 2.0 && o.absolute_tolerance > 0.0 &&
         o.relative_tolerance > 0.0 && std::isfinite(o.rho) && std::isfinite(o.absolute_tolerance) &&
         std::isfinite(o.relative_tolerance)))
-    return pos_fail(PSFM_ERR_INVALID, "options fail the ConstrainedL1Solver options Check()");
+    return fail(entry, PSFM_ERR_INVALID, "options fail the ConstrainedL1Solver options Check()");
   const int F = num_images, R = (int)num_pairs;
+  if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
+  if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
   std::vector<int> used;
-  {
-    std::vector<uint64_t> keys(R);
-    for (int p = 0; p < R; ++p) {
-      const int a = pair_images[2 * p], b = pair_images[2 * p + 1];
-      if (a < 0 || a >= F || b < 0 || b >= F) return pos_fail(PSFM_ERR_INVALID, "an image index is outside [0, num_images)");
-      if (a == b) return pos_fail(PSFM_ERR_INVALID, "a pair of an image with itself");
-      keys[p] = ((uint64_t)std::min(a, b) << 32) | (uint64_t)std::max(a, b);
-      if (!pair_used || pair_used[p]) used.push_back(p);
-    }
-    std::sort(keys.begin(), keys.end());
-    if (std::adjacent_find(keys.begin(), keys.end()) != keys.end())
-      return pos_fail(PSFM_ERR_INVALID, "an unordered image pair is listed twice");
-  }
-  if (used.empty()) return pos_fail(PSFM_ERR_INVALID, "no used image pair");
+  for (int p = 0; p < R; ++p)
+    if (!pair_used || pair_used[p]) used.push_back(p);
+  if (used.empty()) return fail(entry, PSFM_ERR_INVALID, "no used image pair");
   // views: the images of the used pairs, ascending; the first is the gauge
   std::vector<int> vidx(F, -1), views;
   {
@@ -387,13 +373,13 @@ extern "C" int psfm_estimate_global_positions(int32_t num_images, int64_t num_pa
       if (seen[f]) { vidx[f] = (int)views.size(); views.push_back(f); }
   }
   for (int f : views) {
-    if (has_orientation && !has_orientation[f]) return pos_fail(PSFM_ERR_INVALID, "a used pair's image has no orientation");
+    if (has_orientation && !has_orientation[f]) return fail(entry, PSFM_ERR_INVALID, "a used pair's image has no orientation");
     for (int k = 0; k < 4; ++k)
-      if (!std::isfinite(orientations[4 * (size_t)f + k])) return pos_fail(PSFM_ERR_INVALID, "a non-finite orientation");
+      if (!std::isfinite(orientations[4 * (size_t)f + k])) return fail(entry, PSFM_ERR_INVALID, "a non-finite orientation");
   }
   for (int p : used)
     for (int k = 0; k < 3; ++k)
-      if (!std::isfinite(pair_tvec[3 * (size_t)p + k])) return pos_fail(PSFM_ERR_INVALID, "a non-finite pair tvec");
+      if (!std::isfinite(pair_tvec[3 * (size_t)p + k])) return fail(entry, PSFM_ERR_INVALID, "a non-finite pair tvec");
   const int V = (int)views.size(), Ru = (int)used.size();
   {
     std::vector<int> parent(V);
@@ -403,16 +389,12 @@ extern "C" int psfm_estimate_global_positions(int32_t num_images, int64_t num_pa
       const int a = find_root(parent, vidx[pair_images[2 * p]]), b = find_root(parent, vidx[pair_images[2 * p + 1]]);
       if (a != b) { parent[std::max(a, b)] = std::min(a, b); --comps; }
     }
-    if (comps != 1) return pos_fail(PSFM_ERR_INVALID, "the used pairs do not form one connected graph (S is singular)");
+    if (comps != 1) return fail(entry, PSFM_ERR_INVALID, "the used pairs do not form one connected graph (S is singular)");
   }
   const long long n_ll = 3LL * (V - 1);
-  if (n_ll > kMaxUnknowns) return pos_fail(PSFM_ERR_UNSUPPORTED, "more than 2731 views (3 (V - 1) > 8190 unknowns)");
+  if (n_ll > kMaxUnknowns) return fail(entry, PSFM_ERR_UNSUPPORTED, "more than 2731 views (3 (V - 1) > 8190 unknowns)");
   const int n = (int)n_ll;
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return pos_fail(PSFM_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU path)");
-  }
+  if ((rc = require_device(entry)) != PSFM_OK) return rc;
 
   psfm_position_summary sm;
   memset(&sm, 0, sizeof(sm));
@@ -463,12 +445,7 @@ extern "C" int psfm_estimate_global_positions(int32_t num_images, int64_t num_pa
     d_z.zero(nullptr); d_u.zero(nullptr); d_ctl.zero(nullptr);
     PSFM_CUDA(cudaMemsetAsync(d_S.p, 0, sizeof(double) * (size_t)lda * lda, nullptr));
     Ctl* ctl = d_ctl.p;
-    cudaEvent_t ev[4];
-    for (auto& e : ev) PSFM_CUDA(cudaEventCreate(&e));
-    struct EvFree {
-      cudaEvent_t* e;
-      ~EvFree() { for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]); }
-    } ev_free{ev};
+    Event ev[4];
     PSFM_CUDA(cudaEventRecord(ev[0], nullptr));
     k_pos_pair<<<grid_of(Ru), 256>>>(Ru, d_pa.p, d_pb.p, d_tv.p, d_q2.p, d_d.p, d_D.p, d_rs.p, d_w.p, d_S.p, lda);
     PSFM_LAUNCH_CHECK();
@@ -545,12 +522,8 @@ extern "C" int psfm_spd_inverse(const double* A, int32_t n, double* X) {
     set_error("psfm_spd_inverse: needs 1 <= n <= 8190 (the stage's bound)");
     return PSFM_ERR_INVALID;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error("psfm_spd_inverse: no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
+  const int rc = require_device("psfm_spd_inverse");
+  if (rc != PSFM_OK) return rc;
   try {
     const int lda = n + 1, np = dense_chol_panels(n), rmax = dense_chol_rmax(n);
     DBuf<double> d_S, d_xc, d_Lp, d_Ld, d_X;

@@ -6,6 +6,7 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
 #include <string>
 
@@ -14,10 +15,16 @@
 namespace psfm {
 
 void set_error(const std::string& msg);
-// every inlier match's keypoint indices inside its images' keypoint ranges (two_view.cu; host, multi-threaded)
-bool keypoints_in_range(int64_t num_pairs, const int32_t* pair_images, const int64_t* keypoint_ptr,
-                        const int64_t* inlier_ptr, const uint32_t* inlier_matches);
+// sets "<entry>: <msg>" as the last error and returns code
+int fail(const char* entry, int code, const std::string& msg);
+// PSFM_OK, or PSFM_ERR_NO_DEVICE with "<entry>: no CUDA device available (this library has no CPU path)"
+int require_device(const char* entry);
 extern std::atomic<long long> g_launch_count;
+
+// blocks of `block` threads covering n items, at least one (a grid of zero blocks fails at launch)
+inline unsigned grid_of(long long n, int block = 256) { return (unsigned)std::max<long long>(1, (n + block - 1) / block); }
+// the same for grid-stride kernels of 256 threads, capped at 16 blocks per SM of the H100's 132
+inline unsigned grid_stride_of(long long n) { return (unsigned)std::max<long long>(1, std::min<long long>((n + 255) / 256, 132 * 16)); }
 
 struct CudaFail {
   int code;
@@ -80,6 +87,18 @@ struct DBuf {
     if (count) PSFM_CUDA(cudaMemcpyAsync(p, h, count * sizeof(T), cudaMemcpyHostToDevice, s));
   }
   void zero(cudaStream_t s) { PSFM_CUDA(cudaMemsetAsync(p, 0, (n ? n : 1) * sizeof(T), s)); }
+};
+
+// RAII CUDA event (timing enabled) that converts to cudaEvent_t; construction throws CudaFail like PSFM_CUDA
+struct Event {
+  cudaEvent_t e = nullptr;
+  Event() { PSFM_CUDA(cudaEventCreate(&e)); }
+  Event(const Event&) = delete;
+  Event& operator=(const Event&) = delete;
+  ~Event() {
+    if (e) cudaEventDestroy(e);
+  }
+  operator cudaEvent_t() const { return e; }
 };
 
 #ifdef __CUDACC__

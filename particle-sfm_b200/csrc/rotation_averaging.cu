@@ -29,6 +29,7 @@
 #include <vector>
 
 #include "dense_chol.cuh"
+#include "pair_inputs.h"
 #include "psfm_common.cuh"
 #include "quat.cuh"
 #include "rotation_recalled.cuh"
@@ -368,13 +369,6 @@ std::vector<int> largest_component(int F, const int32_t* pair_images, const std:
   return kept;
 }
 
-int rot_fail(int code, const std::string& msg) {
-  set_error("psfm_estimate_global_rotations: " + msg);
-  return code;
-}
-
-inline unsigned grid_of(long long n) { return (unsigned)std::max<long long>(1, (n + 255) / 256); }
-
 }  // namespace
 
 extern "C" void psfm_rotation_default_options(psfm_rotation_options* o) {
@@ -394,32 +388,23 @@ extern "C" int psfm_estimate_global_rotations(int32_t num_images, int64_t num_pa
                                               psfm_rotation_summary* summary) {
   const auto t0 = std::chrono::steady_clock::now();
   const long long launches0 = g_launch_count.load();
-  if (num_images < 0 || num_pairs < 0) return rot_fail(PSFM_ERR_INVALID, "negative size");
-  if (num_pairs > 0x7fffffffLL) return rot_fail(PSFM_ERR_INVALID, "more than 2^31 - 1 pairs");
+  const char* entry = "psfm_estimate_global_rotations";
+  int rc = check_sizes(entry, num_images, 0, num_pairs);
+  if (rc != PSFM_OK) return rc;
   if ((num_pairs > 0 && (!pair_images || !qvec || !num_correspondences || !pair_kept)) ||
       (num_images > 0 && (!orientations || !has_orientation)))
-    return rot_fail(PSFM_ERR_INVALID, "null argument");
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
   psfm_rotation_options o;
   psfm_rotation_default_options(&o);
   if (opts) o = *opts;
   if (!(o.max_num_l1_iterations > 0 && o.l1_step_convergence_threshold > 0.0 && o.max_num_irls_iterations > 0 &&
         o.irls_step_convergence_threshold > 0.0 && o.irls_loss_parameter_sigma > 0.0 && o.rotation_filter_max_degrees > 0.0))
-    return rot_fail(PSFM_ERR_INVALID, "options fail RobustRotationEstimator::Options::Check()");
+    return fail(entry, PSFM_ERR_INVALID, "options fail RobustRotationEstimator::Options::Check()");
   const int F = num_images, R = (int)num_pairs;
-  {
-    std::vector<uint64_t> keys(R);
-    for (int p = 0; p < R; ++p) {
-      const int a = pair_images[2 * p], b = pair_images[2 * p + 1];
-      if (a < 0 || a >= F || b < 0 || b >= F) return rot_fail(PSFM_ERR_INVALID, "an image index is outside [0, num_images)");
-      if (a == b) return rot_fail(PSFM_ERR_INVALID, "a pair of an image with itself");
-      keys[p] = ((uint64_t)std::min(a, b) << 32) | (uint64_t)std::max(a, b);
-    }
-    std::sort(keys.begin(), keys.end());
-    if (std::adjacent_find(keys.begin(), keys.end()) != keys.end())
-      return rot_fail(PSFM_ERR_INVALID, "an unordered image pair is listed twice");
-  }
+  if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
+  if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
   if (o.max_num_l1_iterations > PSFM_ROTATION_MAX_L1_ROUNDS)
-    return rot_fail(PSFM_ERR_UNSUPPORTED, "max_num_l1_iterations above PSFM_ROTATION_MAX_L1_ROUNDS");
+    return fail(entry, PSFM_ERR_UNSUPPORTED, "max_num_l1_iterations above PSFM_ROTATION_MAX_L1_ROUNDS");
 
   psfm_rotation_summary sm;
   memset(&sm, 0, sizeof(sm));
@@ -441,13 +426,12 @@ extern "C" int psfm_estimate_global_rotations(int32_t num_images, int64_t num_pa
   std::vector<char> in_comp;
   const std::vector<int> cp = largest_component(F, pair_images, posed, in_comp);
   if (cp.empty()) {
-    set_error("psfm_estimate_global_rotations: no image pair with a pose");
-    return finish(PSFM_NO_ROTATIONS);
+    return finish(fail(entry, PSFM_NO_ROTATIONS, "no image pair with a pose"));
   }
   std::vector<int> cidx(F, -1), cimg;
   for (int f = 0; f < F; ++f) if (in_comp[f]) { cidx[f] = (int)cimg.size(); cimg.push_back(f); }
   const int nc = (int)cimg.size(), n = nc - 1, Rc = (int)cp.size();
-  if (nc > kMaxComponentImages) return rot_fail(PSFM_ERR_UNSUPPORTED, "more than 8192 images in the kept component");
+  if (nc > kMaxComponentImages) return fail(entry, PSFM_ERR_UNSUPPORTED, "more than 8192 images in the kept component");
   sm.gauge_image = cimg[0];
   sm.num_images_connected = nc;
   sm.num_pairs_connected = Rc;
@@ -510,11 +494,7 @@ extern "C" int psfm_estimate_global_rotations(int32_t num_images, int64_t num_pa
     std::vector<int> fill(inc_ptr.begin(), inc_ptr.end() - 1);
     for (int i = 0; i < Rc; ++i) { inc[fill[pa[i]]++] = 2 * i; inc[fill[pb[i]]++] = 2 * i + 1; }
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return rot_fail(PSFM_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU path)");
-  }
+  if ((rc = require_device(entry)) != PSFM_OK) return rc;
   const auto t1 = std::chrono::steady_clock::now();
   std::vector<unsigned char> kept(Rc);
   try {
@@ -637,12 +617,8 @@ extern "C" int psfm_laplacian_solve(const double* A, const double* B, int32_t n,
     set_error("psfm_laplacian_solve: needs 1 <= n <= 8191 (the stage's bound)");
     return PSFM_ERR_INVALID;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    set_error("psfm_laplacian_solve: no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
+  const int rc = require_device("psfm_laplacian_solve");
+  if (rc != PSFM_OK) return rc;
   try {
     const int lda = n + 1, np = dense_chol_panels(n), rmax = dense_chol_rmax(n);
     DBuf<double> d_A, d_b, d_x, d_xc, d_Lp, d_Ld;

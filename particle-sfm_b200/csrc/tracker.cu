@@ -303,23 +303,11 @@ struct FlagToInt {
   __host__ __device__ int operator()(unsigned char f) const { return f ? 1 : 0; }
 };
 
-int device_ok() {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    set_error("no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
-  return PSFM_OK;
-}
-
-inline unsigned grid_of(size_t n) { return (unsigned)((n + 255) / 256); }
-
 }  // namespace
 
 extern "C" int psfm_grid_sample(const float* map, int32_t h, int32_t w, int32_t channels, const double* xy, int32_t n, float* out) {
   if (!map || !xy || !out || h < 2 || w < 2 || channels < 1 || channels > 2 || n < 0) return PSFM_ERR_INVALID;
-  int rc = device_ok();
+  int rc = require_device("psfm_grid_sample");
   if (rc != PSFM_OK) return rc;
   if (n == 0) return PSFM_OK;
   try {
@@ -335,7 +323,7 @@ extern "C" int psfm_grid_sample(const float* map, int32_t h, int32_t w, int32_t 
 
 extern "C" int psfm_flow_check(const float* flow_f, const float* flow_b, int32_t h, int32_t w, float thres, float* err, uint8_t* occ) {
   if (!flow_f || !flow_b || !occ || h < 2 || w < 2) return PSFM_ERR_INVALID;
-  int rc = device_ok();
+  int rc = require_device("psfm_flow_check");
   if (rc != PSFM_OK) return rc;
   try {
     const size_t hw = (size_t)h * w;
@@ -353,7 +341,7 @@ extern "C" int psfm_flow_check(const float* flow_f, const float* flow_b, int32_t
 extern "C" int psfm_tracker_step(const float* flow, const uint8_t* occ, int32_t h, int32_t w, const double* cur_xy, int32_t n,
                                  int32_t sample_ratio, double* next_xy, uint8_t* flags, uint8_t* reseed_mask) {
   if (!flow || !occ || !cur_xy || !next_xy || !flags || h < 2 || w < 2 || n < 0 || sample_ratio < 1) return PSFM_ERR_INVALID;
-  int rc = device_ok();
+  int rc = require_device("psfm_tracker_step");
   if (rc != PSFM_OK) return rc;
   try {
     const size_t hw = (size_t)h * w;
@@ -386,7 +374,7 @@ extern "C" int psfm_tracker_step(const float* flow, const uint8_t* occ, int32_t 
 extern "C" int psfm_tracker_buffer_inputs(const float* flow01, const float* flow02, const uint8_t* occ02, int32_t h, int32_t w,
                                           const double* x0, int32_t n, double upper_flow, double* ref1, double* ref2, double* scale) {
   if (!flow01 || !flow02 || !occ02 || !x0 || !ref1 || !ref2 || !scale || h < 2 || w < 2 || n < 0) return PSFM_ERR_INVALID;
-  int rc = device_ok();
+  int rc = require_device("psfm_tracker_buffer_inputs");
   if (rc != PSFM_OK) return rc;
   if (n == 0) return PSFM_OK;
   try {
@@ -467,15 +455,10 @@ struct psfm_tracker {
 
 namespace {
 
-int tracker_fail(const std::string& msg) {
-  set_error(msg);
-  return PSFM_ERR_INVALID;
-}
-
 // argument check shared by the calls on a handle: PSFM_OK or the error to return
 int tracker_usable(const psfm_tracker* T, bool args_ok, const char* fn) {
-  if (!T || !args_ok) return tracker_fail(std::string(fn) + ": null argument");
-  if (T->failed) return tracker_fail(std::string(fn) + ": an earlier call on this tracker failed; destroy it");
+  if (!T || !args_ok) return fail(fn, PSFM_ERR_INVALID, "null argument");
+  if (T->failed) return fail(fn, PSFM_ERR_INVALID, "an earlier call on this tracker failed; destroy it");
   return PSFM_OK;
 }
 
@@ -488,9 +471,9 @@ int tracker_broken(psfm_tracker* T, int code) {
 
 extern "C" int psfm_flow_check_device(const float* d_flow_f, const float* d_flow_b, int32_t h, int32_t w, float thres, float* d_err,
                                       uint8_t* d_occ, void* stream) {
-  if (!d_flow_f || !d_flow_b || !d_occ) return tracker_fail("psfm_flow_check_device: null argument");
-  if (h < 2 || w < 2) return tracker_fail("psfm_flow_check_device: bad sizes");
-  int rc = device_ok();
+  if (!d_flow_f || !d_flow_b || !d_occ) return fail("psfm_flow_check_device", PSFM_ERR_INVALID, "null argument");
+  if (h < 2 || w < 2) return fail("psfm_flow_check_device", PSFM_ERR_INVALID, "bad sizes");
+  int rc = require_device("psfm_flow_check_device");
   if (rc != PSFM_OK) return rc;
   try {
     const size_t hw = (size_t)h * w;
@@ -501,10 +484,10 @@ extern "C" int psfm_flow_check_device(const float* d_flow_f, const float* d_flow
 }
 
 extern "C" int psfm_tracker_create(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, void* stream, psfm_tracker** out) {
-  if (!out) return tracker_fail("psfm_tracker_create: null argument");
+  if (!out) return fail("psfm_tracker_create", PSFM_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (h < 2 || w < 2 || sample_ratio < 1 || num_frames < 1) return tracker_fail("psfm_tracker_create: bad sizes");
-  int rc = device_ok();
+  if (h < 2 || w < 2 || sample_ratio < 1 || num_frames < 1) return fail("psfm_tracker_create", PSFM_ERR_INVALID, "bad sizes");
+  int rc = require_device("psfm_tracker_create");
   if (rc != PSFM_OK) return rc;
   psfm_tracker* T = new psfm_tracker;
   try {
@@ -531,13 +514,14 @@ extern "C" int psfm_tracker_create(int32_t h, int32_t w, int32_t sample_ratio, i
 
 extern "C" int psfm_tracker_advance(psfm_tracker* T, const float* d_flow, const uint8_t* d_occ, const float* d_flow_prev,
                                     const float* d_flow2_prev, const uint8_t* d_occ2_prev, int32_t* counts) {
-  int rc = tracker_usable(T, d_flow && d_occ, "psfm_tracker_advance");
+  const char* entry = "psfm_tracker_advance";
+  int rc = tracker_usable(T, d_flow && d_occ, entry);
   if (rc != PSFM_OK) return rc;
-  if (T->finished) return tracker_fail("psfm_tracker_advance: the track set was already assembled");
-  if (T->n_buf > 0) return tracker_fail("psfm_tracker_advance: the buffered set of the previous frame was not optimised");
-  if (T->t + 1 >= T->num_frames) return tracker_fail("psfm_tracker_advance: more frames than the tracker was created for");
+  if (T->finished) return fail(entry, PSFM_ERR_INVALID, "the track set was already assembled");
+  if (T->n_buf > 0) return fail(entry, PSFM_ERR_INVALID, "the buffered set of the previous frame was not optimised");
+  if (T->t + 1 >= T->num_frames) return fail(entry, PSFM_ERR_INVALID, "more frames than the tracker was created for");
   if (T->t >= 1 && (!d_flow_prev || !d_flow2_prev || !d_occ2_prev))
-    return tracker_fail("psfm_tracker_advance: from frame 1 on, flows[t-1], flows_f2[t-1] and occ_maps_s2[t-1] are needed");
+    return fail(entry, PSFM_ERR_INVALID, "from frame 1 on, flows[t-1], flows_f2[t-1] and occ_maps_s2[t-1] are needed");
   try {
     cudaStream_t st = T->st;
     const int t = T->t, G = T->gh * T->gw, H = T->h, W = T->w;
@@ -647,7 +631,7 @@ extern "C" int psfm_tracker_optimize(psfm_tracker* T, const psfm_traj_options* o
   if (summary) memset(summary, 0, sizeof(*summary));
   int rc = tracker_usable(T, true, "psfm_tracker_optimize");
   if (rc != PSFM_OK) return rc;
-  if (T->n_buf <= 0) return tracker_fail("psfm_tracker_optimize: no buffered trajectory");
+  if (T->n_buf <= 0) return fail("psfm_tracker_optimize", PSFM_ERR_INVALID, "no buffered trajectory");
   try {
     // HP1 runs on the tracker's stream, after k_buffer_inputs.  NULL (the legacy default stream) is passed as
     // cudaStreamLegacy: a NULL stream would make solve_device use the HP1 workspace's non-blocking stream, which
@@ -662,7 +646,7 @@ extern "C" int psfm_tracker_optimize(psfm_tracker* T, const psfm_traj_options* o
 extern "C" int psfm_tracker_get_buffer(psfm_tracker* T, double* uv12, double* ref1, double* ref2, double* scale) {
   int rc = tracker_usable(T, uv12 && ref1 && ref2 && scale, "psfm_tracker_get_buffer");
   if (rc != PSFM_OK) return rc;
-  if (T->n_buf <= 0) return tracker_fail("psfm_tracker_get_buffer: no buffered trajectory");
+  if (T->n_buf <= 0) return fail("psfm_tracker_get_buffer", PSFM_ERR_INVALID, "no buffered trajectory");
   try {
     const size_t n = T->n_buf;
     PSFM_CUDA(cudaMemcpyAsync(uv12, T->buv.p, 4 * n * sizeof(double), cudaMemcpyDeviceToHost, T->st));
@@ -677,7 +661,7 @@ extern "C" int psfm_tracker_get_buffer(psfm_tracker* T, double* uv12, double* re
 extern "C" int psfm_tracker_set_buffer(psfm_tracker* T, const double* uv12) {
   int rc = tracker_usable(T, uv12 != nullptr, "psfm_tracker_set_buffer");
   if (rc != PSFM_OK) return rc;
-  if (T->n_buf <= 0) return tracker_fail("psfm_tracker_set_buffer: no buffered trajectory");
+  if (T->n_buf <= 0) return fail("psfm_tracker_set_buffer", PSFM_ERR_INVALID, "no buffered trajectory");
   try {
     PSFM_CUDA(cudaMemcpyAsync(T->bout.p, uv12, 4 * (size_t)T->n_buf * sizeof(double), cudaMemcpyHostToDevice, T->st));
     rc = tracker_writeback(T);
@@ -689,8 +673,8 @@ extern "C" int psfm_tracker_set_buffer(psfm_tracker* T, const double* uv12) {
 extern "C" int psfm_tracker_finish(psfm_tracker* T, int32_t traj_min_len, int64_t* num_trajs, int64_t* num_obs) {
   int rc = tracker_usable(T, num_trajs && num_obs, "psfm_tracker_finish");
   if (rc != PSFM_OK) return rc;
-  if (T->finished) return tracker_fail("psfm_tracker_finish: already finished");
-  if (T->n_buf > 0) return tracker_fail("psfm_tracker_finish: the buffered set of the last frame was not optimised");
+  if (T->finished) return fail("psfm_tracker_finish", PSFM_ERR_INVALID, "already finished");
+  if (T->n_buf > 0) return fail("psfm_tracker_finish", PSFM_ERR_INVALID, "the buffered set of the last frame was not optimised");
   try {
     cudaStream_t st = T->st;
     const int t = T->t;
@@ -735,7 +719,7 @@ extern "C" int psfm_tracker_finish(psfm_tracker* T, int32_t traj_min_len, int64_
 extern "C" int psfm_tracker_result(psfm_tracker* T, int64_t* ids, int64_t* ptr, int32_t* frame_ids, double* xy) {
   int rc = tracker_usable(T, ids && ptr && frame_ids && xy, "psfm_tracker_result");
   if (rc != PSFM_OK) return rc;
-  if (!T->finished) return tracker_fail("psfm_tracker_result: call psfm_tracker_finish first");
+  if (!T->finished) return fail("psfm_tracker_result", PSFM_ERR_INVALID, "call psfm_tracker_finish first");
   try {
     const size_t nt = T->res_trajs, m = T->res_obs;
     if (T->next_id == 0) { ptr[0] = 0; return PSFM_OK; }

@@ -595,16 +595,6 @@ extern "C" void psfm_traj_default_options(psfm_traj_options* o) {
   o->jacobi_scaling = 1;
 }
 
-static int traj_check_device() {
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    set_error("no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
-  return PSFM_OK;
-}
-
 extern "C" int psfm_traj_optimize_device(const double* d_uv12, const double* d_ref1, const double* d_ref2,
                                          const double* d_scale, const float* d_flow12, int32_t n, int32_t w,
                                          int32_t h, const psfm_traj_options* opts, double* d_out_uv12,
@@ -612,7 +602,7 @@ extern "C" int psfm_traj_optimize_device(const double* d_uv12, const double* d_r
   if (summary) memset(summary, 0, sizeof(*summary));
   if (n < 0 || w <= 0 || h <= 0) { set_error("psfm_traj_optimize: bad sizes"); return PSFM_ERR_INVALID; }
   if (n == 0) return PSFM_OK;
-  int rc = traj_check_device();
+  int rc = require_device("psfm_traj_optimize_device");
   if (rc != PSFM_OK) return rc;
   return traj::solve_device(d_uv12, d_ref1, d_ref2, d_scale, d_flow12, n, w, h, opts, d_out_uv12, summary,
                             (cudaStream_t)stream);
@@ -624,7 +614,7 @@ extern "C" int psfm_traj_optimize(const double* uv12, const double* ref1, const 
   if (summary) memset(summary, 0, sizeof(*summary));
   if (n < 0 || w <= 0 || h <= 0) { set_error("psfm_traj_optimize: bad sizes"); return PSFM_ERR_INVALID; }
   if (n == 0) return PSFM_OK;
-  int rc = traj_check_device();
+  int rc = require_device("psfm_traj_optimize");
   if (rc != PSFM_OK) return rc;
   traj::Workspace& ws = traj::g_ws;
   std::lock_guard<std::mutex> lock(ws.mu);

@@ -29,7 +29,6 @@
 // Memory: the sort holds 24 bytes per directed entry (48 per match) with the matches (8) beside it; from the replay on,
 // 8 bytes per match (the neighbour lists) and about 70 bytes per keypoint stay resident.  The handle keeps 20 bytes per
 // keypoint (keypoint, image, point row) for psfm_ba_create_from_triangulation beside the points and tracks.
-#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
@@ -38,8 +37,10 @@
 #include <vector>
 
 #include "dlt.cuh"
+#include "pair_inputs.h"
 #include "psfm_common.cuh"
 #include "quat.cuh"
+#include "radix_sort.cuh"
 #include "triangulation_handle.cuh"
 #include "triangulation_recalled.cuh"
 
@@ -84,8 +85,6 @@ struct Ctx {
   long long trial_cap;             // the RANSAC constructor's cap of max_num_trials
 };
 
-inline unsigned grid_of(long long n) { return (unsigned)std::max<long long>(1, (n + 255) / 256); }
-inline unsigned grid_stride_of(long long n) { return (unsigned)std::max<long long>(1, std::min<long long>((n + 255) / 256, 132 * 16)); }
 
 __device__ __forceinline__ int pair_of(const long long* iptr, int R, long long i) {
   int lo = 0, hi = R;
@@ -614,27 +613,6 @@ __global__ void k_kp_points(long long K, const int* __restrict__ pt_of, const in
   out[k] = pt_of[k] >= 0 ? new_id[pt_of[k]] : -1;
 }
 
-template <typename K, typename V>
-void sort_pairs(cub::DoubleBuffer<K>& keys, cub::DoubleBuffer<V>& vals, long long n, int end_bit) {
-  size_t bytes = 0;
-  PSFM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys, vals, n, 0, end_bit, nullptr));
-  DBuf<unsigned char> tmp;
-  tmp.alloc(bytes);
-  PSFM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, keys, vals, n, 0, end_bit, nullptr));
-  PSFM_LAUNCH_CHECK();
-}
-
-int tri_fail(int code, const std::string& msg) {
-  set_error("psfm_triangulation_create: " + msg);
-  return code;
-}
-
-int bits_for(unsigned long long v) {
-  int b = 1;
-  while (b < 64 && (v >> b)) ++b;
-  return b;
-}
-
 }  // namespace
 
 // ---- hand-off to the bundle adjustment (psfm_ba_create_from_triangulation) ------------------------------------------
@@ -712,13 +690,14 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
                                          int64_t* num_points3D, int64_t* num_track_elements) {
   const auto t0 = std::chrono::steady_clock::now();
   const long long launches0 = g_launch_count.load();
-  if (!out) return tri_fail(PSFM_ERR_INVALID, "null argument");
+  const char* entry = "psfm_triangulation_create";
+  if (!out) return fail(entry, PSFM_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (num_images < 0 || num_cameras < 0 || num_pairs < 0) return tri_fail(PSFM_ERR_INVALID, "negative size");
-  if (num_pairs > 0x7fffffffLL) return tri_fail(PSFM_ERR_INVALID, "more than 2^31 - 1 pairs");
+  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+  if (rc != PSFM_OK) return rc;
   if (!keypoint_ptr || (num_images > 0 && (!image_camera || !orientations || !image_tvec || !registered)) ||
       (num_cameras > 0 && (!cameras || !camera_size)) || (num_pairs > 0 && (!pair_images || !inlier_ptr)))
-    return tri_fail(PSFM_ERR_INVALID, "null argument");
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
   psfm_triangulator_options o;
   psfm_triangulator_default_options(&o);
   if (opts) o = *opts;
@@ -726,35 +705,21 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
         o.min_focal_length_ratio > 0 && o.max_focal_length_ratio > 0 && o.max_extra_param >= 0 &&
         std::isfinite(o.create_max_angle_error) && std::isfinite(o.continue_max_angle_error) && std::isfinite(o.min_angle) &&
         std::isfinite(o.min_focal_length_ratio) && std::isfinite(o.max_focal_length_ratio) && std::isfinite(o.max_extra_param)))
-    return tri_fail(PSFM_ERR_INVALID, "options fail the IncrementalTriangulator::Options Check()");
-  if (o.max_transitivity != 1) return tri_fail(PSFM_ERR_UNSUPPORTED, "max_transitivity != 1 is not supported");
+    return fail(entry, PSFM_ERR_INVALID, "options fail the IncrementalTriangulator::Options Check()");
+  if (o.max_transitivity != 1) return fail(entry, PSFM_ERR_UNSUPPORTED, "max_transitivity != 1 is not supported");
   const int F = num_images, R = (int)num_pairs;
-  if (keypoint_ptr[0] != 0) return tri_fail(PSFM_ERR_INVALID, "keypoint_ptr[0] must be 0");
-  for (int f = 0; f < F; ++f)
-    if (keypoint_ptr[f + 1] < keypoint_ptr[f]) return tri_fail(PSFM_ERR_INVALID, "keypoint_ptr must be non-decreasing");
+  if ((rc = check_keypoint_ptr(entry, F, keypoint_ptr)) != PSFM_OK) return rc;
   const long long K = keypoint_ptr[F];
-  if (K >= 0x7fffffffLL) return tri_fail(PSFM_ERR_UNSUPPORTED, "2^31 - 1 keypoints or more");
-  if (K > 0 && !keypoints) return tri_fail(PSFM_ERR_INVALID, "null argument");
-  for (int f = 0; f < F; ++f)
-    if (image_camera[f] < 0 || image_camera[f] >= num_cameras) return tri_fail(PSFM_ERR_INVALID, "a camera index is outside [0, num_cameras)");
-  for (int i = 0; i < num_cameras; ++i)
-    if (!(camera_size[2 * i] > 0 && camera_size[2 * i + 1] > 0)) return tri_fail(PSFM_ERR_INVALID, "a camera size <= 0");
+  if (K >= 0x7fffffffLL) return fail(entry, PSFM_ERR_UNSUPPORTED, "2^31 - 1 keypoints or more");
+  if (K > 0 && !keypoints) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  if ((rc = check_image_cameras(entry, F, image_camera, num_cameras)) != PSFM_OK) return rc;
+  if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
   if (R > 0) {
-    if (inlier_ptr[0] != 0) return tri_fail(PSFM_ERR_INVALID, "inlier_ptr[0] must be 0");
-    std::vector<uint64_t> keys(R);
-    for (int p = 0; p < R; ++p) {
-      if (inlier_ptr[p + 1] < inlier_ptr[p]) return tri_fail(PSFM_ERR_INVALID, "inlier_ptr must be non-decreasing");
-      const int a = pair_images[2 * p], b = pair_images[2 * p + 1];
-      if (a < 0 || a >= F || b < 0 || b >= F) return tri_fail(PSFM_ERR_INVALID, "an image index is outside [0, num_images)");
-      if (a == b) return tri_fail(PSFM_ERR_INVALID, "a pair of an image with itself");
-      keys[p] = ((uint64_t)std::min(a, b) << 32) | (uint64_t)std::max(a, b);
-    }
-    std::sort(keys.begin(), keys.end());
-    if (std::adjacent_find(keys.begin(), keys.end()) != keys.end())
-      return tri_fail(PSFM_ERR_INVALID, "an unordered image pair is listed twice");
-    if (inlier_ptr[R] > 0 && !inlier_matches) return tri_fail(PSFM_ERR_INVALID, "null argument");
-    if (!keypoints_in_range(R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches))
-      return tri_fail(PSFM_ERR_INVALID, "a keypoint index is outside its image's keypoints");
+    if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
+    if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
+    if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
+    if (inlier_ptr[R] > 0 && !inlier_matches) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
   }
   // per image: P = [R | t], the projection centre -R' t, qvec, tvec; eligible = registered with a non-bogus camera
   // (Camera::HasBogusParams, SIMPLE_PINHOLE: principal point in [0, w] x [0, h], f / max(w, h) in the ratio range)
@@ -765,11 +730,11 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
     const double* q = orientations + 4 * (size_t)f;
     const double* t = image_tvec + 3 * (size_t)f;
     for (int i = 0; i < 4; ++i)
-      if (!std::isfinite(q[i])) return tri_fail(PSFM_ERR_INVALID, "a registered image with a non-finite pose");
+      if (!std::isfinite(q[i])) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
     for (int i = 0; i < 3; ++i)
-      if (!std::isfinite(t[i])) return tri_fail(PSFM_ERR_INVALID, "a registered image with a non-finite pose");
+      if (!std::isfinite(t[i])) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
     const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    if (!(n > 0.0)) return tri_fail(PSFM_ERR_INVALID, "a registered image with a non-finite pose");
+    if (!(n > 0.0)) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
     const double w = q[0] / n, x = q[1] / n, y = q[2] / n, z = q[3] / n;
     const double Rm[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y),
                           2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x),
@@ -789,23 +754,14 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
     const double ratio = fl / std::max(wd, ht);
     elig[f] = !(bogus_pp || ratio < o.min_focal_length_ratio || ratio > o.max_focal_length_ratio);
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return tri_fail(PSFM_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU path)");
-  }
+  if ((rc = require_device(entry)) != PSFM_OK) return rc;
   const long long N = R > 0 ? inlier_ptr[R] : 0, E = 2 * N;
   psfm_triangulation_summary sm;
   memset(&sm, 0, sizeof(sm));
   sm.host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   auto h = new psfm_triangulation();
   try {
-    cudaEvent_t ev[5];
-    for (auto& e : ev) PSFM_CUDA(cudaEventCreate(&e));
-    struct EvFree {
-      cudaEvent_t* e;
-      ~EvFree() { for (int i = 0; i < 5; ++i) cudaEventDestroy(e[i]); }
-    } ev_free{ev};
+    Event ev[5];
     // the keypoints, their images and keypoint_ptr stay with the handle for psfm_ba_create_from_triangulation
     DBuf<long long>& d_kp_ptr = h->kp_ptr;
     DBuf<float2>& d_kps = h->kps;
@@ -841,7 +797,6 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
     }
     d_flag.zero(nullptr); d_cnt.zero(nullptr);
     const unsigned sentinel = (unsigned)K;
-    const int key_bits = bits_for((unsigned long long)K);
     PSFM_CUDA(cudaEventRecord(ev[0], nullptr));
     // ---- graph
     k_kp_image<<<std::max(F, 1), 256>>>(F, d_kp_ptr.p, d_img_of.p, d_pt_of.p, d_parent.p, d_active.p);
@@ -851,7 +806,7 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
     PSFM_LAUNCH_CHECK();
     cub::DoubleBuffer<unsigned> keys(d_key0.p, d_key1.p);
     cub::DoubleBuffer<u64> vals(d_val0.p, d_val1.p);
-    sort_pairs(keys, vals, E, key_bits);
+    sort_pairs(keys, vals, E, key_bits((unsigned long long)K));
     const unsigned* skey = keys.Current();
     const u64* sval = vals.Current();
     d_nbr.alloc(E);

@@ -27,14 +27,13 @@
 //     reference reads an unset R; here candidate 0, tri_angle 0.
 // Memory: 8 bytes per match (its indices) and 1 byte (its mask) during steps 2-4, 24 bytes per kept match in the
 // sorts (the matches are released before them): about 21 GB at the DAVIS shape (636 M matches).
-#include <cub/device/device_radix_sort.cuh>
-
 #include <algorithm>
-#include <thread>
 #include <vector>
 
 #include "dlt.cuh"
+#include "pair_inputs.h"
 #include "psfm_common.cuh"
+#include "radix_sort.cuh"
 
 namespace {
 
@@ -449,56 +448,7 @@ __global__ void k_median(int R, const long long* __restrict__ run_start, const l
   tri_angle[p] = m;
 }
 
-int two_view_fail(const std::string& msg) {
-  set_error("psfm_two_view_relative_poses: " + msg);
-  return PSFM_ERR_INVALID;
-}
-
-inline unsigned grid_of(long long n) { return (unsigned)((n + 255) / 256); }
-inline unsigned grid_stride_of(long long n) { return (unsigned)std::max<long long>(1, std::min<long long>((n + 255) / 256, 132 * 16)); }
-
-template <typename K, typename V>
-void sort_pairs(cub::DoubleBuffer<K>& keys, cub::DoubleBuffer<V>& vals, long long n, int end_bit) {
-  size_t bytes = 0;
-  PSFM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, keys, vals, n, 0, end_bit, nullptr));
-  DBuf<unsigned char> tmp;
-  tmp.alloc(bytes);
-  PSFM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, bytes, keys, vals, n, 0, end_bit, nullptr));
-  PSFM_LAUNCH_CHECK();
-}
-
 }  // namespace
-
-// every match's keypoint indices inside its images' keypoint ranges (host, split over threads: up to 10^9 indices)
-bool psfm::keypoints_in_range(int64_t R, const int32_t* pair_images, const int64_t* kp_ptr, const int64_t* iptr, const uint32_t* m) {
-  const unsigned nt = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
-  std::vector<char> ok(nt, 1);
-  std::vector<std::thread> th;
-  const long long N = iptr[R];
-  for (unsigned w = 0; w < nt; ++w)
-    th.emplace_back([&, w] {
-      const long long lo = N * w / nt, hi = N * (w + 1) / nt;
-      if (lo >= hi) return;
-      int64_t p = std::upper_bound(iptr, iptr + R + 1, (int64_t)lo) - iptr - 1;
-      for (long long i = lo; i < hi;) {
-        while (iptr[p + 1] <= i) ++p;
-        const long long e = std::min<long long>(hi, iptr[p + 1]);
-        const uint64_t na = (uint64_t)(kp_ptr[pair_images[2 * p] + 1] - kp_ptr[pair_images[2 * p]]);
-        const uint64_t nb = (uint64_t)(kp_ptr[pair_images[2 * p + 1] + 1] - kp_ptr[pair_images[2 * p + 1]]);
-        uint32_t ma = 0, mb = 0;
-        bool any = false;
-        for (long long k = i; k < e; ++k) {
-          ma = std::max(ma, m[2 * k]);
-          mb = std::max(mb, m[2 * k + 1]);
-          any = true;
-        }
-        if (any && ((uint64_t)ma >= na || (uint64_t)mb >= nb)) { ok[w] = 0; return; }
-        i = e;
-      }
-    });
-  for (auto& t : th) t.join();
-  return std::all_of(ok.begin(), ok.end(), [](char c) { return c != 0; });
-}
 
 extern "C" int psfm_two_view_relative_poses(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
                                             const int32_t* image_camera, const double* cameras, int32_t num_cameras,
@@ -506,36 +456,24 @@ extern "C" int psfm_two_view_relative_poses(int32_t num_images, const int64_t* k
                                             const double* E, const double* F, const double* H, const int64_t* inlier_ptr,
                                             const uint32_t* inlier_matches, double* qvec, double* tvec, double* tri_angle,
                                             int32_t* config_out, int64_t* num_points3D, uint8_t* estimated) {
-  if (num_images < 0 || num_cameras < 0 || num_pairs < 0) return two_view_fail("negative size");
-  if (num_pairs > 0x7fffffffLL) return two_view_fail("more than 2^31 - 1 pairs");
+  const char* entry = "psfm_two_view_relative_poses";
+  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+  if (rc != PSFM_OK) return rc;
   if (num_pairs > 0 && (!keypoint_ptr || !image_camera || !cameras || !pair_images || !config || !E || !F || !H ||
                         !inlier_ptr || !qvec || !tvec || !tri_angle || !config_out || !num_points3D || !estimated))
-    return two_view_fail("null argument");
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
   const int R = (int)num_pairs;
   if (R > 0) {
-    if (keypoint_ptr[0] != 0) return two_view_fail("keypoint_ptr[0] must be 0");
-    for (int32_t f = 0; f < num_images; ++f)
-      if (keypoint_ptr[f + 1] < keypoint_ptr[f]) return two_view_fail("keypoint_ptr must be non-decreasing");
-    for (int32_t f = 0; f < num_images; ++f)
-      if (image_camera[f] < 0 || image_camera[f] >= num_cameras) return two_view_fail("a camera index is outside [0, num_cameras)");
-    if (inlier_ptr[0] != 0) return two_view_fail("inlier_ptr[0] must be 0");
-    for (int p = 0; p < R; ++p) {
-      if (inlier_ptr[p + 1] < inlier_ptr[p]) return two_view_fail("inlier_ptr must be non-decreasing");
-      for (int k = 0; k < 2; ++k)
-        if (pair_images[2 * p + k] < 0 || pair_images[2 * p + k] >= num_images)
-          return two_view_fail("an image index is outside [0, num_images)");
-    }
+    // no check_distinct_pairs: this stage accepts self pairs and repeated pairs
+    if ((rc = check_keypoint_ptr(entry, num_images, keypoint_ptr)) != PSFM_OK) return rc;
+    if ((rc = check_image_cameras(entry, num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
+    if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
+    if ((rc = check_pair_images(entry, R, pair_images, num_images)) != PSFM_OK) return rc;
     if (inlier_ptr[R] > 0 && (!inlier_matches || (keypoint_ptr[num_images] > 0 && !keypoints)))
-      return two_view_fail("null argument");
-    if (!keypoints_in_range(R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches))
-      return two_view_fail("a keypoint index is outside its image's keypoints");
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
   }
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
-    cudaGetLastError();
-    set_error("no CUDA device available (this library has no CPU path)");
-    return PSFM_ERR_NO_DEVICE;
-  }
+  if ((rc = require_device(entry)) != PSFM_OK) return rc;
   if (R == 0) return PSFM_OK;
   const long long N = inlier_ptr[R], K = keypoint_ptr[num_images];
   try {
@@ -600,9 +538,7 @@ extern "C" int psfm_two_view_relative_poses(int32_t num_images, const int64_t* k
     sort_pairs(keys, vals, M, 64);
     cub::DoubleBuffer<int> pkeys(vals.Current(), vals.Alternate());
     cub::DoubleBuffer<double> pvals(keys.Current(), keys.Alternate());
-    int bits = 1;
-    while (bits < 31 && ((R - 1) >> bits)) ++bits;
-    sort_pairs(pkeys, pvals, M, bits);
+    sort_pairs(pkeys, pvals, M, key_bits(R - 1));
     DBuf<long long> d_run;
     d_run.alloc((size_t)R + 1);
     d_run.upload(run_start.data(), (size_t)R + 1, nullptr);

@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "dlt.cuh"
+#include "pair_inputs.h"
 #include "psfm_common.cuh"
 #include "verification_recalled.cuh"
 
@@ -684,11 +685,6 @@ __global__ void k_compact(int R, const long long* __restrict__ mptr, const long 
   for (long long j = threadIdx.x; j < n; j += blockDim.x) out[o + j] = m[b + inl_idx[b + j]];
 }
 
-int ver_fail(int code, const std::string& msg) {
-  set_error("psfm_verify_two_view_geometries: " + msg);
-  return code;
-}
-
 }  // namespace
 
 extern "C" void psfm_verification_default_options(psfm_verification_options* o) {
@@ -716,11 +712,12 @@ extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t
                                                int32_t* pair_trials, psfm_verification_summary* summary) {
   const auto t0 = std::chrono::steady_clock::now();
   const long long launches0 = g_launch_count.load();
-  if (num_images < 0 || num_cameras < 0 || num_pairs < 0) return ver_fail(PSFM_ERR_INVALID, "negative size");
-  if (num_pairs > 0x7fffffffLL) return ver_fail(PSFM_ERR_INVALID, "more than 2^31 - 1 pairs");
+  const char* entry = "psfm_verify_two_view_geometries";
+  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+  if (rc != PSFM_OK) return rc;
   if (!keypoint_ptr || (num_images > 0 && !image_camera) || (num_cameras > 0 && !camera_size) ||
       (num_pairs > 0 && (!pair_images || !match_ptr || !config || !F || !E || !H)) || !inlier_ptr)
-    return ver_fail(PSFM_ERR_INVALID, "null argument");
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
   psfm_verification_options o;
   psfm_verification_default_options(&o);
   if (opts) o = *opts;
@@ -729,43 +726,29 @@ extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t
         o.dyn_num_trials_multiplier > 0 && o.max_H_inlier_ratio >= 0 && o.watermark_min_inlier_ratio >= 0 &&
         o.watermark_min_inlier_ratio <= 1 && o.watermark_border_size >= 0 && o.watermark_border_size <= 1 &&
         std::isfinite(o.max_error) && std::isfinite(o.dyn_num_trials_multiplier) && std::isfinite(o.max_H_inlier_ratio)))
-    return ver_fail(PSFM_ERR_INVALID, "options fail the TwoViewGeometry::Options Check()");
+    return fail(entry, PSFM_ERR_INVALID, "options fail the TwoViewGeometry::Options Check()");
   const int Fimg = num_images, R = (int)num_pairs;
-  if (keypoint_ptr[0] != 0) return ver_fail(PSFM_ERR_INVALID, "keypoint_ptr[0] must be 0");
-  for (int f = 0; f < Fimg; ++f)
-    if (keypoint_ptr[f + 1] < keypoint_ptr[f]) return ver_fail(PSFM_ERR_INVALID, "keypoint_ptr must be non-decreasing");
+  if ((rc = check_keypoint_ptr(entry, Fimg, keypoint_ptr)) != PSFM_OK) return rc;
   const long long K = keypoint_ptr[Fimg];
-  if (K > 0 && !keypoints) return ver_fail(PSFM_ERR_INVALID, "null argument");
-  for (int f = 0; f < Fimg; ++f)
-    if (image_camera[f] < 0 || image_camera[f] >= num_cameras)
-      return ver_fail(PSFM_ERR_INVALID, "a camera index is outside [0, num_cameras)");
-  for (int i = 0; i < num_cameras; ++i)
-    if (!(camera_size[2 * i] > 0 && camera_size[2 * i + 1] > 0)) return ver_fail(PSFM_ERR_INVALID, "a camera size <= 0");
+  if (K > 0 && !keypoints) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  if ((rc = check_image_cameras(entry, Fimg, image_camera, num_cameras)) != PSFM_OK) return rc;
+  if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
   long long M = 0;
   if (R > 0) {
-    if (match_ptr[0] != 0) return ver_fail(PSFM_ERR_INVALID, "match_ptr[0] must be 0");
-    std::vector<uint64_t> keys(R);
-    for (int p = 0; p < R; ++p) {
-      if (match_ptr[p + 1] < match_ptr[p]) return ver_fail(PSFM_ERR_INVALID, "match_ptr must be non-decreasing");
+    if ((rc = check_match_ptr(entry, "match_ptr", R, match_ptr)) != PSFM_OK) return rc;
+    for (int p = 0; p < R; ++p)
       if (match_ptr[p + 1] - match_ptr[p] > 0x7fffffffLL)
-        return ver_fail(PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
-      const int a = pair_images[2 * p], b = pair_images[2 * p + 1];
-      if (a < 0 || a >= Fimg || b < 0 || b >= Fimg) return ver_fail(PSFM_ERR_INVALID, "an image index is outside [0, num_images)");
-      if (a == b) return ver_fail(PSFM_ERR_INVALID, "a pair of an image with itself");
-      keys[p] = ((uint64_t)std::min(a, b) << 32) | (uint64_t)std::max(a, b);
-    }
-    std::sort(keys.begin(), keys.end());
-    if (std::adjacent_find(keys.begin(), keys.end()) != keys.end())
-      return ver_fail(PSFM_ERR_INVALID, "an unordered image pair is listed twice");
+        return fail(entry, PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
+    if ((rc = check_pair_images(entry, R, pair_images, Fimg)) != PSFM_OK) return rc;
+    if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
     M = match_ptr[R];
-    if (M > 0 && (!matches || !inlier_matches)) return ver_fail(PSFM_ERR_INVALID, "null argument");
-    if (!keypoints_in_range(R, pair_images, keypoint_ptr, match_ptr, matches))
-      return ver_fail(PSFM_ERR_INVALID, "a keypoint index is outside its image's keypoints");
+    if (M > 0 && (!matches || !inlier_matches)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, match_ptr, matches)) != PSFM_OK) return rc;
     if (prior_focal_length)
       for (int p = 0; p < R; ++p)
         if (prior_focal_length[image_camera[pair_images[2 * p]]] && prior_focal_length[image_camera[pair_images[2 * p + 1]]])
-          return ver_fail(PSFM_ERR_UNSUPPORTED,
-                          "both cameras of a pair have a prior focal length (EstimateCalibrated is not supported)");
+          return fail(entry, PSFM_ERR_UNSUPPORTED,
+                      "both cameras of a pair have a prior focal length (EstimateCalibrated is not supported)");
   }
   psfm_verification_summary sm;
   memset(&sm, 0, sizeof(sm));
@@ -775,11 +758,7 @@ extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t
     if (summary) *summary = sm;
     return PSFM_OK;
   }
-  int ndev = 0;
-  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
-    cudaGetLastError();
-    return ver_fail(PSFM_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU path)");
-  }
+  if ((rc = require_device(entry)) != PSFM_OK) return rc;
   std::vector<int> sizes(4 * (size_t)R);
   for (int p = 0; p < R; ++p)
     for (int k = 0; k < 2; ++k) {
@@ -789,12 +768,7 @@ extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t
     }
   sm.host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   try {
-    cudaEvent_t ev[4];
-    for (auto& e : ev) PSFM_CUDA(cudaEventCreate(&e));
-    struct EvFree {
-      cudaEvent_t* e;
-      ~EvFree() { for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]); }
-    } ev_free{ev};
+    Event ev[4];
     DBuf<long long> d_kp_ptr, d_mptr, d_iptr, d_count;
     DBuf<float2> d_kps;
     DBuf<int2> d_pairs, d_sizes;

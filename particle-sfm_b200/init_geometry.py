@@ -37,6 +37,23 @@ def _ptr(sizes):
     return p
 
 
+def _pair_graph(keypoint_ptr, keypoints, image_camera, pair_images, ptr, matches):
+    """The image-pair graph the pair stages take, as the library reads it: keypoint_ptr [F + 1] int64, keypoints [K][2]
+    float32, image_camera [F] int32, pair_images [R][2] int32, ptr [R + 1] int64 (inlier_ptr or match_ptr) and
+    matches [N][2] uint32, all contiguous.  Raises ValueError when the sizes do not describe one graph."""
+    kp_ptr = np.ascontiguousarray(keypoint_ptr, np.int64)
+    kps = np.ascontiguousarray(keypoints, np.float32).reshape(-1, 2)
+    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
+    ptr = np.ascontiguousarray(ptr, np.int64)
+    m = np.ascontiguousarray(matches, np.uint32).reshape(-1, 2)
+    if ptr.shape[0] != pairs.shape[0] + 1 or cam_of.shape[0] != kp_ptr.shape[0] - 1:
+        raise ValueError("the match pointer must have one entry per pair and one more, image_camera one per image")
+    if ptr[-1] != m.shape[0] or kp_ptr[-1] != kps.shape[0]:
+        raise ValueError("the match pointer / keypoint_ptr must end at the number of matches / keypoints")
+    return kp_ptr, kps, cam_of, pairs, ptr, m
+
+
 def batch_optimize_relative_position_with_known_rotation(pairs, return_iterations=False):
     """pairs: sequence of (points1 [n][2], points2 [n][2], rotation1 [4], rotation2 [4]); returns [len(pairs)][3]."""
     pairs = list(pairs)
@@ -96,21 +113,15 @@ def estimate_relative_poses(keypoint_ptr, keypoints, image_camera, cameras, pair
     stored in the database), image_camera [F], cameras [C][3] SIMPLE_PINHOLE (f, cx, cy), pair_images [R][2] image
     indices, config [R], E / F / H [R][3][3], inlier_ptr [R + 1], inlier_matches [N][2] (keypoint in image 1,
     keypoint in image 2).  Returns RelativePoses (psfm_two_view_relative_poses, csrc/two_view.cu)."""
-    kp_ptr = np.ascontiguousarray(keypoint_ptr, np.int64)
-    kps = np.ascontiguousarray(keypoints, np.float32).reshape(-1, 2)
-    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    kp_ptr, kps, cam_of, pairs, iptr, m = _pair_graph(keypoint_ptr, keypoints, image_camera, pair_images, inlier_ptr,
+                                                      inlier_matches)
     cams = np.ascontiguousarray(cameras, np.float64).reshape(-1, 3)
-    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
     cfg = np.ascontiguousarray(config, np.int32)
     R = cfg.shape[0]
     E, F, H = (np.ascontiguousarray(m, np.float64).reshape(R, 9) for m in (E, F, H))
-    iptr = np.ascontiguousarray(inlier_ptr, np.int64)
-    m = np.ascontiguousarray(inlier_matches, np.uint32).reshape(-1, 2)
     num_images = kp_ptr.shape[0] - 1
-    if pairs.shape[0] != R or iptr.shape[0] != R + 1 or cam_of.shape[0] != num_images:
-        raise ValueError("pair_images, config, E, F, H and inlier_ptr must describe the same pairs, image_camera the same images")
-    if iptr[-1] != m.shape[0] or kp_ptr[-1] != kps.shape[0]:
-        raise ValueError("inlier_ptr / keypoint_ptr must end at the number of matches / keypoints")
+    if pairs.shape[0] != R:
+        raise ValueError("pair_images, config, E, F and H must describe the same pairs")
     out = RelativePoses(np.zeros((R, 4)), np.zeros((R, 3)), np.zeros(R), np.zeros(R, np.int32), np.zeros(R, np.int64),
                         np.zeros(R, np.uint8))
     i32, i64 = C.POINTER(C.c_int32), C.POINTER(C.c_int64)
@@ -194,20 +205,14 @@ def optimize_pairwise_translations(keypoint_ptr, keypoints, image_camera, camera
     world-to-camera, `GlobalRotations.orientations`), pair_used [R] (None: every pair; normally
     `GlobalRotations.pair_kept`).  Returns tvec [R][3] (zeros for unused pairs), and the IRLS iterations [R] with
     return_iterations (psfm_optimize_pairwise_translations, csrc/init_geometry.cu)."""
-    kp_ptr = np.ascontiguousarray(keypoint_ptr, np.int64)
-    kps = np.ascontiguousarray(keypoints, np.float32).reshape(-1, 2)
-    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    kp_ptr, kps, cam_of, pairs, iptr, m = _pair_graph(keypoint_ptr, keypoints, image_camera, pair_images, inlier_ptr,
+                                                      inlier_matches)
     cams = np.ascontiguousarray(cameras, np.float64).reshape(-1, 3)
-    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
     R = pairs.shape[0]
-    iptr = np.ascontiguousarray(inlier_ptr, np.int64)
-    m = np.ascontiguousarray(inlier_matches, np.uint32).reshape(-1, 2)
     q = np.ascontiguousarray(orientations, np.float64).reshape(-1, 4)
     num_images = kp_ptr.shape[0] - 1
-    if iptr.shape[0] != R + 1 or cam_of.shape[0] != num_images or q.shape[0] != num_images:
-        raise ValueError("pair_images and inlier_ptr must describe the same pairs, image_camera and orientations the same images")
-    if iptr[-1] != m.shape[0] or kp_ptr[-1] != kps.shape[0]:
-        raise ValueError("inlier_ptr / keypoint_ptr must end at the number of matches / keypoints")
+    if q.shape[0] != num_images:
+        raise ValueError("orientations must have one entry per image")
     used = None
     if pair_used is not None:
         used = np.ascontiguousarray(pair_used, np.uint8)
@@ -356,26 +361,19 @@ class Triangulation:
 def _triangulation_create(keypoint_ptr, keypoints, image_camera, cameras, pair_images, inlier_ptr, inlier_matches,
                           camera_size, orientations, image_tvec, registered, pair_used=None, options=None):
     """psfm_triangulation_create: returns (handle, P, E, inputs)."""
-    kp_ptr = np.ascontiguousarray(keypoint_ptr, np.int64)
-    kps = np.ascontiguousarray(keypoints, np.float32).reshape(-1, 2)
-    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    kp_ptr, kps, cam_of, pairs, iptr, m = _pair_graph(keypoint_ptr, keypoints, image_camera, pair_images, inlier_ptr,
+                                                      inlier_matches)
     cams = np.ascontiguousarray(cameras, np.float64).reshape(-1, 3)
     size = np.ascontiguousarray(camera_size, np.int32).reshape(-1, 2)
-    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
     R = pairs.shape[0]
-    iptr = np.ascontiguousarray(inlier_ptr, np.int64)
-    m = np.ascontiguousarray(inlier_matches, np.uint32).reshape(-1, 2)
     q = np.ascontiguousarray(orientations, np.float64).reshape(-1, 4)
     t = np.ascontiguousarray(image_tvec, np.float64).reshape(-1, 3)
     reg = np.ascontiguousarray(registered, np.uint8)
     F = kp_ptr.shape[0] - 1
-    if iptr.shape[0] != R + 1 or cam_of.shape[0] != F or q.shape[0] != F or t.shape[0] != F or reg.shape != (F,):
-        raise ValueError("pair_images and inlier_ptr must describe the same pairs; image_camera, orientations, image_tvec "
-                         "and registered the same images")
+    if q.shape[0] != F or t.shape[0] != F or reg.shape != (F,):
+        raise ValueError("orientations, image_tvec and registered must have one entry per image")
     if size.shape[0] != cams.shape[0]:
         raise ValueError("camera_size must have one (width, height) per camera")
-    if iptr[-1] != m.shape[0] or kp_ptr[-1] != kps.shape[0]:
-        raise ValueError("inlier_ptr / keypoint_ptr must end at the number of matches / keypoints")
     used = None
     if pair_used is not None:
         used = np.ascontiguousarray(pair_used, np.uint8)
@@ -524,19 +522,10 @@ def verify_two_view_geometries(keypoint_ptr, keypoints, image_camera, camera_siz
     match_ptr [R + 1], matches [M][2] (point2D_idx1, point2D_idx2), prior_focal_length [C] (None: no camera has one),
     options TwoViewVerificationOptions.  handoff.MatchTables.verification_inputs() gives these arguments.  Returns
     TwoViewVerification (psfm_verify_two_view_geometries, csrc/verification.cu)."""
-    kp_ptr = np.ascontiguousarray(keypoint_ptr, np.int64)
-    kps = np.ascontiguousarray(keypoints, np.float32).reshape(-1, 2)
-    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    kp_ptr, kps, cam_of, pairs, mptr, m = _pair_graph(keypoint_ptr, keypoints, image_camera, pair_images, match_ptr, matches)
     size = np.ascontiguousarray(camera_size, np.int32).reshape(-1, 2)
-    pairs = np.ascontiguousarray(pair_images, np.int32).reshape(-1, 2)
     R = pairs.shape[0]
-    mptr = np.ascontiguousarray(match_ptr, np.int64)
-    m = np.ascontiguousarray(matches, np.uint32).reshape(-1, 2)
     F = kp_ptr.shape[0] - 1
-    if mptr.shape[0] != R + 1 or cam_of.shape[0] != F:
-        raise ValueError("pair_images and match_ptr must describe the same pairs, image_camera the images")
-    if mptr[-1] != m.shape[0] or kp_ptr[-1] != kps.shape[0]:
-        raise ValueError("match_ptr / keypoint_ptr must end at the number of matches / keypoints")
     prior = None
     if prior_focal_length is not None:
         prior = np.ascontiguousarray(prior_focal_length, np.uint8)
