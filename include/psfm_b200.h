@@ -789,6 +789,41 @@ int psfm_convert_result(psfm_convert* c, int32_t first_batch, int32_t num_batche
                         psfm_convert_summary* summary);
 void psfm_convert_destroy(psfm_convert* c);
 
+/* ------------------------------------------------------------------------- */
+/* The 3D points' colours from the decoded images                            */
+/* (Reconstruction::ExtractColorsForAllImages, csrc/colors.cu).              */
+/* ------------------------------------------------------------------------- */
+typedef struct psfm_colors psfm_colors;
+typedef struct {
+  int32_t num_batches;       /* psfm_colors_add_images calls that took images */
+  int32_t num_images;        /* images added */
+  int64_t num_observations;  /* keypoints with a point */
+  double setup_ms;           /* create: the observations' upload, the sort and the point lists (CUDA events) */
+  double upload_ms;          /* the batches' host-to-device copies, summed (CUDA events) */
+  double sample_ms;          /* the batches' k_sample, summed (CUDA events; overlaps the next batch's upload) */
+  double mean_ms;            /* result: k_mean (CUDA events) */
+  double stage_ms;           /* host wall time of the copies of the caller's pixels into the pinned buffers */
+} psfm_colors_summary;
+/* Uploads the observations of a model and orders each point's observations by image, then keypoint.
+     keypoint_ptr [F + 1] over keypoints [K][2] (x, y in COLMAP's convention: the upper-left pixel's centre is at
+     (0.5, 0.5)) and point_of_keypoint [K] (point row in [0, num_points), -1: no point), K < 2^31, num_points < 2^31.
+   summary (nullable) receives num_observations and setup_ms.  PSFM_ERR_INVALID before any launch for a bad
+   keypoint_ptr or a point row out of range; PSFM_ERR_NO_DEVICE without a device. */
+int psfm_colors_create(int32_t num_images, const int64_t* keypoint_ptr, const double* keypoints,
+                       const int32_t* point_of_keypoint, int64_t num_points, psfm_colors** out,
+                       psfm_colors_summary* summary);
+/* Samples the observations of images first .. first + count - 1 in their decoded pixels: width [count],
+   height [count], pixels the images one after the other, each top-down rows of w RGB8 triples.  The call copies the
+   pixels and returns while the device works; the k-th call runs on stream k % 2.  PSFM_ERR_INVALID before any launch
+   for an image index out of range or already added, or a zero width or height.  An image never added contributes
+   nothing. */
+int psfm_colors_add_images(psfm_colors* c, int32_t first, int32_t count, const int32_t* width, const int32_t* height,
+                           const uint8_t* pixels);
+/* rgb [num_points][3]: per point the mean of its samples (image ascending, then keypoint; summed in double) rounded
+   half away from zero, black without a sample.  summary (nullable) receives the totals. */
+int psfm_colors_result(psfm_colors* c, uint8_t* rgb, psfm_colors_summary* summary);
+void psfm_colors_destroy(psfm_colors* c);
+
 /* Measured fp64 roof of the current device (bench.py's roofline denominator for the kernels
    that are bounded by the fp64 FMA pipe rather than by HBM): sustained fused multiply-adds
    per second over the whole chip, and the latency in SM cycles of one dependent DFMA. */

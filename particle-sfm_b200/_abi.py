@@ -393,3 +393,17 @@ class ConvertSummary(C.Structure):
         ("alloc_ms", C.c_double),
         ("host_copy_ms", C.c_double),
     ]
+
+
+class ColorsSummary(C.Structure):
+    """psfm_colors_summary: sizes and times of psfm_colors_create / psfm_colors_result."""
+    _fields_ = [
+        ("num_batches", C.c_int32),
+        ("num_images", C.c_int32),
+        ("num_observations", C.c_int64),
+        ("setup_ms", C.c_double),
+        ("upload_ms", C.c_double),
+        ("sample_ms", C.c_double),
+        ("mean_ms", C.c_double),
+        ("stage_ms", C.c_double),
+    ]

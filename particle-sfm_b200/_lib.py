@@ -31,6 +31,7 @@ EXPORTS = [
     "psfm_triangulation_destroy", "psfm_verification_default_options", "psfm_verify_two_view_geometries",
     "psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse",
     "psfm_convert_create", "psfm_convert_result", "psfm_convert_destroy",
+    "psfm_colors_create", "psfm_colors_add_images", "psfm_colors_result", "psfm_colors_destroy",
     "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
@@ -150,6 +151,11 @@ def lib():
     L.psfm_convert_result.argtypes = [vp, C.c_int32, C.c_int32, dp, u8p, C.POINTER(_abi.ConvertSummary)]
     L.psfm_convert_destroy.argtypes = [vp]
     L.psfm_convert_destroy.restype = None
+    L.psfm_colors_create.argtypes = [C.c_int32, i64p, dp, ip, C.c_int64, C.POINTER(vp), C.POINTER(_abi.ColorsSummary)]
+    L.psfm_colors_add_images.argtypes = [vp, C.c_int32, C.c_int32, ip, ip, u8p]
+    L.psfm_colors_result.argtypes = [vp, u8p, C.POINTER(_abi.ColorsSummary)]
+    L.psfm_colors_destroy.argtypes = [vp]
+    L.psfm_colors_destroy.restype = None
     L.psfm_dist_get_unique_id.argtypes = [C.POINTER(C.c_uint8)]
     L.psfm_dist_init.argtypes = [C.POINTER(C.c_uint8), C.c_int32, C.c_int32]
     L.psfm_dist_finalize.restype = None

@@ -24,7 +24,8 @@ COMMON = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", CXX
 
 # (source, extra flags).  traj_solver.cu: -fmad=false so that its iterates are
 # bit-identical to the oracle compiled with -ffp-contract=off (DESIGN.md §4).  convert.cu: the same, so that its
-# depths and percentiles equal the numpy restatement's (DESIGN.md §4.10).
+# depths and percentiles equal the numpy restatement's (DESIGN.md §4.10).  colors.cu: the same, so that its
+# interpolated samples equal the oracle's (DESIGN.md §4.11).
 UNITS = [
     ("common.cu", []),
     ("pair_inputs.cu", []),
@@ -38,6 +39,7 @@ UNITS = [
     ("triangulation.cu", []),
     ("verification.cu", []),
     ("convert.cu", ["-fmad=false"]),
+    ("colors.cu", ["-fmad=false"]),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

@@ -146,13 +146,14 @@ _PT_HDR = np.dtype([("id", "<i8"), ("xyz", "<f8", 3), ("rgb", "u1", 3), ("error"
 
 def write_model_arrays(path, camera_ids, camera_size, cam_params, image_ids, image_names, image_camera, qvec, tvec,
                        keypoint_ptr, keypoints, point3D_ids, point_ids, xyz, error, track_ptr, track_image_ids,
-                       track_point2D, camera_model=0):
+                       track_point2D, camera_model=0, rgb=None):
     """cameras.bin, images.bin and points3D.bin from flat arrays, byte for byte what write_model writes for the
-    equivalent Reconstruction (cameras, images and points in array order, rgb 0).
+    equivalent Reconstruction (cameras, images and points in array order).
       cameras   camera_ids [C], camera_size [C][2] (width, height), cam_params [C][k] of `camera_model`
       images    the images to write: image_ids [F], image_names [F], image_camera [F] (index into the cameras),
                 qvec [F][4], tvec [F][3], keypoint_ptr [F + 1] over keypoints [K][2] and point3D_ids [K] (-1: none)
-      points    point_ids [P], xyz [P][3], error [P], track_ptr [P + 1] over track_image_ids / track_point2D [E]
+      points    point_ids [P], xyz [P][3], error [P], track_ptr [P + 1] over track_image_ids / track_point2D [E],
+                rgb [P][3] uint8 (None: every point black)
     The per-observation and per-track-element bytes are laid out with numpy, without a loop over them."""
     os.makedirs(path, exist_ok=True)
     cam_params = np.asarray(cam_params, "<f8").reshape(len(camera_ids), -1)
@@ -187,6 +188,8 @@ def write_model_arrays(path, camera_ids, camera_size, cam_params, image_ids, ima
             lo, hi = int(tp[a]), int(tp[b])
             hdr = np.zeros(b - a, _PT_HDR)
             hdr["id"], hdr["xyz"], hdr["error"], hdr["len"] = point_ids[a:b], xyz[a:b], error[a:b], np.diff(tp[a:b + 1])
+            if rgb is not None:
+                hdr["rgb"] = np.asarray(rgb, np.uint8).reshape(-1, 3)[a:b]
             trk = np.empty(hi - lo, _TRK)
             trk["image_id"], trk["point2D_idx"] = track_image_ids[lo:hi], track_point2D[lo:hi]
             # within the chunk, point p's header starts at 51 p + 8 (track_ptr[p] - lo); element e at 51 (p + 1) + 8 e

@@ -16,14 +16,17 @@ GlobalMapperController::Reconstruct (reference controllers/global_mapper.cc:136-
      9  refinement pass A           psfm_ba_iterative_refinement, known rotations
     10  refinement pass B           the same resident solver, rotations and focal length
     11  model                       psfm_ba_get_model
-    12  write                       colmap_io.write_model_arrays -> OUT/0/{cameras,images,points3D}.bin
-    13  convert (convert_path set)  convert.save_depth_pose_arrays on the same arrays -> CONVERT/{depths,poses,
+    12  colors (image_path set and  colors.extract_colors_for_all_images on the registered images: each point's
+        extract_colors)             mean bilinear colour (ExtractColorsForAllImages, DESIGN.md §4.11)
+    13  write                       colmap_io.write_model_arrays -> OUT/0/{cameras,images,points3D}.bin
+    14  convert (convert_path set)  convert.save_depth_pose_arrays on the same arrays -> CONVERT/{depths,poses,
                                     intrinsics}, what sfm/convert.py writes from the model (DESIGN.md §4.10)
 
 The model differs from gcolmap's by exactly the steps this library does not run: CompleteAndMergeTracks and
-Retriangulate inside the refinement loop, FilterImages after it, and the colour extraction (points are written with
-rgb 0).  As in the reference, a failed rotation or position stage leaves no model and is not an error: the run ends
-with exit status 0 and no OUT/0.
+Retriangulate inside the refinement loop, FilterImages after it, and, without an image path, the colour extraction
+(points are then written with rgb 0).  Images that cannot be read leave their observations out of the colours, as in
+the reference; they are listed in the colors stage's summary and are not an error.  As in the reference, a failed
+rotation or position stage leaves no model and is not an error: the run ends with exit status 0 and no OUT/0.
 """
 import argparse
 import ctypes as C
@@ -33,8 +36,9 @@ import time
 
 import numpy as np
 
-from . import _abi, _lib, ba, colmap_io, convert, handoff, init_geometry
+from . import _abi, _lib, ba, colmap_io, colors, convert, handoff, init_geometry
 
+# the reference steps this mapper leaves out; ExtractColors only when no image path is given (or extract_colors is off)
 NOT_RUN = ("CompleteAndMergeTracks", "Retriangulate", "FilterImages", "ExtractColors")
 
 
@@ -48,7 +52,7 @@ class GlobalMapperOptions:
         self.min_num_matches = 15
         self.ignore_watermarks = False
         self.num_threads = -1                       # meaningless on the GPU; kept for the surface
-        self.extract_colors = True                  # not built: points are written with rgb 0
+        self.extract_colors = True                  # with an image path: the colors stage
         self.min_track_length = 2
         self.max_track_length = 2 ** 31 - 1
         self.min_focal_length_ratio = 0.1
@@ -152,9 +156,11 @@ def poses_and_points(g, used, o, report):
     return used, rot, pos, tri
 
 
-def global_mapper(database_path, output_path, options=None, convert_path=None):
+def global_mapper(database_path, output_path, options=None, convert_path=None, image_path=None):
     """Run the mapper on `database_path` and write OUT/0/{cameras,images,points3D}.bin under `output_path`.  Returns
-    a MapperReport; a failed rotation or position stage writes nothing and is not an exception.  With convert_path,
+    a MapperReport; a failed rotation or position stage writes nothing and is not an exception.  With image_path and
+    options.extract_colors, the points are coloured from the registered images under image_path (stage `colors`; its
+    summary lists the images that could not be read, which are not an error).  With convert_path,
     the model's depth maps, poses and intrinsics are then written there from the arrays in memory (stage `convert`),
     as convert.write_depth_pose_from_colmap_format would write them from OUT/0.  OUT/0 is written first: a registered
     image with no pixel of positive depth leaves it in place, writes nothing under convert_path and raises the
@@ -196,10 +202,19 @@ def global_mapper(database_path, output_path, options=None, convert_path=None):
         report.add("model", t0)
     finally:
         S.close()
+    arrays = model_arrays(g, pos.has_position, model)
+    rgb = None
+    if image_path is not None and o.extract_colors:
+        t0 = time.perf_counter()
+        rgb, c = colors.extract_colors_for_all_images(image_path, arrays[4], arrays[8], arrays[9],
+                                                      colors.point_rows(arrays[10], arrays[11]), len(arrays[11]),
+                                                      verbose=False)
+        report.add("colors", t0, {"images": c.images, "unread": c.unread, "batches": c.num_batches,
+                                  "observations": c.num_observations})
+        report.not_run = tuple(n for n in NOT_RUN if n != "ExtractColors")
     t0 = time.perf_counter()
     out = os.path.join(output_path, "0")
-    arrays = model_arrays(g, pos.has_position, model)
-    colmap_io.write_model_arrays(out, *arrays)
+    colmap_io.write_model_arrays(out, *arrays, rgb=rgb)
     report.add("write", t0, {"points": int((np.diff(model.track_ptr) > 0).sum()), "observations": int(model.track_ptr[-1])})
     if convert_path is not None:
         t0 = time.perf_counter()
@@ -241,7 +256,7 @@ def _flag(ap, name, default, help_=""):
 def build_parser():
     ap = argparse.ArgumentParser(prog="global_mapper", description=__doc__.split("\n\n")[0])
     ap.add_argument("--database_path", required=True)
-    ap.add_argument("--image_path", default="", help="accepted for gcolmap's surface; colours are not extracted")
+    ap.add_argument("--image_path", default="", help="the images, to colour the points (empty: every point black)")
     ap.add_argument("--output_path", required=True, help="the model is written to OUTPUT_PATH/0")
     ap.add_argument("--random_seed", type=int, default=0, help="accepted; every stage is deterministic")
     ap.add_argument("--quiet", action="store_true")
@@ -251,6 +266,7 @@ def build_parser():
                  "ba_global_max_refinement_change", "filter_max_reproj_error", "filter_min_tri_angle"):
         _flag(ap, name, getattr(d, name))
     _flag(ap, "fix_prior_rotation", False, "keep rotations fixed in pass B too")
+    _flag(ap, "extract_colors", True, "colour the points from the images under --image_path")
     # the reference's selectors of paths this mapper does not build: refused before any device call
     _flag(ap, "filter_with_1dsfm", False, "only 0 is supported")
     ap.add_argument("--GlobalMapper.position_method", dest="position_method", default="lud", help="only lud is supported")
@@ -277,6 +293,7 @@ def options_from_args(args):
     for k in ("ignore_watermarks", "ba_refine_focal_length", "ba_refine_principal_point", "ba_refine_extra_params"):
         setattr(o, k, bool(getattr(o, k)))
     o.ba_fix_prior_rotation = bool(args.fix_prior_rotation)
+    o.extract_colors = bool(args.extract_colors)
     return o
 
 
@@ -293,12 +310,16 @@ def main(argv=None):
         print(f"global_mapper: no database at {args.database_path}", file=sys.stderr)
         return 2
     try:
-        rep = global_mapper(args.database_path, args.output_path, options_from_args(args))
+        rep = global_mapper(args.database_path, args.output_path, options_from_args(args),
+                            image_path=args.image_path or None)
     except _lib.PsfmError as e:
         print(f"global_mapper: {e}", file=sys.stderr)
         return 1
     if not args.quiet:
         for name, s, summary in rep.stages:
+            if name == "colors":
+                for n in summary["unread"]:
+                    print(f"Could not read image {n} at path {os.path.join(args.image_path, n)}.")
             print(f"global_mapper: {name:22s} {1e3 * s:9.1f} ms")
         if rep.success:
             print(f"global_mapper: wrote {rep.output} (not run: {', '.join(rep.not_run)})")
