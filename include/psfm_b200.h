@@ -212,6 +212,27 @@ int psfm_matches_result(const psfm_matches* m, int64_t* keypoint_ptr, double* ke
                         int64_t* pair_ptr, int64_t* matches);
 void psfm_matches_destroy(psfm_matches* m);
 
+/* The COLMAP database's match table, built on the device from a psfm_matches handle (csrc/handoff.cu): bit for bit
+   the arrays of handoff.import_keypoints_matches_arrays followed by MatchTables.from_rows, without the int64 host copy.
+   image_ids [num_images] is the database id of every frame (distinct, in [0, 2^31 - 1), any permutation).  Images in
+   image_id order; keypoints float32(x + 0.5), float32(y + 0.5) (the double sum rounded once to nearest).  Of the two
+   ordered pairs (a, b) and (b, a) of one unordered pair the one with the smaller first frame is kept, else the other
+   one: the first occurrence in get_image_ids order (import_feature_matches.py:88-99), which is name order because
+   SQLite answers that query from the unique index on name.  Its columns are swapped when its first image has the
+   larger id.  Pairs in pair_id order, image 1 the smaller id; matches uint32.
+   On success the handle's keypoints and int64 matches move into the table and are freed: psfm_matches_result then
+   takes NULL keypoints and matches and writes the other arrays only.  num_keypoints / num_pairs / num_matches receive
+   the table's sizes.  PSFM_ERR_INVALID before any launch for an id out of range or given twice, a handle whose matches
+   were already moved, or an ordered pair of a frame with itself (a trajectory visiting one frame twice). */
+typedef struct psfm_match_table psfm_match_table;
+int psfm_matches_table(psfm_matches* m, const int32_t* image_ids, psfm_match_table** out, int64_t* num_keypoints,
+                       int64_t* num_pairs, int64_t* num_matches);
+/* host copies: keypoint_ptr [num_images + 1], keypoints [num_keypoints][2], pair_images [num_pairs][2] image rows,
+   match_ptr [num_pairs + 1], matches [num_matches][2] (point2D_idx1, point2D_idx2) */
+int psfm_match_table_result(const psfm_match_table* t, int64_t* keypoint_ptr, float* keypoints, int32_t* pair_images,
+                            int64_t* match_ptr, uint32_t* matches);
+void psfm_match_table_destroy(psfm_match_table* t);
+
 /* ------------------------------------------------------------------------- */
 /* SURVEY.md 8(f) row f-4: the RANSAC-free steps that initialise HP2, batched (csrc/init_geometry.cu). */
 /* Host buffers in, host buffers out.                                          */
@@ -502,6 +523,15 @@ int psfm_verify_two_view_geometries(int32_t num_images, const int64_t* keypoint_
                                     const psfm_verification_options* opts, int32_t* config, double* F, double* E,
                                     double* H, int64_t* inlier_ptr, uint32_t* inlier_matches, int32_t* pair_trials,
                                     psfm_verification_summary* summary);
+/* psfm_verify_two_view_geometries on a resident match table (psfm_matches_table): the same launches and the same
+   outputs as the host entry given psfm_match_table_result's arrays.  image_camera [num_images] over num_cameras
+   cameras, camera_size, prior_focal_length and opts as there.  The table holds valid keypoint indices and distinct
+   pairs by construction; the other checks and statuses are the host entry's. */
+int psfm_match_table_verify(const psfm_match_table* t, const int32_t* image_camera, int32_t num_cameras,
+                            const int32_t* camera_size, const uint8_t* prior_focal_length,
+                            const psfm_verification_options* opts, int32_t* config, double* F, double* E, double* H,
+                            int64_t* inlier_ptr, uint32_t* inlier_matches, int32_t* pair_trials,
+                            psfm_verification_summary* summary);
 
 /* ------------------------------------------------------------------------- */
 /* HP2 — global bundle adjustment                                             */

@@ -24,7 +24,9 @@ EXPORTS = [
     "psfm_grid_sample", "psfm_flow_check", "psfm_tracker_step", "psfm_tracker_buffer_inputs",
     "psfm_tracker_create", "psfm_tracker_advance", "psfm_tracker_optimize", "psfm_tracker_get_buffer", "psfm_tracker_set_buffer",
     "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy",
-    "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy", "psfm_known_rotation_translations", "psfm_triangulate_tracks",
+    "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy",
+    "psfm_matches_table", "psfm_match_table_result", "psfm_match_table_verify", "psfm_match_table_destroy",
+    "psfm_known_rotation_translations", "psfm_triangulate_tracks",
     "psfm_two_view_relative_poses", "psfm_rotation_default_options", "psfm_estimate_global_rotations",
     "psfm_optimize_pairwise_translations", "psfm_lud_default_options", "psfm_estimate_global_positions",
     "psfm_triangulator_default_options", "psfm_triangulation_create", "psfm_triangulation_result",
@@ -129,6 +131,12 @@ def lib():
     L.psfm_matches_result.argtypes = [vp, i64p, dp, i64p, i64p, i64p]
     L.psfm_matches_destroy.argtypes = [vp]
     L.psfm_matches_destroy.restype = None
+    L.psfm_matches_table.argtypes = [vp, ip, C.POINTER(vp), i64p, i64p, i64p]
+    L.psfm_match_table_result.argtypes = [vp, i64p, fp, ip, i64p, u32p]
+    L.psfm_match_table_verify.argtypes = [vp, ip, C.c_int32, ip, C.POINTER(C.c_uint8), C.POINTER(_abi.VerificationOptions),
+                                          ip, dp, dp, dp, i64p, u32p, ip, C.POINTER(_abi.VerificationSummary)]
+    L.psfm_match_table_destroy.argtypes = [vp]
+    L.psfm_match_table_destroy.restype = None
     L.psfm_ba_default_refine_options.argtypes = [C.POINTER(_abi.BARefineOptions)]
     L.psfm_ba_default_refine_options.restype = None
     L.psfm_ba_filter_negative_depth.argtypes = [C.c_void_p, i64p]

@@ -14,12 +14,23 @@
 //   7. k_scatter      each record to pair_ptr[rank of its run] + its place in the run, as (kp[src], kp[dst])
 // Memory: 32 bytes per record during the sort (keys and values, double-buffered), 24 bytes per record in the
 // scatter (sorted values and the int64 output), about 80 bytes per sample besides.
+//
+// psfm_matches_table then moves the result into the database match table (match_table.cuh), what
+// handoff.import_keypoints_matches_arrays followed by MatchTables.from_rows builds on the host:
+//   8. k_table_keypoints  per keypoint: float32(x + 0.5) at its image's row in image_id order (16 B in, 8 B out)
+//   9. k_table_matches    per kept match: its run's record, columns swapped where the run's source image has the
+//                         larger id, as uint32 (16 B in, 8 B out)
+// Of the two ordered runs of one image pair the one whose source frame comes first by name is kept: the reference
+// visits images in get_image_ids order, which SQLite returns in name order (tests/golden/import_small.npz).
+// The host picks one ordered run per unordered pair and orders the pairs by pair_id; the handle's int64 matches and
+// double keypoints are freed once the table exists, so the peak stays at or below the record sort's.
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <numeric>
 #include <vector>
 
+#include "match_table.cuh"
 #include "psfm_common.cuh"
 #include "radix_sort.cuh"
 
@@ -148,6 +159,28 @@ __global__ void k_scatter(long long M, const long long* run_start, int R, const 
   }
 }
 
+// keypoint s of the handle (frame-major) -> its row in image_id order, shifted to COLMAP's origin: the double sum
+// rounded once to nearest, which is numpy's float64 -> float32 cast
+__global__ void k_table_keypoints(long long N, const long long* kstart, int NI, const long long* dst_start,
+                                  const double2* kxy, float2* out) {
+  for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < N; s += (long long)gridDim.x * blockDim.x) {
+    const long long f = upper_bound_ll(kstart, (long long)NI + 1, s) - 1;
+    const double2 v = kxy[s];
+    out[dst_start[f] + (s - kstart[f])] = make_float2(__double2float_rn(__dadd_rn(v.x, 0.5)), __double2float_rn(__dadd_rn(v.y, 0.5)));
+  }
+}
+
+// match q of the table -> record src[p] + (q - mptr[p]) of the handle, columns swapped when swap[p]
+__global__ void k_table_matches(long long M, const long long* mptr, int R, const long long* src, const unsigned char* swap,
+                                const long long* in, uint2* out) {
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < M; q += (long long)gridDim.x * blockDim.x) {
+    const long long p = upper_bound_ll(mptr, (long long)R + 1, q) - 1;
+    const long long r = src[p] + (q - mptr[p]);
+    const unsigned a = (unsigned)in[2 * r], b = (unsigned)in[2 * r + 1];
+    out[q] = swap[p] ? make_uint2(b, a) : make_uint2(a, b);
+  }
+}
+
 // of two buffers, free the one a CUB double buffer does not currently point at
 template <typename T>
 void release_other(DBuf<T>& a, DBuf<T>& b, const T* current) {
@@ -164,6 +197,7 @@ struct psfm_matches {
   std::vector<long long> pair_images, pair_ptr;
   DBuf<double> kxy;                            // [num_obs][2] keypoints, image-major
   DBuf<long long> matches;                     // [num_matches][2]
+  bool moved = false;                          // kxy and matches were moved into a match table
 };
 
 extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, const int64_t* frame_ids, const double* xy,
@@ -321,12 +355,17 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
 
 extern "C" int psfm_matches_result(const psfm_matches* H, int64_t* keypoint_ptr, double* keypoints, int64_t* pair_images,
                                    int64_t* pair_ptr, int64_t* matches) {
-  if (!H || !keypoint_ptr || !pair_ptr || (H->num_obs && !keypoints) || (H->num_matches && (!pair_images || !matches)))
+  if (H && H->moved && (keypoints || matches))
+    return fail("psfm_matches_result", PSFM_ERR_INVALID,
+                "the keypoints and matches were moved into a match table; pass NULL for them");
+  if (!H || !keypoint_ptr || !pair_ptr || (H->num_obs && !H->moved && !keypoints) ||
+      (H->num_matches && (!pair_images || (!H->moved && !matches))))
     return fail("psfm_matches_result", PSFM_ERR_INVALID, "null argument");
   try {
     std::copy(H->kstart.begin(), H->kstart.end(), keypoint_ptr);
     std::copy(H->pair_ptr.begin(), H->pair_ptr.end(), pair_ptr);
     std::copy(H->pair_images.begin(), H->pair_images.end(), pair_images);
+    if (H->moved) return PSFM_OK;
     if (H->num_obs)
       PSFM_CUDA(cudaMemcpy(keypoints, H->kxy.p, sizeof(double) * 2 * (size_t)H->num_obs, cudaMemcpyDeviceToHost));
     if (H->num_matches)
@@ -337,5 +376,137 @@ extern "C" int psfm_matches_result(const psfm_matches* H, int64_t* keypoint_ptr,
 
 extern "C" void psfm_matches_destroy(psfm_matches* H) {
   delete H;
+  cudaGetLastError();
+}
+
+extern "C" int psfm_matches_table(psfm_matches* H, const int32_t* image_ids, psfm_match_table** out, int64_t* num_keypoints,
+                                  int64_t* num_pairs, int64_t* num_matches) {
+  const char* entry = "psfm_matches_table";
+  if (!H || !out || !num_keypoints || !num_pairs || !num_matches) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  *out = nullptr;
+  if (H->moved) return fail(entry, PSFM_ERR_INVALID, "the handle's matches were already moved into a match table");
+  const int NI = H->num_images;
+  if (NI > 0 && !image_ids) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  for (int f = 0; f < NI; ++f)
+    if (image_ids[f] < 0 || image_ids[f] == 0x7fffffff)
+      return fail(entry, PSFM_ERR_INVALID, "an image id is outside [0, 2^31 - 1)");
+  std::vector<int> row_frame(NI);                   // frame of every row in image_id order
+  std::iota(row_frame.begin(), row_frame.end(), 0);
+  std::sort(row_frame.begin(), row_frame.end(), [&](int x, int y) { return image_ids[x] < image_ids[y]; });
+  for (int r = 1; r < NI; ++r)
+    if (image_ids[row_frame[r]] == image_ids[row_frame[r - 1]]) return fail(entry, PSFM_ERR_INVALID, "an image id is given twice");
+  const long long Rh = (long long)H->pair_ptr.size() - 1;
+  for (long long k = 0; k < Rh; ++k)
+    if (H->pair_images[2 * k] == H->pair_images[2 * k + 1])
+      return fail(entry, PSFM_ERR_INVALID, "a trajectory visits one frame twice (a pair of an image with itself)");
+  int rc = require_device(entry);
+  if (rc != PSFM_OK) return rc;
+  psfm_match_table* T = new psfm_match_table;
+  try {
+    T->num_images = NI;
+    std::vector<int> row_of(NI);
+    for (int r = 0; r < NI; ++r) row_of[row_frame[r]] = r;
+    // images: keypoint rows in image_id order
+    T->keypoint_ptr.assign((size_t)NI + 1, 0);
+    std::vector<long long> dst_start(NI);
+    for (int r = 0; r < NI; ++r) {
+      const int f = row_frame[r];
+      dst_start[f] = T->keypoint_ptr[r];
+      T->keypoint_ptr[r + 1] = T->keypoint_ptr[r] + (H->kstart[f + 1] - H->kstart[f]);
+    }
+    const long long N = T->keypoint_ptr[NI];
+    T->num_keypoints = N;
+    // pairs: per unordered pair the first run in get_image_ids order (import_feature_matches.py:88-99), which is name
+    // order, i.e. frame order: SQLite answers "SELECT name, image_id FROM images" from the unique index on name.  So
+    // the run whose source frame is the smaller one, else the other one; its columns are swapped when its source has
+    // the larger id (add_matches).  Then pair_id order.
+    struct Run { int lo, hi; bool later, swap; long long k; };
+    std::vector<Run> runs((size_t)Rh);
+    for (long long k = 0; k < Rh; ++k) {
+      const long long a = H->pair_images[2 * k], b = H->pair_images[2 * k + 1];
+      const int ia = image_ids[a], ib = image_ids[b];
+      runs[k] = {std::min(ia, ib), std::max(ia, ib), a > b, ia > ib, k};
+    }
+    std::sort(runs.begin(), runs.end(), [](const Run& x, const Run& y) {
+      return x.lo != y.lo ? x.lo < y.lo : x.hi != y.hi ? x.hi < y.hi : x.later < y.later;
+    });
+    std::vector<long long> src;
+    std::vector<unsigned char> swap;
+    T->match_ptr.assign(1, 0);
+    for (size_t i = 0; i < runs.size(); ++i) {
+      if (i > 0 && runs[i].lo == runs[i - 1].lo && runs[i].hi == runs[i - 1].hi) continue;
+      const long long k = runs[i].k;
+      const int a = (int)H->pair_images[2 * k], b = (int)H->pair_images[2 * k + 1];
+      src.push_back(H->pair_ptr[k]);
+      swap.push_back(runs[i].swap);
+      T->pair_images.push_back(runs[i].swap ? row_of[b] : row_of[a]);
+      T->pair_images.push_back(runs[i].swap ? row_of[a] : row_of[b]);
+      T->match_ptr.push_back(T->match_ptr.back() + (H->pair_ptr[k + 1] - H->pair_ptr[k]));
+    }
+    const int R = (int)src.size();
+    const long long M = T->match_ptr[R];
+    T->num_pairs = R;
+    T->num_matches = M;
+    T->d_keypoint_ptr.alloc((size_t)NI + 1);
+    T->d_keypoint_ptr.upload(T->keypoint_ptr.data(), (size_t)NI + 1, nullptr);
+    T->d_match_ptr.alloc((size_t)R + 1);
+    T->d_match_ptr.upload(T->match_ptr.data(), (size_t)R + 1, nullptr);
+    T->pairs.alloc(R);
+    T->pairs.upload(reinterpret_cast<const int2*>(T->pair_images.data()), R, nullptr);
+    T->keypoints.alloc(N);
+    T->matches.alloc(M);
+    if (N > 0) {
+      DBuf<long long> d_kstart, d_dst;
+      d_kstart.alloc((size_t)NI + 1); d_dst.alloc(NI);
+      d_kstart.upload(H->kstart.data(), (size_t)NI + 1, nullptr);
+      d_dst.upload(dst_start.data(), NI, nullptr);
+      k_table_keypoints<<<grid_stride_of(N), 256>>>(N, d_kstart.p, NI, d_dst.p, reinterpret_cast<const double2*>(H->kxy.p),
+                                                    T->keypoints.p);
+      PSFM_LAUNCH_CHECK();
+      PSFM_CUDA(cudaDeviceSynchronize());
+    }
+    if (M > 0) {
+      DBuf<long long> d_src;
+      DBuf<unsigned char> d_swap;
+      d_src.alloc(R); d_swap.alloc(R);
+      d_src.upload(src.data(), R, nullptr);
+      d_swap.upload(swap.data(), R, nullptr);
+      k_table_matches<<<grid_stride_of(M), 256>>>(M, T->d_match_ptr.p, R, d_src.p, d_swap.p, H->matches.p, T->matches.p);
+      PSFM_LAUNCH_CHECK();
+      PSFM_CUDA(cudaDeviceSynchronize());
+    }
+    H->kxy.release();
+    H->matches.release();
+    H->moved = true;
+    *num_keypoints = N;
+    *num_pairs = R;
+    *num_matches = M;
+    *out = T;
+    return PSFM_OK;
+  } catch (const CudaFail& f) {
+    delete T;
+    return f.code;
+  }
+}
+
+extern "C" int psfm_match_table_result(const psfm_match_table* T, int64_t* keypoint_ptr, float* keypoints, int32_t* pair_images,
+                                       int64_t* match_ptr, uint32_t* matches) {
+  if (!T || !keypoint_ptr || !match_ptr || (T->num_keypoints && !keypoints) || (T->num_pairs && !pair_images) ||
+      (T->num_matches && !matches))
+    return fail("psfm_match_table_result", PSFM_ERR_INVALID, "null argument");
+  try {
+    std::copy(T->keypoint_ptr.begin(), T->keypoint_ptr.end(), keypoint_ptr);
+    std::copy(T->match_ptr.begin(), T->match_ptr.end(), match_ptr);
+    std::copy(T->pair_images.begin(), T->pair_images.end(), pair_images);
+    if (T->num_keypoints)
+      PSFM_CUDA(cudaMemcpy(keypoints, T->keypoints.p, sizeof(float2) * (size_t)T->num_keypoints, cudaMemcpyDeviceToHost));
+    if (T->num_matches)
+      PSFM_CUDA(cudaMemcpy(matches, T->matches.p, sizeof(uint2) * (size_t)T->num_matches, cudaMemcpyDeviceToHost));
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return f.code; }
+}
+
+extern "C" void psfm_match_table_destroy(psfm_match_table* T) {
+  delete T;
   cudaGetLastError();
 }

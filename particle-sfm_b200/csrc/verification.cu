@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "dlt.cuh"
+#include "match_table.cuh"
 #include "pair_inputs.h"
 #include "psfm_common.cuh"
 #include "verification_recalled.cuh"
@@ -703,53 +704,53 @@ extern "C" void psfm_verification_default_options(psfm_verification_options* o) 
   o->random_seed = 0;
 }
 
-extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
-                                               const int32_t* image_camera, int32_t num_cameras, const int32_t* camera_size,
-                                               const uint8_t* prior_focal_length, int64_t num_pairs,
-                                               const int32_t* pair_images, const int64_t* match_ptr, const uint32_t* matches,
-                                               const psfm_verification_options* opts, int32_t* config, double* F, double* E,
-                                               double* H, int64_t* inlier_ptr, uint32_t* inlier_matches,
-                                               int32_t* pair_trials, psfm_verification_summary* summary) {
-  const auto t0 = std::chrono::steady_clock::now();
-  const long long launches0 = g_launch_count.load();
-  const char* entry = "psfm_verify_two_view_geometries";
-  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
-  if (rc != PSFM_OK) return rc;
-  if (!keypoint_ptr || (num_images > 0 && !image_camera) || (num_cameras > 0 && !camera_size) ||
-      (num_pairs > 0 && (!pair_images || !match_ptr || !config || !F || !E || !H)) || !inlier_ptr)
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  psfm_verification_options o;
-  psfm_verification_default_options(&o);
-  if (opts) o = *opts;
-  if (!(o.max_error > 0 && o.confidence >= 0 && o.confidence <= 1 && o.min_inlier_ratio >= 0 && o.min_inlier_ratio <= 1 &&
-        o.min_num_trials >= 0 && o.min_num_trials <= o.max_num_trials && o.min_num_inliers >= 0 &&
-        o.dyn_num_trials_multiplier > 0 && o.max_H_inlier_ratio >= 0 && o.watermark_min_inlier_ratio >= 0 &&
-        o.watermark_min_inlier_ratio <= 1 && o.watermark_border_size >= 0 && o.watermark_border_size <= 1 &&
-        std::isfinite(o.max_error) && std::isfinite(o.dyn_num_trials_multiplier) && std::isfinite(o.max_H_inlier_ratio)))
+namespace {
+
+// TwoViewGeometry::Options::Check() on the options (NULL: the defaults)
+int check_options(const char* entry, const psfm_verification_options* opts, psfm_verification_options* o) {
+  psfm_verification_default_options(o);
+  if (opts) *o = *opts;
+  if (!(o->max_error > 0 && o->confidence >= 0 && o->confidence <= 1 && o->min_inlier_ratio >= 0 &&
+        o->min_inlier_ratio <= 1 && o->min_num_trials >= 0 && o->min_num_trials <= o->max_num_trials &&
+        o->min_num_inliers >= 0 && o->dyn_num_trials_multiplier > 0 && o->max_H_inlier_ratio >= 0 &&
+        o->watermark_min_inlier_ratio >= 0 && o->watermark_min_inlier_ratio <= 1 && o->watermark_border_size >= 0 &&
+        o->watermark_border_size <= 1 && std::isfinite(o->max_error) && std::isfinite(o->dyn_num_trials_multiplier) &&
+        std::isfinite(o->max_H_inlier_ratio)))
     return fail(entry, PSFM_ERR_INVALID, "options fail the TwoViewGeometry::Options Check()");
-  const int Fimg = num_images, R = (int)num_pairs;
-  if ((rc = check_keypoint_ptr(entry, Fimg, keypoint_ptr)) != PSFM_OK) return rc;
-  const long long K = keypoint_ptr[Fimg];
-  if (K > 0 && !keypoints) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if ((rc = check_image_cameras(entry, Fimg, image_camera, num_cameras)) != PSFM_OK) return rc;
-  if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
-  long long M = 0;
-  if (R > 0) {
-    if ((rc = check_match_ptr(entry, "match_ptr", R, match_ptr)) != PSFM_OK) return rc;
+  return PSFM_OK;
+}
+
+// the pairs whose two cameras both have a prior focal length go to EstimateCalibrated, which is not supported
+int check_prior_focal_length(const char* entry, int R, const int32_t* pair_images, const int32_t* image_camera,
+                             const uint8_t* prior_focal_length) {
+  if (prior_focal_length)
     for (int p = 0; p < R; ++p)
-      if (match_ptr[p + 1] - match_ptr[p] > 0x7fffffffLL)
-        return fail(entry, PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
-    if ((rc = check_pair_images(entry, R, pair_images, Fimg)) != PSFM_OK) return rc;
-    if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
-    M = match_ptr[R];
-    if (M > 0 && (!matches || !inlier_matches)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, match_ptr, matches)) != PSFM_OK) return rc;
-    if (prior_focal_length)
-      for (int p = 0; p < R; ++p)
-        if (prior_focal_length[image_camera[pair_images[2 * p]]] && prior_focal_length[image_camera[pair_images[2 * p + 1]]])
-          return fail(entry, PSFM_ERR_UNSUPPORTED,
-                      "both cameras of a pair have a prior focal length (EstimateCalibrated is not supported)");
-  }
+      if (prior_focal_length[image_camera[pair_images[2 * p]]] && prior_focal_length[image_camera[pair_images[2 * p + 1]]])
+        return fail(entry, PSFM_ERR_UNSUPPORTED,
+                    "both cameras of a pair have a prior focal length (EstimateCalibrated is not supported)");
+  return PSFM_OK;
+}
+
+// The graph both entries verify.  Host copies of keypoint_ptr, pair_images and match_ptr; keypoints and matches on the
+// host (uploaded here) unless `table` holds every array on the device already.
+struct Graph {
+  int num_images = 0, R = 0;
+  long long K = 0, M = 0;
+  const int64_t* keypoint_ptr = nullptr;
+  const float* keypoints = nullptr;
+  const int32_t* pair_images = nullptr;
+  const int64_t* match_ptr = nullptr;
+  const uint32_t* matches = nullptr;
+  const psfm_match_table* table = nullptr;
+};
+
+// Everything after the host checks: gather, LORANSAC per pair, compaction and the copies back.
+int verify_graph(const char* entry, std::chrono::steady_clock::time_point t0, long long launches0, const Graph& g,
+                 const int32_t* image_camera, const int32_t* camera_size, const psfm_verification_options& o,
+                 int32_t* config, double* F, double* E, double* H, int64_t* inlier_ptr, uint32_t* inlier_matches,
+                 int32_t* pair_trials, psfm_verification_summary* summary) {
+  const int R = g.R;
+  const long long M = g.M;
   psfm_verification_summary sm;
   memset(&sm, 0, sizeof(sm));
   inlier_ptr[0] = 0;
@@ -758,40 +759,51 @@ extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t
     if (summary) *summary = sm;
     return PSFM_OK;
   }
-  if ((rc = require_device(entry)) != PSFM_OK) return rc;
+  int rc = require_device(entry);
+  if (rc != PSFM_OK) return rc;
   std::vector<int> sizes(4 * (size_t)R);
   for (int p = 0; p < R; ++p)
     for (int k = 0; k < 2; ++k) {
-      const int c = image_camera[pair_images[2 * p + k]];
+      const int c = image_camera[g.pair_images[2 * p + k]];
       sizes[4 * p + 2 * k] = camera_size[2 * c];
       sizes[4 * p + 2 * k + 1] = camera_size[2 * c + 1];
     }
   sm.host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   try {
     Event ev[4];
-    DBuf<long long> d_kp_ptr, d_mptr, d_iptr, d_count;
-    DBuf<float2> d_kps;
-    DBuf<int2> d_pairs, d_sizes;
-    DBuf<uint2> d_m, d_out;
+    DBuf<long long> up_kp_ptr, up_mptr, d_iptr, d_count;
+    DBuf<float2> up_kps;
+    DBuf<int2> up_pairs, d_sizes;
+    DBuf<uint2> up_m, d_out;
     DBuf<float4> d_pts;
     DBuf<int> d_inl, d_config, d_trials, d_rounds;
     DBuf<double> d_F, d_H;
-    d_kp_ptr.alloc(Fimg + 1); d_kps.alloc(K); d_mptr.alloc(R + 1); d_iptr.alloc(R + 1); d_count.alloc(R);
-    d_pairs.alloc(R); d_sizes.alloc(2 * (size_t)R); d_m.alloc(M); d_pts.alloc(M); d_inl.alloc(M);
+    const long long *kp_ptr, *mptr;
+    const float2* kps;
+    const int2* pairs;
+    const uint2* m;
+    if (g.table) {
+      kp_ptr = g.table->d_keypoint_ptr.p; kps = g.table->keypoints.p; mptr = g.table->d_match_ptr.p;
+      pairs = g.table->pairs.p; m = g.table->matches.p;
+    } else {
+      up_kp_ptr.alloc(g.num_images + 1); up_kps.alloc(g.K); up_mptr.alloc(R + 1); up_pairs.alloc(R); up_m.alloc(M);
+      up_kp_ptr.upload(reinterpret_cast<const long long*>(g.keypoint_ptr), g.num_images + 1, nullptr);
+      up_kps.upload(reinterpret_cast<const float2*>(g.keypoints), g.K, nullptr);
+      up_mptr.upload(reinterpret_cast<const long long*>(g.match_ptr), R + 1, nullptr);
+      up_pairs.upload(reinterpret_cast<const int2*>(g.pair_images), R, nullptr);
+      up_m.upload(reinterpret_cast<const uint2*>(g.matches), M, nullptr);
+      kp_ptr = up_kp_ptr.p; kps = up_kps.p; mptr = up_mptr.p; pairs = up_pairs.p; m = up_m.p;
+    }
+    d_iptr.alloc(R + 1); d_count.alloc(R); d_sizes.alloc(2 * (size_t)R); d_pts.alloc(M); d_inl.alloc(M);
     d_config.alloc(R); d_trials.alloc(3 * (size_t)R); d_rounds.alloc(3 * (size_t)R); d_F.alloc(9 * (size_t)R);
     d_H.alloc(9 * (size_t)R);
-    d_kp_ptr.upload(reinterpret_cast<const long long*>(keypoint_ptr), Fimg + 1, nullptr);
-    d_kps.upload(reinterpret_cast<const float2*>(keypoints), K, nullptr);
-    d_mptr.upload(reinterpret_cast<const long long*>(match_ptr), R + 1, nullptr);
-    d_pairs.upload(reinterpret_cast<const int2*>(pair_images), R, nullptr);
     d_sizes.upload(reinterpret_cast<const int2*>(sizes.data()), 2 * (size_t)R, nullptr);
-    d_m.upload(reinterpret_cast<const uint2*>(matches), M, nullptr);
     PSFM_CUDA(cudaEventRecord(ev[0], nullptr));
-    k_gather<<<R, 256>>>(R, d_mptr.p, d_pairs.p, d_kp_ptr.p, d_kps.p, d_m.p, d_pts.p);
+    k_gather<<<R, 256>>>(R, mptr, pairs, kp_ptr, kps, m, d_pts.p);
     PSFM_LAUNCH_CHECK();
     PSFM_CUDA(cudaEventRecord(ev[1], nullptr));
     Args a;
-    a.R = R; a.mptr = d_mptr.p; a.pts = d_pts.p; a.sizes = d_sizes.p; a.inl_idx = d_inl.p; a.config = d_config.p;
+    a.R = R; a.mptr = mptr; a.pts = d_pts.p; a.sizes = d_sizes.p; a.inl_idx = d_inl.p; a.config = d_config.p;
     a.F = d_F.p; a.H = d_H.p; a.count = d_count.p; a.trials = d_trials.p; a.rounds = d_rounds.p;
     a.thr = o.max_error * o.max_error;
     a.confidence = o.confidence; a.multiplier = o.dyn_num_trials_multiplier;
@@ -814,7 +826,7 @@ extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t
     const long long N = inlier_ptr[R];
     d_iptr.upload(reinterpret_cast<const long long*>(inlier_ptr), R + 1, nullptr);
     d_out.alloc(N);
-    k_compact<<<R, 256>>>(R, d_mptr.p, d_iptr.p, d_inl.p, d_m.p, d_out.p);
+    k_compact<<<R, 256>>>(R, mptr, d_iptr.p, d_inl.p, m, d_out.p);
     PSFM_LAUNCH_CHECK();
     PSFM_CUDA(cudaEventRecord(ev[3], nullptr));
     PSFM_CUDA(cudaEventSynchronize(ev[3]));
@@ -844,4 +856,84 @@ extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t
   sm.num_launches = g_launch_count.load() - launches0;
   if (summary) *summary = sm;
   return PSFM_OK;
+}
+
+}  // namespace
+
+extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
+                                               const int32_t* image_camera, int32_t num_cameras, const int32_t* camera_size,
+                                               const uint8_t* prior_focal_length, int64_t num_pairs,
+                                               const int32_t* pair_images, const int64_t* match_ptr, const uint32_t* matches,
+                                               const psfm_verification_options* opts, int32_t* config, double* F, double* E,
+                                               double* H, int64_t* inlier_ptr, uint32_t* inlier_matches,
+                                               int32_t* pair_trials, psfm_verification_summary* summary) {
+  const auto t0 = std::chrono::steady_clock::now();
+  const long long launches0 = g_launch_count.load();
+  const char* entry = "psfm_verify_two_view_geometries";
+  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+  if (rc != PSFM_OK) return rc;
+  if (!keypoint_ptr || (num_images > 0 && !image_camera) || (num_cameras > 0 && !camera_size) ||
+      (num_pairs > 0 && (!pair_images || !match_ptr || !config || !F || !E || !H)) || !inlier_ptr)
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
+  psfm_verification_options o;
+  if ((rc = check_options(entry, opts, &o)) != PSFM_OK) return rc;
+  const int Fimg = num_images, R = (int)num_pairs;
+  if ((rc = check_keypoint_ptr(entry, Fimg, keypoint_ptr)) != PSFM_OK) return rc;
+  const long long K = keypoint_ptr[Fimg];
+  if (K > 0 && !keypoints) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  if ((rc = check_image_cameras(entry, Fimg, image_camera, num_cameras)) != PSFM_OK) return rc;
+  if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
+  long long M = 0;
+  if (R > 0) {
+    if ((rc = check_match_ptr(entry, "match_ptr", R, match_ptr)) != PSFM_OK) return rc;
+    for (int p = 0; p < R; ++p)
+      if (match_ptr[p + 1] - match_ptr[p] > 0x7fffffffLL)
+        return fail(entry, PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
+    if ((rc = check_pair_images(entry, R, pair_images, Fimg)) != PSFM_OK) return rc;
+    if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
+    M = match_ptr[R];
+    if (M > 0 && (!matches || !inlier_matches)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, match_ptr, matches)) != PSFM_OK) return rc;
+    if ((rc = check_prior_focal_length(entry, R, pair_images, image_camera, prior_focal_length)) != PSFM_OK) return rc;
+  }
+  Graph g;
+  g.num_images = Fimg; g.R = R; g.K = K; g.M = M;
+  g.keypoint_ptr = keypoint_ptr; g.keypoints = keypoints; g.pair_images = pair_images; g.match_ptr = match_ptr;
+  g.matches = matches;
+  return verify_graph(entry, t0, launches0, g, image_camera, camera_size, o, config, F, E, H, inlier_ptr, inlier_matches,
+                      pair_trials, summary);
+}
+
+extern "C" int psfm_match_table_verify(const psfm_match_table* t, const int32_t* image_camera, int32_t num_cameras,
+                                       const int32_t* camera_size, const uint8_t* prior_focal_length,
+                                       const psfm_verification_options* opts, int32_t* config, double* F, double* E,
+                                       double* H, int64_t* inlier_ptr, uint32_t* inlier_matches, int32_t* pair_trials,
+                                       psfm_verification_summary* summary) {
+  const auto t0 = std::chrono::steady_clock::now();
+  const long long launches0 = g_launch_count.load();
+  const char* entry = "psfm_match_table_verify";
+  if (!t) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  int rc = check_sizes(entry, t->num_images, num_cameras, t->num_pairs);
+  if (rc != PSFM_OK) return rc;
+  const int R = (int)t->num_pairs;
+  if ((t->num_images > 0 && !image_camera) || (num_cameras > 0 && !camera_size) ||
+      (R > 0 && (!config || !F || !E || !H)) || !inlier_ptr || (t->num_matches > 0 && !inlier_matches))
+    return fail(entry, PSFM_ERR_INVALID, "null argument");
+  psfm_verification_options o;
+  if ((rc = check_options(entry, opts, &o)) != PSFM_OK) return rc;
+  if ((rc = check_image_cameras(entry, t->num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
+  if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
+  for (int p = 0; p < R; ++p)
+    if (t->match_ptr[p + 1] - t->match_ptr[p] > 0x7fffffffLL)
+      return fail(entry, PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
+  if ((rc = check_prior_focal_length(entry, R, t->pair_images.data(), image_camera, prior_focal_length)) != PSFM_OK)
+    return rc;
+  Graph g;
+  g.num_images = t->num_images; g.R = R; g.K = t->num_keypoints; g.M = t->num_matches;
+  g.keypoint_ptr = reinterpret_cast<const int64_t*>(t->keypoint_ptr.data());
+  g.match_ptr = reinterpret_cast<const int64_t*>(t->match_ptr.data());
+  g.pair_images = t->pair_images.data();
+  g.table = t;
+  return verify_graph(entry, t0, launches0, g, image_camera, camera_size, o, config, F, E, H, inlier_ptr, inlier_matches,
+                      pair_trials, summary);
 }

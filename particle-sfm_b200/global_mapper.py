@@ -4,7 +4,8 @@
 
 GlobalMapperController::Reconstruct (reference controllers/global_mapper.cc:136-184), every stage on the device:
 
-     1  database cache              handoff.load_database_cache (DatabaseCache::Load pair rules)
+     1  database cache              handoff.load_database_cache (DatabaseCache::Load pair rules); stages 2-14 are
+                                    global_mapper_from_cache, which takes the cache from memory
      2  relative poses              init_geometry.estimate_relative_poses, then the cache drops what it leaves UNDEFINED
      3  rotations                   init_geometry.estimate_global_rotations
      4  pairwise translations       init_geometry.optimize_pairwise_translations on the rotation stage's kept pairs
@@ -90,11 +91,12 @@ class GlobalMapperOptions:
 class MapperReport:
     """success (a model was written), failed_stage (None, "rotations" or "positions") and reason (why it failed),
     stages [(name, seconds, summary dict)], output (the model directory or None), not_run (the reference steps this
-    mapper does not run)."""
+    mapper does not run), stats (model_stats of the written model, or None)."""
 
     def __init__(self):
         self.success, self.failed_stage, self.reason, self.output = False, None, None, None
         self.stages, self.not_run = [], NOT_RUN
+        self.stats = None
 
     def add(self, name, t0, summary=None):
         self.stages.append((name, time.perf_counter() - t0, summary or {}))
@@ -170,6 +172,15 @@ def global_mapper(database_path, output_path, options=None, convert_path=None, i
     t0 = time.perf_counter()
     g, used = handoff.load_database_cache(database_path, o.min_num_matches, o.ignore_watermarks)
     report.add("database_cache", t0, {"images": int(len(g.image_ids)), "pairs": int(len(used)), "pairs_used": int(used.sum())})
+    return global_mapper_from_cache(g, used, output_path, o, convert_path, image_path, report)
+
+
+def global_mapper_from_cache(g, used, output_path, options=None, convert_path=None, image_path=None, report=None):
+    """Stages 2-14 of global_mapper on a database cache already in memory: g a handoff.TwoViewGeometries, used its
+    pair_used (handoff.pair_rules).  The stages are appended to `report` (a new MapperReport when None), which is
+    returned; everything else is as global_mapper.  A written model's stats are in report.stats (model_stats)."""
+    o = options or GlobalMapperOptions()
+    report = report if report is not None else MapperReport()
     staged = poses_and_points(g, used, o, report)
     if staged is None:
         return report
@@ -216,12 +227,27 @@ def global_mapper(database_path, output_path, options=None, convert_path=None, i
     out = os.path.join(output_path, "0")
     colmap_io.write_model_arrays(out, *arrays, rgb=rgb)
     report.add("write", t0, {"points": int((np.diff(model.track_ptr) > 0).sum()), "observations": int(model.track_ptr[-1])})
+    report.stats = model_stats(arrays)
     if convert_path is not None:
         t0 = time.perf_counter()
         c = convert.save_depth_pose_arrays(convert_path, *arrays)
         report.add("convert", t0, {"images": c.images, "batches": c.num_batches})
     report.success, report.output = True, out
     return report
+
+
+def model_stats(arrays):
+    """The six numbers sfm/main_sfm.py:73-90 parses from `colmap model_analyzer`, from model_arrays' arrays:
+    registered images, points, observations, mean track length, mean observations per registered image, and the mean
+    reprojection error as Reconstruction::ComputeMeanReprojectionError computes it (recalled: the mean of the points'
+    errors over the points that have one, error != -1; 0 without any).  The means are exact; model_analyzer prints
+    them with six decimals."""
+    images, point_ids, error, track_ptr = arrays[3], arrays[11], np.asarray(arrays[13], np.float64), arrays[14]
+    reg, pts, obs = len(images), len(point_ids), int(track_ptr[-1])
+    has = error != -1.0
+    return {"num_reg_images": reg, "num_sparse_points": pts, "num_observations": obs,
+            "mean_track_length": obs / pts if pts else 0.0, "num_observations_per_image": obs / reg if reg else 0.0,
+            "mean_reproj_error": float(error[has].mean()) if has.any() else 0.0}
 
 
 def write_model(path, g, registered, model):

@@ -531,18 +531,45 @@ def verify_two_view_geometries(keypoint_ptr, keypoints, image_camera, camera_siz
         prior = np.ascontiguousarray(prior_focal_length, np.uint8)
         if prior.shape != (size.shape[0],):
             raise ValueError("prior_focal_length must have one entry per camera")
+    i32, i64, u32 = C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_uint32)
+    return _verify(R, m.shape[0], options, "psfm_verify_two_view_geometries",
+                   lambda *out: _lib.lib().psfm_verify_two_view_geometries(
+                       F, kp_ptr.ctypes.data_as(i64), kps.ctypes.data_as(C.POINTER(C.c_float)), cam_of.ctypes.data_as(i32),
+                       size.shape[0], size.ctypes.data_as(i32),
+                       prior.ctypes.data_as(C.POINTER(C.c_uint8)) if prior is not None else None, R,
+                       pairs.ctypes.data_as(i32), mptr.ctypes.data_as(i64), m.ctypes.data_as(u32), *out))
+
+
+def verify_match_table(table, image_camera, camera_size, prior_focal_length=None, options=None):
+    """verify_two_view_geometries on a handoff.ResidentMatchTable where it lies on the device (psfm_match_table_verify):
+    the same result as verify_two_view_geometries(**table.tables(...).verification_inputs()).  image_camera
+    [num_images] in image_id order, camera_size [C][2], prior_focal_length [C] (None: no camera has one)."""
+    cam_of = np.ascontiguousarray(image_camera, np.int32)
+    size = np.ascontiguousarray(camera_size, np.int32).reshape(-1, 2)
+    if cam_of.shape != (table.num_images,):
+        raise ValueError("image_camera must have one entry per image of the table")
+    prior = None
+    if prior_focal_length is not None:
+        prior = np.ascontiguousarray(prior_focal_length, np.uint8)
+        if prior.shape != (size.shape[0],):
+            raise ValueError("prior_focal_length must have one entry per camera")
+    i32 = C.POINTER(C.c_int32)
+    return _verify(table.num_pairs, table.num_matches, options, "psfm_match_table_verify",
+                   lambda *out: _lib.lib().psfm_match_table_verify(
+                       table.handle, cam_of.ctypes.data_as(i32), size.shape[0], size.ctypes.data_as(i32),
+                       prior.ctypes.data_as(C.POINTER(C.c_uint8)) if prior is not None else None, *out))
+
+
+def _verify(R, M, options, name, call):
+    """Allocate the outputs of R pairs and M raw matches, call(options, outputs...) and wrap them."""
     opts = (options or TwoViewVerificationOptions()).to_struct()
     config, Fm, Em, Hm = np.zeros(R, np.int32), np.zeros((R, 3, 3)), np.zeros((R, 3, 3)), np.zeros((R, 3, 3))
-    iptr, out = np.zeros(R + 1, np.int64), np.zeros((m.shape[0], 2), np.uint32)
+    iptr, out = np.zeros(R + 1, np.int64), np.zeros((M, 2), np.uint32)
     trials = np.zeros((R, 3), np.int32)
     s = _abi.VerificationSummary()
     i32, i64, u32 = C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_uint32)
-    _lib.check(_lib.lib().psfm_verify_two_view_geometries(
-        F, kp_ptr.ctypes.data_as(i64), kps.ctypes.data_as(C.POINTER(C.c_float)), cam_of.ctypes.data_as(i32),
-        size.shape[0], size.ctypes.data_as(i32), prior.ctypes.data_as(C.POINTER(C.c_uint8)) if prior is not None else None,
-        R, pairs.ctypes.data_as(i32), mptr.ctypes.data_as(i64), m.ctypes.data_as(u32), C.byref(opts),
-        config.ctypes.data_as(i32), _lib.dptr(Fm), _lib.dptr(Em), _lib.dptr(Hm), iptr.ctypes.data_as(i64),
-        out.ctypes.data_as(u32), trials.ctypes.data_as(i32), C.byref(s)), "psfm_verify_two_view_geometries")
+    _lib.check(call(C.byref(opts), config.ctypes.data_as(i32), _lib.dptr(Fm), _lib.dptr(Em), _lib.dptr(Hm),
+                    iptr.ctypes.data_as(i64), out.ctypes.data_as(u32), trials.ctypes.data_as(i32), C.byref(s)), name)
     summary = {n: (list(getattr(s, n)) if n.startswith(("num_trials", "num_local", "num_config")) else getattr(s, n))
                for n, _ in _abi.VerificationSummary._fields_}
     return TwoViewVerification(config, Fm, Em, Hm, iptr, np.ascontiguousarray(out[:iptr[-1]]), trials, summary)
