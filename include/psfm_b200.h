@@ -187,6 +187,29 @@ int psfm_tracker_finish(psfm_tracker* t, int32_t traj_min_len, int64_t* num_traj
    ptr[k] .. ptr[k + 1]), frame_ids [num_obs], xy [num_obs][2] */
 int psfm_tracker_result(psfm_tracker* t, int64_t* ids, int64_t* ptr, int32_t* frame_ids, double* xy);
 void psfm_tracker_destroy(psfm_tracker* t);
+/* psfm_tracker_create with the mode: path_consistency 1 is psfm_tracker_create (track_optimize.py:24-54); 0 is
+   track.py:24-50, the same tracker without the buffer: psfm_tracker_advance needs only flow and occ on every frame,
+   reports 0 buffered and never asks for psfm_tracker_optimize, and a frame without survivors is not an error */
+int psfm_tracker_create_mode(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, int32_t path_consistency,
+                             void* stream, psfm_tracker** out);
+
+/* ------------------------------------------------------------------------- */
+/* track.npy's pickled TrajectorySet state written on the device                */
+/* (csrc/track_npy.cu, DESIGN.md 4.13): the body {id: {"frame_ids": [...],        */
+/* "locations": [(x, y), ...], "labels": [False, ...]}, ...} as protocol-2 pickle  */
+/* opcodes without memo, trajectories in the given order.  The bytes wait in a     */
+/* pinned host buffer owned by the handle.                                         */
+/* ------------------------------------------------------------------------- */
+typedef struct psfm_track_npy psfm_track_npy;
+/* host arrays: ids [num_trajs] in [0, 2^31), ptr [num_trajs + 1] monotone from 0 to num_obs, frame_ids [num_obs]
+   >= 0, xy [num_obs][2]; anything else is PSFM_ERR_INVALID before the device is used */
+int psfm_track_npy_create(const int64_t* ids, const int64_t* ptr, const int32_t* frame_ids, const double* xy, int64_t num_trajs,
+                          int64_t num_obs, psfm_track_npy** out, int64_t* nbytes);
+/* the finished track set of a tracker (after psfm_tracker_finish), encoded where it lies, on the tracker's stream */
+int psfm_tracker_track_npy(psfm_tracker* t, psfm_track_npy** out, int64_t* nbytes);
+/* the body's nbytes bytes, valid until psfm_track_npy_destroy */
+const uint8_t* psfm_track_npy_data(const psfm_track_npy* h);
+void psfm_track_npy_destroy(psfm_track_npy* h);
 
 /* ------------------------------------------------------------------------- */
 /* SURVEY.md 8(f) row f-2: track set -> COLMAP keypoints and matches          */

@@ -24,6 +24,8 @@ EXPORTS = [
     "psfm_grid_sample", "psfm_flow_check", "psfm_tracker_step", "psfm_tracker_buffer_inputs",
     "psfm_tracker_create", "psfm_tracker_advance", "psfm_tracker_optimize", "psfm_tracker_get_buffer", "psfm_tracker_set_buffer",
     "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy",
+    "psfm_tracker_create_mode", "psfm_tracker_track_npy", "psfm_track_npy_create", "psfm_track_npy_data",
+    "psfm_track_npy_destroy",
     "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy",
     "psfm_matches_table", "psfm_match_table_result", "psfm_match_table_verify", "psfm_match_table_destroy",
     "psfm_known_rotation_translations", "psfm_triangulate_tracks",
@@ -127,6 +129,13 @@ def lib():
     L.psfm_tracker_result.argtypes = [vp, i64p, i64p, ip, dp]
     L.psfm_tracker_destroy.argtypes = [vp]
     L.psfm_tracker_destroy.restype = None
+    L.psfm_tracker_create_mode.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, vp, C.POINTER(vp)]
+    L.psfm_tracker_track_npy.argtypes = [vp, C.POINTER(vp), i64p]
+    L.psfm_track_npy_create.argtypes = [i64p, i64p, ip, dp, C.c_int64, C.c_int64, C.POINTER(vp), i64p]
+    L.psfm_track_npy_data.argtypes = [vp]
+    L.psfm_track_npy_data.restype = vp
+    L.psfm_track_npy_destroy.argtypes = [vp]
+    L.psfm_track_npy_destroy.restype = None
     L.psfm_matches_create.argtypes = [i64p, C.c_int64, i64p, dp, C.c_int32, C.c_int32, C.POINTER(vp), i64p, i64p]
     L.psfm_matches_result.argtypes = [vp, i64p, dp, i64p, i64p, i64p]
     L.psfm_matches_destroy.argtypes = [vp]

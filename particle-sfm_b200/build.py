@@ -31,6 +31,7 @@ UNITS = [
     ("pair_inputs.cu", []),
     ("microbench.cu", []),
     ("tracker.cu", []),
+    ("track_npy.cu", []),
     ("handoff.cu", []),
     ("init_geometry.cu", []),
     ("two_view.cu", []),

@@ -26,6 +26,7 @@
 #include <vector>
 
 #include "psfm_common.cuh"
+#include "track_npy.cuh"
 #include "traj_solver.cuh"
 
 namespace {
@@ -414,6 +415,7 @@ void grow(DBuf<T>& b, size_t need, size_t keep, cudaStream_t st) {
 
 struct psfm_tracker {
   int h = 0, w = 0, ratio = 1, gh = 0, gw = 0, num_frames = 0;
+  bool path_consistency = true;   // false: track.py:24-50, no buffer and no HP1
   cudaStream_t st = nullptr;
   int t = 0;                      // frames advanced; the active particles live at time t
   int n_active = 0;               // = history[t]'s survivors until the next seeding
@@ -483,15 +485,20 @@ extern "C" int psfm_flow_check_device(const float* d_flow_f, const float* d_flow
   } catch (const CudaFail& f) { return f.code; }
 }
 
-extern "C" int psfm_tracker_create(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, void* stream, psfm_tracker** out) {
-  if (!out) return fail("psfm_tracker_create", PSFM_ERR_INVALID, "null argument");
+namespace {
+
+int tracker_create(const char* entry, int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, int32_t path_consistency,
+                   void* stream, psfm_tracker** out) {
+  if (!out) return fail(entry, PSFM_ERR_INVALID, "null argument");
   *out = nullptr;
-  if (h < 2 || w < 2 || sample_ratio < 1 || num_frames < 1) return fail("psfm_tracker_create", PSFM_ERR_INVALID, "bad sizes");
-  int rc = require_device("psfm_tracker_create");
+  if (h < 2 || w < 2 || sample_ratio < 1 || num_frames < 1) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
+  if (path_consistency != 0 && path_consistency != 1) return fail(entry, PSFM_ERR_INVALID, "path_consistency must be 0 or 1");
+  int rc = require_device(entry);
   if (rc != PSFM_OK) return rc;
   psfm_tracker* T = new psfm_tracker;
   try {
     T->h = h; T->w = w; T->ratio = sample_ratio; T->num_frames = num_frames;
+    T->path_consistency = path_consistency != 0;
     T->gh = (h + sample_ratio - 1) / sample_ratio; T->gw = (w + sample_ratio - 1) / sample_ratio;
     T->st = (cudaStream_t)stream;
     T->hoff.assign(1, 0);
@@ -512,6 +519,17 @@ extern "C" int psfm_tracker_create(int32_t h, int32_t w, int32_t sample_ratio, i
   return PSFM_OK;
 }
 
+}  // namespace
+
+extern "C" int psfm_tracker_create(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, void* stream, psfm_tracker** out) {
+  return tracker_create("psfm_tracker_create", h, w, sample_ratio, num_frames, 1, stream, out);
+}
+
+extern "C" int psfm_tracker_create_mode(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, int32_t path_consistency,
+                                        void* stream, psfm_tracker** out) {
+  return tracker_create("psfm_tracker_create_mode", h, w, sample_ratio, num_frames, path_consistency, stream, out);
+}
+
 extern "C" int psfm_tracker_advance(psfm_tracker* T, const float* d_flow, const uint8_t* d_occ, const float* d_flow_prev,
                                     const float* d_flow2_prev, const uint8_t* d_occ2_prev, int32_t* counts) {
   const char* entry = "psfm_tracker_advance";
@@ -520,7 +538,7 @@ extern "C" int psfm_tracker_advance(psfm_tracker* T, const float* d_flow, const 
   if (T->finished) return fail(entry, PSFM_ERR_INVALID, "the track set was already assembled");
   if (T->n_buf > 0) return fail(entry, PSFM_ERR_INVALID, "the buffered set of the previous frame was not optimised");
   if (T->t + 1 >= T->num_frames) return fail(entry, PSFM_ERR_INVALID, "more frames than the tracker was created for");
-  if (T->t >= 1 && (!d_flow_prev || !d_flow2_prev || !d_occ2_prev))
+  if (T->path_consistency && T->t >= 1 && (!d_flow_prev || !d_flow2_prev || !d_occ2_prev))
     return fail(entry, PSFM_ERR_INVALID, "from frame 1 on, flows[t-1], flows_f2[t-1] and occ_maps_s2[t-1] are needed");
   try {
     cudaStream_t st = T->st;
@@ -537,10 +555,12 @@ extern "C" int psfm_tracker_advance(psfm_tracker* T, const float* d_flow, const 
     const size_t ids_now = (size_t)T->next_id + seeds;
     grow(T->rank, ids_now, T->next_id, st); grow(T->rlen, ids_now, T->next_id, st); grow(T->rstart, ids_now, T->next_id, st);
     grow(T->next, 2 * (size_t)n, 0, st); grow(T->flags, n, 0, st); grow(T->pos, n, 0, st);
-    grow(T->bflags, n, 0, st); grow(T->bpos, n, 0, st);
-    grow(T->bx0, 2 * (size_t)n, 0, st); grow(T->buv, 4 * (size_t)n, 0, st); grow(T->bslot, n, 0, st);
-    grow(T->bref1, 2 * (size_t)n, 0, st); grow(T->bref2, 2 * (size_t)n, 0, st); grow(T->bscale, n, 0, st);
-    grow(T->bout, 4 * (size_t)n, 0, st);
+    if (T->path_consistency) {
+      grow(T->bflags, n, 0, st); grow(T->bpos, n, 0, st);
+      grow(T->bx0, 2 * (size_t)n, 0, st); grow(T->buv, 4 * (size_t)n, 0, st); grow(T->bslot, n, 0, st);
+      grow(T->bref1, 2 * (size_t)n, 0, st); grow(T->bref2, 2 * (size_t)n, 0, st); grow(T->bscale, n, 0, st);
+      grow(T->bout, 4 * (size_t)n, 0, st);
+    }
     int* hid_t = T->hid.p + h0;
     double* hxy_t = T->hxy.p + 2 * h0;
     // 1. seed (new_traj_all)
@@ -574,8 +594,8 @@ extern "C" int psfm_tracker_advance(psfm_tracker* T, const float* d_flow, const 
     T->scan_flags(T->mask.p, T->mpos.p, G);
     k_total<<<1, 1, 0, st>>>(T->mask.p, T->mpos.p, G, T->d_counts.p + 1);
     PSFM_LAUNCH_CHECK();
-    // 4. buffer (optimize_buffer's selection and gather), from frame 1 on
-    if (t >= 1 && n) {
+    // 4. buffer (optimize_buffer's selection and gather), from frame 1 on, with path consistency only
+    if (T->path_consistency && t >= 1 && n) {
       k_buffer_flags<<<grid_of(n), 256, 0, st>>>(T->act_len[d].p, T->d_counts.p, n, T->bflags.p);
       PSFM_LAUNCH_CHECK();
       T->scan_flags(T->bflags.p, T->bpos.p, n);
@@ -730,6 +750,17 @@ extern "C" int psfm_tracker_result(psfm_tracker* T, int64_t* ids, int64_t* ptr, 
     T->sync();
     return PSFM_OK;
   } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+}
+
+extern "C" int psfm_tracker_track_npy(psfm_tracker* T, psfm_track_npy** out, int64_t* nbytes) {
+  int rc = tracker_usable(T, out && nbytes, "psfm_tracker_track_npy");
+  if (rc != PSFM_OK) return rc;
+  *out = nullptr;
+  *nbytes = 0;
+  if (!T->finished) return fail("psfm_tracker_track_npy", PSFM_ERR_INVALID, "call psfm_tracker_finish first");
+  // the tracker's ids are retire ranks (< 2^31, int counters), its frame ids times, its ptr an exclusive scan
+  rc = track_npy_encode(T->ids.p, T->ptr.p, T->res_frames.p, T->res_xy.p, T->res_trajs, T->st, out, nbytes);
+  return rc == PSFM_OK ? rc : tracker_broken(T, rc);
 }
 
 extern "C" void psfm_tracker_destroy(psfm_tracker* T) {

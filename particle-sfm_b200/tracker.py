@@ -24,6 +24,9 @@ Semantics that decide the INTEGER TRACK CONNECTIVITY are kept bit-for-bit:
     ratio-strided grid,
   * trajectory ids are the positions in the reference's `full_trajs` list (retire order).
 
+track mirrors point_trajectory/track.py:24-50, the same loop without path consistency (no buffer, no HP1);
+track_device runs it resident on the GPU.
+
 track_optimize_device / main_connect_point_trajectories_device run the same loop with every particle array
 resident on the GPU (csrc/tracker.cu, psfm_tracker_*) and return a TrackArrays; DESIGN.md §4.1.
 """
@@ -320,6 +323,29 @@ def track_optimize(flows, flows_f2, occ_maps, occ_maps_s2, sample_ratio, optimiz
     return trajs.full_trajs(traj_min_len)
 
 
+def track(flows, occ_maps, sample_ratio, traj_min_len=0, device=False):
+    """Sequentially track point trajectories without path consistency (track.py:24-50): track_optimize with a
+    trajectory set of buffer_size 0, so no optimize_buffer, and a frame without survivors is not an error.  The
+    motion-boundary mask the reference computes there is not used by its step_forward (trajectory.py:61).  Same
+    result type and ids as track_optimize; device=True: track_device(...).to_dict(), same bits."""
+    if device:
+        return track_device(flows, occ_maps, sample_ratio, traj_min_len).to_dict()
+    import torch
+    n_flows = len(flows)
+    h, w = flows[0].shape[:2]
+    trajs = BatchedTrajectorySet(n_flows + 1, h, w, sample_ratio, None)
+    for frame_id in range(n_flows):
+        trajs.new_traj_all(frame_id, trajs.sample_candidates)
+        cur_xys = trajs.get_cur_pos()
+        flow_sample = grid_sample(torch.from_numpy(flows[frame_id]).permute(2, 0, 1).float(), cur_xys)
+        occ = grid_sample(torch.from_numpy(occ_maps[frame_id]).unsqueeze(0).float(), cur_xys) > 0.1
+        next_xys = cur_xys + flow_sample
+        valid = (next_xys[:, 0] > 0) * (next_xys[:, 0] < w - 1) * (next_xys[:, 1] > 0) * (next_xys[:, 1] < h - 1)
+        trajs.extend_all(next_xys, frame_id + 1, valid * (1.0 - np.squeeze(occ, axis=-1)))
+    trajs.clear_active()
+    return trajs.full_trajs(traj_min_len)
+
+
 def main_connect_point_trajectories(flows_f, flows_b, flows_f2, flows_b2, sample_ratio=2, flow_check_thres=1.0,
                                     traj_min_len=3, optimize_fn=None, device=False):
     """In-memory equivalent of main_connect_point_trajectories.py:27-62 with
@@ -353,9 +379,10 @@ def _on_host(a):
 
 
 class _ResidentTracker:
-    """A psfm_tracker handle (csrc/tracker.cu) on torch's current stream."""
+    """A psfm_tracker handle (csrc/tracker.cu) on torch's current stream; path_consistency=False: the mode of
+    track.py (no buffer, no HP1)."""
 
-    def __init__(self, h, w, sample_ratio, num_frames):
+    def __init__(self, h, w, sample_ratio, num_frames, path_consistency=True):
         from . import _lib
         self.L, self.check = _lib.lib(), _lib.check
         self.h, self.w = h, w
@@ -364,17 +391,21 @@ class _ResidentTracker:
         if self.L.psfm_device_count() > 0:      # without a device the library refuses below, before torch touches CUDA
             import torch
             self.stream = torch.cuda.current_stream().cuda_stream
-        self.check(self.L.psfm_tracker_create(h, w, sample_ratio, num_frames, self.stream, _C.byref(self.handle)),
-                   "psfm_tracker_create")
+        if path_consistency:
+            self.check(self.L.psfm_tracker_create(h, w, sample_ratio, num_frames, self.stream, _C.byref(self.handle)),
+                       "psfm_tracker_create")
+        else:
+            self.check(self.L.psfm_tracker_create_mode(h, w, sample_ratio, num_frames, 0, self.stream, _C.byref(self.handle)),
+                       "psfm_tracker_create_mode")
 
     def close(self):
         if self.handle:
             self.L.psfm_tracker_destroy(self.handle)
             self.handle = _C.c_void_p()
 
-    def flow_check(self, flow_f, flow_b, thres):
+    def flow_check(self, flow_f, flow_b, thres, out=None):
         import torch
-        occ = torch.empty((self.h, self.w), dtype=torch.uint8, device=flow_f.device)
+        occ = torch.empty((self.h, self.w), dtype=torch.uint8, device=flow_f.device) if out is None else out
         self.check(self.L.psfm_flow_check_device(flow_f.data_ptr(), flow_b.data_ptr(), self.h, self.w, float(thres), None,
                                                  occ.data_ptr(), self.stream), "psfm_flow_check_device")
         return occ
@@ -411,6 +442,72 @@ class _ResidentTracker:
         self.check(self.L.psfm_tracker_result(self.handle, i64(ids), i64(ptr), frame_ids.ctypes.data_as(_C.POINTER(_C.c_int32)),
                                               _lib.dptr(xy)), "psfm_tracker_result")
         return TrackArrays(ids, ptr, frame_ids, xy)
+
+    def track_npy_body(self):
+        """After finish(): the finished track set's track.npy state body, encoded on the device where the set lies
+        (csrc/track_npy.cu) -> a TrackNpyBody."""
+        body = TrackNpyBody()
+        self.check(self.L.psfm_tracker_track_npy(self.handle, _C.byref(body.handle), _C.byref(body.nbytes)),
+                   "psfm_tracker_track_npy")
+        return body
+
+
+class TrackNpyBody:
+    """The bytes of a track.npy state body in a pinned host buffer the library owns; view() is valid until close()."""
+
+    def __init__(self):
+        from . import _lib
+        self.L = _lib.lib()
+        self.handle, self.nbytes = _C.c_void_p(), _C.c_int64()
+
+    def view(self):
+        n = self.nbytes.value
+        return memoryview((_C.c_uint8 * n).from_address(self.L.psfm_track_npy_data(self.handle))).cast("B")
+
+    def close(self):
+        if self.handle:
+            self.L.psfm_track_npy_destroy(self.handle)
+            self.handle = _C.c_void_p()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+
+def track_npy_body_device(arrays):
+    """The track.npy state body of any TrackArrays (host arrays, uploaded), encoded by csrc/track_npy.cu.  Ids
+    outside [0, 2^31), negative frame ids and a ptr that does not run monotonically from 0 to the number of
+    observations are refused (PsfmError, PSFM_ERR_INVALID) before the device is used."""
+    from . import _lib
+    ids = np.ascontiguousarray(arrays.ids, np.int64)
+    ptr = np.ascontiguousarray(arrays.ptr, np.int64)
+    frame_ids = np.ascontiguousarray(arrays.frame_ids, np.int32)
+    xy = np.ascontiguousarray(arrays.xy, np.float64).reshape(-1, 2)
+    if ptr.shape != (ids.shape[0] + 1,) or frame_ids.shape[0] != xy.shape[0]:
+        raise ValueError("TrackArrays: ptr must have one entry more than ids, frame_ids as many as xy rows")
+    i64 = lambda a: a.ctypes.data_as(_C.POINTER(_C.c_int64))
+    body = TrackNpyBody()
+    _lib.check(body.L.psfm_track_npy_create(i64(ids), i64(ptr), frame_ids.ctypes.data_as(_C.POINTER(_C.c_int32)), _lib.dptr(xy),
+                                            ids.shape[0], frame_ids.shape[0], _C.byref(body.handle), _C.byref(body.nbytes)),
+               "psfm_track_npy_create")
+    return body
+
+
+def track_device(flows, occ_maps, sample_ratio, traj_min_len=0):
+    """track (track.py:24-50) resident on the GPU -> TrackArrays, bit for bit the host path's track set.  Maps as
+    track_optimize_device takes them."""
+    n_flows = len(flows)
+    h, w = flows[0].shape[:2]
+    trk = _ResidentTracker(h, w, sample_ratio, n_flows + 1, path_consistency=False)
+    try:
+        import torch
+        for frame_id in range(n_flows):
+            trk.step(_on_device(flows[frame_id], torch.float32), _on_device(occ_maps[frame_id], torch.uint8))
+        return trk.finish(traj_min_len)
+    finally:
+        trk.close()
 
 
 def track_optimize_device(flows, flows_f2, occ_maps, occ_maps_s2, sample_ratio, optimize_fn=None, traj_min_len=0):
