@@ -908,6 +908,31 @@ int psfm_blocked_cholesky_solve(const double* A, const double* b, int32_t ns, in
 int psfm_laplacian_solve(const double* A, const double* B, int32_t n, double* X);
 int psfm_spd_inverse(const double* A, int32_t n, double* X);
 
+/* Test entries of the small null-vector solvers of the geometry stages (csrc/dlt.cuh) and of the verification's local
+   step.  Each returns PSFM_OK, PSFM_ERR_INVALID on a bad argument (psfm_last_error says which), PSFM_ERR_NO_DEVICE
+   without a device; argument checks come first.
+   psfm_null_vectors: one solver per thread on `count` (1 .. 2^24) row-major N x N matrices A, its raw outputs in out:
+     PSFM_NV_JACOBI_3, _4   one_sided_jacobi<N>: A V [N][N], then V [N][N]
+     PSFM_NV_DLT_POINT      dlt_point_4x4 (N = 4): X [3], then the null vector v [4] before hnormalisation
+     PSFM_NV_EIGEN_3, _4    smallest_eigenvector<N> of a symmetric A: v [N]
+     PSFM_NV_JACOBI_9       one_sided_jacobi_mem on 9 x 9, the local step's solve: A V [9][9], V [9][9], then V's
+                            column of the smallest column norm of A V [9]
+   psfm_verification_local_model: the local step of the verification's LORANSAC (local_estimate in one 256-thread
+     CTA, k_verify's code path) for kind 0 (eight-point F) or 1 (normalised DLT H) on the inliers of `best` [9]
+     (residual <= max_squared_error) among n points [n][4] = (x1, y1, x2, y2).  null_vector [9]: the normalised
+     solve's null vector (unit norm, any sign); normalization [6]: (s1, c1x, c1y, s2, c2x, c2y), T = [s 0 -s cx;
+     0 s -s cy; 0 0 1]; local_model [9]: the denormalised model that k_verify scores next (F after the rank-2 step). */
+#define PSFM_NV_JACOBI_3 0
+#define PSFM_NV_JACOBI_4 1
+#define PSFM_NV_DLT_POINT 2
+#define PSFM_NV_EIGEN_3 3
+#define PSFM_NV_EIGEN_4 4
+#define PSFM_NV_JACOBI_9 5
+int psfm_null_vectors(int32_t form, const double* A, int64_t count, double* out);
+int psfm_verification_local_model(int32_t kind, const float* points, int64_t n, const double* best,
+                                  double max_squared_error, double* null_vector, double* normalization,
+                                  double* local_model);
+
 /* ------------------------------------------------------------------------- */
 /* Multi-GPU (HP2): points sharded across ranks, one all-reduce of the         */
 /* camera-side vector per PCG step (SURVEY.md §8e).                            */

@@ -39,6 +39,7 @@ UNITS = [
     ("position_estimation.cu", []),
     ("triangulation.cu", []),
     ("verification.cu", []),
+    ("dlt.cu", []),
     ("convert.cu", ["-fmad=false"]),
     ("colors.cu", ["-fmad=false"]),
     ("dist.cu", []),

@@ -1,5 +1,6 @@
 // dlt.cuh — the triangulation pieces shared by the two-view relative pose (two_view.cu), the multi-view DLT of
-// init_geometry.cu and the triangulation of every registered image (triangulation.cu).
+// init_geometry.cu and the triangulation of every registered image (triangulation.cu), and the null-vector solve of
+// the verification's local step (verification.cu).  psfm_null_vectors (dlt.cu) runs each solver alone for the tests.
 #pragma once
 #include <cmath>
 
@@ -46,9 +47,9 @@ __device__ __forceinline__ void one_sided_jacobi(double (&A)[N][N], double (&V)[
   }
 }
 
-// TriangulatePoint's solve: the right singular vector of the smallest singular value of the 4 x 4 DLT matrix A
-// (destroyed), hnormalized
-__device__ __forceinline__ void dlt_point_4x4(double (&A)[4][4], double* X) {
+// TriangulatePoint's null vector: the right singular vector of the smallest singular value of the 4 x 4 DLT matrix A
+// (destroyed), before hnormalisation
+__device__ __forceinline__ void dlt_null_vector_4x4(double (&A)[4][4], double (&v)[4]) {
   double V[4][4];
   one_sided_jacobi<4>(A, V);
   int best = 0;
@@ -58,7 +59,6 @@ __device__ __forceinline__ void dlt_point_4x4(double (&A)[4][4], double* X) {
     const double nj = A[0][j] * A[0][j] + A[1][j] * A[1][j] + A[2][j] * A[2][j] + A[3][j] * A[3][j];
     if (nj < bn) { bn = nj; best = j; }
   }
-  double v[4];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     double x = V[i][0];
@@ -67,6 +67,12 @@ __device__ __forceinline__ void dlt_point_4x4(double (&A)[4][4], double* X) {
       if (j == best) x = V[i][j];
     v[i] = x;
   }
+}
+
+// TriangulatePoint's solve: dlt_null_vector_4x4, hnormalized
+__device__ __forceinline__ void dlt_point_4x4(double (&A)[4][4], double* X) {
+  double v[4];
+  dlt_null_vector_4x4(A, v);
   X[0] = v[0] / v[3]; X[1] = v[1] / v[3]; X[2] = v[2] / v[3];
 }
 
@@ -127,43 +133,44 @@ __device__ __forceinline__ void smallest_eigenvector(double (&A)[N][N], double (
   }
 }
 
-// smallest_eigenvector's cyclic Jacobi with A (n x n row-major, destroyed) and the workspace V (n x n) in memory, for a
-// caller that cannot hold 2 n^2 doubles in registers (the 9 x 9 normal matrices of verification.cu)
-__device__ inline void smallest_eigenvector_mem(double* A, double* V, int n, double* v) {
+// one_sided_jacobi with A (n x n row-major, destroyed) and V (n x n) in memory, for a caller that cannot hold 2 n^2
+// doubles in registers (the 9 x 9 R factors of verification.cu's local step); returns the index of the column of A V
+// with the smallest norm, whose column of V is the right singular vector of A's smallest singular value
+__device__ inline int one_sided_jacobi_mem(double* A, double* V, int n) {
   for (int i = 0; i < n; ++i)
     for (int j = 0; j < n; ++j) V[i * n + j] = i == j ? 1.0 : 0.0;
-  for (int sweep = 0; sweep < 30; ++sweep) {
-    double off = 0.0, dia = 0.0;
-    for (int i = 0; i < n; ++i) {
-      dia += A[i * n + i] * A[i * n + i];
-      for (int j = i + 1; j < n; ++j) off += A[i * n + j] * A[i * n + j];
-    }
-    if (!(off > 1e-34 * dia)) break;
+  for (int sweep = 0; sweep < 40; ++sweep) {
+    bool rotated = false;
     for (int p = 0; p < n - 1; ++p)
       for (int q = p + 1; q < n; ++q) {
-        const double apq = A[p * n + q];
-        if (apq == 0.0) continue;
-        const double theta = (A[q * n + q] - A[p * n + p]) / (2.0 * apq);
-        const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        double alpha = 0.0, beta = 0.0, gamma = 0.0;
         for (int k = 0; k < n; ++k) {
-          const double akp = A[k * n + p], akq = A[k * n + q];
-          A[k * n + p] = c * akp - s * akq; A[k * n + q] = s * akp + c * akq;
+          alpha += A[k * n + p] * A[k * n + p];
+          beta += A[k * n + q] * A[k * n + q];
+          gamma += A[k * n + p] * A[k * n + q];
         }
+        if (!(fabs(gamma) > kJacobiTol * sqrt(alpha * beta))) continue;
+        rotated = true;
+        const double zeta = (beta - alpha) / (2.0 * gamma);
+        const double t = (zeta >= 0.0 ? 1.0 : -1.0) / (fabs(zeta) + sqrt(1.0 + zeta * zeta));
+        const double c = 1.0 / sqrt(1.0 + t * t), s = c * t;
         for (int k = 0; k < n; ++k) {
-          const double apk = A[p * n + k], aqk = A[q * n + k];
-          A[p * n + k] = c * apk - s * aqk; A[q * n + k] = s * apk + c * aqk;
-        }
-        for (int k = 0; k < n; ++k) {
-          const double vkp = V[k * n + p], vkq = V[k * n + q];
-          V[k * n + p] = c * vkp - s * vkq; V[k * n + q] = s * vkp + c * vkq;
+          const double ap = A[k * n + p], aq = A[k * n + q];
+          A[k * n + p] = c * ap - s * aq; A[k * n + q] = s * ap + c * aq;
+          const double vp = V[k * n + p], vq = V[k * n + q];
+          V[k * n + p] = c * vp - s * vq; V[k * n + q] = s * vp + c * vq;
         }
       }
+    if (!rotated) break;
   }
   int best = 0;
-  for (int i = 1; i < n; ++i)
-    if (A[i * n + i] < A[best * n + best]) best = i;
-  for (int i = 0; i < n; ++i) v[i] = V[i * n + best];
+  double bn = 0.0;
+  for (int j = 0; j < n; ++j) {
+    double nj = 0.0;
+    for (int k = 0; k < n; ++k) nj += A[k * n + j] * A[k * n + j];
+    if (j == 0 || nj < bn) { bn = nj; best = j; }
+  }
+  return best;
 }
 
 // TriangulateMultiViewPoint's accumulation of one view: A += (P - r r' P)' (P - r r' P), r = (x, y, 1) / |(x, y, 1)|,

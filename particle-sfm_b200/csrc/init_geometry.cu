@@ -179,14 +179,9 @@ __global__ void __launch_bounds__(128) k_known_rotation(const Points pts, const 
                        {0.0, -1.0, ay, 0.0},
                        {bx * R[6] - R[0], bx * R[7] - R[1], bx * R[8] - R[2], bx * pos[2] - pos[0]},
                        {by * R[6] - R[3], by * R[7] - R[4], by * R[8] - R[5], by * pos[2] - pos[1]}};
-    double G[4][4];
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-      for (int c = 0; c < 4; ++c) G[r][c] = Am[0][r] * Am[0][c] + Am[1][r] * Am[1][c] + Am[2][r] * Am[2][c] + Am[3][r] * Am[3][c];
-    double v[4];
-    smallest_eigenvector<4>(G, v);
-    const double X0 = v[0] / v[3], X1 = v[1] / v[3], X2 = v[2] / v[3];
+    double X[3];
+    dlt_point_4x4(Am, X);                           // TriangulatePoint: the SVD of Am itself, never Am'Am
+    const double X0 = X[0], X1 = X[1], X2 = X[2];
     const double d1 = X2;
     if (d1 > eps && d1 < max_depth) {
       const double d2 = (R[6] * X0 + R[7] * X1 + R[8] * X2 + pos[2]) * sqrt(R[2] * R[2] + R[5] * R[5] + R[8] * R[8]);

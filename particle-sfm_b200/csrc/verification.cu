@@ -13,9 +13,9 @@
 //            the CTA scores all models of the sample in one sweep over the pair's matches (per-thread partials, then a
 //            fixed-order block reduction); the leader applies the support comparison, the dynamic trial bound and the
 //            stopping test in model order.  Local optimisation sweeps the best model's inliers for their moments and
-//            the 9 x 9 Gram matrix of the normalised rows, solves it with the Jacobi eigen-solver of dlt.cuh, and
-//            scores the local model.  Then F's inliers are compacted in match order, the watermark test and its
-//            translation LORANSAC run on them, and the config is decided.
+//            the R factor of the normalised rows (Givens rotations, never A'A), takes R's smallest right singular
+//            vector with the one-sided Jacobi of dlt.cuh, and scores the local model.  Then F's inliers are compacted
+//            in match order, the watermark test and its translation LORANSAC run on them, and the config is decided.
 //   compact  k_compact: the inlier matches packed by the host's prefix sum of the per-pair counts
 // Trials run in the sequential order, so every scored trial is a trial of the reference loop (no trial is scored and
 // discarded).  Three launches per call with pairs, none without; no floating-point atomics: two calls are
@@ -309,7 +309,8 @@ struct Shared {
   double local[9];
   double red[kWarps][45];
   double tot[45];
-  double G[81], GV[81];            // the local step's 9 x 9 eigenproblem (leader only)
+  double G[81], GV[81];            // the local step's 9 x 9 R factor and its right singular vectors (leader only)
+  double lnull[9], lnorm[6];       // the local step's normalised null vector and (s1, c1x, c1y, s2, c2x, c2y)
   double best_sum;
   long long best_n;
   long long dyn;
@@ -363,6 +364,41 @@ __device__ void score(const double (*models)[9], int nm, const float4* pts, cons
   block_reduce<6>(v, s);
 }
 
+// The local step's R factor: the 9 x 9 upper triangle of the normalised design matrix's QR, packed by rows.  Solving R
+// instead of the Gram matrix A'A keeps the null vector's error proportional to A's condition number, not its square.
+__device__ __forceinline__ constexpr int tri(int j, int k) { return j * (17 - j) / 2 + k; }
+
+// fold the row r (zero before column j0) into R by Givens rotations, column by column; r is destroyed
+__device__ __forceinline__ void givens_fold(double (&R)[45], double (&r)[9], int j0) {
+#pragma unroll
+  for (int j = 0; j < 9; ++j) {
+    if (j < j0) continue;
+    const double b = r[j];
+    if (b == 0.0) continue;
+    const double a = R[tri(j, j)];
+    const double h = sqrt(a * a + b * b), c = a / h, sn = b / h;
+    R[tri(j, j)] = h;
+#pragma unroll
+    for (int k = j + 1; k < 9; ++k) {
+      const double x = R[tri(j, k)], y = r[k];
+      R[tri(j, k)] = c * x + sn * y; r[k] = c * y - sn * x;
+    }
+  }
+}
+
+// fold the triangle of lane + o into this lane's (a shuffle tree: lane 0 ends with the warp's triangle).  Every lane
+// folds at once, so the rows go last to first: folding row i changes rows i .. 8 only, and row i of the source lane is
+// still its own when it is read.
+__device__ __forceinline__ void givens_merge_down(double (&R)[45], int o) {
+#pragma unroll
+  for (int i = 8; i >= 0; --i) {
+    double r[9];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) r[k] = k < i ? 0.0 : __shfl_down_sync(0xffffffffu, R[tri(i, k)], o);
+    givens_fold(R, r, i);
+  }
+}
+
 template <int KIND>
 __device__ __noinline__ void local_model(Shared& s, double s1, double c1x, double c1y, double s2, double c2x, double c2y);
 
@@ -398,47 +434,55 @@ __device__ void local_estimate(const float4* pts, const int* list, int n, double
     block_reduce<2>(v, s);
   }
   const double s1 = sqrt(2.0) / sqrt(s.tot[0] / cnt), s2 = sqrt(2.0) / sqrt(s.tot[1] / cnt);
-  {                                                      // Gram matrix of the normalised rows (upper triangle)
-    double g[45];
+  {                                                      // R factor of the normalised rows
+    double R[45];
 #pragma unroll
-    for (int k = 0; k < 45; ++k) g[k] = 0.0;
+    for (int k = 0; k < 45; ++k) R[k] = 0.0;
     for (int i = threadIdx.x; i < n; i += kThreads) {
       const float4 p = point<KIND>(pts, list, i);
       if (!(residual<KIND>(best, p) <= thr)) continue;
       const double a0 = (p.x - c1x) * s1, a1 = (p.y - c1y) * s1, d0 = (p.z - c2x) * s2, d1 = (p.w - c2y) * s2;
       if (KIND == kKindF) {
-        const double r[9] = {d0 * a0, d0 * a1, d0, d1 * a0, d1 * a1, d1, a0, a1, 1.0};
-        int k = 0;
-#pragma unroll
-        for (int u = 0; u < 9; ++u)
-#pragma unroll
-          for (int w = u; w < 9; ++w) g[k++] += r[u] * r[w];
+        double r[9] = {d0 * a0, d0 * a1, d0, d1 * a0, d1 * a1, d1, a0, a1, 1.0};
+        givens_fold(R, r, 0);
       } else {
-        const double r[9] = {-a0, -a1, -1.0, 0.0, 0.0, 0.0, a0 * d0, a1 * d0, d0};
-        const double q[9] = {0.0, 0.0, 0.0, -a0, -a1, -1.0, a0 * d1, a1 * d1, d1};
-        int k = 0;
-#pragma unroll
-        for (int u = 0; u < 9; ++u)
-#pragma unroll
-          for (int w = u; w < 9; ++w) g[k++] += r[u] * r[w] + q[u] * q[w];
+        double r[9] = {-a0, -a1, -1.0, 0.0, 0.0, 0.0, a0 * d0, a1 * d0, d0};
+        double q[9] = {0.0, 0.0, 0.0, -a0, -a1, -1.0, a0 * d1, a1 * d1, d1};
+        givens_fold(R, r, 0);
+        givens_fold(R, q, 3);
       }
     }
-    block_reduce<45>(g, s);
+    for (int o = 16; o > 0; o >>= 1) givens_merge_down(R, o);
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    if (lane == 0)
+#pragma unroll
+      for (int k = 0; k < 45; ++k) s.red[wid][k] = R[k];
+    __syncthreads();
   }
   if (threadIdx.x == 0) local_model<KIND>(s, s1, c1x, c1y, s2, c2x, c2y);
   __syncthreads();
 }
 
-// the leader's part of the local step: the smallest eigenvector of the Gram matrix in s.tot, the rank-2 constraint
-// for F, denormalised into s.local
+// the leader's part of the local step: the warps' R factors (s.red) folded in warp order, the right singular vector of
+// the smallest singular value of R, the rank-2 constraint for F, denormalised into s.local
 template <int KIND>
 __device__ __noinline__ void local_model(Shared& s, double s1, double c1x, double c1y, double s2, double c2x, double c2y) {
   {
-    double f[9];
-    int k = 0;
+    double R[45];
+    for (int k = 0; k < 45; ++k) R[k] = s.red[0][k];
+    for (int w = 1; w < kWarps; ++w)
+      for (int i = 0; i < 9; ++i) {
+        double r[9];
+        for (int k = 0; k < 9; ++k) r[k] = k < i ? 0.0 : s.red[w][tri(i, k)];
+        givens_fold(R, r, i);
+      }
     for (int u = 0; u < 9; ++u)
-      for (int w = u; w < 9; ++w) { s.G[9 * u + w] = s.tot[k]; s.G[9 * w + u] = s.tot[k]; ++k; }
-    smallest_eigenvector_mem(s.G, s.GV, 9, f);
+      for (int w = 0; w < 9; ++w) s.G[9 * u + w] = w < u ? 0.0 : R[tri(u, w)];
+    const int mn9 = one_sided_jacobi_mem(s.G, s.GV, 9);
+    double f[9];
+    for (int i = 0; i < 9; ++i) f[i] = s.GV[9 * i + mn9];
+    for (int i = 0; i < 9; ++i) s.lnull[i] = f[i];
+    s.lnorm[0] = s1; s.lnorm[1] = c1x; s.lnorm[2] = c1y; s.lnorm[3] = s2; s.lnorm[4] = c2x; s.lnorm[5] = c2y;
     if (KIND == kKindF) {
       double A[3][3], V[3][3];                           // rank 2: the smallest singular value set to zero
       for (int r = 0; r < 3; ++r)
@@ -684,6 +728,22 @@ __global__ void k_compact(int R, const long long* __restrict__ mptr, const long 
   if (p >= R) return;
   const long long b = mptr[p], o = iptr[p], n = iptr[p + 1] - iptr[p];
   for (long long j = threadIdx.x; j < n; j += blockDim.x) out[o + j] = m[b + inl_idx[b + j]];
+}
+
+// psfm_verification_local_model: one local step of k_verify on one point stream, through the same Shared layout;
+// out = the normalised null vector (9), (s1, c1x, c1y, s2, c2x, c2y) (6), the denormalised local model (9)
+template <int KIND>
+__global__ void __launch_bounds__(kThreads) k_local_model(const float4* __restrict__ pts, int n,
+                                                           const double* __restrict__ best, double thr, double* out) {
+  __shared__ Shared s;
+  if (threadIdx.x < 9) s.best[threadIdx.x] = best[threadIdx.x];
+  __syncthreads();
+  local_estimate<KIND>(pts, nullptr, n, thr, s);
+  if (threadIdx.x < 9) {
+    out[threadIdx.x] = s.lnull[threadIdx.x];
+    out[15 + threadIdx.x] = s.local[threadIdx.x];
+  }
+  if (threadIdx.x < 6) out[9 + threadIdx.x] = s.lnorm[threadIdx.x];
 }
 
 }  // namespace
@@ -936,4 +996,32 @@ extern "C" int psfm_match_table_verify(const psfm_match_table* t, const int32_t*
   g.table = t;
   return verify_graph(entry, t0, launches0, g, image_camera, camera_size, o, config, F, E, H, inlier_ptr, inlier_matches,
                       pair_trials, summary);
+}
+
+extern "C" int psfm_verification_local_model(int32_t kind, const float* points, int64_t n, const double* best,
+                                             double max_squared_error, double* null_vector, double* normalization,
+                                             double* local_model) {
+  const char* entry = "psfm_verification_local_model";
+  if (!points || !best || !null_vector || !normalization || !local_model) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  if (kind != kKindF && kind != kKindH) return fail(entry, PSFM_ERR_INVALID, "kind must be 0 (F) or 1 (H)");
+  if (n < 1 || n > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "needs 1 <= n < 2^31");
+  if (!(max_squared_error >= 0.0)) return fail(entry, PSFM_ERR_INVALID, "max_squared_error must be >= 0");
+  const int rc = require_device(entry);
+  if (rc != PSFM_OK) return rc;
+  try {
+    DBuf<float4> d_pts;
+    DBuf<double> d_best, d_out;
+    d_pts.alloc(n); d_best.alloc(9); d_out.alloc(24);
+    d_pts.upload(reinterpret_cast<const float4*>(points), n, nullptr);
+    d_best.upload(best, 9, nullptr);
+    if (kind == kKindF) k_local_model<kKindF><<<1, kThreads>>>(d_pts.p, (int)n, d_best.p, max_squared_error, d_out.p);
+    else k_local_model<kKindH><<<1, kThreads>>>(d_pts.p, (int)n, d_best.p, max_squared_error, d_out.p);
+    PSFM_LAUNCH_CHECK();
+    double out[24];
+    PSFM_CUDA(cudaMemcpy(out, d_out.p, sizeof(out), cudaMemcpyDeviceToHost));
+    memcpy(null_vector, out, 9 * sizeof(double));
+    memcpy(normalization, out + 9, 6 * sizeof(double));
+    memcpy(local_model, out + 15, 9 * sizeof(double));
+    return PSFM_OK;
+  } catch (const CudaFail& f) { return f.code; }
 }

@@ -143,3 +143,59 @@ def test_no_cpu_fallback_of_the_initialisation_ops():
         ig.triangulate_multi_view_points([(np.zeros((2, 3, 4)), np.zeros((2, 2)))])
     assert ig.batch_optimize_relative_position_with_known_rotation([]).shape == (0, 3)      # nothing to do: no device needed
     assert ig.triangulate_multi_view_points([]).shape == (0, 3)
+
+
+def _null_vector_entries(form=0, A=np.eye(3), count=1, kind=0, n=8, best=np.eye(3).reshape(9), thr=16.0,
+                         points=np.zeros((8, 4), np.float32), out=True, only=None):
+    """The two null-vector test entries on the same kind of arguments: (name, status, psfm_last_error).  The outputs
+    are sized for one good call; a call with more is refused before it reads or writes anything."""
+    L = _lib.lib()
+    o = np.zeros(171) if out else None
+    v, T, m = (np.zeros(9), np.zeros(6), np.zeros(9)) if out else (None, None, None)
+    pts = None if points is None else points.ctypes.data_as(C.POINTER(C.c_float))
+    res = []
+    for name, call in (("psfm_null_vectors", lambda: L.psfm_null_vectors(form, _lib.dptr(A), count, _lib.dptr(o))),
+                       ("psfm_verification_local_model",
+                        lambda: L.psfm_verification_local_model(kind, pts, n, _lib.dptr(best), thr, _lib.dptr(v),
+                                                                _lib.dptr(T), _lib.dptr(m)))):
+        if only is None or name in only:
+            rc = call()
+            res.append((name, rc, L.psfm_last_error().decode()))
+    return res
+
+
+NULL_VECTOR_BAD = {
+    "null_input": (dict(A=None, points=None), {"psfm_null_vectors", "psfm_verification_local_model"}),
+    "null_output": (dict(out=False), {"psfm_null_vectors", "psfm_verification_local_model"}),
+    "null_best": (dict(best=None), {"psfm_verification_local_model"}),
+    "form_negative": (dict(form=-1), {"psfm_null_vectors"}),
+    "form_unknown": (dict(form=6), {"psfm_null_vectors"}),
+    "count0": (dict(count=0), {"psfm_null_vectors"}),
+    "count_above_2e24": (dict(count=(1 << 24) + 1), {"psfm_null_vectors"}),
+    "kind_watermark": (dict(kind=2), {"psfm_verification_local_model"}),
+    "n0": (dict(n=0), {"psfm_verification_local_model"}),
+    "n2e31": (dict(n=1 << 31), {"psfm_verification_local_model"}),
+    "threshold_negative": (dict(thr=-1.0), {"psfm_verification_local_model"}),
+    "threshold_nan": (dict(thr=float("nan")), {"psfm_verification_local_model"}),
+}
+
+
+@pytest.mark.parametrize("case", list(NULL_VECTOR_BAD))
+def test_null_vector_entries_check_arguments_before_the_device(case):
+    """Bad arguments are PSFM_ERR_INVALID, named in psfm_last_error, on any machine and before any launch."""
+    change, refused = NULL_VECTOR_BAD[case]
+    n0 = _lib.lib().psfm_launch_count()
+    for name, rc, msg in _null_vector_entries(**change, only=refused):
+        assert rc == _abi.PSFM_ERR_INVALID and msg.startswith(name + ":"), (name, rc, msg)
+    if _lib.lib().psfm_device_count() == 0:
+        assert _lib.lib().psfm_launch_count() == n0
+
+
+@pytest.mark.skipif(_lib.lib().psfm_device_count() > 0, reason="needs a machine WITHOUT a GPU")
+def test_no_cpu_fallback_of_the_null_vector_entries():
+    for name, rc, msg in _null_vector_entries():
+        assert rc == _abi.PSFM_ERR_NO_DEVICE and "no CUDA device" in msg, (name, rc, msg)
+    for form in range(6):
+        A = np.zeros((1, 81))
+        name, rc, msg = _null_vector_entries(form=form, A=A, only={"psfm_null_vectors"})[0]
+        assert rc == _abi.PSFM_ERR_NO_DEVICE, (form, rc, msg)

@@ -181,7 +181,7 @@ def _raised(fn):
 
 def _no_device_calls():
     from particlesfm_b200 import ba, handoff, init_geometry as ig, synthetic as syn, traj
-    from test_abi import _dense_chol_entries
+    from test_abi import _dense_chol_entries, _null_vector_entries
     from test_abi_convert import _args, _create
     L = _lib.lib()
     calls = {name: (lambda c=call: (c(_graph()), L.psfm_last_error().decode())) for name, (call, _, _) in STAGES.items()}
@@ -224,13 +224,15 @@ def _no_device_calls():
     })
     for name in ("psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse"):
         calls[name] = lambda n=name: _dense_chol_entries(np.eye(4), np.ones(4), 4, 4, 4, 0, only={n})[0][1:]
+    for name in ("psfm_null_vectors", "psfm_verification_local_model"):
+        calls[name] = lambda n=name: _null_vector_entries(only={n})[0][1:]
     return calls
 
 
 NO_DEVICE_ENTRIES = list(STAGES) + ["psfm_ba_solve", "psfm_traj_optimize", "psfm_known_rotation_translations",
                                     "psfm_triangulate_tracks", "psfm_matches_create", "psfm_tracker_create",
                                     "psfm_convert_create", "psfm_blocked_cholesky_solve", "psfm_laplacian_solve",
-                                    "psfm_spd_inverse"]
+                                    "psfm_spd_inverse", "psfm_null_vectors", "psfm_verification_local_model"]
 
 
 @pytest.mark.skipif(device_count() > 0, reason="checks the refusal without a device")
