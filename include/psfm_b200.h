@@ -934,6 +934,32 @@ int psfm_verification_local_model(int32_t kind, const float* points, int64_t n, 
                                   double* local_model);
 
 /* ------------------------------------------------------------------------- */
+/* RAFT's correlation, lookup, upsampling and flow image on the device          */
+/* (csrc/optical_flow.cu, DESIGN.md 4.14).  DEVICE pointers, work enqueued on    */
+/* `stream` without synchronising.  Each returns PSFM_OK, PSFM_ERR_INVALID on a  */
+/* bad argument (argument checks come first), PSFM_ERR_NO_DEVICE without a      */
+/* device.  h x w is the 1/8 grid (8 <= h, w and h w <= 2^20 where a pyramid is  */
+/* involved); a pyramid holds, level l = 0 .. 3 after level l - 1, h w images of */
+/* (h >> l) x (w >> l) floats: psfm_corr_pyramid_floats(h, w) of them.           */
+/* ------------------------------------------------------------------------- */
+/* psfm_corr_pyramids: fwd [h w][h w] holds fmap1^T fmap2 (row = pixel of image 1) on entry; on return fwd is the
+   forward pyramid (level 0 = the product / 16) and bwd the backward one, built from the transposed product. */
+int psfm_corr_pyramids(float* fwd, float* bwd, int32_t h, int32_t w, void* stream);
+int64_t psfm_corr_pyramid_floats(int32_t h, int32_t w);
+/* psfm_corr_lookup: CorrBlock.__call__ (radius 4) of num_problems pyramids laid end to end: coords [P][2][h][w]
+   (x, y at 1/8) -> out [P][324][h][w]; channel l * 81 + a * 9 + b samples level l at (x / 2^l + a - 4,
+   y / 2^l + b - 4), zero outside. */
+int psfm_corr_lookup(const float* pyramids, int32_t num_problems, int32_t h, int32_t w, const float* coords, float* out,
+                     void* stream);
+/* psfm_flow_upsample: upsample_flow then InputPadder.unpad: flow [P][2][h][w] (coords1 - coords0), mask [P][576][h][w]
+   (the mask head's output before its 0.25 scale), pad [4] = (left, right, top, bottom), each 0 .. 7 ->
+   out [P][8 h - top - bottom][8 w - left - right][2]. */
+int psfm_flow_upsample(const float* flow, const float* mask, int32_t num_problems, int32_t h, int32_t w, const int32_t* pad,
+                       float* out, void* stream);
+/* psfm_flow_to_image: flow_to_image(flow, convert_to_bgr=True) of num_maps maps [M][h][w][2] -> bgr [M][h][w][3] */
+int psfm_flow_to_image(const float* flow, int32_t num_maps, int32_t h, int32_t w, uint8_t* bgr, void* stream);
+
+/* ------------------------------------------------------------------------- */
 /* Multi-GPU (HP2): points sharded across ranks, one all-reduce of the         */
 /* camera-side vector per PCG step (SURVEY.md §8e).                            */
 /* ------------------------------------------------------------------------- */

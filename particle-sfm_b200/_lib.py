@@ -37,6 +37,7 @@ EXPORTS = [
     "psfm_null_vectors", "psfm_verification_local_model",
     "psfm_convert_create", "psfm_convert_result", "psfm_convert_destroy",
     "psfm_colors_create", "psfm_colors_add_images", "psfm_colors_result", "psfm_colors_destroy",
+    "psfm_corr_pyramids", "psfm_corr_pyramid_floats", "psfm_corr_lookup", "psfm_flow_upsample", "psfm_flow_to_image",
     "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
@@ -176,6 +177,12 @@ def lib():
     L.psfm_colors_result.argtypes = [vp, u8p, C.POINTER(_abi.ColorsSummary)]
     L.psfm_colors_destroy.argtypes = [vp]
     L.psfm_colors_destroy.restype = None
+    L.psfm_corr_pyramids.argtypes = [vp, vp, C.c_int32, C.c_int32, vp]
+    L.psfm_corr_pyramid_floats.argtypes = [C.c_int32, C.c_int32]
+    L.psfm_corr_pyramid_floats.restype = C.c_int64
+    L.psfm_corr_lookup.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp]
+    L.psfm_flow_upsample.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, ip, vp, vp]
+    L.psfm_flow_to_image.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, vp]
     L.psfm_dist_get_unique_id.argtypes = [C.POINTER(C.c_uint8)]
     L.psfm_dist_init.argtypes = [C.POINTER(C.c_uint8), C.c_int32, C.c_int32]
     L.psfm_dist_finalize.restype = None

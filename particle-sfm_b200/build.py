@@ -42,6 +42,7 @@ UNITS = [
     ("dlt.cu", []),
     ("convert.cu", ["-fmad=false"]),
     ("colors.cu", ["-fmad=false"]),
+    ("optical_flow.cu", ["-fmad=false"]),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),
