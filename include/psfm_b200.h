@@ -247,6 +247,13 @@ void psfm_matches_destroy(psfm_matches* m);
    takes NULL keypoints and matches and writes the other arrays only.  num_keypoints / num_pairs / num_matches receive
    the table's sizes.  PSFM_ERR_INVALID before any launch for an id out of range or given twice, a handle whose matches
    were already moved, or an ordered pair of a frame with itself (a trajectory visiting one frame twice). */
+/* The psfm_matches handle of a finished tracker's track set (after psfm_tracker_finish), built on the tracker's stream
+   from its device arrays without a host copy: the handle psfm_matches_create returns for the host copy of those arrays
+   (psfm_tracker_result: ptr as traj_ptr, frame_ids widened to int64, xy), bit for bit.  PSFM_ERR_INVALID for a tracker
+   that is not finished, num_images below the tracker's number of frames, or sample_k < 1. */
+int psfm_tracker_matches(psfm_tracker* t, int32_t num_images, int32_t sample_k, psfm_matches** out, int64_t* num_pairs,
+                         int64_t* num_matches);
+
 typedef struct psfm_match_table psfm_match_table;
 int psfm_matches_table(psfm_matches* m, const int32_t* image_ids, psfm_match_table** out, int64_t* num_keypoints,
                        int64_t* num_pairs, int64_t* num_matches);

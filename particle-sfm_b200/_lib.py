@@ -26,7 +26,7 @@ EXPORTS = [
     "psfm_flow_check_device", "psfm_tracker_finish", "psfm_tracker_result", "psfm_tracker_destroy",
     "psfm_tracker_create_mode", "psfm_tracker_track_npy", "psfm_track_npy_create", "psfm_track_npy_data",
     "psfm_track_npy_destroy",
-    "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy",
+    "psfm_matches_create", "psfm_matches_result", "psfm_matches_destroy", "psfm_tracker_matches",
     "psfm_matches_table", "psfm_match_table_result", "psfm_match_table_verify", "psfm_match_table_destroy",
     "psfm_known_rotation_translations", "psfm_triangulate_tracks",
     "psfm_two_view_relative_poses", "psfm_rotation_default_options", "psfm_estimate_global_rotations",
@@ -141,6 +141,7 @@ def lib():
     L.psfm_matches_create.argtypes = [i64p, C.c_int64, i64p, dp, C.c_int32, C.c_int32, C.POINTER(vp), i64p, i64p]
     L.psfm_matches_result.argtypes = [vp, i64p, dp, i64p, i64p, i64p]
     L.psfm_matches_destroy.argtypes = [vp]
+    L.psfm_tracker_matches.argtypes = [vp, C.c_int32, C.c_int32, C.POINTER(vp), i64p, i64p]
     L.psfm_matches_destroy.restype = None
     L.psfm_matches_table.argtypes = [vp, ip, C.POINTER(vp), i64p, i64p, i64p]
     L.psfm_match_table_result.argtypes = [vp, i64p, fp, ip, i64p, u32p]

@@ -24,6 +24,10 @@
 // visits images in get_image_ids order, which SQLite returns in name order (tests/golden/import_small.npz).
 // The host picks one ordered run per unordered pair and orders the pairs by pair_id; the handle's int64 matches and
 // double keypoints are freed once the table exists, so the peak stays at or below the record sort's.
+//
+// Steps 1-7 (psfm::matches_build) start from the track set on the device: psfm_matches_create uploads the host arrays
+// and hands them over to be freed as soon as they are read; psfm_tracker_matches (csrc/tracker.cu) passes the finished
+// tracker's own arrays, which stay where they are, and runs on the tracker's stream.
 #include <cub/device/device_scan.cuh>
 
 #include <algorithm>
@@ -200,22 +204,11 @@ struct psfm_matches {
   bool moved = false;                          // kxy and matches were moved into a match table
 };
 
-extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, const int64_t* frame_ids, const double* xy,
-                                   int32_t num_images, int32_t sample_k, psfm_matches** out, int64_t* num_pairs,
-                                   int64_t* num_matches) {
-  const char* entry = "psfm_matches_create";
-  if (!out || !num_pairs || !num_matches || !traj_ptr) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (num_trajs < 0 || num_images < 0 || sample_k < 1)
-    return fail(entry, PSFM_ERR_INVALID, "num_trajs and num_images must be >= 0, sample_k >= 1");
-  if (traj_ptr[0] != 0) return fail(entry, PSFM_ERR_INVALID, "traj_ptr[0] must be 0");
-  for (int64_t t = 0; t < num_trajs; ++t)
-    if (traj_ptr[t + 1] < traj_ptr[t]) return fail(entry, PSFM_ERR_INVALID, "traj_ptr must be non-decreasing");
-  const long long N = traj_ptr[num_trajs];
-  if (N > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 samples");
-  if (N > 0 && (!frame_ids || !xy)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
+namespace psfm {
+
+int matches_build(const char* entry, TrackSetDev& in, int num_images, int sample_k, cudaStream_t st, psfm_matches** out,
+                  int64_t* num_pairs, int64_t* num_matches) {
+  const long long N = in.num_obs, num_trajs = in.num_trajs;
   psfm_matches* H = new psfm_matches;
   H->num_images = num_images;
   H->num_obs = N;
@@ -228,32 +221,29 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
   }
   try {
     const int n = (int)N, K = sample_k, NI = num_images;
-    DBuf<long long> tptr, frames, cnt, off, kstart;
-    DBuf<double> dxy;
+    DBuf<long long> cnt, off, kstart;
     DBuf<int> f32a, f32b, ida, idb, kp, bad;
-    tptr.alloc((size_t)num_trajs + 1); frames.alloc(N); dxy.alloc(2 * (size_t)N);
-    tptr.upload(reinterpret_cast<const long long*>(traj_ptr), tptr.n, nullptr);
-    frames.upload(reinterpret_cast<const long long*>(frame_ids), N, nullptr); dxy.upload(xy, 2 * (size_t)N, nullptr);
     f32a.alloc(N); f32b.alloc(N); ida.alloc(N); idb.alloc(N); cnt.alloc(N + 1); bad.alloc(1);
-    bad.zero(nullptr);
-    k_count<<<grid_of(N + 1), 256>>>(n, tptr.p, num_trajs, frames.p, NI, K, f32a.p, ida.p, cnt.p, bad.p);
+    bad.zero(st);
+    k_count<<<grid_of(N + 1), 256, 0, st>>>(n, in.tptr, num_trajs, in.frames, NI, K, f32a.p, ida.p, cnt.p, bad.p);
     PSFM_LAUNCH_CHECK();
-    frames.release();
     // visiting positions: exclusive int64 scan of the per-sample counts, off[N] = number of records
     off.alloc(N + 1);
     {
       size_t bytes = 0;
-      PSFM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, cnt.p, off.p, n + 1, nullptr));
+      PSFM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, cnt.p, off.p, n + 1, st));
       DBuf<unsigned char> tmp;
-      tmp.alloc(bytes);
-      PSFM_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, cnt.p, off.p, n + 1, nullptr));
+      tmp.alloc(bytes, st);
+      PSFM_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, cnt.p, off.p, n + 1, st));
       PSFM_LAUNCH_CHECK();
     }
-    cnt.release();
     int h_bad = 0;
     long long M = 0;
-    PSFM_CUDA(cudaMemcpy(&h_bad, bad.p, sizeof(int), cudaMemcpyDeviceToHost));
-    PSFM_CUDA(cudaMemcpy(&M, off.p + N, sizeof(long long), cudaMemcpyDeviceToHost));
+    PSFM_CUDA(cudaMemcpyAsync(&h_bad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaMemcpyAsync(&M, off.p + N, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaStreamSynchronize(st));
+    cnt.release();
+    drop(in.own_frames);
     if (h_bad) {
       delete H;
       return fail(entry, PSFM_ERR_INVALID, "a frame id is outside [0, num_images)");
@@ -263,28 +253,31 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
     // k_records reads the unsorted frames: sort copies of them
     DBuf<int> frame32;
     frame32.alloc(N);
-    PSFM_CUDA(cudaMemcpy(frame32.p, f32a.p, sizeof(int) * (size_t)N, cudaMemcpyDeviceToDevice));
-    sort_pairs(fk, fv, n, key_bits(NI > 0 ? (u64)(NI - 1) : 0));
+    PSFM_CUDA(cudaMemcpyAsync(frame32.p, f32a.p, sizeof(int) * (size_t)N, cudaMemcpyDeviceToDevice, st));
+    sort_pairs(fk, fv, n, key_bits(NI > 0 ? (u64)(NI - 1) : 0), st);
     kstart.alloc((size_t)NI + 1);
-    k_kp_start<<<grid_of((long long)NI + 1), 256>>>(NI, fk.Current(), n, kstart.p);
+    k_kp_start<<<grid_of((long long)NI + 1), 256, 0, st>>>(NI, fk.Current(), n, kstart.p);
     PSFM_LAUNCH_CHECK();
     kp.alloc(N);
     H->kxy.alloc(2 * (size_t)N);
-    k_kp<<<grid_of(N), 256>>>(n, fk.Current(), fv.Current(), kstart.p, reinterpret_cast<const double2*>(dxy.p), kp.p,
-                              reinterpret_cast<double2*>(H->kxy.p));
+    k_kp<<<grid_of(N), 256, 0, st>>>(n, fk.Current(), fv.Current(), kstart.p, reinterpret_cast<const double2*>(in.xy), kp.p,
+                                     reinterpret_cast<double2*>(H->kxy.p));
     PSFM_LAUNCH_CHECK();
-    PSFM_CUDA(cudaMemcpy(H->kstart.data(), kstart.p, sizeof(long long) * ((size_t)NI + 1), cudaMemcpyDeviceToHost));
-    f32a.release(); f32b.release(); ida.release(); idb.release(); dxy.release();
+    PSFM_CUDA(cudaMemcpyAsync(H->kstart.data(), kstart.p, sizeof(long long) * ((size_t)NI + 1), cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaStreamSynchronize(st));
+    f32a.release(); f32b.release(); ida.release(); idb.release(); drop(in.own_xy);
     H->num_matches = M;
     if (M > 0) {
       // match records at their visiting positions, then stable by pair key
       DBuf<u64> ka, kb, va, vb;
       ka.alloc(M); kb.alloc(M); va.alloc(M); vb.alloc(M);
-      k_records<<<grid_of(N), 256>>>(n, tptr.p, num_trajs, frame32.p, off.p, K, NI, ka.p, va.p);
+      k_records<<<grid_of(N), 256, 0, st>>>(n, in.tptr, num_trajs, frame32.p, off.p, K, NI, ka.p, va.p);
       PSFM_LAUNCH_CHECK();
-      off.release(); frame32.release(); tptr.release();
+      PSFM_CUDA(cudaStreamSynchronize(st));
+      off.release(); frame32.release(); drop(in.own_tptr);
       cub::DoubleBuffer<u64> rk(ka.p, kb.p), rv(va.p, vb.p);
-      sort_pairs(rk, rv, (long long)M, key_bits((u64)NI * (u64)NI - 1));
+      sort_pairs(rk, rv, (long long)M, key_bits((u64)NI * (u64)NI - 1), st);
+      PSFM_CUDA(cudaStreamSynchronize(st));
       release_other(ka, kb, rk.Current());
       release_other(va, vb, rv.Current());
       const u64* skey = rk.Current();
@@ -294,21 +287,23 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
       DBuf<long long> heads;
       DBuf<unsigned long long> nheads;
       heads.alloc(max_runs); nheads.alloc(1);
-      nheads.zero(nullptr);
-      k_run_heads<<<grid_stride_of(M), 256>>>(M, skey, heads.p, nheads.p);
+      nheads.zero(st);
+      k_run_heads<<<grid_stride_of(M), 256, 0, st>>>(M, skey, heads.p, nheads.p);
       PSFM_LAUNCH_CHECK();
       unsigned long long R64 = 0;
-      PSFM_CUDA(cudaMemcpy(&R64, nheads.p, sizeof(R64), cudaMemcpyDeviceToHost));
+      PSFM_CUDA(cudaMemcpyAsync(&R64, nheads.p, sizeof(R64), cudaMemcpyDeviceToHost, st));
+      PSFM_CUDA(cudaStreamSynchronize(st));
       const int R = (int)R64;
       DBuf<u64> rkey, rfirst;
       rkey.alloc(R); rfirst.alloc(R);
-      k_run_info<<<grid_of(R), 256>>>(R, heads.p, skey, sval, rkey.p, rfirst.p);
+      k_run_info<<<grid_of(R), 256, 0, st>>>(R, heads.p, skey, sval, rkey.p, rfirst.p);
       PSFM_LAUNCH_CHECK();
       std::vector<long long> h_heads(R);
       std::vector<u64> h_key(R), h_first(R);
-      PSFM_CUDA(cudaMemcpy(h_heads.data(), heads.p, sizeof(long long) * R, cudaMemcpyDeviceToHost));
-      PSFM_CUDA(cudaMemcpy(h_key.data(), rkey.p, sizeof(u64) * R, cudaMemcpyDeviceToHost));
-      PSFM_CUDA(cudaMemcpy(h_first.data(), rfirst.p, sizeof(u64) * R, cudaMemcpyDeviceToHost));
+      PSFM_CUDA(cudaMemcpyAsync(h_heads.data(), heads.p, sizeof(long long) * R, cudaMemcpyDeviceToHost, st));
+      PSFM_CUDA(cudaMemcpyAsync(h_key.data(), rkey.p, sizeof(u64) * R, cudaMemcpyDeviceToHost, st));
+      PSFM_CUDA(cudaMemcpyAsync(h_first.data(), rfirst.p, sizeof(u64) * R, cudaMemcpyDeviceToHost, st));
+      PSFM_CUDA(cudaStreamSynchronize(st));
       if (rk.Current() == ka.p) ka.release();
       else kb.release();
       // runs in sorted-record order (their heads), and the pair list: by image a, then first appearance
@@ -337,11 +332,11 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
       for (int r = 0; r < R; ++r) { h_start[r] = h_heads[by_head[r]]; h_dest[r] = dest[by_head[r]]; }
       DBuf<long long> d_start, d_dest;
       d_start.alloc(R); d_dest.alloc(R);
-      d_start.upload(h_start.data(), R, nullptr); d_dest.upload(h_dest.data(), R, nullptr);
+      d_start.upload(h_start.data(), R, st); d_dest.upload(h_dest.data(), R, st);
       H->matches.alloc(2 * (size_t)M);
-      k_scatter<<<grid_stride_of(M), 256>>>(M, d_start.p, R, d_dest.p, sval, kp.p, H->matches.p);
+      k_scatter<<<grid_stride_of(M), 256, 0, st>>>(M, d_start.p, R, d_dest.p, sval, kp.p, H->matches.p);
       PSFM_LAUNCH_CHECK();
-      PSFM_CUDA(cudaDeviceSynchronize());
+      PSFM_CUDA(cudaStreamSynchronize(st));
     }
     *num_pairs = (int64_t)(H->pair_ptr.size() - 1);
     *num_matches = M;
@@ -351,6 +346,41 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
     delete H;
     return f.code;
   }
+}
+
+}  // namespace psfm
+
+extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, const int64_t* frame_ids, const double* xy,
+                                   int32_t num_images, int32_t sample_k, psfm_matches** out, int64_t* num_pairs,
+                                   int64_t* num_matches) {
+  const char* entry = "psfm_matches_create";
+  if (!out || !num_pairs || !num_matches || !traj_ptr) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  *out = nullptr;
+  if (num_trajs < 0 || num_images < 0 || sample_k < 1)
+    return fail(entry, PSFM_ERR_INVALID, "num_trajs and num_images must be >= 0, sample_k >= 1");
+  if (traj_ptr[0] != 0) return fail(entry, PSFM_ERR_INVALID, "traj_ptr[0] must be 0");
+  for (int64_t t = 0; t < num_trajs; ++t)
+    if (traj_ptr[t + 1] < traj_ptr[t]) return fail(entry, PSFM_ERR_INVALID, "traj_ptr must be non-decreasing");
+  const long long N = traj_ptr[num_trajs];
+  if (N > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 samples");
+  if (N > 0 && (!frame_ids || !xy)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+  int rc = require_device(entry);
+  if (rc != PSFM_OK) return rc;
+  try {
+    DBuf<long long> tptr, frames;
+    DBuf<double> dxy;
+    TrackSetDev in;
+    in.num_trajs = num_trajs;
+    in.num_obs = N;
+    if (N > 0) {
+      tptr.alloc((size_t)num_trajs + 1); frames.alloc(N); dxy.alloc(2 * (size_t)N);
+      tptr.upload(reinterpret_cast<const long long*>(traj_ptr), tptr.n, nullptr);
+      frames.upload(reinterpret_cast<const long long*>(frame_ids), N, nullptr); dxy.upload(xy, 2 * (size_t)N, nullptr);
+      in.tptr = tptr.p; in.frames = frames.p; in.xy = dxy.p;
+      in.own_tptr = &tptr; in.own_frames = &frames; in.own_xy = &dxy;
+    }
+    return matches_build(entry, in, num_images, sample_k, nullptr, out, num_pairs, num_matches);
+  } catch (const CudaFail& f) { return f.code; }
 }
 
 extern "C" int psfm_matches_result(const psfm_matches* H, int64_t* keypoint_ptr, double* keypoints, int64_t* pair_images,

@@ -25,6 +25,7 @@
 #include <cub/device/device_scan.cuh>
 #include <vector>
 
+#include "match_table.cuh"
 #include "psfm_common.cuh"
 #include "track_npy.cuh"
 #include "traj_solver.cuh"
@@ -761,6 +762,43 @@ extern "C" int psfm_tracker_track_npy(psfm_tracker* T, psfm_track_npy** out, int
   // the tracker's ids are retire ranks (< 2^31, int counters), its frame ids times, its ptr an exclusive scan
   rc = track_npy_encode(T->ids.p, T->ptr.p, T->res_frames.p, T->res_xy.p, T->res_trajs, T->st, out, nbytes);
   return rc == PSFM_OK ? rc : tracker_broken(T, rc);
+}
+
+namespace {
+
+__global__ void k_widen(long long n, const int* in, long long* out) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (i < n) out[i] = in[i];
+}
+
+}  // namespace
+
+extern "C" int psfm_tracker_matches(psfm_tracker* T, int32_t num_images, int32_t sample_k, psfm_matches** out,
+                                    int64_t* num_pairs, int64_t* num_matches) {
+  const char* entry = "psfm_tracker_matches";
+  int rc = tracker_usable(T, out && num_pairs && num_matches, entry);
+  if (rc != PSFM_OK) return rc;
+  *out = nullptr;
+  if (!T->finished) return fail(entry, PSFM_ERR_INVALID, "call psfm_tracker_finish first");
+  if (num_images < T->num_frames) return fail(entry, PSFM_ERR_INVALID, "num_images is below the tracker's number of frames");
+  if (sample_k < 1) return fail(entry, PSFM_ERR_INVALID, "sample_k must be >= 1");
+  if (T->res_obs > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 samples");
+  try {
+    // the tracker's ptr and xy are read where they are; its int32 frame ids are widened to the build's int64
+    psfm::DBuf<long long> frames;
+    psfm::TrackSetDev in;
+    in.num_trajs = T->res_trajs;
+    in.num_obs = T->res_obs;
+    if (T->res_obs > 0) {
+      frames.alloc((size_t)T->res_obs);
+      k_widen<<<grid_of(T->res_obs), 256, 0, T->st>>>(T->res_obs, T->res_frames.p, frames.p);
+      PSFM_LAUNCH_CHECK();
+      in.tptr = T->ptr.p; in.frames = frames.p; in.xy = T->res_xy.p;
+      in.own_frames = &frames;
+    }
+    rc = psfm::matches_build(entry, in, num_images, sample_k, T->st, out, num_pairs, num_matches);
+    return rc == PSFM_OK ? rc : tracker_broken(T, rc);
+  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
 }
 
 extern "C" void psfm_tracker_destroy(psfm_tracker* T) {

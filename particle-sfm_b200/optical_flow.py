@@ -448,70 +448,104 @@ def compute_optical_flows(image_dir, model_path, path_consistency=True):
     return out[1][0], out[1][1], (out[2][0] if path_consistency else []), (out[2][1] if path_consistency else [])
 
 
-def write_optical_flows(image_dir, output_dir, model_path, skip_path_consistency=False, skip_exists=False):
-    """compute_raft_custom_folder (and _stride2 unless skip_path_consistency) into output_dir.  With skip_exists, a
-    pair whose three files exist is skipped, as the reference does.  Files are written on a writer thread while the
-    next batch runs.  Returns the number of pairs computed."""
-    import torch
-    paths, h, w = frame_list(image_dir)
-    sd = load_weights(model_path)
-    for s in ((1,) if skip_path_consistency else (1, 2)):
-        for d in _subdirs(s):
-            os.makedirs(os.path.join(output_dir, d), exist_ok=True)
+class FlowWriter:
+    """A sink for _run that writes each batch's files on a writer thread while the next batch runs: the maps and
+    images go to pinned host buffers on torch's current stream, and the thread writes them once that copy is done.
+    files(t, stride) -> (forward .flo, backward .flo, flow image) paths.  close() waits for the thread and raises
+    the first failed write (join() only waits); a failed write also makes the next call raise."""
 
-    def files(t, s):
-        f, b, i = output_names(paths[t])
-        df, db, di = _subdirs(s)
-        return os.path.join(output_dir, df, f), os.path.join(output_dir, db, b), os.path.join(output_dir, di, i)
+    def __init__(self, files):
+        self.files = files
+        self.work, self.failure = queue.Queue(maxsize=2), []
+        self.thread = threading.Thread(target=self._write, name="psfm-flow-writer", daemon=True)
+        self.thread.start()
 
-    pairs = _pairs(len(paths), not skip_path_consistency)
-    if skip_exists:
-        pairs = [p for p in pairs if not all(os.path.exists(f) for f in files(*p))]
-    if not pairs:
-        return 0
-    _require_device()
-    import cv2
-    work, failure = queue.Queue(maxsize=2), []
-
-    def writer():
+    def _write(self):
+        import cv2
         while True:
-            item = work.get()
+            item = self.work.get()
             if item is None:
                 return
-            if failure:
+            if self.failure:
                 continue
             try:
                 batch, flows, images, ev = item
                 ev.synchronize()
                 for j, (t, s) in enumerate(batch):
-                    ff, fb, fi = files(t, s)
+                    ff, fb, fi = self.files(t, s)
                     if not cv2.imwrite(fi, images[j].numpy()):
                         raise OSError("%s: could not be written" % fi)
                     write_flo(ff, flows[j].numpy())
                     write_flo(fb, flows[len(batch) + j].numpy())
             except BaseException as e:
-                failure.append(e)
+                self.failure.append(e)
 
-    def send(batch, flows, images):
-        if failure:
-            raise failure[0]
+    def __call__(self, batch, flows, images):
+        import torch
+        if self.failure:
+            raise self.failure[0]
         hf = torch.empty(flows.shape, dtype=flows.dtype, pin_memory=True)
         hi = torch.empty(images.shape, dtype=images.dtype, pin_memory=True)
         hf.copy_(flows, non_blocking=True)
         hi.copy_(images, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record(torch.cuda.current_stream())
-        work.put((batch, hf, hi, ev))
+        self.work.put((batch, hf, hi, ev))
 
-    th = threading.Thread(target=writer, name="psfm-flow-writer", daemon=True)
-    th.start()
+    def join(self):
+        """Ends the thread once the batches sent so far are written (or skipped after a failure)."""
+        if self.thread is not None:
+            self.work.put(None)
+            self.thread.join()
+            self.thread = None
+
+    def close(self):
+        self.join()
+        if self.failure:
+            raise self.failure[0]
+
+
+def flow_files(paths, output_dir):
+    """files(t, stride) of the flow directory output_dir for the frames `paths`: the forward .flo, backward .flo and
+    flow image of pair (t, t + stride), named as compute_raft_custom_folder names them."""
+    def files(t, s):
+        f, b, i = output_names(paths[t])
+        df, db, di = _subdirs(s)
+        return os.path.join(output_dir, df, f), os.path.join(output_dir, db, b), os.path.join(output_dir, di, i)
+    return files
+
+
+def make_flow_dirs(output_dir, path_consistency):
+    for s in ((1, 2) if path_consistency else (1,)):
+        for d in _subdirs(s):
+            os.makedirs(os.path.join(output_dir, d), exist_ok=True)
+
+
+def missing_pairs(paths, output_dir, path_consistency):
+    """The pairs of the frames `paths` whose three files are not all in output_dir (skip_exists)."""
+    files = flow_files(paths, output_dir)
+    return [p for p in _pairs(len(paths), path_consistency) if not all(os.path.exists(f) for f in files(*p))]
+
+
+def write_optical_flows(image_dir, output_dir, model_path, skip_path_consistency=False, skip_exists=False):
+    """compute_raft_custom_folder (and _stride2 unless skip_path_consistency) into output_dir.  With skip_exists, a
+    pair whose three files exist is skipped, as the reference does.  Files are written on a writer thread while the
+    next batch runs.  Returns the number of pairs computed."""
+    paths, h, w = frame_list(image_dir)
+    sd = load_weights(model_path)
+    make_flow_dirs(output_dir, not skip_path_consistency)
+    pairs = _pairs(len(paths), not skip_path_consistency)
+    if skip_exists:
+        pairs = missing_pairs(paths, output_dir, not skip_path_consistency)
+    if not pairs:
+        return 0
+    _require_device()
+    writer = FlowWriter(flow_files(paths, output_dir))
     try:
-        _run(paths, h, w, sd, pairs, send)
+        _run(paths, h, w, sd, pairs, writer)
     finally:
-        work.put(None)
-        th.join()
-    if failure:
-        raise failure[0]
+        writer.join()
+    writer.close()
     return len(pairs)
 
 

@@ -229,7 +229,6 @@ def connect_point_trajectories(flow_dir, sample_ratio=2, flow_check_thres=1.0, t
                                npy_path=None):
     """The stage from a checked flow directory -> tracker.TrackArrays; with npy_path, the track set is also written
     there as track.npy from the device."""
-    import torch
     frames, h, w = flow_frames(flow_dir, skip_path_consistency)
     n_flows = len(frames)
     pc = not skip_path_consistency
@@ -237,8 +236,6 @@ def connect_point_trajectories(flow_dir, sample_ratio=2, flow_check_thres=1.0, t
     stream = None
     try:
         stream = _FlowStream(frames, h, w)
-        occ = torch.empty((h, w), dtype=torch.uint8, device="cuda")
-        occ2 = torch.empty((h, w), dtype=torch.uint8, device="cuda") if pc else None
         stream.upload(0)
         prev = None
         for t in range(n_flows):
@@ -246,12 +243,8 @@ def connect_point_trajectories(flow_dir, sample_ratio=2, flow_check_thres=1.0, t
                 stream.upload(t + 1)           # crosses the bus while frame t runs
             m = stream.maps(t)
             flow = m[0]
-            trk.flow_check(flow, m[1], flow_check_thres, out=occ)
-            if pc and t >= 1:
-                trk.flow_check(m[2], m[3], flow_check_thres, out=occ2)
-                trk.optimize_buffer(trk.step(flow, occ, prev, m[2], occ2), None, None)
-            else:
-                trk.step(flow, occ)
+            f2, b2 = (m[2], m[3]) if pc and t >= 1 else (None, None)
+            trk.advance(t, flow, m[1], prev, f2, b2, flow_check_thres)
             if t >= 1:
                 stream.release(t - 1)
             prev = flow

@@ -177,23 +177,32 @@ def mapper_options(min_num_matches=None):
 def main_global_sfm(sfm_dir, image_dir, trajectories, single_camera=True, remove_dynamic=True,
                     skip_geometric_verification=False, min_num_matches=None, convert_path=None):
     """sfm/main_sfm.py:127-159 on the GPU: SFM/database.db, SFM/image_match_pairs.txt and SFM/model/0/*.bin (copied to
-    SFM/model/), the points coloured from image_dir.  trajectories: a directory holding track.npy, the dict, or a
-    tracker.TrackArrays.  With convert_path, the converted depth maps and poses are written there from the arrays in
+    SFM/model/), the points coloured from image_dir.  trajectories: a directory holding track.npy, the dict, a
+    tracker.TrackArrays, or a finished tracker._ResidentTracker, whose track set goes into the match table on the device
+    (no host copy, no frame-range scan) and which is closed once the table is built.  With convert_path, the converted depth maps and poses are written there from the arrays in
     memory.  Returns a global_mapper.MapperReport whose stages add import, table, verification and database, and whose
     stats are the model's stats (None, and success False, when the rotation or position stage fails and no model is
     written).  Raises ValueError before any device call or file write for an input the importer cannot take."""
     if not single_camera:
         raise ValueError("single_camera=False is not supported: every image would get its own camera, and the bundle "
                          "adjustment refines the focal length of one camera only")
+    from .tracker import _ResidentTracker
     report = gm.MapperReport()
     t0 = time.perf_counter()
     images = read_image_set(image_dir)
-    flat = handoff._flatten(load_trajectories(trajectories), remove_dynamic)
-    frames = flat[2]
-    if frames.size and (frames.min() < 0 or frames.max() >= len(images.names)):
-        k = int(np.nonzero((frames < 0) | (frames >= len(images.names)))[0][0])
-        raise ValueError(f"trajectory {flat[0][int(flat[1][k])]!r} has frame id {int(frames[k])}, not below the number "
-                         f"of images ({len(images.names)}) in {image_dir}")
+    resident = isinstance(trajectories, _ResidentTracker)
+    if resident:
+        # its frame ids are below its number of frames, which the caller has checked against the images
+        if trajectories.num_frames > len(images.names):
+            raise ValueError(f"the tracker has {trajectories.num_frames} frames, {image_dir} holds {len(images.names)} "
+                             "images")
+    else:
+        flat = handoff._flatten(load_trajectories(trajectories), remove_dynamic)
+        frames = flat[2]
+        if frames.size and (frames.min() < 0 or frames.max() >= len(images.names)):
+            k = int(np.nonzero((frames < 0) | (frames >= len(images.names)))[0][0])
+            raise ValueError(f"trajectory {flat[0][int(flat[1][k])]!r} has frame id {int(frames[k])}, not below the "
+                             f"number of images ({len(images.names)}) in {image_dir}")
     os.makedirs(sfm_dir, exist_ok=True)
     db_path = os.path.join(sfm_dir, "database.db")
     pair_path = os.path.join(sfm_dir, "image_match_pairs.txt")
@@ -204,8 +213,12 @@ def main_global_sfm(sfm_dir, image_dir, trajectories, single_camera=True, remove
     writer.submit(write_schema, images)
     table = None
     try:
-        table = handoff.ResidentMatchTable(flat, images.image_ids)
-        del flat, frames
+        if resident:
+            table = handoff.ResidentMatchTable.from_tracker(trajectories, images.image_ids)
+            trajectories.close()            # the track set has moved into the table
+        else:
+            table = handoff.ResidentMatchTable(flat, images.image_ids)
+            del flat, frames
         table.pairs.write_pair_list(pair_path, images.names)
         report.add("import", t0, {"images": len(images.names), "ordered_pairs": int(len(table.pairs.pair_images))})
         t0 = time.perf_counter()

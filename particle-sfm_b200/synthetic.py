@@ -152,6 +152,87 @@ def umeyama_ate(est_centres, gt_centres):
     return float(np.sqrt((err ** 2).sum(1).mean()))
 
 
+# ----------------------------------------------------------------------------- a rigid video with exact flows
+
+ROOM_HALF = np.array([4.0, 2.5, 4.0])          # the box room's half extents (x, y down, z)
+
+
+def _room_camera(t, n_frames, seed_shift):
+    """World-to-camera rotation R and centre C of frame t of the room sequence: a smooth path near the room's
+    middle, turning left and right."""
+    u = t / max(1, n_frames - 1)
+    a, b = seed_shift
+    c = np.array([-0.6 + 1.2 * u + 0.2 * a, 0.2 * np.sin(2 * np.pi * u + b), 0.4 * np.sin(np.pi * u) - 0.2])
+    yaw, pitch = 0.15 * np.sin(np.pi * u + a) - 0.05, 0.04 * np.sin(2 * np.pi * u)
+    cy, sy, cp, sp = np.cos(yaw), np.sin(yaw), np.cos(pitch), np.sin(pitch)
+    ry = np.array([[cy, 0, sy], [0, 1, 0], [-sy, 0, cy]])
+    rx = np.array([[1, 0, 0], [0, cp, -sp], [0, sp, cp]])
+    return (ry @ rx).T, c
+
+
+def _room_points(R, C, h, w, camera):
+    """The wall point seen at every pixel (i, j) (image point (j + 0.5, i + 0.5), COLMAP's pixel centre) from a
+    camera inside the room: [h][w][3] world coordinates.  From inside a convex room every ray meets one wall."""
+    f, cx, cy = camera
+    jj, ii = np.meshgrid(np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64))
+    d = np.stack([(jj + 0.5 - cx) / f, (ii + 0.5 - cy) / f, np.ones_like(jj)], -1) @ R       # rays in the world
+    with np.errstate(divide="ignore"):
+        hit = np.where(d > 0, (ROOM_HALF - C) / d, np.where(d < 0, (-ROOM_HALF - C) / d, np.inf))
+    return C + hit.min(-1)[..., None] * d
+
+
+def _room_texture(P, rng):
+    """uint8 RGB of wall points: a few sinusoids of the 3D point per channel."""
+    k = rng.uniform(-1, 1, (3, 4, 3)) * np.array([3.0, 7.0, 13.0, 23.0])[None, :, None]
+    ph = rng.uniform(0, 2 * np.pi, (3, 4))
+    amp = np.array([50.0, 35.0, 22.0, 12.0])
+    out = np.empty(P.shape[:-1] + (3,))
+    for c in range(3):
+        out[..., c] = 128 + sum(amp[m] * np.sin(P @ k[c, m] + ph[c, m]) for m in range(4))
+    return np.clip(np.rint(out), 0, 255).astype(np.uint8)
+
+
+def _room_flow(P, R, C, camera):
+    """Flow of the pixels whose world points are P [h][w][3] into the camera (R, C): the projection's pixel position
+    minus the pixel's own; a point behind that camera gets a flow far outside the frame."""
+    f, cx, cy = camera
+    h, w = P.shape[:2]
+    X = (P - C) @ R.T
+    z = X[..., 2]
+    front = z > 1e-9
+    zs = np.where(front, z, 1.0)
+    jj, ii = np.meshgrid(np.arange(w, dtype=np.float64), np.arange(h, dtype=np.float64))
+    flow = np.stack([f * X[..., 0] / zs + cx - 0.5 - jj, f * X[..., 1] / zs + cy - 0.5 - ii], -1)
+    flow[~front] = 1e6
+    return flow.astype(np.float32)
+
+
+def make_room_sequence(n_frames, h, w, seed=0):
+    """A rigid video with exact flows: a camera (SIMPLE_PINHOLE, f = 1.2 max(w, h), principal point at the centre,
+    what the SfM importer assumes) moves along a smooth path inside a convex box room, so no pixel is ever occluded;
+    the walls are textured procedurally from the 3D point.  Returns (frames [n][h][w][3] uint8, flows {(t, stride):
+    (forward, backward)} for strides 1 and 2, [h][w][2] float32 computed in closed form from every pixel's wall point
+    and the two poses, qvec [n][4], tvec [n][3] (world to camera, COLMAP's convention))."""
+    rng = np.random.default_rng(seed)
+    camera = (1.2 * max(w, h), w / 2.0, h / 2.0)
+    shift = rng.uniform(-1, 1, 2) * [0.5, np.pi]
+    poses = [_room_camera(t, n_frames, shift) for t in range(n_frames)]
+    tex = np.random.default_rng(rng.integers(1 << 31))
+    frames, flows = [], {}
+    pts = [_room_points(R, C, h, w, camera) for R, C in poses]
+    tex_state = tex.bit_generator.state
+    for P in pts:
+        tex.bit_generator.state = tex_state                # the same texture on every frame
+        frames.append(_room_texture(P, tex))
+    for t in range(n_frames):
+        for s in (1, 2):
+            if t + s < n_frames:
+                flows[(t, s)] = (_room_flow(pts[t], *poses[t + s], camera), _room_flow(pts[t + s], *poses[t], camera))
+    qvec = np.array([rotmat_to_qvec(R) for R, _ in poses])
+    tvec = np.array([-R @ C for R, C in poses])
+    return np.stack(frames), flows, qvec, tvec
+
+
 # ----------------------------------------------------------------------------- HP1
 
 def bilinear_zeros(img, xy):

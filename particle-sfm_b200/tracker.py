@@ -385,7 +385,9 @@ class _ResidentTracker:
     def __init__(self, h, w, sample_ratio, num_frames, path_consistency=True):
         from . import _lib
         self.L, self.check = _lib.lib(), _lib.check
-        self.h, self.w = h, w
+        self.h, self.w, self.num_frames = h, w, num_frames
+        self.path_consistency = path_consistency
+        self.occ = self.occ2 = None             # advance()'s occlusion maps, reused frame after frame
         self.handle = _C.c_void_p()
         self.stream = None
         if self.L.psfm_device_count() > 0:      # without a device the library refuses below, before torch touches CUDA
@@ -432,16 +434,48 @@ class _ResidentTracker:
         new = np.ascontiguousarray(np.asarray(new, np.float64).reshape(n, 4))
         self.check(self.L.psfm_tracker_set_buffer(self.handle, _lib.dptr(new)), "psfm_tracker_set_buffer")
 
-    def finish(self, traj_min_len):
+    def advance(self, t, flow_f, flow_b, flow_prev=None, flow_f2=None, flow_b2=None, thres=1.0, optimize_fn=None,
+                flow12_map=None):
+        """Frame t of main_connect_point_trajectories.py: the flow check of pair (t, 1) (flow_f, flow_b), with path
+        consistency from t = 1 on the flow check of pair (t-1, 2) (flow_f2, flow_b2), the step (flow_prev: the
+        forward map of pair (t-1, 1)) and optimize_buffer (optimize_fn None: HP1 on the device; otherwise it gets
+        flow12_map, default flow_f, as optimize_buffer gives it).  Maps are CUDA tensors on the tracker's stream;
+        they may be dropped once this returns, as the stream orders any reuse of their memory after this work."""
+        import torch
+        if self.occ is None:
+            self.occ = torch.empty((self.h, self.w), dtype=torch.uint8, device=flow_f.device)
+        self.flow_check(flow_f, flow_b, thres, out=self.occ)
+        if self.path_consistency and t >= 1:
+            if self.occ2 is None:
+                self.occ2 = torch.empty((self.h, self.w), dtype=torch.uint8, device=flow_f.device)
+            self.flow_check(flow_f2, flow_b2, thres, out=self.occ2)
+            n = self.step(flow_f, self.occ, flow_prev, flow_f2, self.occ2)
+            self.optimize_buffer(n, optimize_fn, flow_f if flow12_map is None else flow12_map)
+        else:
+            self.step(flow_f, self.occ)
+
+    def finish(self, traj_min_len, result=True):
+        """psfm_tracker_finish -> the track set's TrackArrays (host copies); result=False: (number of trajectories,
+        number of observations) only, the set left on the device for matches() and track_npy_body()."""
         from . import _lib
         nt, m = _C.c_int64(), _C.c_int64()
         self.check(self.L.psfm_tracker_finish(self.handle, int(traj_min_len), _C.byref(nt), _C.byref(m)), "psfm_tracker_finish")
+        if not result:
+            return nt.value, m.value
         ids, ptr = np.empty(nt.value, np.int64), np.empty(nt.value + 1, np.int64)
         frame_ids, xy = np.empty(m.value, np.int32), np.empty((m.value, 2), np.float64)
         i64 = lambda a: a.ctypes.data_as(_C.POINTER(_C.c_int64))
         self.check(self.L.psfm_tracker_result(self.handle, i64(ids), i64(ptr), frame_ids.ctypes.data_as(_C.POINTER(_C.c_int32)),
                                               _lib.dptr(xy)), "psfm_tracker_result")
         return TrackArrays(ids, ptr, frame_ids, xy)
+
+    def matches(self, num_images, sample_k):
+        """After finish(): psfm_tracker_matches, the hand-off's psfm_matches handle built from the track set where it
+        lies -> (handle, number of ordered pairs, number of matches); the caller destroys the handle."""
+        handle, npairs, nmatches = _C.c_void_p(), _C.c_int64(), _C.c_int64()
+        self.check(self.L.psfm_tracker_matches(self.handle, int(num_images), int(sample_k), _C.byref(handle),
+                                               _C.byref(npairs), _C.byref(nmatches)), "psfm_tracker_matches")
+        return handle, npairs.value, nmatches.value
 
     def track_npy_body(self):
         """After finish(): the finished track set's track.npy state body, encoded on the device where the set lies
@@ -549,14 +583,11 @@ def main_connect_point_trajectories_device(flows_f, flows_b, flows_f2, flows_b2,
         prev = None
         for frame_id in range(n_flows):
             flow = _on_device(flows_f[frame_id], f32)
-            occ = trk.flow_check(flow, _on_device(flows_b[frame_id], f32), flow_check_thres)
-            if frame_id + 1 >= 2:
-                f2 = _on_device(flows_f2[frame_id - 1], f32)
-                occ2 = trk.flow_check(f2, _on_device(flows_b2[frame_id - 1], f32), flow_check_thres)
-                n = trk.step(flow, occ, prev, f2, occ2)
-                trk.optimize_buffer(n, optimize_fn, flows_f[frame_id])
-            else:
-                trk.step(flow, occ)
+            f2 = b2 = None
+            if frame_id >= 1:
+                f2, b2 = _on_device(flows_f2[frame_id - 1], f32), _on_device(flows_b2[frame_id - 1], f32)
+            trk.advance(frame_id, flow, _on_device(flows_b[frame_id], f32), prev, f2, b2, flow_check_thres, optimize_fn,
+                        flows_f[frame_id])
             prev = flow
         return trk.finish(traj_min_len)
     finally:
