@@ -967,6 +967,25 @@ int psfm_flow_upsample(const float* flow, const float* mask, int32_t num_problem
 int psfm_flow_to_image(const float* flow, int32_t num_maps, int32_t h, int32_t w, uint8_t* bgr, void* stream);
 
 /* ------------------------------------------------------------------------- */
+/* Monocular depth (MiDaS midas_v21, DESIGN.md §4.16): the steps the reference */
+/* runs on the host around the network.  Device pointers, torch's stream.      */
+/* ------------------------------------------------------------------------- */
+/* psfm_depth_prepare: uint8 RGB frames [n][h][w][3] -> the network input [n][3][net_h][net_w] with channels_last
+   strides (memory [n][net_h][net_w][3]), float32 or (half = 1) fp16: / 255, cv2.resize(INTER_CUBIC) in float64,
+   (x - ImageNet mean) / std, rounded once to float32 (then to fp16). */
+int psfm_depth_prepare(const uint8_t* rgb, int32_t num_frames, int32_t h, int32_t w, int32_t net_h, int32_t net_w,
+                       int32_t half, void* out, void* stream);
+/* psfm_depth_upsample: the prediction [n][net_h][net_w] (float32, or fp16 with half = 1) -> F.interpolate(bicubic,
+   align_corners=False) at h x w, rounded to the prediction's dtype, written as float32 [n][h][w] with the rows
+   flipped (the PFM payload); minmax [n][2] receives each frame's minimum and maximum. */
+int psfm_depth_upsample(const void* pred, int32_t num_frames, int32_t net_h, int32_t net_w, int32_t half, int32_t h,
+                        int32_t w, float* flipped, float* minmax, void* stream);
+/* psfm_depth_quantize: write_depth's 16-bit pixels [n][h][w] (frame orientation) from the flipped maps and their
+   minmax: (uint16)(65535 * (d - min) / (max - min)) in float32, zeros where max - min <= float64 eps. */
+int psfm_depth_quantize(const float* flipped, int32_t num_frames, int32_t h, int32_t w, const float* minmax,
+                        uint16_t* pixels, void* stream);
+
+/* ------------------------------------------------------------------------- */
 /* Multi-GPU (HP2): points sharded across ranks, one all-reduce of the         */
 /* camera-side vector per PCG step (SURVEY.md §8e).                            */
 /* ------------------------------------------------------------------------- */

@@ -38,6 +38,7 @@ EXPORTS = [
     "psfm_convert_create", "psfm_convert_result", "psfm_convert_destroy",
     "psfm_colors_create", "psfm_colors_add_images", "psfm_colors_result", "psfm_colors_destroy",
     "psfm_corr_pyramids", "psfm_corr_pyramid_floats", "psfm_corr_lookup", "psfm_flow_upsample", "psfm_flow_to_image",
+    "psfm_depth_prepare", "psfm_depth_upsample", "psfm_depth_quantize",
     "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
@@ -184,6 +185,9 @@ def lib():
     L.psfm_corr_lookup.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp]
     L.psfm_flow_upsample.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, ip, vp, vp]
     L.psfm_flow_to_image.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, vp, vp]
+    L.psfm_depth_prepare.argtypes = [vp] + [C.c_int32] * 6 + [vp, vp]
+    L.psfm_depth_upsample.argtypes = [vp] + [C.c_int32] * 6 + [vp, vp, vp]
+    L.psfm_depth_quantize.argtypes = [vp] + [C.c_int32] * 3 + [vp, vp, vp]
     L.psfm_dist_get_unique_id.argtypes = [C.POINTER(C.c_uint8)]
     L.psfm_dist_init.argtypes = [C.POINTER(C.c_uint8), C.c_int32, C.c_int32]
     L.psfm_dist_finalize.restype = None

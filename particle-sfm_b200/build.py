@@ -25,7 +25,8 @@ COMMON = ["-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", CXX
 # (source, extra flags).  traj_solver.cu: -fmad=false so that its iterates are
 # bit-identical to the oracle compiled with -ffp-contract=off (DESIGN.md §4).  convert.cu: the same, so that its
 # depths and percentiles equal the numpy restatement's (DESIGN.md §4.10).  colors.cu: the same, so that its
-# interpolated samples equal the oracle's (DESIGN.md §4.11).
+# interpolated samples equal the oracle's (DESIGN.md §4.11).  midas.cu: the same, so that its input transform
+# restates cv2's unfused float64 arithmetic (DESIGN.md §4.16).
 UNITS = [
     ("common.cu", []),
     ("pair_inputs.cu", []),
@@ -43,6 +44,7 @@ UNITS = [
     ("convert.cu", ["-fmad=false"]),
     ("colors.cu", ["-fmad=false"]),
     ("optical_flow.cu", ["-fmad=false"]),
+    ("midas.cu", ["-fmad=false"]),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

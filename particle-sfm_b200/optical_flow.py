@@ -322,16 +322,23 @@ def write_flo(path, flow):
 
 # ----------------------------------------------------------------------------- the stage
 
+def decode_rgb(path):
+    """A frame as RAFT's custom folder scripts read it: PIL's decode, [H][W][3] uint8 RGB."""
+    from PIL import Image
+    with Image.open(path) as im:
+        return np.asarray(im, dtype=np.uint8)
+
+
 class _FrameReader:
     """Decodes the frames a run needs, in order, on host threads into pinned [H][W][3] uint8 tensors, a few ahead of
     their use; upload(i) copies frame i on the copy stream and returns the device tensor, ordered before torch's
-    current stream."""
+    current stream.  decode(path) gives a frame as an [H][W][3] uint8 RGB array (decode_rgb by default)."""
 
     AHEAD = 6
 
-    def __init__(self, paths, order):
+    def __init__(self, paths, order, decode=decode_rgb):
         import torch
-        self.paths, self.order, self.next = paths, list(order), 0
+        self.paths, self.order, self.next, self.decode = paths, list(order), 0, decode
         self.pool = ThreadPoolExecutor(max_workers=4, thread_name_prefix="psfm-frame-reader")
         self.pending = OrderedDict()
         self.copy = torch.cuda.Stream()
@@ -339,9 +346,7 @@ class _FrameReader:
 
     def _decode(self, i):
         import torch
-        from PIL import Image
-        with Image.open(self.paths[i]) as im:
-            a = np.asarray(im, dtype=np.uint8)
+        a = self.decode(self.paths[i])
         t = torch.empty(a.shape, dtype=torch.uint8, pin_memory=True)
         t.numpy()[...] = a
         return t
