@@ -19,15 +19,14 @@ import argparse
 import ctypes
 import glob
 import os
-import queue
 import sys
-import threading
 from collections import OrderedDict
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
-from . import _abi, _lib
+from . import _lib
+from ._stage import FrameReader, PinnedSink, check_keys, load_checkpoint, require_device, stream
 
 C_void = ctypes.c_void_p
 
@@ -87,7 +86,6 @@ def check_state_dict(sd, what):
     """midas_v21's weights from a checkpoint's contents: a dict holding an "optimizer" key is unwrapped to its "model"
     entry, as BaseModel.load does.  ValueError naming the key for a DPT or midas_v21_small key, an unexpected or
     missing key, or a wrong shape (what the reference's strict load_state_dict refuses)."""
-    import torch
     if isinstance(sd, dict) and "optimizer" in sd:
         sd = sd.get("model")
     if not isinstance(sd, dict):
@@ -96,28 +94,14 @@ def check_state_dict(sd, what):
     for k in sd:
         if isinstance(k, str) and _other_model(k):
             raise ValueError("%s: key %r is a DPT or midas_v21_small model's; only midas_v21 is built" % (what, k))
-    for k, v in sd.items():
-        if k not in shapes:
-            raise ValueError("%s: unexpected key %r" % (what, k))
-        if not isinstance(v, torch.Tensor) or tuple(v.shape) != shapes[k]:
-            raise ValueError("%s: key %r has shape %s, expected %s" % (what, k, tuple(getattr(v, "shape", ())), shapes[k]))
-    for k in shapes:
-        if k not in sd:
-            raise ValueError("%s: missing key %r" % (what, k))
+    check_keys(sd, shapes, what)
     return {k: sd[k].float() for k in shapes if not k.endswith("num_batches_tracked")}
 
 
 def load_weights(path):
-    """check_state_dict of torch.load(path, weights_only=True) on the host; ValueError naming the file when it does
-    not exist or cannot be read as a checkpoint."""
-    import torch
-    if not os.path.isfile(path):
-        raise ValueError("%s: no such weights file" % path)
-    try:
-        sd = torch.load(path, map_location="cpu", weights_only=True)
-    except Exception as e:
-        raise ValueError("%s: not a readable checkpoint (%s)" % (path, e)) from None
-    return check_state_dict(sd, path)
+    """check_state_dict of load_checkpoint(path): ValueError naming the file when it does not exist or cannot be read
+    as a checkpoint."""
+    return check_state_dict(load_checkpoint(path), path)
 
 
 def network_weights(sd, device, optimize):
@@ -228,11 +212,6 @@ def get_size(width, height):
             _constrain_to_multiple_of(scale_height * height, NET_SIZE))
 
 
-def _stream():
-    import torch
-    return C_void(torch.cuda.current_stream().cuda_stream)
-
-
 def prepare(rgb, net_h, net_w, half):
     """psfm_depth_prepare: uint8 RGB frames [n][h][w][3] on the device -> the network input [n][3][net_h][net_w]
     (channels_last), fp16 when half else float32."""
@@ -242,7 +221,7 @@ def prepare(rgb, net_h, net_w, half):
     out = torch.empty((n, 3, net_h, net_w), dtype=torch.float16 if half else torch.float32, device=rgb.device,
                       memory_format=torch.channels_last)
     _lib.check(_lib.lib().psfm_depth_prepare(C_void(rgb.data_ptr()), n, h, w, net_h, net_w, int(half),
-                                             C_void(out.data_ptr()), _stream()), "psfm_depth_prepare")
+                                             C_void(out.data_ptr()), stream()), "psfm_depth_prepare")
     return out
 
 
@@ -255,7 +234,7 @@ def upsample(pred, h, w):
     flipped = torch.empty((n, h, w), dtype=torch.float32, device=pred.device)
     minmax = torch.empty((n, 2), dtype=torch.float32, device=pred.device)
     _lib.check(_lib.lib().psfm_depth_upsample(C_void(pred.data_ptr()), n, H, W, int(pred.dtype == torch.float16), h, w,
-                                              C_void(flipped.data_ptr()), C_void(minmax.data_ptr()), _stream()),
+                                              C_void(flipped.data_ptr()), C_void(minmax.data_ptr()), stream()),
                "psfm_depth_upsample")
     return flipped, minmax
 
@@ -267,7 +246,7 @@ def quantize(flipped, minmax):
     n, h, w = flipped.shape
     out = torch.empty((n, h, w), dtype=torch.uint16, device=flipped.device)
     _lib.check(_lib.lib().psfm_depth_quantize(C_void(flipped.data_ptr()), n, h, w, C_void(minmax.data_ptr()),
-                                              C_void(out.data_ptr()), _stream()), "psfm_depth_quantize")
+                                              C_void(out.data_ptr()), stream()), "psfm_depth_quantize")
     return out
 
 
@@ -338,21 +317,18 @@ def pfm_bytes(flipped):
 # ----------------------------------------------------------------------------- the step
 
 def _require_device():
-    from . import device_count
-    if device_count() <= 0:
-        raise _lib.PsfmError("midas: no CUDA device (the product has no CPU path)", _abi.PSFM_ERR_NO_DEVICE)
+    require_device("midas")
 
 
 def _run(paths, h, w, sd, optimize, sink):
-    """The depth maps of the frames `paths` (h x w), in batches; sink(ids, flipped, minmax, pixels) gets each batch's
-    frame indices, its flipped float32 maps [b][h][w], their (min, max) [b][2] and the uint16 pixels [b][h][w], all
-    on the device and ordered on torch's current stream.  Returns the seconds of device time spent in the network."""
+    """The depth maps of the frames `paths` (h x w), in batches; sink(ids, flipped, pixels) gets each batch's frame
+    indices, its flipped float32 maps [b][h][w] and the uint16 pixels [b][h][w], both on the device and ordered on
+    torch's current stream.  Returns the seconds of device time spent in the network."""
     import torch
-    from .optical_flow import _FrameReader
     net_w, net_h = get_size(w, h)
     per = frames_per_batch(net_h, net_w, optimize)
     weights = network_weights(sd, "cuda", optimize)
-    reader = _FrameReader(paths, range(len(paths)), decode=decode_rgb)
+    reader = FrameReader(paths, range(len(paths)), decode_rgb)
     events = []
     try:
         with torch.no_grad():
@@ -368,7 +344,7 @@ def _run(paths, h, w, sd, optimize, sink):
                 del x
                 flipped, minmax = upsample(pred, h, w)
                 del pred
-                sink(ids, flipped, minmax, quantize(flipped, minmax))
+                sink(ids, flipped, quantize(flipped, minmax))
     finally:
         reader.close()
     torch.cuda.current_stream().synchronize()
@@ -387,7 +363,7 @@ def compute_depth_maps(image_dir, model_path, optimize=True):
     _require_device()
     maps, pixels = [], []
 
-    def keep(ids, flipped, minmax, px):
+    def keep(ids, flipped, px):
         maps.append(torch.flip(flipped, [1]))
         pixels.append(px)
 
@@ -395,65 +371,31 @@ def compute_depth_maps(image_dir, model_path, optimize=True):
     return paths, torch.cat(maps), torch.cat(pixels)
 
 
-class DepthWriter:
-    """A sink for _run that writes each batch's files on a writer thread while the next batch runs: the flipped maps
-    and the pixels go to pinned host buffers on torch's current stream, and once that copy is done the thread writes
-    the batch's NAME.pfm and NAME.png files on 4 file threads.  bases[i] is frame i's output path without extension.  close() waits for the thread and
-    raises the first failed write (join() only waits); a failed write also makes the next call raise."""
+class DepthWriter(PinnedSink):
+    """A sink for _run that writes each batch's NAME.pfm and NAME.png files on a writer thread while the next batch
+    runs, the batch's frames on 4 file threads; the first failed write is raised by the next call, by close() and on
+    leaving a with block (PinnedSink).  bases[i] is frame i's output path without extension."""
 
     def __init__(self, bases):
         self.bases = bases
-        self.work, self.failure = queue.Queue(maxsize=2), []
         self.pool = ThreadPoolExecutor(max_workers=4, thread_name_prefix="psfm-depth-files")
-        self.thread = threading.Thread(target=self._write, name="psfm-depth-writer", daemon=True)
-        self.thread.start()
+        super().__init__("psfm-depth-writer")
 
-    def _write(self):
+    def write(self, ids, flipped, pixels):
         import cv2
-        while True:
-            item = self.work.get()
-            if item is None:
-                return
-            if self.failure:
-                continue
-            try:
-                ids, flipped, pixels, ev = item
-                ev.synchronize()
 
-                def write(j):
-                    base = self.bases[ids[j]]
-                    with open(base + ".pfm", "wb") as f:
-                        f.write(pfm_bytes(flipped[j].numpy()))
-                    if not cv2.imwrite(base + ".png", pixels[j].numpy()):
-                        raise OSError("%s.png: could not be written" % base)
-                list(self.pool.map(write, range(len(ids))))      # PNG encoding releases the GIL
-            except BaseException as e:
-                self.failure.append(e)
-
-    def __call__(self, ids, flipped, minmax, pixels):
-        import torch
-        if self.failure:
-            raise self.failure[0]
-        hf = torch.empty(flipped.shape, dtype=flipped.dtype, pin_memory=True)
-        hp = torch.empty(pixels.shape, dtype=pixels.dtype, pin_memory=True)
-        hf.copy_(flipped, non_blocking=True)
-        hp.copy_(pixels, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream())
-        self.work.put((ids, hf, hp, ev))
+        def one(j):
+            base = self.bases[ids[j]]
+            with open(base + ".pfm", "wb") as f:
+                f.write(pfm_bytes(flipped[j].numpy()))
+            if not cv2.imwrite(base + ".png", pixels[j].numpy()):
+                raise OSError("%s.png: could not be written" % base)
+        list(self.pool.map(one, range(len(ids))))      # PNG encoding releases the GIL
 
     def join(self):
-        """Ends the thread once the batches sent so far are written (or skipped after a failure)."""
-        if self.thread is not None:
-            self.work.put(None)
-            self.thread.join()
-            self.thread = None
-            self.pool.shutdown(wait=True)
-
-    def close(self):
-        self.join()
-        if self.failure:
-            raise self.failure[0]
+        error = super().join()
+        self.pool.shutdown(wait=True)
+        return error
 
 
 def write_depth_maps(image_dir, output_dir, model_path, skip_exists=False, optimize=True):
@@ -469,12 +411,8 @@ def write_depth_maps(image_dir, output_dir, model_path, skip_exists=False, optim
     if not paths:
         return 0
     _require_device()
-    writer = DepthWriter(bases)
-    try:
+    with DepthWriter(bases) as writer:
         _run(paths, h, w, sd, optimize, writer)
-    finally:
-        writer.join()
-    writer.close()
     return len(paths)
 
 

@@ -20,15 +20,13 @@ import argparse
 import ctypes
 import glob
 import os
-import queue
 import sys
-import threading
 from collections import OrderedDict
-from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
-from . import _abi, _lib
+from . import _lib
+from ._stage import FrameReader, PinnedSink, check_keys, load_checkpoint, require_device, stream
 
 C_void = ctypes.c_void_p
 
@@ -94,7 +92,6 @@ def state_shapes():
 def check_state_dict(sd, what):
     """The basic model's weights from a state dict, DataParallel's `module.` prefix stripped.  ValueError naming the
     key for the small model's keys, an unexpected or missing key, or a wrong shape."""
-    import torch
     if not isinstance(sd, dict):
         raise ValueError("%s: holds a %s, not a state dict" % (what, type(sd).__name__))
     sd = {(k[7:] if k.startswith("module.") else k): v for k, v in sd.items()}
@@ -102,28 +99,14 @@ def check_state_dict(sd, what):
     for k in _SMALL_ONLY:
         if k in sd:
             raise ValueError("%s: key %r is the small RAFT model's; only the basic model (raft-things) is supported" % (what, k))
-    for k, v in sd.items():
-        if k not in shapes:
-            raise ValueError("%s: unexpected key %r" % (what, k))
-        if not isinstance(v, torch.Tensor) or tuple(v.shape) != shapes[k]:
-            raise ValueError("%s: key %r has shape %s, expected %s" % (what, k, tuple(getattr(v, "shape", ())), shapes[k]))
-    for k in shapes:
-        if k not in sd:
-            raise ValueError("%s: missing key %r" % (what, k))
+    check_keys(sd, shapes, what)
     return {k: (sd[k] if k.endswith("num_batches_tracked") else sd[k].float()) for k in shapes}
 
 
 def load_weights(path):
-    """check_state_dict of torch.load(path, weights_only=True) on the host; ValueError naming the file when it does
-    not exist or cannot be read as a checkpoint."""
-    import torch
-    if not os.path.isfile(path):
-        raise ValueError("%s: no such weights file" % path)
-    try:
-        sd = torch.load(path, map_location="cpu", weights_only=True)
-    except Exception as e:
-        raise ValueError("%s: not a readable checkpoint (%s)" % (path, e)) from None
-    return check_state_dict(sd, path)
+    """check_state_dict of load_checkpoint(path): ValueError naming the file when it does not exist or cannot be read
+    as a checkpoint."""
+    return check_state_dict(load_checkpoint(path), path)
 
 
 # ----------------------------------------------------------------------------- the network
@@ -201,11 +184,6 @@ def coords_grid(n, h, w, device):
     return torch.stack([x, y]).float()[None].repeat(n, 1, 1, 1)
 
 
-def _stream():
-    import torch
-    return C_void(torch.cuda.current_stream().cuda_stream)
-
-
 def corr_pyramid_floats(h, w):
     return int(_lib.check(_lib.lib().psfm_corr_pyramid_floats(h, w), "psfm_corr_pyramid_floats"))
 
@@ -216,7 +194,7 @@ def corr_pyramids(fmap1, fmap2, fwd, bwd):
     import torch
     c, h, w = fmap1.shape
     torch.matmul(fmap1.reshape(c, h * w).t(), fmap2.reshape(c, h * w), out=fwd[:h * w * h * w].view(h * w, h * w))
-    _lib.check(_lib.lib().psfm_corr_pyramids(C_void(fwd.data_ptr()), C_void(bwd.data_ptr()), h, w, _stream()),
+    _lib.check(_lib.lib().psfm_corr_pyramids(C_void(fwd.data_ptr()), C_void(bwd.data_ptr()), h, w, stream()),
                "psfm_corr_pyramids")
 
 
@@ -224,7 +202,7 @@ def corr_lookup(pyramids, coords, out):
     """psfm_corr_lookup: pyramids [P][corr_pyramid_floats], coords [P][2][h][w] -> out [P][324][h][w]."""
     P, _, h, w = coords.shape
     _lib.check(_lib.lib().psfm_corr_lookup(C_void(pyramids.data_ptr()), P, h, w, C_void(coords.data_ptr()),
-                                           C_void(out.data_ptr()), _stream()), "psfm_corr_lookup")
+                                           C_void(out.data_ptr()), stream()), "psfm_corr_lookup")
     return out
 
 
@@ -236,7 +214,7 @@ def upsample(flow, mask, pad):
     out = torch.empty((P, 8 * h - pad[2] - pad[3], 8 * w - pad[0] - pad[1], 2), dtype=torch.float32, device=flow.device)
     p = (ctypes.c_int32 * 4)(*pad)
     _lib.check(_lib.lib().psfm_flow_upsample(C_void(flow.data_ptr()), C_void(mask.data_ptr()), P, h, w, p,
-                                             C_void(out.data_ptr()), _stream()), "psfm_flow_upsample")
+                                             C_void(out.data_ptr()), stream()), "psfm_flow_upsample")
     return out
 
 
@@ -246,7 +224,7 @@ def flow_to_image(flows):
     import torch
     M, H, W, _ = flows.shape
     out = torch.empty((M, H, W, 3), dtype=torch.uint8, device=flows.device)
-    _lib.check(_lib.lib().psfm_flow_to_image(C_void(flows.data_ptr()), M, H, W, C_void(out.data_ptr()), _stream()),
+    _lib.check(_lib.lib().psfm_flow_to_image(C_void(flows.data_ptr()), M, H, W, C_void(out.data_ptr()), stream()),
                "psfm_flow_to_image")
     return out
 
@@ -329,53 +307,6 @@ def decode_rgb(path):
         return np.asarray(im, dtype=np.uint8)
 
 
-class _FrameReader:
-    """Decodes the frames a run needs, in order, on host threads into pinned [H][W][3] uint8 tensors, a few ahead of
-    their use; upload(i) copies frame i on the copy stream and returns the device tensor, ordered before torch's
-    current stream.  decode(path) gives a frame as an [H][W][3] uint8 RGB array (decode_rgb by default)."""
-
-    AHEAD = 6
-
-    def __init__(self, paths, order, decode=decode_rgb):
-        import torch
-        self.paths, self.order, self.next, self.decode = paths, list(order), 0, decode
-        self.pool = ThreadPoolExecutor(max_workers=4, thread_name_prefix="psfm-frame-reader")
-        self.pending = OrderedDict()
-        self.copy = torch.cuda.Stream()
-        self._fill()
-
-    def _decode(self, i):
-        import torch
-        a = self.decode(self.paths[i])
-        t = torch.empty(a.shape, dtype=torch.uint8, pin_memory=True)
-        t.numpy()[...] = a
-        return t
-
-    def _fill(self):
-        while self.next < len(self.order) and len(self.pending) < self.AHEAD:
-            i = self.order[self.next]
-            self.pending[i] = self.pool.submit(self._decode, i)
-            self.next += 1
-
-    def upload(self, i):
-        import torch
-        host = self.pending.pop(i).result()
-        self._fill()
-        with torch.cuda.stream(self.copy):
-            dev = host.to("cuda", non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(self.copy)
-        torch.cuda.current_stream().wait_event(ev)
-        dev.record_stream(torch.cuda.current_stream())
-        ev.synchronize()            # the pinned buffer may be freed once the copy has left it
-        return dev
-
-    def close(self):
-        for f in self.pending.values():
-            f.cancel()
-        self.pool.shutdown(wait=True)
-
-
 def _run(paths, h, w, sd, pairs, sink):
     """The flows of `pairs` [(t, stride)] of the frames `paths` (h x w), in batches; sink(batch, flows, images) gets
     each batch's pairs, its maps [2 n][h][w][2] (forward maps first, then backward, in pair order) and the forward
@@ -389,7 +320,7 @@ def _run(paths, h, w, sd, pairs, sink):
     per = pairs_per_batch(h, w)
     needed = sorted({t for t, s in pairs} | {t + s for t, s in pairs})
     sd = {k: v.to(dev) for k, v in sd.items()}
-    reader = _FrameReader(paths, needed)
+    reader = FrameReader(paths, needed, decode_rgb)
     cache = {}          # frame -> (fmap, net, inp)
     try:
         with torch.no_grad():
@@ -430,9 +361,7 @@ def _run(paths, h, w, sd, pairs, sink):
 
 
 def _require_device():
-    from . import device_count
-    if device_count() <= 0:
-        raise _lib.PsfmError("optical flow: no CUDA device (the product has no CPU path)", _abi.PSFM_ERR_NO_DEVICE)
+    require_device("optical flow")
 
 
 def compute_optical_flows(image_dir, model_path, path_consistency=True):
@@ -453,61 +382,23 @@ def compute_optical_flows(image_dir, model_path, path_consistency=True):
     return out[1][0], out[1][1], (out[2][0] if path_consistency else []), (out[2][1] if path_consistency else [])
 
 
-class FlowWriter:
-    """A sink for _run that writes each batch's files on a writer thread while the next batch runs: the maps and
-    images go to pinned host buffers on torch's current stream, and the thread writes them once that copy is done.
-    files(t, stride) -> (forward .flo, backward .flo, flow image) paths.  close() waits for the thread and raises
-    the first failed write (join() only waits); a failed write also makes the next call raise."""
+class FlowWriter(PinnedSink):
+    """A sink for _run that writes each batch's files on a writer thread while the next batch runs; the first failed
+    write is raised by the next call, by close() and on leaving a with block (PinnedSink).  files(t, stride) ->
+    (forward .flo, backward .flo, flow image) paths."""
 
     def __init__(self, files):
         self.files = files
-        self.work, self.failure = queue.Queue(maxsize=2), []
-        self.thread = threading.Thread(target=self._write, name="psfm-flow-writer", daemon=True)
-        self.thread.start()
+        super().__init__("psfm-flow-writer")
 
-    def _write(self):
+    def write(self, batch, flows, images):
         import cv2
-        while True:
-            item = self.work.get()
-            if item is None:
-                return
-            if self.failure:
-                continue
-            try:
-                batch, flows, images, ev = item
-                ev.synchronize()
-                for j, (t, s) in enumerate(batch):
-                    ff, fb, fi = self.files(t, s)
-                    if not cv2.imwrite(fi, images[j].numpy()):
-                        raise OSError("%s: could not be written" % fi)
-                    write_flo(ff, flows[j].numpy())
-                    write_flo(fb, flows[len(batch) + j].numpy())
-            except BaseException as e:
-                self.failure.append(e)
-
-    def __call__(self, batch, flows, images):
-        import torch
-        if self.failure:
-            raise self.failure[0]
-        hf = torch.empty(flows.shape, dtype=flows.dtype, pin_memory=True)
-        hi = torch.empty(images.shape, dtype=images.dtype, pin_memory=True)
-        hf.copy_(flows, non_blocking=True)
-        hi.copy_(images, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record(torch.cuda.current_stream())
-        self.work.put((batch, hf, hi, ev))
-
-    def join(self):
-        """Ends the thread once the batches sent so far are written (or skipped after a failure)."""
-        if self.thread is not None:
-            self.work.put(None)
-            self.thread.join()
-            self.thread = None
-
-    def close(self):
-        self.join()
-        if self.failure:
-            raise self.failure[0]
+        for j, (t, s) in enumerate(batch):
+            ff, fb, fi = self.files(t, s)
+            if not cv2.imwrite(fi, images[j].numpy()):
+                raise OSError("%s: could not be written" % fi)
+            write_flo(ff, flows[j].numpy())
+            write_flo(fb, flows[len(batch) + j].numpy())
 
 
 def flow_files(paths, output_dir):
@@ -545,12 +436,8 @@ def write_optical_flows(image_dir, output_dir, model_path, skip_path_consistency
     if not pairs:
         return 0
     _require_device()
-    writer = FlowWriter(flow_files(paths, output_dir))
-    try:
+    with FlowWriter(flow_files(paths, output_dir)) as writer:
         _run(paths, h, w, sd, pairs, writer)
-    finally:
-        writer.join()
-    writer.close()
     return len(pairs)
 
 

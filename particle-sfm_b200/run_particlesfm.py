@@ -193,24 +193,19 @@ def _fused(report, paths, h, w, source, output_dir, pc, sample_ratio, flow_check
     flow_dir, traj_dir, npy = workspace_paths(output_dir)
     t0 = time.perf_counter()
     trk = tracker._ResidentTracker(h, w, sample_ratio, len(paths), path_consistency=pc)
-    writer = None
     try:
         feed = FrameFeed(len(paths), pc, lambda t, f, b, prev, f2, b2: trk.advance(t, f, b, prev, f2, b2, flow_check_thres))
-        sink = feed
+        pairs = optical_flow._pairs(len(paths), pc)
         if report.plan.write_flows:
             optical_flow.make_flow_dirs(flow_dir, pc)
-            writer = optical_flow.FlowWriter(optical_flow.flow_files(paths, flow_dir))
+            with optical_flow.FlowWriter(optical_flow.flow_files(paths, flow_dir)) as writer:
 
-            def sink(batch, flows, images):
-                writer(batch, flows, images)
-                feed(batch, flows, images)
-        try:
-            source(paths, h, w, optical_flow._pairs(len(paths), pc), sink)
-        finally:
-            if writer is not None:
-                writer.join()
-        if writer is not None:
-            writer.close()
+                def sink(batch, flows, images):
+                    writer(batch, flows, images)
+                    feed(batch, flows, images)
+                source(paths, h, w, pairs, sink)
+        else:
+            source(paths, h, w, pairs, feed)
         feed.done()
         trk.finish(traj_min_len, result=False)         # returns once the set is assembled on the device
         report.add("flows_trajectories", t0)
@@ -233,12 +228,8 @@ def _from_flow_dir(report, paths, h, w, source, output_dir, pc, sample_ratio, fl
     optical_flow.make_flow_dirs(flow_dir, pc)
     missing = optical_flow.missing_pairs(paths, flow_dir, pc)
     if missing:
-        writer = optical_flow.FlowWriter(optical_flow.flow_files(paths, flow_dir))
-        try:
+        with optical_flow.FlowWriter(optical_flow.flow_files(paths, flow_dir)) as writer:
             source(paths, h, w, missing, writer)
-        finally:
-            writer.join()
-        writer.close()
     report.add("flows", t0)
     t0 = time.perf_counter()
     if report.plan.write_track:

@@ -22,16 +22,15 @@ matches_importer.  The mapper reads none of it back.
 """
 import argparse
 import os
-import queue
 import shutil
 import sqlite3
 import sys
-import threading
 import time
 
 import numpy as np
 
 from . import _lib, convert, global_mapper as gm, handoff, init_geometry
+from ._stage import Worker
 
 # ---------------------------------------------------------------------------------------------------------------------
 # What `colmap feature_importer --ImageReader.single_camera 1 --ImageReader.camera_model SIMPLE_PINHOLE` writes, as
@@ -129,42 +128,6 @@ def write_schema(db, images):
     db.commit()
 
 
-class DatabaseWriter:
-    """One thread that owns the SQLite connection and runs the submitted writes in order.  A failed write skips the
-    rest; join() ends the thread and returns that exception (or None).  seconds: the thread's time in writes."""
-
-    def __init__(self, path):
-        self.error, self.seconds = None, 0.0
-        self._q = queue.Queue()
-        self._thread = threading.Thread(target=self._run, args=(path,), name="psfm-sfm-database")
-        self._thread.start()
-
-    def submit(self, fn, *args):
-        self._q.put((fn, args))
-
-    def _run(self, path):
-        db = sqlite3.connect(path)
-        try:
-            while True:
-                item = self._q.get()
-                if item is None:
-                    return
-                if self.error is None:
-                    t0 = time.perf_counter()
-                    try:
-                        item[0](db, *item[1])
-                    except BaseException as e:          # handed to the calling thread by join()
-                        self.error = e
-                    self.seconds += time.perf_counter() - t0
-        finally:
-            db.close()
-
-    def join(self):
-        self._q.put(None)
-        self._thread.join()
-        return self.error
-
-
 def mapper_options(min_num_matches=None):
     """The GlobalMapper flags of main_sfm.py:139-149: principal point and extra parameters not refined, and
     min_num_matches when given."""
@@ -209,8 +172,10 @@ def main_global_sfm(sfm_dir, image_dir, trajectories, single_camera=True, remove
     for p in (db_path, pair_path):
         if os.path.exists(p):
             os.remove(p)
-    writer = DatabaseWriter(db_path)
-    writer.submit(write_schema, images)
+    # one worker thread writes the database beside the device work and is the only user of the connection
+    db = sqlite3.connect(db_path, check_same_thread=False)
+    writer = Worker("psfm-sfm-database")
+    writer.submit(write_schema, db, images)
     table = None
     try:
         if resident:
@@ -223,7 +188,7 @@ def main_global_sfm(sfm_dir, image_dir, trajectories, single_camera=True, remove
         report.add("import", t0, {"images": len(images.names), "ordered_pairs": int(len(table.pairs.pair_images))})
         t0 = time.perf_counter()
         tables = table.tables(images.names, images.camera, (images.width, images.height))
-        writer.submit(handoff.insert_rows, *tables.rows())
+        writer.submit(handoff.insert_rows, db, *tables.rows())
         report.add("table", t0, {"keypoints": table.num_keypoints, "pairs": table.num_pairs,
                                  "matches": table.num_matches})
         t0 = time.perf_counter()
@@ -235,7 +200,7 @@ def main_global_sfm(sfm_dir, image_dir, trajectories, single_camera=True, remove
             g = ver.to_two_view_geometries(tables)
             two_view = ver.two_view_rows(tables.pair_ids)
         table.close()
-        writer.submit(handoff.insert_rows, (), (), two_view)
+        writer.submit(handoff.insert_rows, db, (), (), two_view)
         report.add("verification", t0, {"pairs": int(len(g.pair_ids)), "inlier_matches": int(g.inlier_ptr[-1]),
                                         "skipped": bool(skip_geometric_verification)})
         o = mapper_options(min_num_matches)
@@ -248,6 +213,7 @@ def main_global_sfm(sfm_dir, image_dir, trajectories, single_camera=True, remove
             table.close()
         t0 = time.perf_counter()
         error = writer.join()
+        db.close()
         report.add("database", t0, {"writer_seconds": writer.seconds})
     if error is not None:
         raise error

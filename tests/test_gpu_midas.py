@@ -2,6 +2,8 @@
 (oracle/midas_oracle.py) and the reference's own float32 run (tests/golden/depth_small.npz): the kernels one by one,
 then the whole step in float32 and in fp16, then the written files."""
 import os
+import re
+import threading
 
 import cv2
 import numpy as np
@@ -159,3 +161,24 @@ def test_written_files_equal_the_returned_tensors(gpu, tmp_path, monkeypatch):
         depth = cv2.imread(base + ".png", -1) / 65535.0
         assert depth.max() == 1.0 and np.count_nonzero(depth) > 0.5 * depth.size
     assert midas.main(["--image_dir", d, "--output_dir", out, "--model", w, "--skip_exists"]) == 0
+
+
+@pytest.mark.gpu
+def test_a_failed_write_raises_and_writes_no_later_batch(gpu, tmp_path, monkeypatch):
+    """A directory where one .pfm file goes: the step raises the OSError naming it, writes no later batch and leaves
+    no thread behind, and the command exits 1."""
+    d = _write_frames(str(tmp_path / "img"), mo.seeded_frames(4, 40, 192, seed=0))
+    w = str(tmp_path / "w.pt")
+    torch.save(mo.seeded_state_dict(0), w)
+    monkeypatch.setattr(midas, "_BUDGET", 1)       # a batch per frame
+    out = str(tmp_path / "midas_depth")
+    bad = os.path.join(out, "00001.pfm")
+    os.makedirs(bad)
+    before = set(threading.enumerate())
+    with pytest.raises(OSError, match=re.escape(bad)):
+        midas.write_depth_maps(d, out, w)
+    assert [t.name for t in threading.enumerate() if t not in before] == []
+    assert os.path.isfile(os.path.join(out, "00000.pfm")) and os.path.isfile(os.path.join(out, "00000.png"))
+    assert not any(os.path.exists(os.path.join(out, "%05d.%s" % (i, e))) for i in (2, 3) for e in ("pfm", "png"))
+    assert midas.main(["--image_dir", d, "--output_dir", out, "--model", w]) == 1
+    assert [t.name for t in threading.enumerate() if t not in before] == []

@@ -2,7 +2,9 @@
 reference call structure (oracle/raft_oracle.py) run on the same GPU: the kernels one by one, then the whole stage,
 then the point-trajectory stage fed from the written directory and from the returned tensors."""
 import os
+import re
 import sys
+import threading
 
 import numpy as np
 import pytest
@@ -179,3 +181,27 @@ def test_point_trajectory_from_the_directory_equals_the_tensors(gpu, tmp_path):
     arrays = pt.main_connect_point_trajectories(out, str(tmp_path / "traj"))
     assert arrays.ids.shape[0] > 0
     _same(arrays.to_dict(), dev.to_dict())
+
+
+@pytest.mark.gpu
+def test_a_failed_write_raises_and_writes_no_later_batch(gpu, tmp_path, monkeypatch):
+    """A directory where one .flo file goes: the step raises the OSError naming it, writes no later batch and leaves
+    no thread behind, and the command exits 1."""
+    d = _write_frames(str(tmp_path / "img"), ro.seeded_frames(5, 123, 125, seed=2))
+    weights = str(tmp_path / "w.pth")
+    torch.save(ro.seeded_state_dict(3), weights)
+    monkeypatch.setattr(of, "_BUDGET", 1)          # a batch per pair
+    out = str(tmp_path / "flows")
+    bad = os.path.join(out, "flow_f", "00001.flo")
+    os.makedirs(bad)
+    pairs = of._pairs(5, True)
+    files = of.flow_files(of.frame_list(d)[0], out)
+    before = set(threading.enumerate())
+    with pytest.raises(OSError, match=re.escape(bad)):
+        of.write_optical_flows(d, out, weights)
+    assert [t.name for t in threading.enumerate() if t not in before] == []
+    k = pairs.index((1, 1))
+    assert all(os.path.isfile(f) for p in pairs[:k] for f in files(*p))
+    assert not any(os.path.exists(f) for p in pairs[k + 1:] for f in files(*p))
+    assert of.main(["--image_dir", d, "--output_dir", out, "--model", weights]) == 1
+    assert [t.name for t in threading.enumerate() if t not in before] == []

@@ -61,13 +61,8 @@ def main():
         def step(out):
             bases = [midas.output_base(out, q) for q in paths]
             os.makedirs(out, exist_ok=True)
-            writer = midas.DepthWriter(bases)
-            try:
-                net = midas._run(paths, h, w, midas.load_weights(wpath), optimize, writer)
-            finally:
-                writer.join()
-            writer.close()
-            return net
+            with midas.DepthWriter(bases) as writer:
+                return midas._run(paths, h, w, midas.load_weights(wpath), optimize, writer)
 
         step(os.path.join(tmp, "warm_step"))                    # module load, cuDNN heuristics
         mo.run_directory(weights, d, os.path.join(tmp, "warm_oracle"), optimize)

@@ -88,12 +88,8 @@ def staged_room(img, out, source):
 
     def flows():
         of.make_flow_dirs(flow_dir, True)
-        writer = of.FlowWriter(of.flow_files(paths, flow_dir))
-        try:
+        with of.FlowWriter(of.flow_files(paths, flow_dir)) as writer:
             source(paths, h, w, of._pairs(len(paths), True), writer)
-        finally:
-            writer.join()
-        writer.close()
     clock(s, "flows", flows)
     clock(s, "trajectories", lambda: pt.main_connect_point_trajectories(flow_dir, traj))
     rep = clock(s, "sfm", lambda: sfm.sfm_reconstruction(img, out, traj, assume_static=True))
