@@ -985,6 +985,45 @@ int psfm_depth_upsample(const void* pred, int32_t num_frames, int32_t net_h, int
 int psfm_depth_quantize(const float* flipped, int32_t num_frames, int32_t h, int32_t w, const float* minmax,
                         uint16_t* pixels, void* stream);
 
+/* ---- trajectory labeller (motion segmentation; DESIGN.md §4.17) ----
+   The track set is CSR on the device: trajectory t owns observations ptr[t] .. ptr[t + 1] of frames / xy, its frames
+   strictly ascending.  Windows are win_start[w] .. win_start[w] + L - 1. */
+/* psfm_seg_max_window: the longest window psfm_seg_encode takes (its per-row state must fit in shared memory). */
+int psfm_seg_max_window(void);
+/* psfm_seg_hits: hits [num_windows][num_trajs], the number of window frames each trajectory is seen in. */
+int psfm_seg_hits(const int64_t* ptr, const int32_t* frames, int32_t num_trajs, const int32_t* win_start,
+                  int32_t num_windows, int32_t L, int32_t* hits, void* stream);
+/* psfm_seg_shuffle (host): perm [K], the permutation of 0 .. K-1 that std::shuffle with std::mt19937(5489) makes,
+   the one TrajectorySet::sample_inside_window applies before cutting an over-full window. */
+int psfm_seg_shuffle(int32_t K, int32_t* perm);
+/* psfm_seg_windows: for row r (trajectory rows[r] in window row_window[r]) the float64 locations loc [R][L][2] (0
+   where the trajectory is not seen) and valid [R][L] (1 where it is). */
+int psfm_seg_windows(const int64_t* ptr, const int32_t* frames, const double* xy, const int32_t* rows,
+                     const int32_t* row_window, int32_t num_rows, const int32_t* win_start, int32_t L, double* loc,
+                     uint8_t* valid, void* stream);
+/* psfm_seg_depth_resize: uint16 depth pixels [n][h][w] -> float32 [n][240][424], cv2.resize(INTER_LINEAR) of
+   pixels / 65535.0 in float64, then cast. */
+int psfm_seg_depth_resize(const uint16_t* pixels, int32_t num_frames, int32_t h, int32_t w, float* out, void* stream);
+/* psfm_seg_encode: the encoder features feat [R][16] of the window rows (loc, valid as psfm_seg_windows writes them)
+   over the depth maps [num_frames][240][424], frames raw_h x raw_w; weights: the 15881 floats of
+   motion_seg.pack_encoder. */
+int psfm_seg_encode(const double* loc, const uint8_t* valid, const int32_t* row_window, const int32_t* win_start,
+                    int32_t num_windows, int32_t num_rows, int32_t L, const float* depth, int32_t num_frames,
+                    int32_t raw_h, int32_t raw_w, const float* weights, float* feat, void* stream);
+/* psfm_seg_merge: with row_of [num_windows][num_trajs] (the row of trajectory t in window w, -1 when not sampled) and
+   the rows' labels pred [R]: labels [M] (the label of the first window that sampled the trajectory and holds the
+   frame, -1 for none) and first_row [num_trajs] (the first row that sampled the trajectory, -1 for none). */
+int psfm_seg_merge(const int64_t* ptr, const int32_t* frames, int32_t num_trajs, const int32_t* win_start,
+                   int32_t num_windows, int32_t L, const int32_t* row_of, const uint8_t* pred, int8_t* labels,
+                   int32_t* first_row, void* stream);
+/* psfm_seg_draw: draw_traj_cls's video frames out [L][960][424][3] (BGR) of one window of K rows: the frames
+   [L][240][424][3] (BGR), then the labels, the points and the num_draws trajectories draws[], stamped with the pixel
+   offsets stamps [(na + nb + nc)][2] (dx, dy) of the three circles; order [L][3][240][424] is scratch. */
+int psfm_seg_draw(const uint8_t* frames, const double* loc, const uint8_t* valid, const uint8_t* pred, int32_t K,
+                  int32_t L, int32_t raw_h, int32_t raw_w, const int32_t* draws, int32_t num_draws,
+                  const int16_t* stamps, int32_t na, int32_t nb, int32_t nc, int32_t* order, uint8_t* out,
+                  void* stream);
+
 /* ------------------------------------------------------------------------- */
 /* Multi-GPU (HP2): points sharded across ranks, one all-reduce of the         */
 /* camera-side vector per PCG step (SURVEY.md §8e).                            */

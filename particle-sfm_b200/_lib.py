@@ -39,6 +39,8 @@ EXPORTS = [
     "psfm_colors_create", "psfm_colors_add_images", "psfm_colors_result", "psfm_colors_destroy",
     "psfm_corr_pyramids", "psfm_corr_pyramid_floats", "psfm_corr_lookup", "psfm_flow_upsample", "psfm_flow_to_image",
     "psfm_depth_prepare", "psfm_depth_upsample", "psfm_depth_quantize",
+    "psfm_seg_max_window", "psfm_seg_hits", "psfm_seg_shuffle", "psfm_seg_windows", "psfm_seg_depth_resize",
+    "psfm_seg_encode", "psfm_seg_merge", "psfm_seg_draw",
     "psfm_dist_get_unique_id", "psfm_dist_init", "psfm_dist_world_size",
     "psfm_dist_rank", "psfm_dist_finalize",
 ]
@@ -188,6 +190,14 @@ def lib():
     L.psfm_depth_prepare.argtypes = [vp] + [C.c_int32] * 6 + [vp, vp]
     L.psfm_depth_upsample.argtypes = [vp] + [C.c_int32] * 6 + [vp, vp, vp]
     L.psfm_depth_quantize.argtypes = [vp] + [C.c_int32] * 3 + [vp, vp, vp]
+    L.psfm_seg_max_window.argtypes = []
+    L.psfm_seg_hits.argtypes = [vp, vp, C.c_int32, vp, C.c_int32, C.c_int32, vp, vp]
+    L.psfm_seg_shuffle.argtypes = [C.c_int32, vp]
+    L.psfm_seg_windows.argtypes = [vp, vp, vp, vp, vp, C.c_int32, vp, C.c_int32, vp, vp, vp]
+    L.psfm_seg_depth_resize.argtypes = [vp] + [C.c_int32] * 3 + [vp, vp]
+    L.psfm_seg_encode.argtypes = [vp, vp, vp, vp] + [C.c_int32] * 3 + [vp] + [C.c_int32] * 3 + [vp, vp, vp]
+    L.psfm_seg_merge.argtypes = [vp, vp, C.c_int32, vp, C.c_int32, C.c_int32, vp, vp, vp, vp, vp]
+    L.psfm_seg_draw.argtypes = [vp, vp, vp, vp] + [C.c_int32] * 4 + [vp, C.c_int32, vp] + [C.c_int32] * 3 + [vp, vp, vp]
     L.psfm_dist_get_unique_id.argtypes = [C.POINTER(C.c_uint8)]
     L.psfm_dist_init.argtypes = [C.POINTER(C.c_uint8), C.c_int32, C.c_int32]
     L.psfm_dist_finalize.restype = None

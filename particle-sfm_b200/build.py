@@ -45,6 +45,7 @@ UNITS = [
     ("colors.cu", ["-fmad=false"]),
     ("optical_flow.cu", ["-fmad=false"]),
     ("midas.cu", ["-fmad=false"]),
+    ("motion_seg.cu", []),
     ("dist.cu", []),
     ("ba_solver.cu", []),
     ("traj_solver.cu", ["-fmad=false"]),

@@ -143,6 +143,35 @@ TrajectorySet set_from_dict(const std::map<int, py::dict>& in) {
   return s;
 }
 
+// The track set as the window sampler reads it: trajectories in ascending id order; for each, the first observation of
+// every frame among its first min(times, xys) entries (build_invert_indexes keeps the first), frames ascending.
+py::tuple set_csr(const TrajectorySet& s) {
+  std::vector<int64_t> ids, ptr{0};
+  std::vector<int32_t> frames;
+  std::vector<double> xy;
+  for (const auto& kv : s.trajs) {
+    const Trajectory& t = kv.second;
+    const size_t n = std::min(t.times.size(), t.xys.size());
+    std::map<int, size_t> first;
+    for (size_t i = 0; i < n; ++i) first.emplace(t.times[i], i);
+    for (const auto& f : first) {
+      frames.push_back(f.first);
+      xy.push_back(t.xys[f.second].x);
+      xy.push_back(t.xys[f.second].y);
+    }
+    ids.push_back(kv.first);
+    ptr.push_back((int64_t)frames.size());
+  }
+  py::array_t<int64_t> a_ids((py::ssize_t)ids.size()), a_ptr((py::ssize_t)ptr.size());
+  py::array_t<int32_t> a_frames((py::ssize_t)frames.size());
+  py::array_t<double> a_xy({(py::ssize_t)frames.size(), (py::ssize_t)2});
+  std::copy(ids.begin(), ids.end(), a_ids.mutable_data());
+  std::copy(ptr.begin(), ptr.end(), a_ptr.mutable_data());
+  std::copy(frames.begin(), frames.end(), a_frames.mutable_data());
+  std::copy(xy.begin(), xy.end(), a_xy.mutable_data());
+  return py::make_tuple(a_ids, a_ptr, a_frames, a_xy);
+}
+
 }  // namespace
 
 PYBIND11_MODULE(particlesfm, m) {
@@ -201,5 +230,8 @@ PYBIND11_MODULE(particlesfm, m) {
              out["traj_ids"] = w.traj_ids;
              return out;
            },
-           py::arg("frame_ids"), py::arg("min_length") = 3, py::arg("max_num_tracks") = 100000);
+           py::arg("frame_ids"), py::arg("min_length") = 3, py::arg("max_num_tracks") = 100000)
+      .def("csr", &set_csr,
+           "(ids [T] int64 ascending, ptr [T+1] int64, frame_ids [M] int32, xy [M, 2] float64): every trajectory's "
+           "observations as sample_inside_window sees them, one per frame (its first), frames ascending.");
 }

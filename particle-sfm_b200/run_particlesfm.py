@@ -1,7 +1,9 @@
-"""ParticleSfM's --assume_static pipeline as one command on the GPU, from the frames to the converted poses
-(DESIGN.md §4.15).
+"""ParticleSfM's pipeline as one command on the GPU, from the frames to the converted poses (DESIGN.md §4.15,
+§4.17).
 
-    python -m particlesfm_b200.run_particlesfm --model raft-things.pth --assume_static
+    python -m particlesfm_b200.run_particlesfm --model raft-things.pth
+        (--assume_static | --midas_model midas_v21-f6b98070.pt --motion_seg_model checkpoint.pth
+                           [--window_size 10] [--traj_max_num 100000])
         (-i IMAGES -o OUT | --workspace_dir WS [--image_folder images] | --root_dir ROOT [--image_folder images])
         [--sample_ratio 2] [--traj_min_len 3] [--flow_check_thres 1.0] [--skip_path_consistency] [--skip_sfm]
         [--skip_exists] [--keep_intermediate]
@@ -13,18 +15,25 @@ optical_flow, point_trajectory and sfm, joined in one process so that nothing pa
                           advances as soon as its pairs are computed (FrameFeed), so the device holds one batch's
                           maps plus the few a later frame still needs, whatever the clip length
     track.npy             written from the device (psfm_tracker_track_npy) with --skip_sfm or --keep_intermediate
+    motion segmentation   without --assume_static: the depth maps (midas) are resized to 240 x 424 on the device
+                          as each batch is computed, the finished tracker's track set goes to the labeller
+                          (motion_seg), which writes OUT/motion_seg.mp4, and its labelled arrays go to the SfM step
+                          with the dynamic observations removed
     sfm                   the finished tracker's track set goes into the database match table on the device
                           (psfm_tracker_matches), then verification, the global mapper and the conversion as in sfm
 
 Deliberate differences from the reference:
   * Intermediates are not written unless asked for (OUT/optical_flows with --keep_intermediate, OUT/trajectories/
-    track.npy with --skip_sfm or --keep_intermediate), and nothing is ever deleted: an intermediate an earlier run
-    left stays where it is.
+    track.npy with --skip_sfm or --keep_intermediate, OUT/midas_depth with --keep_intermediate, OUT/
+    trajectories_labeled/track.npy with --skip_sfm or --keep_intermediate), and nothing is ever deleted: an
+    intermediate an earlier run left stays where it is.
   * --traj_min_len reaches the tracker; the reference parses it and never passes it on.  The default, 3, is the
     reference's behaviour.
-  * With --skip_exists an existing OUT/trajectories/track.npy skips the flows as well as the tracking.
+  * With --skip_exists an existing OUT/trajectories/track.npy skips the flows as well as the tracking, and without
+    --assume_static an existing OUT/trajectories_labeled/track.npy goes straight to the SfM step.
   * --root_dir runs the sequences in child processes, one per visible GPU at a time.
-  * Motion segmentation is not built: --assume_static is required.  Only --sfm_type global_theia is built.
+  * The MiDaS and labeller weights are files named on the command line (--midas_model, --motion_seg_model).  Only
+    --sfm_type global_theia is built.
 """
 import argparse
 import os
@@ -34,7 +43,7 @@ import time
 
 import numpy as np
 
-from . import _lib, optical_flow, point_trajectory, sfm, tracker
+from . import _lib, midas, motion_seg, optical_flow, point_trajectory, sfm, tracker
 
 PROG = "run_particlesfm"
 
@@ -43,16 +52,25 @@ PROG = "run_particlesfm"
 
 class Plan:
     """What a run does in OUT.  route: "fused" (frames -> flows -> track set on the device), "flow_dir" (the missing
-    pairs of an existing OUT/optical_flows filled in, then the track set from that directory) or "track_npy" (an
-    existing OUT/trajectories/track.npy, no flow and no tracking).  write_flows / write_track: whether files are
-    written under OUT/optical_flows and to OUT/trajectories/track.npy; sfm: whether the SfM step runs."""
+    pairs of an existing OUT/optical_flows filled in, then the track set from that directory), "track_npy" (an
+    existing OUT/trajectories/track.npy, no flow and no tracking) or "labeled_npy" (an existing OUT/
+    trajectories_labeled/track.npy straight to the SfM step).  write_flows / write_track: whether files are written
+    under OUT/optical_flows and to OUT/trajectories/track.npy; sfm: whether the SfM step runs; motion_seg: whether the
+    depth maps and the labeller run, write_depth / write_labeled: whether they write OUT/midas_depth and OUT/
+    trajectories_labeled/track.npy."""
 
-    def __init__(self, route, write_flows, write_track, sfm):
+    def __init__(self, route, write_flows, write_track, sfm, motion_seg=False, write_depth=False, write_labeled=False):
         self.route, self.write_flows, self.write_track, self.sfm = route, write_flows, write_track, sfm
+        self.motion_seg, self.write_depth, self.write_labeled = motion_seg, write_depth, write_labeled
 
     def stages(self):
-        flows = {"fused": ["flows_trajectories"], "flow_dir": ["flows", "trajectories"], "track_npy": []}[self.route]
-        return flows + (["sfm"] if self.sfm else [])
+        flows = {"fused": ["flows_trajectories"], "flow_dir": ["flows", "trajectories"], "track_npy": [],
+                 "labeled_npy": []}[self.route]
+        return flows + (["depth", "motion_seg"] if self.motion_seg else []) + (["sfm"] if self.sfm else [])
+
+
+def labeled_dir(output_dir):
+    return os.path.join(output_dir, "trajectories_labeled")
 
 
 def workspace_paths(output_dir):
@@ -61,8 +79,11 @@ def workspace_paths(output_dir):
     return os.path.join(output_dir, "optical_flows"), traj, os.path.join(traj, "track.npy")
 
 
-def plan(output_dir, skip_sfm=False, skip_exists=False, keep_intermediate=False):
+def plan(output_dir, skip_sfm=False, skip_exists=False, keep_intermediate=False, motion_segmentation=False):
+    """The Plan of a run; motion_segmentation: the route without --assume_static."""
     flow_dir, _, track = workspace_paths(output_dir)
+    if motion_segmentation and skip_exists and os.path.isfile(os.path.join(labeled_dir(output_dir), "track.npy")):
+        return Plan("labeled_npy", False, False, sfm=not skip_sfm)
     if skip_exists and os.path.isfile(track):
         route = "track_npy"
     elif skip_exists and os.path.isdir(flow_dir):
@@ -70,7 +91,9 @@ def plan(output_dir, skip_sfm=False, skip_exists=False, keep_intermediate=False)
     else:
         route = "fused"
     return Plan(route, write_flows=route == "flow_dir" or (route == "fused" and keep_intermediate),
-                write_track=route != "track_npy" and (skip_sfm or keep_intermediate), sfm=not skip_sfm)
+                write_track=route != "track_npy" and (skip_sfm or keep_intermediate), sfm=not skip_sfm,
+                motion_seg=motion_segmentation, write_depth=motion_segmentation and keep_intermediate,
+                write_labeled=motion_segmentation and (skip_sfm or keep_intermediate))
 
 
 # ----------------------------------------------------------------------------- flows -> tracker, frame by frame
@@ -207,7 +230,8 @@ def _fused(report, paths, h, w, source, output_dir, pc, sample_ratio, flow_check
         else:
             source(paths, h, w, pairs, feed)
         feed.done()
-        trk.finish(traj_min_len, result=False)         # returns once the set is assembled on the device
+        # returns once the set is assembled on the device; the labeller takes host copies of it
+        arrays = trk.finish(traj_min_len, result=report.plan.motion_seg)
         report.add("flows_trajectories", t0)
         if report.plan.write_track:
             t0 = time.perf_counter()
@@ -215,7 +239,7 @@ def _fused(report, paths, h, w, source, output_dir, pc, sample_ratio, flow_check
             with trk.track_npy_body() as body:
                 point_trajectory.write_track_npy(npy, body.view())
             report.add("track_npy", t0)
-        return trk
+        return trk, arrays if report.plan.motion_seg else None
     except BaseException:
         trk.close()
         raise
@@ -240,39 +264,105 @@ def _from_flow_dir(report, paths, h, w, source, output_dir, pc, sample_ratio, fl
     return arrays
 
 
+def check_motion_seg_inputs(image_dir, midas_model, motion_seg_model, window_size, traj_max_num):
+    """The labelling route's inputs, checked before anything is written -> (MiDaS weights, labeller weights).
+    ValueError naming the flag or file: a missing weights flag, weights either loader refuses, frames the depth step
+    refuses, a window size or trajectory cap below 1."""
+    if midas_model is None or motion_seg_model is None:
+        raise ValueError("without --assume_static, motion segmentation needs --midas_model and --motion_seg_model")
+    if window_size < 1 or traj_max_num < 1:
+        raise ValueError("--window_size and --traj_max_num must be at least 1")
+    paths = midas.frame_list(image_dir)[0]
+    motion_seg.check_window_length(len(paths), window_size)
+    return midas.load_weights(midas_model), motion_seg.load_weights(motion_seg_model)
+
+
+def _motion_seg(report, paths, h, w, tracks, output_dir, midas_sd, seg_sd, window_size, traj_max_num):
+    """The depth maps, kept on the device at the labeller's 240 x 424, then the labeller -> its labelled TrackArrays;
+    OUT/motion_seg.mp4 always, OUT/midas_depth and OUT/trajectories_labeled/track.npy as the plan says."""
+    import torch
+    t0 = time.perf_counter()
+    maps = torch.empty((len(paths), motion_seg.H, motion_seg.W), dtype=torch.float32, device="cuda")
+    writer = None
+    if report.plan.write_depth:
+        depth_dir = os.path.join(output_dir, "midas_depth")
+        os.makedirs(depth_dir, exist_ok=True)
+        writer = midas.DepthWriter([midas.output_base(depth_dir, p) for p in paths])
+
+    def sink(ids, flipped, pixels):
+        maps[ids[0]:ids[-1] + 1] = motion_seg.depth_resize(pixels)
+        if writer is not None:
+            writer(ids, flipped, pixels)
+    try:
+        midas._run(paths, h, w, midas_sd, True, sink)
+    finally:
+        if writer is not None:
+            writer.close()
+    report.add("depth", t0)
+    t0 = time.perf_counter()
+    frames = torch.from_numpy(np.stack([motion_seg.resized_frame(p) for p in paths])).cuda()
+    with motion_seg.VideoWriter(os.path.join(output_dir, "motion_seg.mp4")) as video:
+        out = motion_seg.label_trajectories(tracks, maps, (h, w), seg_sd, window_size, traj_max_num, video, frames)
+    if report.plan.write_labeled:
+        os.makedirs(labeled_dir(output_dir), exist_ok=True)
+        np.save(os.path.join(labeled_dir(output_dir), "track.npy"),
+                motion_seg.labelled_dict(out, window_size >= len(paths)))
+    report.add("motion_seg", t0)
+    return out
+
+
 def particlesfm(image_dir, output_dir, model=None, flow_source=None, sample_ratio=2, flow_check_thres=1.0,
                 traj_min_len=3, skip_path_consistency=False, skip_sfm=False, skip_exists=False, keep_intermediate=False,
-                quiet=False):
-    """run_particlesfm.py's particlesfm(args, image_dir, output_dir, ...) with --assume_static and --sfm_type
-    global_theia, for one sequence.  flow_source(paths, h, w, pairs, sink) computes the flows of `pairs` and hands
-    them to sink(batch, flows, images) in batches as optical_flow._run does; None: the RAFT stage with the weights
-    `model`.  Returns a RunReport (its success False when the SfM step wrote no model).  Raises ValueError before
+                quiet=False, assume_static=True, midas_model=None, motion_seg_model=None, window_size=10,
+                traj_max_num=100000):
+    """run_particlesfm.py's particlesfm(args, image_dir, output_dir, ...) with --sfm_type global_theia, for one
+    sequence.  flow_source(paths, h, w, pairs, sink) computes the flows of `pairs` and hands them to sink(batch, flows,
+    images) in batches as optical_flow._run does; None: the RAFT stage with the weights `model`.  assume_static=False:
+    the motion segmentation with the weights files midas_model and motion_seg_model, the SfM step without the dynamic
+    observations.  Returns a RunReport (its success False when the SfM step wrote no model).  Raises ValueError before
     anything is written or the device is touched (check_inputs), PsfmError without a device."""
     say = (lambda *a: None) if quiet else print
-    p = plan(output_dir, skip_sfm, skip_exists, keep_intermediate)
+    p = plan(output_dir, skip_sfm, skip_exists, keep_intermediate, not assume_static)
     report = RunReport(p)
     pc = not skip_path_consistency
     paths, h, w, source = check_inputs(image_dir, model, flow_source, p.sfm)
+    if not assume_static:
+        midas_sd, seg_sd = check_motion_seg_inputs(image_dir, midas_model, motion_seg_model, window_size, traj_max_num)
     if not p.stages():
         return report
     optical_flow._require_device()
     os.makedirs(output_dir, exist_ok=True)
     _, traj_dir, _ = workspace_paths(output_dir)
-    trajectories = traj_dir
-    if p.route != "track_npy":
+    trajectories = labeled_dir(output_dir) if p.route == "labeled_npy" else traj_dir
+    arrays = None
+    if p.route in ("fused", "flow_dir"):
         # the reference's messages (run_particlesfm.py:32-40), "ParticleSFM" in the first as it prints it
         say("[ParticleSFM] Running pairwise optical flow inference......")
         if pc:
             say("[ParticleSfM] Running pairwise optical flow inference (stride 2)......")
         say("[ParticleSfM] Connecting (optimization {0}) point trajectories from optical flows......."
             .format("enabled" if pc else "disabled"))
-        run = _fused if p.route == "fused" else _from_flow_dir
-        trajectories = run(report, paths, h, w, source, output_dir, pc, sample_ratio, flow_check_thres, traj_min_len)
+        if p.route == "fused":
+            trajectories, arrays = _fused(report, paths, h, w, source, output_dir, pc, sample_ratio, flow_check_thres,
+                                          traj_min_len)
+        else:
+            trajectories = arrays = _from_flow_dir(report, paths, h, w, source, output_dir, pc, sample_ratio,
+                                                   flow_check_thres, traj_min_len)
     try:
+        if p.motion_seg:
+            say("[ParticleSfM] Running motion segmentation........")
+            if arrays is None:
+                arrays = motion_seg.read_tracks(traj_dir)
+            labelled = _motion_seg(report, paths, h, w, arrays, output_dir, midas_sd, seg_sd, window_size,
+                                   traj_max_num)
+            if isinstance(trajectories, tracker._ResidentTracker):
+                trajectories.close()
+            trajectories = labelled
         if p.sfm:
             say("[ParticleSfM] Running global structure-from-motion with Theia........")
             t0 = time.perf_counter()
-            report.sfm = sfm.main_global_sfm(os.path.join(output_dir, "sfm"), image_dir, trajectories, remove_dynamic=False,
+            report.sfm = sfm.main_global_sfm(os.path.join(output_dir, "sfm"), image_dir, trajectories,
+                                             remove_dynamic=not assume_static,
                                              convert_path=os.path.join(output_dir, "colmap_outputs_converted"))
             report.add("sfm", t0)
     finally:
@@ -338,6 +428,9 @@ def child_args(args, workspace_dir):
             "--flow_check_thres", repr(args.flow_check_thres), "--sample_ratio", str(args.sample_ratio),
             "--traj_min_len", str(args.traj_min_len), "--window_size", str(args.window_size),
             "--traj_max_num", str(args.traj_max_num), "--sfm_type", args.sfm_type]
+    for flag in ("midas_model", "motion_seg_model"):
+        if getattr(args, flag) is not None:
+            argv += ["--" + flag, getattr(args, flag)]
     for flag in ("skip_path_consistency", "assume_static", "skip_sfm", "skip_exists", "keep_intermediate"):
         if getattr(args, flag):
             argv.append("--" + flag)
@@ -386,7 +479,7 @@ def run_root(args, devices=None, command=None, out=print):
 
 def build_parser():
     p = argparse.ArgumentParser(PROG, description="Dense point trajectory based colmap reconstruction for videos, on "
-                                                  "the GPU (--assume_static)")
+                                                  "the GPU")
     p.add_argument("--model", required=True, help="the RAFT weights file (raft-things.pth), as optical_flow takes it")
     # point trajectory
     p.add_argument("--flow_check_thres", type=float, default=1.0, help="the forward-backward flow consistency check threshold")
@@ -394,14 +487,18 @@ def build_parser():
     p.add_argument("--traj_min_len", type=int, default=3,
                    help="the minimum length for point trajectories; passed to the tracker (the reference parses it "
                         "and never passes it on, so its runs use the default, 3)")
-    # motion segmentation: accepted and unused, as under --assume_static
-    p.add_argument("--window_size", type=int, default=10, help="unused (motion segmentation is not built)")
-    p.add_argument("--traj_max_num", type=int, default=100000, help="unused (motion segmentation is not built)")
+    # motion segmentation
+    p.add_argument("--midas_model", default=None,
+                   help="the MiDaS weights file (midas_v21-f6b98070.pt); required without --assume_static")
+    p.add_argument("--motion_seg_model", default=None,
+                   help="the labeller's checkpoint (traj_oa_depth, model_state_dict); required without --assume_static")
+    p.add_argument("--window_size", type=int, default=10, help="the labeller's sliding window size")
+    p.add_argument("--traj_max_num", type=int, default=100000, help="the labeller's maximum trajectories per window")
     # sfm
     p.add_argument("--sfm_type", default="global_theia", help="sfm type; only global_theia is built")
     # pipeline control
     p.add_argument("--skip_path_consistency", action="store_true", help="whether to skip the path consistency optimization or not")
-    p.add_argument("--assume_static", action="store_true", help="skip the motion segmentation (required)")
+    p.add_argument("--assume_static", action="store_true", help="skip the motion segmentation")
     p.add_argument("--skip_sfm", action="store_true", help="whether to skip structure-from-motion or not")
     p.add_argument("--skip_exists", action="store_true",
                    help="reuse OUT/trajectories/track.npy (no flows, no tracking), else fill in OUT/optical_flows")
@@ -418,9 +515,9 @@ def build_parser():
 
 def refusal(args):
     """The message for flags this command does not run, or None."""
-    if not args.assume_static:
-        return ("--assume_static is required: motion segmentation (MiDaS and the trajectory network) is not built; "
-                "run with --assume_static")
+    if not args.assume_static and (args.midas_model is None or args.motion_seg_model is None):
+        return ("motion segmentation needs the MiDaS and labeller weights: give --midas_model and --motion_seg_model, "
+                "or run with --assume_static")
     if args.sfm_type != "global_theia":
         return "--sfm_type %s is not supported (only global_theia)" % args.sfm_type
     if not (args.image_dir != "none" and args.output_dir != "none") and args.workspace_dir == "none" \
@@ -448,7 +545,9 @@ def main(argv=None):
     try:
         report = particlesfm(image_dir, output_dir, args.model, None, args.sample_ratio, args.flow_check_thres,
                              args.traj_min_len, args.skip_path_consistency, args.skip_sfm, args.skip_exists,
-                             args.keep_intermediate)
+                             args.keep_intermediate, assume_static=args.assume_static, midas_model=args.midas_model,
+                             motion_seg_model=args.motion_seg_model, window_size=args.window_size,
+                             traj_max_num=args.traj_max_num)
     except ValueError as e:
         print("%s: %s" % (PROG, e), file=sys.stderr)
         return 2

@@ -268,10 +268,11 @@ class BatchedTrajectorySet:
 class TrackArrays:
     """The track set in the reference's `full_trajs` order as four arrays: trajectory k has id ids[k] and owns
     observations ptr[k] .. ptr[k + 1] of frame_ids / xy, in time order.
-        ids [T] int64, ptr [T + 1] int64, frame_ids [M] int32, xy [M, 2] float64"""
+        ids [T] int64, ptr [T + 1] int64, frame_ids [M] int32, xy [M, 2] float64
+    labels [M] bool marks the observations the motion segmentation found dynamic; None: all static."""
 
-    def __init__(self, ids, ptr, frame_ids, xy):
-        self.ids, self.ptr, self.frame_ids, self.xy = ids, ptr, frame_ids, xy
+    def __init__(self, ids, ptr, frame_ids, xy, labels=None):
+        self.ids, self.ptr, self.frame_ids, self.xy, self.labels = ids, ptr, frame_ids, xy, labels
 
     def lengths(self):
         return np.diff(self.ptr)
@@ -284,7 +285,8 @@ class TrackArrays:
         out = {}
         for k, i in enumerate(self.ids.tolist()):
             s, e = ptr[k], ptr[k + 1]
-            out[i] = {"frame_ids": frames[s:e], "locations": rows[s:e], "labels": [False] * (e - s)}
+            out[i] = {"frame_ids": frames[s:e], "locations": rows[s:e],
+                      "labels": [False] * (e - s) if self.labels is None else self.labels[s:e].tolist()}
         return out
 
 
