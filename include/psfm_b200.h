@@ -42,7 +42,8 @@ typedef enum {
   PSFM_ERR_NO_DEVICE = -2,      /* no CUDA device: the product has no CPU path */
   PSFM_ERR_CUDA = -3,           /* CUDA runtime error; see psfm_last_error() */
   PSFM_ERR_UNSUPPORTED = -4,    /* e.g. camera model other than SIMPLE_PINHOLE */
-  PSFM_ERR_NCCL = -5
+  PSFM_ERR_NCCL = -5,
+  PSFM_ERR_HOST = -6            /* host exception, e.g. out of host memory; see psfm_last_error() */
 } psfm_status;
 
 /* Human-readable text of the last error on this thread ("" if none). */

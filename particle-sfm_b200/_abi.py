@@ -12,6 +12,7 @@ PSFM_ERR_NO_DEVICE = -2
 PSFM_ERR_CUDA = -3
 PSFM_ERR_UNSUPPORTED = -4
 PSFM_ERR_NCCL = -5
+PSFM_ERR_HOST = -6
 
 LOSS_TRIVIAL, LOSS_SOFT_L1, LOSS_CAUCHY = 0, 1, 2
 SOLVER_AUTO, SOLVER_EXACT_SCHUR, SOLVER_ITERATIVE_SCHUR = 0, 1, 2

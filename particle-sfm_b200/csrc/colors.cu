@@ -141,21 +141,21 @@ extern "C" int psfm_colors_create(int32_t num_images, const int64_t* keypoint_pt
                                   const int32_t* point_of_keypoint, int64_t num_points, psfm_colors** out,
                                   psfm_colors_summary* summary) {
   const char* entry = "psfm_colors_create";
-  if (!out || !keypoint_ptr) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (num_images < 0 || num_points < 0 || num_points > INT_MAX)
-    return fail(entry, PSFM_ERR_INVALID, "num_images must be >= 0 and num_points in [0, 2^31 - 1]");
-  int rc = check_keypoint_ptr(entry, num_images, keypoint_ptr);
-  if (rc != PSFM_OK) return rc;
-  const long long K = keypoint_ptr[num_images];
-  if (K > INT_MAX) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 keypoints");
-  if (K > 0 && (!keypoints || !point_of_keypoint)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  for (long long k = 0; k < K; ++k)
-    if (point_of_keypoint[k] < -1 || point_of_keypoint[k] >= num_points)
-      return fail(entry, PSFM_ERR_INVALID, "keypoint " + std::to_string(k) + " has a point row out of range (point row)");
-  if ((rc = require_device(entry)) != PSFM_OK) return rc;
-  psfm_colors* H = new psfm_colors;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!out || !keypoint_ptr) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (num_images < 0 || num_points < 0 || num_points > INT_MAX)
+      return fail(entry, PSFM_ERR_INVALID, "num_images must be >= 0 and num_points in [0, 2^31 - 1]");
+    int rc = check_keypoint_ptr(entry, num_images, keypoint_ptr);
+    if (rc != PSFM_OK) return rc;
+    const long long K = keypoint_ptr[num_images];
+    if (K > INT_MAX) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 keypoints");
+    if (K > 0 && (!keypoints || !point_of_keypoint)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    for (long long k = 0; k < K; ++k)
+      if (point_of_keypoint[k] < -1 || point_of_keypoint[k] >= num_points)
+        return fail(entry, PSFM_ERR_INVALID, "keypoint " + std::to_string(k) + " has a point row out of range (point row)");
+    if ((rc = require_device(entry)) != PSFM_OK) return rc;
+    std::unique_ptr<psfm_colors> H(new psfm_colors);
     H->F = num_images;
     H->P = num_points;
     H->added.assign(num_images, 0);
@@ -201,33 +201,30 @@ extern "C" int psfm_colors_create(int32_t num_images, const int64_t* keypoint_pt
       summary->num_observations = N;
       summary->setup_ms = H->setup_ms;
     }
-    *out = H;
+    *out = H.release();
     return PSFM_OK;
-  } catch (const CudaFail& f) {
-    delete H;
-    return f.code;
-  }
+  });
 }
 
 extern "C" int psfm_colors_add_images(psfm_colors* H, int32_t first, int32_t count, const int32_t* width,
                                       const int32_t* height, const uint8_t* pixels) {
   const char* entry = "psfm_colors_add_images";
-  if (!H) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (count < 0 || first < 0 || first > H->F || count > H->F - first)
-    return fail(entry, PSFM_ERR_INVALID, "images [first, first + count) out of range (image index)");
-  if (count == 0) return PSFM_OK;
-  if (!width || !height || !pixels) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  std::vector<ImageMeta> meta(count);
-  long long bytes = 0;
-  for (int j = 0; j < count; ++j) {
-    if (H->added[first + j])
-      return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(first + j) + " was already added (image index)");
-    if (width[j] <= 0 || height[j] <= 0)
-      return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(first + j) + " has a zero size (image size)");
-    meta[j] = ImageMeta{bytes, width[j], height[j]};
-    bytes += 3LL * width[j] * height[j];
-  }
-  try {
+  return guard(entry, [&]() -> int {
+    if (!H) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (count < 0 || first < 0 || first > H->F || count > H->F - first)
+      return fail(entry, PSFM_ERR_INVALID, "images [first, first + count) out of range (image index)");
+    if (count == 0) return PSFM_OK;
+    if (!width || !height || !pixels) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    std::vector<ImageMeta> meta(count);
+    long long bytes = 0;
+    for (int j = 0; j < count; ++j) {
+      if (H->added[first + j])
+        return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(first + j) + " was already added (image index)");
+      if (width[j] <= 0 || height[j] <= 0)
+        return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(first + j) + " has a zero size (image size)");
+      meta[j] = ImageMeta{bytes, width[j], height[j]};
+      bytes += 3LL * width[j] * height[j];
+    }
     Slot& s = H->slots[H->num_batches % 2];
     PSFM_CUDA(cudaStreamSynchronize(s.st));            // the slot's previous batch no longer reads its buffers
     count_batch(H, s);
@@ -265,15 +262,13 @@ extern "C" int psfm_colors_add_images(psfm_colors* H, int32_t first, int32_t cou
     ++H->num_batches;
     H->num_images += count;
     return PSFM_OK;
-  } catch (const CudaFail& f) {
-    return f.code;
-  }
+  });
 }
 
 extern "C" int psfm_colors_result(psfm_colors* H, uint8_t* rgb, psfm_colors_summary* summary) {
   const char* entry = "psfm_colors_result";
-  if (!H || (H->P > 0 && !rgb)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  try {
+  return guard(entry, [&]() -> int {
+    if (!H || (H->P > 0 && !rgb)) return fail(entry, PSFM_ERR_INVALID, "null argument");
     for (Slot& s : H->slots) {
       PSFM_CUDA(cudaStreamSynchronize(s.st));
       count_batch(H, s);
@@ -296,9 +291,7 @@ extern "C" int psfm_colors_result(psfm_colors* H, uint8_t* rgb, psfm_colors_summ
       summary->stage_ms = H->stage_ms;
     }
     return PSFM_OK;
-  } catch (const CudaFail& f) {
-    return f.code;
-  }
+  });
 }
 
 extern "C" void psfm_colors_destroy(psfm_colors* H) {

@@ -41,10 +41,12 @@ extern "C" int psfm_device_count(void) {
   return n;
 }
 extern "C" int psfm_set_device(int device) {
-  if (cudaSetDevice(device) != cudaSuccess) {
-    psfm::set_error(std::string("cudaSetDevice: ") + cudaGetErrorString(cudaGetLastError()));
-    return PSFM_ERR_CUDA;
-  }
-  return PSFM_OK;
+  return psfm::guard("psfm_set_device", [&]() -> int {
+    if (cudaSetDevice(device) != cudaSuccess) {
+      psfm::set_error(std::string("cudaSetDevice: ") + cudaGetErrorString(cudaGetLastError()));
+      return PSFM_ERR_CUDA;
+    }
+    return PSFM_OK;
+  });
 }
 extern "C" int64_t psfm_launch_count(void) { return (int64_t)psfm::g_launch_count.load(); }

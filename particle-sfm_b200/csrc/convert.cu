@@ -255,62 +255,62 @@ extern "C" int psfm_convert_create(int32_t num_cameras, const int32_t* camera_si
                                    const double* xyz, const uint8_t* gray_lut, int64_t memory_budget, psfm_convert** out,
                                    int64_t* valid_count, int32_t* batch_ptr, psfm_convert_summary* summary) {
   const char* entry = "psfm_convert_create";
-  if (!out || !camera_size || !image_camera || !keypoint_ptr || !gray_lut || !valid_count || !batch_ptr ||
-      (num_images > 0 && (!qvec || !tvec)))
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (num_cameras < 0 || num_images < 0 || num_points < 0 || memory_budget <= 0)
-    return fail(entry, PSFM_ERR_INVALID, "num_cameras, num_images, num_points must be >= 0 and memory_budget > 0");
-  for (int c = 0; c < num_cameras; ++c)
-    if (camera_size[2 * c] <= 0 || camera_size[2 * c + 1] <= 0 ||
-        (long long)camera_size[2 * c] * camera_size[2 * c + 1] > 0x7fffffffLL)
-      return fail(entry, PSFM_ERR_INVALID, "camera " + std::to_string(c) + " has a bad size (camera size)");
-  int rc = check_keypoint_ptr(entry, num_images, keypoint_ptr);
-  if (rc != PSFM_OK) return rc;
-  for (int i = 0; i < num_images; ++i)
-    if (image_camera[i] < 0 || image_camera[i] >= num_cameras)
-      return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(i) + " has a camera index out of range (camera index)");
-  const long long K = keypoint_ptr[num_images];
-  if (K > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 keypoints");
-  if (K > 0 && (!keypoints || !point_row)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (num_points > 0 && !xyz) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  for (long long k = 0; k < K; ++k)
-    if (point_row[k] < -1 || point_row[k] >= num_points)
-      return fail(entry, PSFM_ERR_INVALID, "keypoint " + std::to_string(k) + " has a point row out of range (point row)");
-  if ((rc = require_device(entry)) != PSFM_OK) return rc;
-  psfm_convert* H = new psfm_convert;
-  H->F = num_images;
-  H->K = K;
-  std::copy(gray_lut, gray_lut + 256, H->lut);
-  H->kptr.assign(keypoint_ptr, keypoint_ptr + num_images + 1);
-  H->valid.assign(num_images, 0);
-  // batches: images in order while both slots' buffers stay inside the budget, at least one image per batch
-  std::vector<int> sz(2 * (size_t)num_images);
-  std::vector<long long> local_off(num_images, 0);
-  std::vector<int> seg_begin(num_images, 0);
-  H->num_px.assign(num_images, 0);
-  for (int i = 0; i < num_images; ++i) {
-    sz[2 * i] = camera_size[2 * image_camera[i]];
-    sz[2 * i + 1] = camera_size[2 * image_camera[i] + 1];
-    H->num_px[i] = (long long)sz[2 * i] * sz[2 * i + 1];
-  }
-  for (int i = 0; i < num_images;) {
-    Batch b{i, 0, H->kptr[i], 0, 0};
-    while (i < num_images) {
-      const long long px = H->num_px[i], kp = H->kptr[i + 1] - H->kptr[i];
-      if (b.count > 0 && (b.count == kMaxBatchImages ||
-                          2 * (kBytesPerPixel * (b.num_px + px) + kBytesPerKeypoint * (b.num_kp + kp)) > memory_budget))
-        break;
-      local_off[i] = b.num_px;
-      seg_begin[i] = (int)b.num_kp;
-      b.num_px += px;
-      b.num_kp += kp;
-      ++b.count;
-      ++i;
+  return guard(entry, [&]() -> int {
+    if (!out || !camera_size || !image_camera || !keypoint_ptr || !gray_lut || !valid_count || !batch_ptr ||
+        (num_images > 0 && (!qvec || !tvec)))
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (num_cameras < 0 || num_images < 0 || num_points < 0 || memory_budget <= 0)
+      return fail(entry, PSFM_ERR_INVALID, "num_cameras, num_images, num_points must be >= 0 and memory_budget > 0");
+    for (int c = 0; c < num_cameras; ++c)
+      if (camera_size[2 * c] <= 0 || camera_size[2 * c + 1] <= 0 ||
+          (long long)camera_size[2 * c] * camera_size[2 * c + 1] > 0x7fffffffLL)
+        return fail(entry, PSFM_ERR_INVALID, "camera " + std::to_string(c) + " has a bad size (camera size)");
+    int rc = check_keypoint_ptr(entry, num_images, keypoint_ptr);
+    if (rc != PSFM_OK) return rc;
+    for (int i = 0; i < num_images; ++i)
+      if (image_camera[i] < 0 || image_camera[i] >= num_cameras)
+        return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(i) + " has a camera index out of range (camera index)");
+    const long long K = keypoint_ptr[num_images];
+    if (K > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 keypoints");
+    if (K > 0 && (!keypoints || !point_row)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (num_points > 0 && !xyz) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    for (long long k = 0; k < K; ++k)
+      if (point_row[k] < -1 || point_row[k] >= num_points)
+        return fail(entry, PSFM_ERR_INVALID, "keypoint " + std::to_string(k) + " has a point row out of range (point row)");
+    if ((rc = require_device(entry)) != PSFM_OK) return rc;
+    std::unique_ptr<psfm_convert> H(new psfm_convert);
+    H->F = num_images;
+    H->K = K;
+    std::copy(gray_lut, gray_lut + 256, H->lut);
+    H->kptr.assign(keypoint_ptr, keypoint_ptr + num_images + 1);
+    H->valid.assign(num_images, 0);
+    // batches: images in order while both slots' buffers stay inside the budget, at least one image per batch
+    std::vector<int> sz(2 * (size_t)num_images);
+    std::vector<long long> local_off(num_images, 0);
+    std::vector<int> seg_begin(num_images, 0);
+    H->num_px.assign(num_images, 0);
+    for (int i = 0; i < num_images; ++i) {
+      sz[2 * i] = camera_size[2 * image_camera[i]];
+      sz[2 * i + 1] = camera_size[2 * image_camera[i] + 1];
+      H->num_px[i] = (long long)sz[2 * i] * sz[2 * i + 1];
     }
-    H->batches.push_back(b);
-  }
-  try {
+    for (int i = 0; i < num_images;) {
+      Batch b{i, 0, H->kptr[i], 0, 0};
+      while (i < num_images) {
+        const long long px = H->num_px[i], kp = H->kptr[i + 1] - H->kptr[i];
+        if (b.count > 0 && (b.count == kMaxBatchImages ||
+                            2 * (kBytesPerPixel * (b.num_px + px) + kBytesPerKeypoint * (b.num_kp + kp)) > memory_budget))
+          break;
+        local_off[i] = b.num_px;
+        seg_begin[i] = (int)b.num_kp;
+        b.num_px += px;
+        b.num_kp += kp;
+        ++b.count;
+        ++i;
+      }
+      H->batches.push_back(b);
+    }
     Event e0, e1, e2, e3;
     Slot s;
     const auto t_alloc = std::chrono::steady_clock::now();
@@ -328,13 +328,13 @@ extern "C" int psfm_convert_create(int32_t num_cameras, const int32_t* camera_si
     PSFM_CUDA(cudaEventRecord(e1.e, 0));
     PSFM_CUDA(cudaDeviceSynchronize());
     const auto t_slot = std::chrono::steady_clock::now();
-    alloc_slot(H, s, false);
+    alloc_slot(H.get(), s, false);
     alloc_ms += host_ms_since(t_slot);
     PSFM_CUDA(cudaEventRecord(e2.e, s.st));
     // the counting pass: the valid pixels of every image, before anything is written
     std::vector<int> cnt;
     for (const Batch& b : H->batches) {
-      run_claims(H, b, s, false);
+      run_claims(H.get(), b, s, false);
       cnt.resize(b.count);
       PSFM_CUDA(cudaMemcpyAsync(cnt.data(), s.count.p, sizeof(int) * (size_t)b.count, cudaMemcpyDeviceToHost, s.st));
       PSFM_CUDA(cudaStreamSynchronize(s.st));
@@ -353,28 +353,25 @@ extern "C" int psfm_convert_create(int32_t num_cameras, const int32_t* camera_si
     std::copy(H->valid.begin(), H->valid.end(), valid_count);
     for (size_t j = 0; j < H->batches.size(); ++j) batch_ptr[j] = H->batches[j].first;
     batch_ptr[H->batches.size()] = num_images;
-    *out = H;
+    *out = H.release();
     return PSFM_OK;
-  } catch (const CudaFail& f) {
-    delete H;
-    return f.code;
-  }
+  });
 }
 
 extern "C" int psfm_convert_result(psfm_convert* H, int32_t first_batch, int32_t num_batches, double* depth,
                                    uint8_t* rgba, psfm_convert_summary* summary) {
   const char* entry = "psfm_convert_result";
-  if (!H) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  const int nb = (int)H->batches.size();
-  if (first_batch < 0 || num_batches < 0 || first_batch > nb || num_batches > nb - first_batch)
-    return fail(entry, PSFM_ERR_INVALID, "batches out of range");
-  if (num_batches > 0 && (!depth || !rgba)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  const int j0 = first_batch, j1 = first_batch + num_batches;
-  for (int j = j0; j < j1; ++j)
-    for (int i = H->batches[j].first; i < H->batches[j].first + H->batches[j].count; ++i)
-      if (H->valid[i] == 0)
-        return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(i) + " has no valid pixel (no percentile)");
-  try {
+  return guard(entry, [&]() -> int {
+    if (!H) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    const int nb = (int)H->batches.size();
+    if (first_batch < 0 || num_batches < 0 || first_batch > nb || num_batches > nb - first_batch)
+      return fail(entry, PSFM_ERR_INVALID, "batches out of range");
+    if (num_batches > 0 && (!depth || !rgba)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    const int j0 = first_batch, j1 = first_batch + num_batches;
+    for (int j = j0; j < j1; ++j)
+      for (int i = H->batches[j].first; i < H->batches[j].first + H->batches[j].count; ++i)
+        if (H->valid[i] == 0)
+          return fail(entry, PSFM_ERR_INVALID, "image " + std::to_string(i) + " has no valid pixel (no percentile)");
     Slot* slots = H->slots;
     const auto t_alloc = std::chrono::steady_clock::now();
     if (!H->slots_ready && nb > 0) {
@@ -434,9 +431,7 @@ extern "C" int psfm_convert_result(psfm_convert* H, int32_t first_batch, int32_t
       summary->host_copy_ms = host_copy_ms;
     }
     return PSFM_OK;
-  } catch (const CudaFail& f) {
-    return f.code;
-  }
+  });
 }
 
 extern "C" void psfm_convert_destroy(psfm_convert* H) {

@@ -222,29 +222,33 @@ void allreduce_max(double* buf, size_t n, cudaStream_t stream) {
 using namespace psfm;
 
 extern "C" int psfm_dist_get_unique_id(uint8_t id[PSFM_NCCL_UNIQUE_ID_BYTES]) {
-  if (!dist::load_nccl()) return PSFM_ERR_NCCL;
-  dist::ncclUniqueId u;
-  if (dist::g.GetUniqueId(&u) != dist::ncclSuccess) { set_error("ncclGetUniqueId failed"); return PSFM_ERR_NCCL; }
-  memcpy(id, u.internal, PSFM_NCCL_UNIQUE_ID_BYTES);
-  return PSFM_OK;
+  return guard("psfm_dist_get_unique_id", [&]() -> int {
+    if (!dist::load_nccl()) return PSFM_ERR_NCCL;
+    dist::ncclUniqueId u;
+    if (dist::g.GetUniqueId(&u) != dist::ncclSuccess) { set_error("ncclGetUniqueId failed"); return PSFM_ERR_NCCL; }
+    memcpy(id, u.internal, PSFM_NCCL_UNIQUE_ID_BYTES);
+    return PSFM_OK;
+  });
 }
 
 extern "C" int psfm_dist_init(const uint8_t id[PSFM_NCCL_UNIQUE_ID_BYTES], int32_t rank, int32_t world_size) {
-  if (world_size < 1 || rank < 0 || rank >= world_size) { set_error("psfm_dist_init: bad rank/world"); return PSFM_ERR_INVALID; }
-  if (dist::g.comm) { set_error("psfm_dist_init: already initialised"); return PSFM_ERR_INVALID; }
-  if (world_size == 1) { dist::g.world = 1; dist::g.rank = 0; return PSFM_OK; }
-  if (!dist::load_nccl()) return PSFM_ERR_NCCL;
-  dist::ncclUniqueId u;
-  memcpy(u.internal, id, PSFM_NCCL_UNIQUE_ID_BYTES);
-  const int rc = dist::g.CommInitRank(&dist::g.comm, world_size, u, rank);
-  if (rc != dist::ncclSuccess) {
-    set_error(std::string("ncclCommInitRank: ") + (dist::g.GetErrorString ? dist::g.GetErrorString(rc) : "error"));
-    dist::g.comm = nullptr;
-    return PSFM_ERR_NCCL;
-  }
-  dist::g.world = world_size;
-  dist::g.rank = rank;
-  return PSFM_OK;
+  return guard("psfm_dist_init", [&]() -> int {
+    if (world_size < 1 || rank < 0 || rank >= world_size) { set_error("psfm_dist_init: bad rank/world"); return PSFM_ERR_INVALID; }
+    if (dist::g.comm) { set_error("psfm_dist_init: already initialised"); return PSFM_ERR_INVALID; }
+    if (world_size == 1) { dist::g.world = 1; dist::g.rank = 0; return PSFM_OK; }
+    if (!dist::load_nccl()) return PSFM_ERR_NCCL;
+    dist::ncclUniqueId u;
+    memcpy(u.internal, id, PSFM_NCCL_UNIQUE_ID_BYTES);
+    const int rc = dist::g.CommInitRank(&dist::g.comm, world_size, u, rank);
+    if (rc != dist::ncclSuccess) {
+      set_error(std::string("ncclCommInitRank: ") + (dist::g.GetErrorString ? dist::g.GetErrorString(rc) : "error"));
+      dist::g.comm = nullptr;
+      return PSFM_ERR_NCCL;
+    }
+    dist::g.world = world_size;
+    dist::g.rank = rank;
+    return PSFM_OK;
+  });
 }
 
 extern "C" int psfm_dist_world_size(void) { return dist::g.world; }

@@ -71,14 +71,14 @@ void launch(const double* in, long long count, double* out) {
 
 extern "C" int psfm_null_vectors(int32_t form, const double* A, int64_t count, double* out) {
   const char* entry = "psfm_null_vectors";
-  if (!A || !out) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (form < PSFM_NV_JACOBI_3 || form > PSFM_NV_JACOBI_9) return fail(entry, PSFM_ERR_INVALID, "unknown form");
-  if (count < 1 || count > (1LL << 24)) return fail(entry, PSFM_ERR_INVALID, "needs 1 <= count <= 2^24");
-  const int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  const int isz[6] = {in_size(0), in_size(1), in_size(2), in_size(3), in_size(4), in_size(5)};
-  const int osz[6] = {out_size(0), out_size(1), out_size(2), out_size(3), out_size(4), out_size(5)};
-  try {
+  return guard(entry, [&]() -> int {
+    if (!A || !out) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (form < PSFM_NV_JACOBI_3 || form > PSFM_NV_JACOBI_9) return fail(entry, PSFM_ERR_INVALID, "unknown form");
+    if (count < 1 || count > (1LL << 24)) return fail(entry, PSFM_ERR_INVALID, "needs 1 <= count <= 2^24");
+    const int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
+    const int isz[6] = {in_size(0), in_size(1), in_size(2), in_size(3), in_size(4), in_size(5)};
+    const int osz[6] = {out_size(0), out_size(1), out_size(2), out_size(3), out_size(4), out_size(5)};
     DBuf<double> d_in, d_out;
     d_in.alloc((size_t)count * isz[form]); d_out.alloc((size_t)count * osz[form]);
     d_in.upload(A, (size_t)count * isz[form], nullptr);
@@ -92,5 +92,5 @@ extern "C" int psfm_null_vectors(int32_t form, const double* A, int64_t count, d
     }
     PSFM_CUDA(cudaMemcpy(out, d_out.p, sizeof(double) * (size_t)count * osz[form], cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }

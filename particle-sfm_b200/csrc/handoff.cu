@@ -209,143 +209,135 @@ namespace psfm {
 int matches_build(const char* entry, TrackSetDev& in, int num_images, int sample_k, cudaStream_t st, psfm_matches** out,
                   int64_t* num_pairs, int64_t* num_matches) {
   const long long N = in.num_obs, num_trajs = in.num_trajs;
-  psfm_matches* H = new psfm_matches;
+  std::unique_ptr<psfm_matches> H(new psfm_matches);
   H->num_images = num_images;
   H->num_obs = N;
   H->kstart.assign((size_t)num_images + 1, 0);
   H->pair_ptr.assign(1, 0);
   if (N == 0) {                                     // empty or all-dynamic track set: nothing to launch
-    *out = H;
+    *out = H.release();
     *num_pairs = *num_matches = 0;
     return PSFM_OK;
   }
-  try {
-    const int n = (int)N, K = sample_k, NI = num_images;
-    DBuf<long long> cnt, off, kstart;
-    DBuf<int> f32a, f32b, ida, idb, kp, bad;
-    f32a.alloc(N); f32b.alloc(N); ida.alloc(N); idb.alloc(N); cnt.alloc(N + 1); bad.alloc(1);
-    bad.zero(st);
-    k_count<<<grid_of(N + 1), 256, 0, st>>>(n, in.tptr, num_trajs, in.frames, NI, K, f32a.p, ida.p, cnt.p, bad.p);
+  const int n = (int)N, K = sample_k, NI = num_images;
+  DBuf<long long> cnt, off, kstart;
+  DBuf<int> f32a, f32b, ida, idb, kp, bad;
+  f32a.alloc(N); f32b.alloc(N); ida.alloc(N); idb.alloc(N); cnt.alloc(N + 1); bad.alloc(1);
+  bad.zero(st);
+  k_count<<<grid_of(N + 1), 256, 0, st>>>(n, in.tptr, num_trajs, in.frames, NI, K, f32a.p, ida.p, cnt.p, bad.p);
+  PSFM_LAUNCH_CHECK();
+  // visiting positions: exclusive int64 scan of the per-sample counts, off[N] = number of records
+  off.alloc(N + 1);
+  {
+    size_t bytes = 0;
+    PSFM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, cnt.p, off.p, n + 1, st));
+    DBuf<unsigned char> tmp;
+    tmp.alloc(bytes, st);
+    PSFM_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, cnt.p, off.p, n + 1, st));
     PSFM_LAUNCH_CHECK();
-    // visiting positions: exclusive int64 scan of the per-sample counts, off[N] = number of records
-    off.alloc(N + 1);
-    {
-      size_t bytes = 0;
-      PSFM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, cnt.p, off.p, n + 1, st));
-      DBuf<unsigned char> tmp;
-      tmp.alloc(bytes, st);
-      PSFM_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, bytes, cnt.p, off.p, n + 1, st));
-      PSFM_LAUNCH_CHECK();
-    }
-    int h_bad = 0;
-    long long M = 0;
-    PSFM_CUDA(cudaMemcpyAsync(&h_bad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    PSFM_CUDA(cudaMemcpyAsync(&M, off.p + N, sizeof(long long), cudaMemcpyDeviceToHost, st));
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    cnt.release();
-    drop(in.own_frames);
-    if (h_bad) {
-      delete H;
-      return fail(entry, PSFM_ERR_INVALID, "a frame id is outside [0, num_images)");
-    }
-    // keypoints: stable sort of the samples by frame
-    cub::DoubleBuffer<int> fk(f32a.p, f32b.p), fv(ida.p, idb.p);
-    // k_records reads the unsorted frames: sort copies of them
-    DBuf<int> frame32;
-    frame32.alloc(N);
-    PSFM_CUDA(cudaMemcpyAsync(frame32.p, f32a.p, sizeof(int) * (size_t)N, cudaMemcpyDeviceToDevice, st));
-    sort_pairs(fk, fv, n, key_bits(NI > 0 ? (u64)(NI - 1) : 0), st);
-    kstart.alloc((size_t)NI + 1);
-    k_kp_start<<<grid_of((long long)NI + 1), 256, 0, st>>>(NI, fk.Current(), n, kstart.p);
-    PSFM_LAUNCH_CHECK();
-    kp.alloc(N);
-    H->kxy.alloc(2 * (size_t)N);
-    k_kp<<<grid_of(N), 256, 0, st>>>(n, fk.Current(), fv.Current(), kstart.p, reinterpret_cast<const double2*>(in.xy), kp.p,
-                                     reinterpret_cast<double2*>(H->kxy.p));
-    PSFM_LAUNCH_CHECK();
-    PSFM_CUDA(cudaMemcpyAsync(H->kstart.data(), kstart.p, sizeof(long long) * ((size_t)NI + 1), cudaMemcpyDeviceToHost, st));
-    PSFM_CUDA(cudaStreamSynchronize(st));
-    f32a.release(); f32b.release(); ida.release(); idb.release(); drop(in.own_xy);
-    H->num_matches = M;
-    if (M > 0) {
-      // match records at their visiting positions, then stable by pair key
-      DBuf<u64> ka, kb, va, vb;
-      ka.alloc(M); kb.alloc(M); va.alloc(M); vb.alloc(M);
-      k_records<<<grid_of(N), 256, 0, st>>>(n, in.tptr, num_trajs, frame32.p, off.p, K, NI, ka.p, va.p);
-      PSFM_LAUNCH_CHECK();
-      PSFM_CUDA(cudaStreamSynchronize(st));
-      off.release(); frame32.release(); drop(in.own_tptr);
-      cub::DoubleBuffer<u64> rk(ka.p, kb.p), rv(va.p, vb.p);
-      sort_pairs(rk, rv, (long long)M, key_bits((u64)NI * (u64)NI - 1), st);
-      PSFM_CUDA(cudaStreamSynchronize(st));
-      release_other(ka, kb, rk.Current());
-      release_other(va, vb, rv.Current());
-      const u64* skey = rk.Current();
-      const u64* sval = rv.Current();
-      // runs of equal keys = image pairs
-      const long long max_runs = std::min<long long>(M, (long long)NI * NI);
-      DBuf<long long> heads;
-      DBuf<unsigned long long> nheads;
-      heads.alloc(max_runs); nheads.alloc(1);
-      nheads.zero(st);
-      k_run_heads<<<grid_stride_of(M), 256, 0, st>>>(M, skey, heads.p, nheads.p);
-      PSFM_LAUNCH_CHECK();
-      unsigned long long R64 = 0;
-      PSFM_CUDA(cudaMemcpyAsync(&R64, nheads.p, sizeof(R64), cudaMemcpyDeviceToHost, st));
-      PSFM_CUDA(cudaStreamSynchronize(st));
-      const int R = (int)R64;
-      DBuf<u64> rkey, rfirst;
-      rkey.alloc(R); rfirst.alloc(R);
-      k_run_info<<<grid_of(R), 256, 0, st>>>(R, heads.p, skey, sval, rkey.p, rfirst.p);
-      PSFM_LAUNCH_CHECK();
-      std::vector<long long> h_heads(R);
-      std::vector<u64> h_key(R), h_first(R);
-      PSFM_CUDA(cudaMemcpyAsync(h_heads.data(), heads.p, sizeof(long long) * R, cudaMemcpyDeviceToHost, st));
-      PSFM_CUDA(cudaMemcpyAsync(h_key.data(), rkey.p, sizeof(u64) * R, cudaMemcpyDeviceToHost, st));
-      PSFM_CUDA(cudaMemcpyAsync(h_first.data(), rfirst.p, sizeof(u64) * R, cudaMemcpyDeviceToHost, st));
-      PSFM_CUDA(cudaStreamSynchronize(st));
-      if (rk.Current() == ka.p) ka.release();
-      else kb.release();
-      // runs in sorted-record order (their heads), and the pair list: by image a, then first appearance
-      std::vector<int> by_head(R), by_pair(R);
-      std::iota(by_head.begin(), by_head.end(), 0);
-      std::sort(by_head.begin(), by_head.end(), [&](int x, int y) { return h_heads[x] < h_heads[y]; });
-      std::vector<long long> run_len(R);
-      for (int r = 0; r < R; ++r)
-        run_len[by_head[r]] = (r + 1 < R ? h_heads[by_head[r + 1]] : M) - h_heads[by_head[r]];
-      std::iota(by_pair.begin(), by_pair.end(), 0);
-      std::sort(by_pair.begin(), by_pair.end(), [&](int x, int y) {
-        const u64 ax = h_key[x] / (u64)NI, ay = h_key[y] / (u64)NI;
-        return ax != ay ? ax < ay : h_first[x] < h_first[y];
-      });
-      H->pair_images.resize(2 * (size_t)R);
-      H->pair_ptr.assign((size_t)R + 1, 0);
-      std::vector<long long> dest(R);
-      for (int k = 0; k < R; ++k) {
-        const int r = by_pair[k];
-        H->pair_images[2 * k] = (long long)(h_key[r] / (u64)NI);
-        H->pair_images[2 * k + 1] = (long long)(h_key[r] % (u64)NI);
-        dest[r] = H->pair_ptr[k];
-        H->pair_ptr[k + 1] = H->pair_ptr[k] + run_len[r];
-      }
-      std::vector<long long> h_start(R), h_dest(R);
-      for (int r = 0; r < R; ++r) { h_start[r] = h_heads[by_head[r]]; h_dest[r] = dest[by_head[r]]; }
-      DBuf<long long> d_start, d_dest;
-      d_start.alloc(R); d_dest.alloc(R);
-      d_start.upload(h_start.data(), R, st); d_dest.upload(h_dest.data(), R, st);
-      H->matches.alloc(2 * (size_t)M);
-      k_scatter<<<grid_stride_of(M), 256, 0, st>>>(M, d_start.p, R, d_dest.p, sval, kp.p, H->matches.p);
-      PSFM_LAUNCH_CHECK();
-      PSFM_CUDA(cudaStreamSynchronize(st));
-    }
-    *num_pairs = (int64_t)(H->pair_ptr.size() - 1);
-    *num_matches = M;
-    *out = H;
-    return PSFM_OK;
-  } catch (const CudaFail& f) {
-    delete H;
-    return f.code;
   }
+  int h_bad = 0;
+  long long M = 0;
+  PSFM_CUDA(cudaMemcpyAsync(&h_bad, bad.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  PSFM_CUDA(cudaMemcpyAsync(&M, off.p + N, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  PSFM_CUDA(cudaStreamSynchronize(st));
+  cnt.release();
+  drop(in.own_frames);
+  if (h_bad) return fail(entry, PSFM_ERR_INVALID, "a frame id is outside [0, num_images)");
+  // keypoints: stable sort of the samples by frame
+  cub::DoubleBuffer<int> fk(f32a.p, f32b.p), fv(ida.p, idb.p);
+  // k_records reads the unsorted frames: sort copies of them
+  DBuf<int> frame32;
+  frame32.alloc(N);
+  PSFM_CUDA(cudaMemcpyAsync(frame32.p, f32a.p, sizeof(int) * (size_t)N, cudaMemcpyDeviceToDevice, st));
+  sort_pairs(fk, fv, n, key_bits(NI > 0 ? (u64)(NI - 1) : 0), st);
+  kstart.alloc((size_t)NI + 1);
+  k_kp_start<<<grid_of((long long)NI + 1), 256, 0, st>>>(NI, fk.Current(), n, kstart.p);
+  PSFM_LAUNCH_CHECK();
+  kp.alloc(N);
+  H->kxy.alloc(2 * (size_t)N);
+  k_kp<<<grid_of(N), 256, 0, st>>>(n, fk.Current(), fv.Current(), kstart.p, reinterpret_cast<const double2*>(in.xy), kp.p,
+                                   reinterpret_cast<double2*>(H->kxy.p));
+  PSFM_LAUNCH_CHECK();
+  PSFM_CUDA(cudaMemcpyAsync(H->kstart.data(), kstart.p, sizeof(long long) * ((size_t)NI + 1), cudaMemcpyDeviceToHost, st));
+  PSFM_CUDA(cudaStreamSynchronize(st));
+  f32a.release(); f32b.release(); ida.release(); idb.release(); drop(in.own_xy);
+  H->num_matches = M;
+  if (M > 0) {
+    // match records at their visiting positions, then stable by pair key
+    DBuf<u64> ka, kb, va, vb;
+    ka.alloc(M); kb.alloc(M); va.alloc(M); vb.alloc(M);
+    k_records<<<grid_of(N), 256, 0, st>>>(n, in.tptr, num_trajs, frame32.p, off.p, K, NI, ka.p, va.p);
+    PSFM_LAUNCH_CHECK();
+    PSFM_CUDA(cudaStreamSynchronize(st));
+    off.release(); frame32.release(); drop(in.own_tptr);
+    cub::DoubleBuffer<u64> rk(ka.p, kb.p), rv(va.p, vb.p);
+    sort_pairs(rk, rv, (long long)M, key_bits((u64)NI * (u64)NI - 1), st);
+    PSFM_CUDA(cudaStreamSynchronize(st));
+    release_other(ka, kb, rk.Current());
+    release_other(va, vb, rv.Current());
+    const u64* skey = rk.Current();
+    const u64* sval = rv.Current();
+    // runs of equal keys = image pairs
+    const long long max_runs = std::min<long long>(M, (long long)NI * NI);
+    DBuf<long long> heads;
+    DBuf<unsigned long long> nheads;
+    heads.alloc(max_runs); nheads.alloc(1);
+    nheads.zero(st);
+    k_run_heads<<<grid_stride_of(M), 256, 0, st>>>(M, skey, heads.p, nheads.p);
+    PSFM_LAUNCH_CHECK();
+    unsigned long long R64 = 0;
+    PSFM_CUDA(cudaMemcpyAsync(&R64, nheads.p, sizeof(R64), cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaStreamSynchronize(st));
+    const int R = (int)R64;
+    DBuf<u64> rkey, rfirst;
+    rkey.alloc(R); rfirst.alloc(R);
+    k_run_info<<<grid_of(R), 256, 0, st>>>(R, heads.p, skey, sval, rkey.p, rfirst.p);
+    PSFM_LAUNCH_CHECK();
+    std::vector<long long> h_heads(R);
+    std::vector<u64> h_key(R), h_first(R);
+    PSFM_CUDA(cudaMemcpyAsync(h_heads.data(), heads.p, sizeof(long long) * R, cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaMemcpyAsync(h_key.data(), rkey.p, sizeof(u64) * R, cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaMemcpyAsync(h_first.data(), rfirst.p, sizeof(u64) * R, cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaStreamSynchronize(st));
+    if (rk.Current() == ka.p) ka.release();
+    else kb.release();
+    // runs in sorted-record order (their heads), and the pair list: by image a, then first appearance
+    std::vector<int> by_head(R), by_pair(R);
+    std::iota(by_head.begin(), by_head.end(), 0);
+    std::sort(by_head.begin(), by_head.end(), [&](int x, int y) { return h_heads[x] < h_heads[y]; });
+    std::vector<long long> run_len(R);
+    for (int r = 0; r < R; ++r)
+      run_len[by_head[r]] = (r + 1 < R ? h_heads[by_head[r + 1]] : M) - h_heads[by_head[r]];
+    std::iota(by_pair.begin(), by_pair.end(), 0);
+    std::sort(by_pair.begin(), by_pair.end(), [&](int x, int y) {
+      const u64 ax = h_key[x] / (u64)NI, ay = h_key[y] / (u64)NI;
+      return ax != ay ? ax < ay : h_first[x] < h_first[y];
+    });
+    H->pair_images.resize(2 * (size_t)R);
+    H->pair_ptr.assign((size_t)R + 1, 0);
+    std::vector<long long> dest(R);
+    for (int k = 0; k < R; ++k) {
+      const int r = by_pair[k];
+      H->pair_images[2 * k] = (long long)(h_key[r] / (u64)NI);
+      H->pair_images[2 * k + 1] = (long long)(h_key[r] % (u64)NI);
+      dest[r] = H->pair_ptr[k];
+      H->pair_ptr[k + 1] = H->pair_ptr[k] + run_len[r];
+    }
+    std::vector<long long> h_start(R), h_dest(R);
+    for (int r = 0; r < R; ++r) { h_start[r] = h_heads[by_head[r]]; h_dest[r] = dest[by_head[r]]; }
+    DBuf<long long> d_start, d_dest;
+    d_start.alloc(R); d_dest.alloc(R);
+    d_start.upload(h_start.data(), R, st); d_dest.upload(h_dest.data(), R, st);
+    H->matches.alloc(2 * (size_t)M);
+    k_scatter<<<grid_stride_of(M), 256, 0, st>>>(M, d_start.p, R, d_dest.p, sval, kp.p, H->matches.p);
+    PSFM_LAUNCH_CHECK();
+    PSFM_CUDA(cudaStreamSynchronize(st));
+  }
+  *num_pairs = (int64_t)(H->pair_ptr.size() - 1);
+  *num_matches = M;
+  *out = H.release();
+  return PSFM_OK;
 }
 
 }  // namespace psfm
@@ -354,19 +346,19 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
                                    int32_t num_images, int32_t sample_k, psfm_matches** out, int64_t* num_pairs,
                                    int64_t* num_matches) {
   const char* entry = "psfm_matches_create";
-  if (!out || !num_pairs || !num_matches || !traj_ptr) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (num_trajs < 0 || num_images < 0 || sample_k < 1)
-    return fail(entry, PSFM_ERR_INVALID, "num_trajs and num_images must be >= 0, sample_k >= 1");
-  if (traj_ptr[0] != 0) return fail(entry, PSFM_ERR_INVALID, "traj_ptr[0] must be 0");
-  for (int64_t t = 0; t < num_trajs; ++t)
-    if (traj_ptr[t + 1] < traj_ptr[t]) return fail(entry, PSFM_ERR_INVALID, "traj_ptr must be non-decreasing");
-  const long long N = traj_ptr[num_trajs];
-  if (N > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 samples");
-  if (N > 0 && (!frame_ids || !xy)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!out || !num_pairs || !num_matches || !traj_ptr) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (num_trajs < 0 || num_images < 0 || sample_k < 1)
+      return fail(entry, PSFM_ERR_INVALID, "num_trajs and num_images must be >= 0, sample_k >= 1");
+    if (traj_ptr[0] != 0) return fail(entry, PSFM_ERR_INVALID, "traj_ptr[0] must be 0");
+    for (int64_t t = 0; t < num_trajs; ++t)
+      if (traj_ptr[t + 1] < traj_ptr[t]) return fail(entry, PSFM_ERR_INVALID, "traj_ptr must be non-decreasing");
+    const long long N = traj_ptr[num_trajs];
+    if (N > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 samples");
+    if (N > 0 && (!frame_ids || !xy)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     DBuf<long long> tptr, frames;
     DBuf<double> dxy;
     TrackSetDev in;
@@ -380,18 +372,18 @@ extern "C" int psfm_matches_create(const int64_t* traj_ptr, int64_t num_trajs, c
       in.own_tptr = &tptr; in.own_frames = &frames; in.own_xy = &dxy;
     }
     return matches_build(entry, in, num_images, sample_k, nullptr, out, num_pairs, num_matches);
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_matches_result(const psfm_matches* H, int64_t* keypoint_ptr, double* keypoints, int64_t* pair_images,
                                    int64_t* pair_ptr, int64_t* matches) {
-  if (H && H->moved && (keypoints || matches))
-    return fail("psfm_matches_result", PSFM_ERR_INVALID,
-                "the keypoints and matches were moved into a match table; pass NULL for them");
-  if (!H || !keypoint_ptr || !pair_ptr || (H->num_obs && !H->moved && !keypoints) ||
-      (H->num_matches && (!pair_images || (!H->moved && !matches))))
-    return fail("psfm_matches_result", PSFM_ERR_INVALID, "null argument");
-  try {
+  return guard("psfm_matches_result", [&]() -> int {
+    if (H && H->moved && (keypoints || matches))
+      return fail("psfm_matches_result", PSFM_ERR_INVALID,
+                  "the keypoints and matches were moved into a match table; pass NULL for them");
+    if (!H || !keypoint_ptr || !pair_ptr || (H->num_obs && !H->moved && !keypoints) ||
+        (H->num_matches && (!pair_images || (!H->moved && !matches))))
+      return fail("psfm_matches_result", PSFM_ERR_INVALID, "null argument");
     std::copy(H->kstart.begin(), H->kstart.end(), keypoint_ptr);
     std::copy(H->pair_ptr.begin(), H->pair_ptr.end(), pair_ptr);
     std::copy(H->pair_images.begin(), H->pair_images.end(), pair_images);
@@ -401,7 +393,7 @@ extern "C" int psfm_matches_result(const psfm_matches* H, int64_t* keypoint_ptr,
     if (H->num_matches)
       PSFM_CUDA(cudaMemcpy(matches, H->matches.p, sizeof(long long) * 2 * (size_t)H->num_matches, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" void psfm_matches_destroy(psfm_matches* H) {
@@ -412,27 +404,27 @@ extern "C" void psfm_matches_destroy(psfm_matches* H) {
 extern "C" int psfm_matches_table(psfm_matches* H, const int32_t* image_ids, psfm_match_table** out, int64_t* num_keypoints,
                                   int64_t* num_pairs, int64_t* num_matches) {
   const char* entry = "psfm_matches_table";
-  if (!H || !out || !num_keypoints || !num_pairs || !num_matches) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  *out = nullptr;
-  if (H->moved) return fail(entry, PSFM_ERR_INVALID, "the handle's matches were already moved into a match table");
-  const int NI = H->num_images;
-  if (NI > 0 && !image_ids) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  for (int f = 0; f < NI; ++f)
-    if (image_ids[f] < 0 || image_ids[f] == 0x7fffffff)
-      return fail(entry, PSFM_ERR_INVALID, "an image id is outside [0, 2^31 - 1)");
-  std::vector<int> row_frame(NI);                   // frame of every row in image_id order
-  std::iota(row_frame.begin(), row_frame.end(), 0);
-  std::sort(row_frame.begin(), row_frame.end(), [&](int x, int y) { return image_ids[x] < image_ids[y]; });
-  for (int r = 1; r < NI; ++r)
-    if (image_ids[row_frame[r]] == image_ids[row_frame[r - 1]]) return fail(entry, PSFM_ERR_INVALID, "an image id is given twice");
-  const long long Rh = (long long)H->pair_ptr.size() - 1;
-  for (long long k = 0; k < Rh; ++k)
-    if (H->pair_images[2 * k] == H->pair_images[2 * k + 1])
-      return fail(entry, PSFM_ERR_INVALID, "a trajectory visits one frame twice (a pair of an image with itself)");
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  psfm_match_table* T = new psfm_match_table;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!H || !out || !num_keypoints || !num_pairs || !num_matches) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    *out = nullptr;
+    if (H->moved) return fail(entry, PSFM_ERR_INVALID, "the handle's matches were already moved into a match table");
+    const int NI = H->num_images;
+    if (NI > 0 && !image_ids) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    for (int f = 0; f < NI; ++f)
+      if (image_ids[f] < 0 || image_ids[f] == 0x7fffffff)
+        return fail(entry, PSFM_ERR_INVALID, "an image id is outside [0, 2^31 - 1)");
+    std::vector<int> row_frame(NI);                   // frame of every row in image_id order
+    std::iota(row_frame.begin(), row_frame.end(), 0);
+    std::sort(row_frame.begin(), row_frame.end(), [&](int x, int y) { return image_ids[x] < image_ids[y]; });
+    for (int r = 1; r < NI; ++r)
+      if (image_ids[row_frame[r]] == image_ids[row_frame[r - 1]]) return fail(entry, PSFM_ERR_INVALID, "an image id is given twice");
+    const long long Rh = (long long)H->pair_ptr.size() - 1;
+    for (long long k = 0; k < Rh; ++k)
+      if (H->pair_images[2 * k] == H->pair_images[2 * k + 1])
+        return fail(entry, PSFM_ERR_INVALID, "a trajectory visits one frame twice (a pair of an image with itself)");
+    int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
+    std::unique_ptr<psfm_match_table> T(new psfm_match_table);
     T->num_images = NI;
     std::vector<int> row_of(NI);
     for (int r = 0; r < NI; ++r) row_of[row_frame[r]] = r;
@@ -511,20 +503,17 @@ extern "C" int psfm_matches_table(psfm_matches* H, const int32_t* image_ids, psf
     *num_keypoints = N;
     *num_pairs = R;
     *num_matches = M;
-    *out = T;
+    *out = T.release();
     return PSFM_OK;
-  } catch (const CudaFail& f) {
-    delete T;
-    return f.code;
-  }
+  });
 }
 
 extern "C" int psfm_match_table_result(const psfm_match_table* T, int64_t* keypoint_ptr, float* keypoints, int32_t* pair_images,
                                        int64_t* match_ptr, uint32_t* matches) {
-  if (!T || !keypoint_ptr || !match_ptr || (T->num_keypoints && !keypoints) || (T->num_pairs && !pair_images) ||
-      (T->num_matches && !matches))
-    return fail("psfm_match_table_result", PSFM_ERR_INVALID, "null argument");
-  try {
+  return guard("psfm_match_table_result", [&]() -> int {
+    if (!T || !keypoint_ptr || !match_ptr || (T->num_keypoints && !keypoints) || (T->num_pairs && !pair_images) ||
+        (T->num_matches && !matches))
+      return fail("psfm_match_table_result", PSFM_ERR_INVALID, "null argument");
     std::copy(T->keypoint_ptr.begin(), T->keypoint_ptr.end(), keypoint_ptr);
     std::copy(T->match_ptr.begin(), T->match_ptr.end(), match_ptr);
     std::copy(T->pair_images.begin(), T->pair_images.end(), pair_images);
@@ -533,7 +522,7 @@ extern "C" int psfm_match_table_result(const psfm_match_table* T, int64_t* keypo
     if (T->num_matches)
       PSFM_CUDA(cudaMemcpy(matches, T->matches.p, sizeof(uint2) * (size_t)T->num_matches, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" void psfm_match_table_destroy(psfm_match_table* T) {

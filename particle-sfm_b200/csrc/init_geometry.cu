@@ -220,15 +220,15 @@ __global__ void __launch_bounds__(128) k_triangulate_tracks(const double* __rest
 extern "C" int psfm_known_rotation_translations(const double* points1, const double* points2, const int32_t* pair_ptr,
                                                 const double* qvec1, const double* qvec2, int32_t num_pairs, double* tvec,
                                                 int32_t* iterations) {
-  if (num_pairs < 0 || (num_pairs > 0 && (!pair_ptr || !qvec1 || !qvec2 || !tvec))) return PSFM_ERR_INVALID;
-  int rc = require_device("psfm_known_rotation_translations");
-  if (rc != PSFM_OK) return rc;
-  if (num_pairs == 0) return PSFM_OK;
-  const size_t m = (size_t)pair_ptr[num_pairs];
-  if (pair_ptr[0] != 0 || (m > 0 && (!points1 || !points2))) return PSFM_ERR_INVALID;
-  for (int i = 0; i < num_pairs; ++i)
-    if (pair_ptr[i + 1] < pair_ptr[i]) return PSFM_ERR_INVALID;
-  try {
+  return guard("psfm_known_rotation_translations", [&]() -> int {
+    if (num_pairs < 0 || (num_pairs > 0 && (!pair_ptr || !qvec1 || !qvec2 || !tvec))) return PSFM_ERR_INVALID;
+    int rc = require_device("psfm_known_rotation_translations");
+    if (rc != PSFM_OK) return rc;
+    if (num_pairs == 0) return PSFM_OK;
+    const size_t m = (size_t)pair_ptr[num_pairs];
+    if (pair_ptr[0] != 0 || (m > 0 && (!points1 || !points2))) return PSFM_ERR_INVALID;
+    for (int i = 0; i < num_pairs; ++i)
+      if (pair_ptr[i + 1] < pair_ptr[i]) return PSFM_ERR_INVALID;
     DBuf<double> d1, d2, dq1, dq2, dt;
     DBuf<int> dp, di;
     d1.alloc(2 * m); d2.alloc(2 * m); dq1.alloc(4 * (size_t)num_pairs); dq2.alloc(4 * (size_t)num_pairs);
@@ -241,20 +241,20 @@ extern "C" int psfm_known_rotation_translations(const double* points1, const dou
     PSFM_CUDA(cudaMemcpy(tvec, dt.p, sizeof(double) * dt.n, cudaMemcpyDeviceToHost));
     if (iterations) PSFM_CUDA(cudaMemcpy(iterations, di.p, sizeof(int) * di.n, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_triangulate_tracks(const double* proj_matrices, const double* points, const int32_t* track_ptr,
                                        int32_t num_tracks, double* xyz) {
-  if (num_tracks < 0 || (num_tracks > 0 && (!track_ptr || !xyz))) return PSFM_ERR_INVALID;
-  int rc = require_device("psfm_triangulate_tracks");
-  if (rc != PSFM_OK) return rc;
-  if (num_tracks == 0) return PSFM_OK;
-  const size_t m = (size_t)track_ptr[num_tracks];
-  if (track_ptr[0] != 0 || (m > 0 && (!proj_matrices || !points))) return PSFM_ERR_INVALID;
-  for (int i = 0; i < num_tracks; ++i)
-    if (track_ptr[i + 1] < track_ptr[i]) return PSFM_ERR_INVALID;
-  try {
+  return guard("psfm_triangulate_tracks", [&]() -> int {
+    if (num_tracks < 0 || (num_tracks > 0 && (!track_ptr || !xyz))) return PSFM_ERR_INVALID;
+    int rc = require_device("psfm_triangulate_tracks");
+    if (rc != PSFM_OK) return rc;
+    if (num_tracks == 0) return PSFM_OK;
+    const size_t m = (size_t)track_ptr[num_tracks];
+    if (track_ptr[0] != 0 || (m > 0 && (!proj_matrices || !points))) return PSFM_ERR_INVALID;
+    for (int i = 0; i < num_tracks; ++i)
+      if (track_ptr[i + 1] < track_ptr[i]) return PSFM_ERR_INVALID;
     DBuf<double> dP, dx, dX;
     DBuf<int> dp;
     dP.alloc(12 * m); dx.alloc(2 * m); dX.alloc(3 * (size_t)num_tracks); dp.alloc((size_t)num_tracks + 1);
@@ -263,7 +263,7 @@ extern "C" int psfm_triangulate_tracks(const double* proj_matrices, const double
     PSFM_LAUNCH_CHECK();
     PSFM_CUDA(cudaMemcpy(xyz, dX.p, sizeof(double) * dX.n, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_optimize_pairwise_translations(int32_t num_images, const int64_t* keypoint_ptr, const float* keypoints,
@@ -272,42 +272,42 @@ extern "C" int psfm_optimize_pairwise_translations(int32_t num_images, const int
                                                    const uint32_t* inlier_matches, const double* orientations,
                                                    const uint8_t* pair_used, double* tvec, int32_t* iterations) {
   const char* entry = "psfm_optimize_pairwise_translations";
-  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
-  if (rc != PSFM_OK) return rc;
-  if (num_pairs > 0 && (!keypoint_ptr || !image_camera || !cameras || !pair_images || !inlier_ptr || !orientations ||
-                        !tvec || !iterations))
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  const int R = (int)num_pairs;
-  if (R > 0) {
-    // no check_distinct_pairs: this stage accepts self pairs and repeated pairs
-    if ((rc = check_keypoint_ptr(entry, num_images, keypoint_ptr)) != PSFM_OK) return rc;
-    if ((rc = check_image_cameras(entry, num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
-    if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
-    if ((rc = check_pair_images(entry, R, pair_images, num_images)) != PSFM_OK) return rc;
-    for (int p = 0; p < R; ++p) {
-      if (pair_used && !pair_used[p]) continue;
-      for (int k = 0; k < 2; ++k) {
-        const double* q = orientations + 4 * (size_t)pair_images[2 * p + k];
-        const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-        if (!(std::isfinite(n2) && n2 > 0.0))
-          return fail(entry, PSFM_ERR_INVALID, "a used pair's image has a zero or non-finite orientation");
-      }
-    }
-    if (inlier_ptr[R] > 0 && (!inlier_matches || (keypoint_ptr[num_images] > 0 && !keypoints)))
+  return guard(entry, [&]() -> int {
+    int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+    if (rc != PSFM_OK) return rc;
+    if (num_pairs > 0 && (!keypoint_ptr || !image_camera || !cameras || !pair_images || !inlier_ptr || !orientations ||
+                          !tvec || !iterations))
       return fail(entry, PSFM_ERR_INVALID, "null argument");
-    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
-  }
-  if ((rc = require_device(entry)) != PSFM_OK) return rc;
-  if (R == 0) return PSFM_OK;
-  const long long N = inlier_ptr[R], K = keypoint_ptr[num_images];
-  // the kernel reads one quaternion pair per pair: gathered here from the image orientations
-  std::vector<double> q1(4 * (size_t)R), q2(4 * (size_t)R);
-  for (int p = 0; p < R; ++p)
-    for (int k = 0; k < 4; ++k) {
-      q1[4 * (size_t)p + k] = orientations[4 * (size_t)pair_images[2 * p] + k];
-      q2[4 * (size_t)p + k] = orientations[4 * (size_t)pair_images[2 * p + 1] + k];
+    const int R = (int)num_pairs;
+    if (R > 0) {
+      // no check_distinct_pairs: this stage accepts self pairs and repeated pairs
+      if ((rc = check_keypoint_ptr(entry, num_images, keypoint_ptr)) != PSFM_OK) return rc;
+      if ((rc = check_image_cameras(entry, num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
+      if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
+      if ((rc = check_pair_images(entry, R, pair_images, num_images)) != PSFM_OK) return rc;
+      for (int p = 0; p < R; ++p) {
+        if (pair_used && !pair_used[p]) continue;
+        for (int k = 0; k < 2; ++k) {
+          const double* q = orientations + 4 * (size_t)pair_images[2 * p + k];
+          const double n2 = q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+          if (!(std::isfinite(n2) && n2 > 0.0))
+            return fail(entry, PSFM_ERR_INVALID, "a used pair's image has a zero or non-finite orientation");
+        }
+      }
+      if (inlier_ptr[R] > 0 && (!inlier_matches || (keypoint_ptr[num_images] > 0 && !keypoints)))
+        return fail(entry, PSFM_ERR_INVALID, "null argument");
+      if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
     }
-  try {
+    if ((rc = require_device(entry)) != PSFM_OK) return rc;
+    if (R == 0) return PSFM_OK;
+    const long long N = inlier_ptr[R], K = keypoint_ptr[num_images];
+    // the kernel reads one quaternion pair per pair: gathered here from the image orientations
+    std::vector<double> q1(4 * (size_t)R), q2(4 * (size_t)R);
+    for (int p = 0; p < R; ++p)
+      for (int k = 0; k < 4; ++k) {
+        q1[4 * (size_t)p + k] = orientations[4 * (size_t)pair_images[2 * p] + k];
+        q2[4 * (size_t)p + k] = orientations[4 * (size_t)pair_images[2 * p + 1] + k];
+      }
     DBuf<double> d_q1, d_q2, d_t, d_cams;
     DBuf<int> d_it, d_pairs, d_cam;
     DBuf<long long> d_iptr, d_kp_ptr;
@@ -331,5 +331,5 @@ extern "C" int psfm_optimize_pairwise_translations(int32_t num_images, const int
     PSFM_CUDA(cudaMemcpy(tvec, d_t.p, sizeof(double) * 3 * (size_t)R, cudaMemcpyDeviceToHost));
     PSFM_CUDA(cudaMemcpy(iterations, d_it.p, sizeof(int) * (size_t)R, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }

@@ -41,10 +41,10 @@ __global__ void k_fp64_latency(long long* cycles, double* sink, int n, double se
 // dfma_per_second: fused multiply-adds per second, whole device (x2 = FLOP/s);
 // dependent_latency_cycles: SM cycles from one DFMA to the next dependent one.
 extern "C" int psfm_measure_dfma(double* dfma_per_second, double* dependent_latency_cycles) {
-  using namespace psfm;
-  const int rc = require_device("psfm_measure_dfma");
-  if (rc != PSFM_OK) return rc;
-  try {
+  return psfm::guard("psfm_measure_dfma", [&]() -> int {
+    using namespace psfm;
+    const int rc = require_device("psfm_measure_dfma");
+    if (rc != PSFM_OK) return rc;
     int dev = 0, sms = 0;
     PSFM_CUDA(cudaGetDevice(&dev));
     PSFM_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -76,7 +76,5 @@ extern "C" int psfm_measure_dfma(double* dfma_per_second, double* dependent_late
     if (dfma_per_second) *dfma_per_second = best;
     if (dependent_latency_cycles) *dependent_latency_cycles = (double)h / (16.0 * nl);
     return PSFM_OK;
-  } catch (const CudaFail& f) {
-    return f.code;
-  }
+  });
 }

@@ -203,15 +203,15 @@ int check_sizes(const char* entry, int32_t n, int32_t h, int32_t w) {
 extern "C" int psfm_depth_prepare(const uint8_t* d_rgb, int32_t num_frames, int32_t h, int32_t w, int32_t net_h,
                                   int32_t net_w, int32_t half, void* d_out, void* stream) {
   const char* entry = "psfm_depth_prepare";
-  if (!d_rgb || !d_out) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  int rc = check_sizes(entry, num_frames, h, w);
-  if (rc != PSFM_OK) return rc;
-  if (net_h < 1 || net_w < 1 || (long long)net_h * net_w > (1ll << 28))
-    return fail(entry, PSFM_ERR_INVALID, "bad network input size");
-  if (half != 0 && half != 1) return fail(entry, PSFM_ERR_INVALID, "half must be 0 or 1");
-  rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_rgb || !d_out) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    int rc = check_sizes(entry, num_frames, h, w);
+    if (rc != PSFM_OK) return rc;
+    if (net_h < 1 || net_w < 1 || (long long)net_h * net_w > (1ll << 28))
+      return fail(entry, PSFM_ERR_INVALID, "bad network input size");
+    if (half != 0 && half != 1) return fail(entry, PSFM_ERR_INVALID, "half must be 0 or 1");
+    rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     // cv::resize: inv_scale = dsize / ssize, and resizeGeneric_ takes scale = 1 / inv_scale
     const double scale_x = 1.0 / ((double)net_w / w), scale_y = 1.0 / ((double)net_h / h);
     const dim3 grid(grid_of((long long)net_h * net_w), num_frames);
@@ -220,21 +220,21 @@ extern "C" int psfm_depth_prepare(const uint8_t* d_rgb, int32_t num_frames, int3
     else k_prepare<float><<<grid, 256, 0, st>>>(d_rgb, h, w, net_h, net_w, scale_x, scale_y, (float*)d_out);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_depth_upsample(const void* d_pred, int32_t num_frames, int32_t net_h, int32_t net_w, int32_t half,
                                    int32_t h, int32_t w, float* d_flipped, float* d_minmax, void* stream) {
   const char* entry = "psfm_depth_upsample";
-  if (!d_pred || !d_flipped || !d_minmax) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  int rc = check_sizes(entry, num_frames, h, w);
-  if (rc != PSFM_OK) return rc;
-  if (net_h < 1 || net_w < 1 || (long long)net_h * net_w > (1ll << 28))
-    return fail(entry, PSFM_ERR_INVALID, "bad network output size");
-  if (half != 0 && half != 1) return fail(entry, PSFM_ERR_INVALID, "half must be 0 or 1");
-  rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_pred || !d_flipped || !d_minmax) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    int rc = check_sizes(entry, num_frames, h, w);
+    if (rc != PSFM_OK) return rc;
+    if (net_h < 1 || net_w < 1 || (long long)net_h * net_w > (1ll << 28))
+      return fail(entry, PSFM_ERR_INVALID, "bad network output size");
+    if (half != 0 && half != 1) return fail(entry, PSFM_ERR_INVALID, "half must be 0 or 1");
+    rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     DBuf<unsigned> mm;
     mm.alloc(2 * (size_t)num_frames, st);
@@ -247,21 +247,21 @@ extern "C" int psfm_depth_upsample(const void* d_pred, int32_t num_frames, int32
     k_minmax_decode<<<grid_of(2 * (long long)num_frames), 256, 0, st>>>(mm.p, num_frames, d_minmax);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_depth_quantize(const float* d_flipped, int32_t num_frames, int32_t h, int32_t w,
                                    const float* d_minmax, uint16_t* d_pixels, void* stream) {
   const char* entry = "psfm_depth_quantize";
-  if (!d_flipped || !d_minmax || !d_pixels) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  int rc = check_sizes(entry, num_frames, h, w);
-  if (rc != PSFM_OK) return rc;
-  rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_flipped || !d_minmax || !d_pixels) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    int rc = check_sizes(entry, num_frames, h, w);
+    if (rc != PSFM_OK) return rc;
+    rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     k_quantize<<<dim3(grid_of((long long)h * w), num_frames), 256, 0, (cudaStream_t)stream>>>(d_flipped, h, w, d_minmax,
                                                                                             d_pixels);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }

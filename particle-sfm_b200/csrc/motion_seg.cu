@@ -448,31 +448,33 @@ extern "C" int psfm_seg_hits(const int64_t* d_ptr, const int32_t* d_frames, int3
                              const int32_t* d_win_start, int32_t num_windows, int32_t L, int32_t* d_hits,
                              void* stream) {
   const char* entry = "psfm_seg_hits";
-  if (!d_ptr || !d_frames || !d_win_start || !d_hits) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (num_trajs < 1) return fail(entry, PSFM_ERR_INVALID, "num_trajs must be positive");
-  int rc = check_window(entry, num_windows, L);
-  if (rc != PSFM_OK) return rc;
-  rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_ptr || !d_frames || !d_win_start || !d_hits) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (num_trajs < 1) return fail(entry, PSFM_ERR_INVALID, "num_trajs must be positive");
+    int rc = check_window(entry, num_windows, L);
+    if (rc != PSFM_OK) return rc;
+    rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     const long long n = (long long)num_trajs * num_windows;
     k_hits<<<grid_of(n), 256, 0, (cudaStream_t)stream>>>(d_ptr, d_frames, num_trajs, d_win_start, num_windows, L,
                                                           d_hits);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_seg_shuffle(int32_t K, int32_t* perm) {
   const char* entry = "psfm_seg_shuffle";
-  if (!perm) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (K < 0) return fail(entry, PSFM_ERR_INVALID, "K must not be negative");
-  std::vector<int32_t> p((size_t)K);
-  std::iota(p.begin(), p.end(), 0);
-  std::mt19937 rng(5489u);
-  std::shuffle(p.begin(), p.end(), rng);
-  std::copy(p.begin(), p.end(), perm);
-  return PSFM_OK;
+  return guard(entry, [&]() -> int {
+    if (!perm) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (K < 0) return fail(entry, PSFM_ERR_INVALID, "K must not be negative");
+    std::vector<int32_t> p((size_t)K);
+    std::iota(p.begin(), p.end(), 0);
+    std::mt19937 rng(5489u);
+    std::shuffle(p.begin(), p.end(), rng);
+    std::copy(p.begin(), p.end(), perm);
+    return PSFM_OK;
+  });
 }
 
 extern "C" int psfm_seg_windows(const int64_t* d_ptr, const int32_t* d_frames, const double* d_xy,
@@ -480,38 +482,38 @@ extern "C" int psfm_seg_windows(const int64_t* d_ptr, const int32_t* d_frames, c
                                 const int32_t* d_win_start, int32_t L, double* d_loc, uint8_t* d_valid,
                                 void* stream) {
   const char* entry = "psfm_seg_windows";
-  if (!d_ptr || !d_frames || !d_xy || !d_rows || !d_row_window || !d_win_start || !d_loc || !d_valid)
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (num_rows < 1) return fail(entry, PSFM_ERR_INVALID, "num_rows must be positive");
-  int rc = check_window(entry, 1, L);
-  if (rc != PSFM_OK) return rc;
-  rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_ptr || !d_frames || !d_xy || !d_rows || !d_row_window || !d_win_start || !d_loc || !d_valid)
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (num_rows < 1) return fail(entry, PSFM_ERR_INVALID, "num_rows must be positive");
+    int rc = check_window(entry, 1, L);
+    if (rc != PSFM_OK) return rc;
+    rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     const long long n = (long long)num_rows * L;
     k_windows<<<grid_of(n), 256, 0, (cudaStream_t)stream>>>(d_ptr, d_frames, d_xy, d_rows, d_row_window, num_rows,
                                                              d_win_start, L, d_loc, d_valid);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_seg_depth_resize(const uint16_t* d_pixels, int32_t num_frames, int32_t h, int32_t w, float* d_out,
                                      void* stream) {
   const char* entry = "psfm_seg_depth_resize";
-  if (!d_pixels || !d_out) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (num_frames < 1 || num_frames > 65535) return fail(entry, PSFM_ERR_INVALID, "num_frames must be 1 .. 65535");
-  if (h < 1 || w < 1 || (long long)h * w > (1ll << 28)) return fail(entry, PSFM_ERR_INVALID, "bad frame size");
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_pixels || !d_out) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (num_frames < 1 || num_frames > 65535) return fail(entry, PSFM_ERR_INVALID, "num_frames must be 1 .. 65535");
+    if (h < 1 || w < 1 || (long long)h * w > (1ll << 28)) return fail(entry, PSFM_ERR_INVALID, "bad frame size");
+    int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     // cv::resize: inv_scale = dsize / ssize, and resizeGeneric_ takes scale = 1 / inv_scale
     const double scale_x = 1.0 / ((double)kW / w), scale_y = 1.0 / ((double)kH / h);
     const dim3 grid(grid_of((long long)kH * kW), num_frames);
     k_depth_resize<<<grid, 256, 0, (cudaStream_t)stream>>>(d_pixels, h, w, scale_x, scale_y, d_out);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_seg_encode(const double* d_loc, const uint8_t* d_valid, const int32_t* d_row_window,
@@ -519,19 +521,19 @@ extern "C" int psfm_seg_encode(const double* d_loc, const uint8_t* d_valid, cons
                                const float* d_depth, int32_t num_frames, int32_t raw_h, int32_t raw_w,
                                const float* d_weights, float* d_feat, void* stream) {
   const char* entry = "psfm_seg_encode";
-  if (!d_loc || !d_valid || !d_row_window || !d_win_start || !d_depth || !d_weights || !d_feat)
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (num_rows < 1) return fail(entry, PSFM_ERR_INVALID, "num_rows must be positive");
-  int rc = check_window(entry, num_windows, L);
-  if (rc != PSFM_OK) return rc;
-  if (L > psfm_seg_max_window())
-    return fail(entry, PSFM_ERR_INVALID, "window length " + std::to_string(L) + " exceeds the fused encoder's " +
-                                             std::to_string(psfm_seg_max_window()));
-  if (num_frames < 1) return fail(entry, PSFM_ERR_INVALID, "num_frames must be positive");
-  if (raw_h < 1 || raw_w < 1) return fail(entry, PSFM_ERR_INVALID, "bad frame size");
-  rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_loc || !d_valid || !d_row_window || !d_win_start || !d_depth || !d_weights || !d_feat)
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (num_rows < 1) return fail(entry, PSFM_ERR_INVALID, "num_rows must be positive");
+    int rc = check_window(entry, num_windows, L);
+    if (rc != PSFM_OK) return rc;
+    if (L > psfm_seg_max_window())
+      return fail(entry, PSFM_ERR_INVALID, "window length " + std::to_string(L) + " exceeds the fused encoder's " +
+                                               std::to_string(psfm_seg_max_window()));
+    if (num_frames < 1) return fail(entry, PSFM_ERR_INVALID, "num_frames must be positive");
+    if (raw_h < 1 || raw_w < 1) return fail(entry, PSFM_ERR_INVALID, "bad frame size");
+    rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     const int warps = encode_warps(L);
     const size_t smem = (size_t)(kWeightsPadded + (long long)warps * kWarpFloats * L) * 4;
     PSFM_CUDA(cudaFuncSetAttribute(k_encode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -545,27 +547,27 @@ extern "C" int psfm_seg_encode(const double* d_loc, const uint8_t* d_valid, cons
         (double)raw_h / (double)kH, d_weights, d_feat);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_seg_merge(const int64_t* d_ptr, const int32_t* d_frames, int32_t num_trajs,
                               const int32_t* d_win_start, int32_t num_windows, int32_t L, const int32_t* d_row_of,
                               const uint8_t* d_pred, int8_t* d_labels, int32_t* d_first_row, void* stream) {
   const char* entry = "psfm_seg_merge";
-  if (!d_ptr || !d_frames || !d_win_start || !d_row_of || !d_pred || !d_labels || !d_first_row)
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (num_trajs < 1) return fail(entry, PSFM_ERR_INVALID, "num_trajs must be positive");
-  int rc = check_window(entry, num_windows, L);
-  if (rc != PSFM_OK) return rc;
-  rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_ptr || !d_frames || !d_win_start || !d_row_of || !d_pred || !d_labels || !d_first_row)
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (num_trajs < 1) return fail(entry, PSFM_ERR_INVALID, "num_trajs must be positive");
+    int rc = check_window(entry, num_windows, L);
+    if (rc != PSFM_OK) return rc;
+    rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     k_merge<<<grid_of(num_trajs), 256, 0, (cudaStream_t)stream>>>(d_ptr, d_frames, num_trajs, d_win_start,
                                                                    num_windows, L, d_row_of, d_pred, d_labels,
                                                                    d_first_row);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_seg_draw(const uint8_t* d_frames, const double* d_loc, const uint8_t* d_valid,
@@ -573,18 +575,18 @@ extern "C" int psfm_seg_draw(const uint8_t* d_frames, const double* d_loc, const
                              const int32_t* d_draws, int32_t num_draws, const int16_t* d_stamps, int32_t na,
                              int32_t nb, int32_t nc, int32_t* d_order, uint8_t* d_out, void* stream) {
   const char* entry = "psfm_seg_draw";
-  if (!d_frames || !d_order || !d_out || !d_stamps) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (K > 0 && (!d_loc || !d_valid || !d_pred)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (num_draws > 0 && !d_draws) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (K < 0 || num_draws < 0 || (num_draws > 0 && K == 0))
-    return fail(entry, PSFM_ERR_INVALID, "bad trajectory or draw count");
-  if (na < 1 || nb < 1 || nc < 1) return fail(entry, PSFM_ERR_INVALID, "empty stamp");
-  int rc = check_window(entry, 1, L);
-  if (rc != PSFM_OK) return rc;
-  if (raw_h < 1 || raw_w < 1) return fail(entry, PSFM_ERR_INVALID, "bad frame size");
-  rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_frames || !d_order || !d_out || !d_stamps) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (K > 0 && (!d_loc || !d_valid || !d_pred)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (num_draws > 0 && !d_draws) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (K < 0 || num_draws < 0 || (num_draws > 0 && K == 0))
+      return fail(entry, PSFM_ERR_INVALID, "bad trajectory or draw count");
+    if (na < 1 || nb < 1 || nc < 1) return fail(entry, PSFM_ERR_INVALID, "empty stamp");
+    int rc = check_window(entry, 1, L);
+    if (rc != PSFM_OK) return rc;
+    if (raw_h < 1 || raw_w < 1) return fail(entry, PSFM_ERR_INVALID, "bad frame size");
+    rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     PSFM_CUDA(cudaMemsetAsync(d_order, 0, (size_t)L * 3 * kH * kW * sizeof(int32_t), st));
     const long long n = ((long long)K + num_draws) * L;
@@ -597,5 +599,5 @@ extern "C" int psfm_seg_draw(const uint8_t* d_frames, const double* d_loc, const
     k_draw_colour<<<grid_of((long long)L * 4 * kH * kW), 256, 0, st>>>(d_frames, L, d_order, d_pred, d_draws, d_out);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }

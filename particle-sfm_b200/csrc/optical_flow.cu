@@ -236,12 +236,12 @@ __global__ void k_colour(const float* __restrict__ flow, long long hw, const uns
 
 extern "C" int psfm_corr_pyramids(float* d_fwd, float* d_bwd, int32_t h, int32_t w, void* stream) {
   const char* entry = "psfm_corr_pyramids";
-  if (!d_fwd || !d_bwd) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (h < 8 || w < 8) return fail(entry, PSFM_ERR_INVALID, "bad sizes: every level needs at least one pixel (h, w >= 8)");
-  if ((long long)h * w > (1 << 20)) return fail(entry, PSFM_ERR_INVALID, "bad sizes: more than 2^20 pixels at 1/8");
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_fwd || !d_bwd) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (h < 8 || w < 8) return fail(entry, PSFM_ERR_INVALID, "bad sizes: every level needs at least one pixel (h, w >= 8)");
+    if ((long long)h * w > (1 << 20)) return fail(entry, PSFM_ERR_INVALID, "bad sizes: more than 2^20 pixels at 1/8");
+    int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int n = h * w;
     k_corr_level0<<<dim3((n + 31) / 32, (n + 31) / 32), dim3(32, 8), 0, st>>>(d_fwd, d_bwd, n);
@@ -258,60 +258,62 @@ extern "C" int psfm_corr_pyramids(float* d_fwd, float* d_bwd, int32_t h, int32_t
       wl /= 2;
     }
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int64_t psfm_corr_pyramid_floats(int32_t h, int32_t w) {
-  if (h < 8 || w < 8 || (long long)h * w > (1 << 20)) return fail("psfm_corr_pyramid_floats", PSFM_ERR_INVALID, "bad sizes");
-  return pyramid_floats(h, w);
+  return guard("psfm_corr_pyramid_floats", [&]() -> int64_t {
+    if (h < 8 || w < 8 || (long long)h * w > (1 << 20)) return fail("psfm_corr_pyramid_floats", PSFM_ERR_INVALID, "bad sizes");
+    return pyramid_floats(h, w);
+  });
 }
 
 extern "C" int psfm_corr_lookup(const float* d_pyramids, int32_t num_problems, int32_t h, int32_t w, const float* d_coords,
                                 float* d_out, void* stream) {
   const char* entry = "psfm_corr_lookup";
-  if (!d_pyramids || !d_coords || !d_out) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (h < 8 || w < 8 || (long long)h * w > (1 << 20)) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
-  if (num_problems < 1 || num_problems > 65535) return fail(entry, PSFM_ERR_INVALID, "num_problems must be 1 .. 65535");
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_pyramids || !d_coords || !d_out) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (h < 8 || w < 8 || (long long)h * w > (1 << 20)) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
+    if (num_problems < 1 || num_problems > 65535) return fail(entry, PSFM_ERR_INVALID, "num_problems must be 1 .. 65535");
+    int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     const int hw = h * w;
     k_lookup<<<dim3((hw + 127) / 128, kLevels, num_problems), 128, 0, (cudaStream_t)stream>>>(
         d_pyramids, pyramid_floats(h, w), h, w, d_coords, d_out);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_flow_upsample(const float* d_flow, const float* d_mask, int32_t num_problems, int32_t h, int32_t w,
                                   const int32_t* pad, float* d_out, void* stream) {
   const char* entry = "psfm_flow_upsample";
-  if (!d_flow || !d_mask || !pad || !d_out) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (h < 1 || w < 1 || (long long)h * w > (1 << 20)) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
-  if (num_problems < 1 || num_problems > 65535) return fail(entry, PSFM_ERR_INVALID, "num_problems must be 1 .. 65535");
-  for (int k = 0; k < 4; ++k)
-    if (pad[k] < 0 || pad[k] > 7) return fail(entry, PSFM_ERR_INVALID, "padding must be 0 .. 7");
-  const int out_w = 8 * w - pad[0] - pad[1], out_h = 8 * h - pad[2] - pad[3];
-  if (out_w < 1 || out_h < 1) return fail(entry, PSFM_ERR_INVALID, "padding leaves no pixel");
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_flow || !d_mask || !pad || !d_out) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (h < 1 || w < 1 || (long long)h * w > (1 << 20)) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
+    if (num_problems < 1 || num_problems > 65535) return fail(entry, PSFM_ERR_INVALID, "num_problems must be 1 .. 65535");
+    for (int k = 0; k < 4; ++k)
+      if (pad[k] < 0 || pad[k] > 7) return fail(entry, PSFM_ERR_INVALID, "padding must be 0 .. 7");
+    const int out_w = 8 * w - pad[0] - pad[1], out_h = 8 * h - pad[2] - pad[3];
+    if (out_w < 1 || out_h < 1) return fail(entry, PSFM_ERR_INVALID, "padding leaves no pixel");
+    int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     const long long n = (long long)out_h * out_w;
     k_upsample<<<dim3(grid_of(n), num_problems), 256, 0, (cudaStream_t)stream>>>(d_flow, d_mask, h, w, out_h, out_w,
                                                                                    pad[2], pad[0], d_out);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_flow_to_image(const float* d_flow, int32_t num_maps, int32_t h, int32_t w, uint8_t* d_bgr, void* stream) {
   const char* entry = "psfm_flow_to_image";
-  if (!d_flow || !d_bgr) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (h < 1 || w < 1) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
-  if (num_maps < 1 || num_maps > 65535) return fail(entry, PSFM_ERR_INVALID, "num_maps must be 1 .. 65535");
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!d_flow || !d_bgr) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (h < 1 || w < 1) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
+    if (num_maps < 1 || num_maps > 65535) return fail(entry, PSFM_ERR_INVALID, "num_maps must be 1 .. 65535");
+    int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const long long hw = (long long)h * w;
     DBuf<unsigned> rmax;
@@ -322,5 +324,5 @@ extern "C" int psfm_flow_to_image(const float* d_flow, int32_t num_maps, int32_t
     k_colour<<<dim3(grid_of(hw), num_maps), 256, 0, st>>>(d_flow, hw, rmax.p, d_bgr);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }

@@ -15,30 +15,27 @@ namespace {
 bool keypoints_in_range(int64_t R, const int32_t* pair_images, const int64_t* kp_ptr, const int64_t* iptr, const uint32_t* m) {
   const unsigned nt = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
   std::vector<char> ok(nt, 1);
-  std::vector<std::thread> th;
   const long long N = iptr[R];
-  for (unsigned w = 0; w < nt; ++w)
-    th.emplace_back([&, w] {
-      const long long lo = N * w / nt, hi = N * (w + 1) / nt;
-      if (lo >= hi) return;
-      int64_t p = std::upper_bound(iptr, iptr + R + 1, (int64_t)lo) - iptr - 1;
-      for (long long i = lo; i < hi;) {
-        while (iptr[p + 1] <= i) ++p;
-        const long long e = std::min<long long>(hi, iptr[p + 1]);
-        const uint64_t na = (uint64_t)(kp_ptr[pair_images[2 * p] + 1] - kp_ptr[pair_images[2 * p]]);
-        const uint64_t nb = (uint64_t)(kp_ptr[pair_images[2 * p + 1] + 1] - kp_ptr[pair_images[2 * p + 1]]);
-        uint32_t ma = 0, mb = 0;
-        bool any = false;
-        for (long long k = i; k < e; ++k) {
-          ma = std::max(ma, m[2 * k]);
-          mb = std::max(mb, m[2 * k + 1]);
-          any = true;
-        }
-        if (any && ((uint64_t)ma >= na || (uint64_t)mb >= nb)) { ok[w] = 0; return; }
-        i = e;
+  host_fan(nt, [&](unsigned w) {
+    const long long lo = N * w / nt, hi = N * (w + 1) / nt;
+    if (lo >= hi) return;
+    int64_t p = std::upper_bound(iptr, iptr + R + 1, (int64_t)lo) - iptr - 1;
+    for (long long i = lo; i < hi;) {
+      while (iptr[p + 1] <= i) ++p;
+      const long long e = std::min<long long>(hi, iptr[p + 1]);
+      const uint64_t na = (uint64_t)(kp_ptr[pair_images[2 * p] + 1] - kp_ptr[pair_images[2 * p]]);
+      const uint64_t nb = (uint64_t)(kp_ptr[pair_images[2 * p + 1] + 1] - kp_ptr[pair_images[2 * p + 1]]);
+      uint32_t ma = 0, mb = 0;
+      bool any = false;
+      for (long long k = i; k < e; ++k) {
+        ma = std::max(ma, m[2 * k]);
+        mb = std::max(mb, m[2 * k + 1]);
+        any = true;
       }
-    });
-  for (auto& t : th) t.join();
+      if (any && ((uint64_t)ma >= na || (uint64_t)mb >= nb)) { ok[w] = 0; return; }
+      i = e;
+    }
+  });
   return std::all_of(ok.begin(), ok.end(), [](char c) { return c != 0; });
 }
 

@@ -345,88 +345,88 @@ extern "C" int psfm_estimate_global_positions(int32_t num_images, int64_t num_pa
   const auto t0 = std::chrono::steady_clock::now();
   const long long launches0 = g_launch_count.load();
   const char* entry = "psfm_estimate_global_positions";
-  int rc = check_sizes(entry, num_images, 0, num_pairs);
-  if (rc != PSFM_OK) return rc;
-  if ((num_pairs > 0 && (!pair_images || !pair_tvec || !scales)) ||
-      (num_images > 0 && (!orientations || !positions || !has_position || !image_tvec)))
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  psfm_lud_options o;
-  psfm_lud_default_options(&o);
-  if (opts) o = *opts;
-  if (!(o.max_num_iterations > 0 && o.rho > 0.0 && o.alpha > 0.0 && o.alpha < 2.0 && o.absolute_tolerance > 0.0 &&
-        o.relative_tolerance > 0.0 && std::isfinite(o.rho) && std::isfinite(o.absolute_tolerance) &&
-        std::isfinite(o.relative_tolerance)))
-    return fail(entry, PSFM_ERR_INVALID, "options fail the ConstrainedL1Solver options Check()");
-  const int F = num_images, R = (int)num_pairs;
-  if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
-  if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
-  std::vector<int> used;
-  for (int p = 0; p < R; ++p)
-    if (!pair_used || pair_used[p]) used.push_back(p);
-  if (used.empty()) return fail(entry, PSFM_ERR_INVALID, "no used image pair");
-  // views: the images of the used pairs, ascending; the first is the gauge
-  std::vector<int> vidx(F, -1), views;
-  {
-    std::vector<char> seen(F, 0);
-    for (int p : used) seen[pair_images[2 * p]] = seen[pair_images[2 * p + 1]] = 1;
-    for (int f = 0; f < F; ++f)
-      if (seen[f]) { vidx[f] = (int)views.size(); views.push_back(f); }
-  }
-  for (int f : views) {
-    if (has_orientation && !has_orientation[f]) return fail(entry, PSFM_ERR_INVALID, "a used pair's image has no orientation");
-    for (int k = 0; k < 4; ++k)
-      if (!std::isfinite(orientations[4 * (size_t)f + k])) return fail(entry, PSFM_ERR_INVALID, "a non-finite orientation");
-  }
-  for (int p : used)
-    for (int k = 0; k < 3; ++k)
-      if (!std::isfinite(pair_tvec[3 * (size_t)p + k])) return fail(entry, PSFM_ERR_INVALID, "a non-finite pair tvec");
-  const int V = (int)views.size(), Ru = (int)used.size();
-  {
-    std::vector<int> parent(V);
-    std::iota(parent.begin(), parent.end(), 0);
-    int comps = V;
-    for (int p : used) {
-      const int a = find_root(parent, vidx[pair_images[2 * p]]), b = find_root(parent, vidx[pair_images[2 * p + 1]]);
-      if (a != b) { parent[std::max(a, b)] = std::min(a, b); --comps; }
-    }
-    if (comps != 1) return fail(entry, PSFM_ERR_INVALID, "the used pairs do not form one connected graph (S is singular)");
-  }
-  const long long n_ll = 3LL * (V - 1);
-  if (n_ll > kMaxUnknowns) return fail(entry, PSFM_ERR_UNSUPPORTED, "more than 2731 views (3 (V - 1) > 8190 unknowns)");
-  const int n = (int)n_ll;
-  if ((rc = require_device(entry)) != PSFM_OK) return rc;
-
   psfm_position_summary sm;
   memset(&sm, 0, sizeof(sm));
-  sm.gauge_image = views[0];
-  sm.num_views = V;
-  sm.num_pairs_used = Ru;
   auto finish = [&](int rc) {
     sm.num_launches = g_launch_count.load() - launches0;
     if (summary) *summary = sm;
     return rc;
   };
-  std::vector<int> pa(Ru), pb(Ru);
-  std::vector<double> tv(3 * (size_t)Ru), q2(4 * (size_t)Ru);
-  for (int k = 0; k < Ru; ++k) {
-    const int p = used[k];
-    pa[k] = vidx[pair_images[2 * p]];
-    pb[k] = vidx[pair_images[2 * p + 1]];
-    for (int i = 0; i < 3; ++i) tv[3 * (size_t)k + i] = pair_tvec[3 * (size_t)p + i];
-    for (int i = 0; i < 4; ++i) q2[4 * (size_t)k + i] = orientations[4 * (size_t)pair_images[2 * p + 1] + i];
-  }
-  // view -> incident pairs, in pair order; bit 0: the view is the pair's image 1 (+I in A), else image 2 (-I)
-  std::vector<int> inc_ptr(V + 1, 0), inc(2 * (size_t)Ru);
-  for (int k = 0; k < Ru; ++k) { ++inc_ptr[pa[k] + 1]; ++inc_ptr[pb[k] + 1]; }
-  for (int v = 0; v < V; ++v) inc_ptr[v + 1] += inc_ptr[v];
-  {
-    std::vector<int> fill(inc_ptr.begin(), inc_ptr.end() - 1);
-    for (int k = 0; k < Ru; ++k) { inc[fill[pa[k]]++] = 2 * k + 1; inc[fill[pb[k]]++] = 2 * k; }
-  }
-  std::vector<double> c(n), s(Ru);
-  const auto t1 = std::chrono::steady_clock::now();
-  sm.host_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
-  try {
+  return guard(entry, [&]() -> int {
+    int rc = check_sizes(entry, num_images, 0, num_pairs);
+    if (rc != PSFM_OK) return rc;
+    if ((num_pairs > 0 && (!pair_images || !pair_tvec || !scales)) ||
+        (num_images > 0 && (!orientations || !positions || !has_position || !image_tvec)))
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    psfm_lud_options o;
+    psfm_lud_default_options(&o);
+    if (opts) o = *opts;
+    if (!(o.max_num_iterations > 0 && o.rho > 0.0 && o.alpha > 0.0 && o.alpha < 2.0 && o.absolute_tolerance > 0.0 &&
+          o.relative_tolerance > 0.0 && std::isfinite(o.rho) && std::isfinite(o.absolute_tolerance) &&
+          std::isfinite(o.relative_tolerance)))
+      return fail(entry, PSFM_ERR_INVALID, "options fail the ConstrainedL1Solver options Check()");
+    const int F = num_images, R = (int)num_pairs;
+    if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
+    if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
+    std::vector<int> used;
+    for (int p = 0; p < R; ++p)
+      if (!pair_used || pair_used[p]) used.push_back(p);
+    if (used.empty()) return fail(entry, PSFM_ERR_INVALID, "no used image pair");
+    // views: the images of the used pairs, ascending; the first is the gauge
+    std::vector<int> vidx(F, -1), views;
+    {
+      std::vector<char> seen(F, 0);
+      for (int p : used) seen[pair_images[2 * p]] = seen[pair_images[2 * p + 1]] = 1;
+      for (int f = 0; f < F; ++f)
+        if (seen[f]) { vidx[f] = (int)views.size(); views.push_back(f); }
+    }
+    for (int f : views) {
+      if (has_orientation && !has_orientation[f]) return fail(entry, PSFM_ERR_INVALID, "a used pair's image has no orientation");
+      for (int k = 0; k < 4; ++k)
+        if (!std::isfinite(orientations[4 * (size_t)f + k])) return fail(entry, PSFM_ERR_INVALID, "a non-finite orientation");
+    }
+    for (int p : used)
+      for (int k = 0; k < 3; ++k)
+        if (!std::isfinite(pair_tvec[3 * (size_t)p + k])) return fail(entry, PSFM_ERR_INVALID, "a non-finite pair tvec");
+    const int V = (int)views.size(), Ru = (int)used.size();
+    {
+      std::vector<int> parent(V);
+      std::iota(parent.begin(), parent.end(), 0);
+      int comps = V;
+      for (int p : used) {
+        const int a = find_root(parent, vidx[pair_images[2 * p]]), b = find_root(parent, vidx[pair_images[2 * p + 1]]);
+        if (a != b) { parent[std::max(a, b)] = std::min(a, b); --comps; }
+      }
+      if (comps != 1) return fail(entry, PSFM_ERR_INVALID, "the used pairs do not form one connected graph (S is singular)");
+    }
+    const long long n_ll = 3LL * (V - 1);
+    if (n_ll > kMaxUnknowns) return fail(entry, PSFM_ERR_UNSUPPORTED, "more than 2731 views (3 (V - 1) > 8190 unknowns)");
+    const int n = (int)n_ll;
+    if ((rc = require_device(entry)) != PSFM_OK) return rc;
+
+    sm.gauge_image = views[0];
+    sm.num_views = V;
+    sm.num_pairs_used = Ru;
+    std::vector<int> pa(Ru), pb(Ru);
+    std::vector<double> tv(3 * (size_t)Ru), q2(4 * (size_t)Ru);
+    for (int k = 0; k < Ru; ++k) {
+      const int p = used[k];
+      pa[k] = vidx[pair_images[2 * p]];
+      pb[k] = vidx[pair_images[2 * p + 1]];
+      for (int i = 0; i < 3; ++i) tv[3 * (size_t)k + i] = pair_tvec[3 * (size_t)p + i];
+      for (int i = 0; i < 4; ++i) q2[4 * (size_t)k + i] = orientations[4 * (size_t)pair_images[2 * p + 1] + i];
+    }
+    // view -> incident pairs, in pair order; bit 0: the view is the pair's image 1 (+I in A), else image 2 (-I)
+    std::vector<int> inc_ptr(V + 1, 0), inc(2 * (size_t)Ru);
+    for (int k = 0; k < Ru; ++k) { ++inc_ptr[pa[k] + 1]; ++inc_ptr[pb[k] + 1]; }
+    for (int v = 0; v < V; ++v) inc_ptr[v + 1] += inc_ptr[v];
+    {
+      std::vector<int> fill(inc_ptr.begin(), inc_ptr.end() - 1);
+      for (int k = 0; k < Ru; ++k) { inc[fill[pa[k]]++] = 2 * k + 1; inc[fill[pb[k]]++] = 2 * k; }
+    }
+    std::vector<double> c(n), s(Ru);
+    const auto t1 = std::chrono::steady_clock::now();
+    sm.host_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
     const int lda = n + 1, np = dense_chol_panels(n), rmax = dense_chol_rmax(n);
     DBuf<int> d_pa, d_pb, d_inc_ptr, d_inc, d_fail;
     DBuf<double> d_tv, d_q2, d_d, d_D, d_rs, d_w, d_z, d_u, d_dz, d_s, d_part, d_ipart, d_rhs, d_c, d_S, d_xc, d_Lp, d_Ld,
@@ -494,37 +494,37 @@ extern "C" int psfm_estimate_global_positions(int32_t num_images, int64_t num_pa
     sm.converged = h.done;
     sm.primal_residual = h.r_norm; sm.primal_tolerance = h.primal_eps;
     sm.dual_residual = h.s_norm; sm.dual_tolerance = h.dual_eps;
-  } catch (const CudaFail& f) { return finish(f.code); }
-  // outputs; RegisterAllImages: tvec = -QuaternionRotatePoint(q, c)
-  for (int f = 0; f < F; ++f) {
-    has_position[f] = 0;
-    for (int k = 0; k < 3; ++k) positions[3 * (size_t)f + k] = image_tvec[3 * (size_t)f + k] = 0.0;
-  }
-  for (int p = 0; p < R; ++p) scales[p] = 0.0;
-  for (int k = 0; k < Ru; ++k) scales[used[k]] = s[k];
-  for (int v = 0; v < V; ++v) {
-    const int f = views[v];
-    double* cf = positions + 3 * (size_t)f;
-    for (int k = 0; k < 3; ++k) cf[k] = v == 0 ? 0.0 : c[3 * (v - 1) + k];
-    double t[3];
-    qrotate(load_q(orientations + 4 * (size_t)f), cf, t);
-    for (int k = 0; k < 3; ++k) image_tvec[3 * (size_t)f + k] = -t[k];
-    has_position[f] = 1;
-  }
-  return finish(PSFM_OK);
+    // outputs; RegisterAllImages: tvec = -QuaternionRotatePoint(q, c)
+    for (int f = 0; f < F; ++f) {
+      has_position[f] = 0;
+      for (int k = 0; k < 3; ++k) positions[3 * (size_t)f + k] = image_tvec[3 * (size_t)f + k] = 0.0;
+    }
+    for (int p = 0; p < R; ++p) scales[p] = 0.0;
+    for (int k = 0; k < Ru; ++k) scales[used[k]] = s[k];
+    for (int v = 0; v < V; ++v) {
+      const int f = views[v];
+      double* cf = positions + 3 * (size_t)f;
+      for (int k = 0; k < 3; ++k) cf[k] = v == 0 ? 0.0 : c[3 * (v - 1) + k];
+      double t[3];
+      qrotate(load_q(orientations + 4 * (size_t)f), cf, t);
+      for (int k = 0; k < 3; ++k) image_tvec[3 * (size_t)f + k] = -t[k];
+      has_position[f] = 1;
+    }
+    return finish(PSFM_OK);
+  }, finish);
 }
 
 // test entry: the stage's explicit inverse of one SPD matrix, dense_cholesky_launch then k_pos_inverse, failure through
 // Ctl.failed
 extern "C" int psfm_spd_inverse(const double* A, int32_t n, double* X) {
-  if (!A || !X) { set_error("psfm_spd_inverse: null argument"); return PSFM_ERR_INVALID; }
-  if (n < 1 || n > kMaxUnknowns) {
-    set_error("psfm_spd_inverse: needs 1 <= n <= 8190 (the stage's bound)");
-    return PSFM_ERR_INVALID;
-  }
-  const int rc = require_device("psfm_spd_inverse");
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard("psfm_spd_inverse", [&]() -> int {
+    if (!A || !X) { set_error("psfm_spd_inverse: null argument"); return PSFM_ERR_INVALID; }
+    if (n < 1 || n > kMaxUnknowns) {
+      set_error("psfm_spd_inverse: needs 1 <= n <= 8190 (the stage's bound)");
+      return PSFM_ERR_INVALID;
+    }
+    const int rc = require_device("psfm_spd_inverse");
+    if (rc != PSFM_OK) return rc;
     const int lda = n + 1, np = dense_chol_panels(n), rmax = dense_chol_rmax(n);
     DBuf<double> d_S, d_xc, d_Lp, d_Ld, d_X;
     DBuf<int> d_fail;
@@ -544,5 +544,5 @@ extern "C" int psfm_spd_inverse(const double* A, int32_t n, double* X) {
     if (h.failed) { set_error("psfm_spd_inverse: matrix is not positive definite"); return PSFM_ERR_INVALID; }
     PSFM_CUDA(cudaMemcpy(X, d_X.p, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }

@@ -8,7 +8,12 @@
 
 #include <algorithm>
 #include <atomic>
+#include <exception>
+#include <memory>
+#include <new>
 #include <string>
+#include <thread>
+#include <vector>
 
 #include "../../include/psfm_b200.h"
 
@@ -29,6 +34,42 @@ inline unsigned grid_stride_of(long long n) { return (unsigned)std::max<long lon
 struct CudaFail {
   int code;
 };
+
+inline int same_code(int code) { return code; }
+
+// The exception boundary of a C entry point: returns body()'s status and lets no exception out.  CudaFail returns its
+// code (its thrower set the message); any other exception sets "<entry>: <what>" and returns PSFM_ERR_HOST.  Only after
+// an exception, on_throw(code) runs and its value is returned (by default the code itself).
+template <typename Body, typename OnThrow = int (&)(int)>
+auto guard(const char* entry, Body&& body, OnThrow&& on_throw = same_code) -> decltype(body()) {
+  int code;
+  try {
+    return body();
+  } catch (const CudaFail& f) {
+    code = f.code;
+  } catch (const std::bad_alloc&) {
+    code = fail(entry, PSFM_ERR_HOST, "out of host memory");
+  } catch (const std::exception& e) {
+    code = fail(entry, PSFM_ERR_HOST, e.what());
+  } catch (...) {
+    code = fail(entry, PSFM_ERR_HOST, "unknown host exception");
+  }
+  return on_throw(code);
+}
+
+// Runs fn(0) .. fn(nt - 1), fn(0) on the calling thread and the others on threads of their own.  The calls must be
+// independent: when a thread cannot be created, the calling thread runs the remaining calls itself.
+template <typename Fn>
+void host_fan(unsigned nt, Fn&& fn) {
+  std::vector<std::thread> th;
+  unsigned w = 1;
+  try {
+    for (; w < nt; ++w) th.emplace_back([&fn, w] { fn(w); });
+  } catch (const std::exception&) {}
+  for (; w < nt; ++w) fn(w);
+  fn(0);
+  for (auto& t : th) t.join();
+}
 
 #define PSFM_CUDA(expr)                                                                   \
   do {                                                                                    \

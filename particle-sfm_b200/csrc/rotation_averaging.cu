@@ -389,115 +389,115 @@ extern "C" int psfm_estimate_global_rotations(int32_t num_images, int64_t num_pa
   const auto t0 = std::chrono::steady_clock::now();
   const long long launches0 = g_launch_count.load();
   const char* entry = "psfm_estimate_global_rotations";
-  int rc = check_sizes(entry, num_images, 0, num_pairs);
-  if (rc != PSFM_OK) return rc;
-  if ((num_pairs > 0 && (!pair_images || !qvec || !num_correspondences || !pair_kept)) ||
-      (num_images > 0 && (!orientations || !has_orientation)))
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  psfm_rotation_options o;
-  psfm_rotation_default_options(&o);
-  if (opts) o = *opts;
-  if (!(o.max_num_l1_iterations > 0 && o.l1_step_convergence_threshold > 0.0 && o.max_num_irls_iterations > 0 &&
-        o.irls_step_convergence_threshold > 0.0 && o.irls_loss_parameter_sigma > 0.0 && o.rotation_filter_max_degrees > 0.0))
-    return fail(entry, PSFM_ERR_INVALID, "options fail RobustRotationEstimator::Options::Check()");
-  const int F = num_images, R = (int)num_pairs;
-  if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
-  if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
-  if (o.max_num_l1_iterations > PSFM_ROTATION_MAX_L1_ROUNDS)
-    return fail(entry, PSFM_ERR_UNSUPPORTED, "max_num_l1_iterations above PSFM_ROTATION_MAX_L1_ROUNDS");
-
   psfm_rotation_summary sm;
   memset(&sm, 0, sizeof(sm));
   sm.gauge_image = -1;
-  for (int f = 0; f < F; ++f) { has_orientation[f] = 0; for (int k = 0; k < 4; ++k) orientations[4 * f + k] = 0.0; }
-  for (int p = 0; p < R; ++p) pair_kept[p] = 0;
   auto finish = [&](int rc) {
     sm.num_launches = g_launch_count.load() - launches0;
     if (summary) *summary = sm;
     return rc;
   };
-  // AllPairs(only_with_pose), then the first RemoveDisconnectedViewPairs
-  std::vector<int> posed;
-  for (int p = 0; p < R; ++p) {
-    bool ok = !has_pose || has_pose[p];
-    for (int k = 0; k < 4; ++k) ok = ok && std::isfinite(qvec[4 * p + k]);
-    if (ok) posed.push_back(p);
-  }
-  std::vector<char> in_comp;
-  const std::vector<int> cp = largest_component(F, pair_images, posed, in_comp);
-  if (cp.empty()) {
-    return finish(fail(entry, PSFM_NO_ROTATIONS, "no image pair with a pose"));
-  }
-  std::vector<int> cidx(F, -1), cimg;
-  for (int f = 0; f < F; ++f) if (in_comp[f]) { cidx[f] = (int)cimg.size(); cimg.push_back(f); }
-  const int nc = (int)cimg.size(), n = nc - 1, Rc = (int)cp.size();
-  if (nc > kMaxComponentImages) return fail(entry, PSFM_ERR_UNSUPPORTED, "more than 8192 images in the kept component");
-  sm.gauge_image = cimg[0];
-  sm.num_images_connected = nc;
-  sm.num_pairs_connected = Rc;
-  std::vector<int> pa(Rc), pb(Rc);
-  std::vector<double> rq(4 * (size_t)Rc);
-  for (int i = 0; i < Rc; ++i) {
-    pa[i] = cidx[pair_images[2 * cp[i]]];
-    pb[i] = cidx[pair_images[2 * cp[i] + 1]];
-    for (int k = 0; k < 4; ++k) rq[4 * i + k] = qvec[4 * (size_t)cp[i] + k];
-  }
-  // OrientationsFromMaximumSpanningTree: Kruskal on (-num_correspondences, image 1, image 2), then chaining from
-  // the gauge image (on a tree the traversal order does not change the result)
-  std::vector<int> order(Rc);
-  std::iota(order.begin(), order.end(), 0);
-  std::sort(order.begin(), order.end(), [&](int i, int j) {
-    const int ni = num_correspondences[cp[i]], nj = num_correspondences[cp[j]];
-    if (ni != nj) return ni > nj;
-    if (pa[i] != pa[j]) return pa[i] < pa[j];
-    return pb[i] < pb[j];
-  });
-  std::vector<std::vector<int>> tree(nc);
-  {
-    UnionFind uf(nc);
-    for (int i : order)
-      if (uf.unite(pa[i], pb[i])) { tree[pa[i]].push_back(i); tree[pb[i]].push_back(i); }
-  }
-  std::vector<double> Rq(4 * (size_t)nc, 0.0);
-  {
-    std::vector<char> done(nc, 0);
-    std::vector<int> queue(1, 0);
-    Rq[0] = 1.0;
-    done[0] = 1;
-    for (size_t h = 0; h < queue.size(); ++h) {
-      const int s = queue[h];
-      double Rs[3][3], Rr[3][3], Rn[3][3];
-      quat_to_matrix({Rq[4 * s], Rq[4 * s + 1], Rq[4 * s + 2], Rq[4 * s + 3]}, Rs);
-      for (int i : tree[s]) {
-        const bool src_first = pa[i] == s;
-        const int t = src_first ? pb[i] : pa[i];
-        if (done[t]) continue;
-        quat_to_matrix({rq[4 * i], rq[4 * i + 1], rq[4 * i + 2], rq[4 * i + 3]}, Rr);
-        for (int r = 0; r < 3; ++r)
-          for (int c = 0; c < 3; ++c) {
-            double v = 0.0;
-            for (int k = 0; k < 3; ++k) v += (src_first ? Rr[r][k] : Rr[k][r]) * Rs[k][c];
-            Rn[r][c] = v;
-          }
-        const Quat q = matrix_to_quat(Rn);
-        Rq[4 * t] = q.w; Rq[4 * t + 1] = q.x; Rq[4 * t + 2] = q.y; Rq[4 * t + 3] = q.z;
-        done[t] = 1;
-        queue.push_back(t);
+  return guard(entry, [&]() -> int {
+    int rc = check_sizes(entry, num_images, 0, num_pairs);
+    if (rc != PSFM_OK) return rc;
+    if ((num_pairs > 0 && (!pair_images || !qvec || !num_correspondences || !pair_kept)) ||
+        (num_images > 0 && (!orientations || !has_orientation)))
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    psfm_rotation_options o;
+    psfm_rotation_default_options(&o);
+    if (opts) o = *opts;
+    if (!(o.max_num_l1_iterations > 0 && o.l1_step_convergence_threshold > 0.0 && o.max_num_irls_iterations > 0 &&
+          o.irls_step_convergence_threshold > 0.0 && o.irls_loss_parameter_sigma > 0.0 && o.rotation_filter_max_degrees > 0.0))
+      return fail(entry, PSFM_ERR_INVALID, "options fail RobustRotationEstimator::Options::Check()");
+    const int F = num_images, R = (int)num_pairs;
+    if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
+    if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
+    if (o.max_num_l1_iterations > PSFM_ROTATION_MAX_L1_ROUNDS)
+      return fail(entry, PSFM_ERR_UNSUPPORTED, "max_num_l1_iterations above PSFM_ROTATION_MAX_L1_ROUNDS");
+
+    for (int f = 0; f < F; ++f) { has_orientation[f] = 0; for (int k = 0; k < 4; ++k) orientations[4 * f + k] = 0.0; }
+    for (int p = 0; p < R; ++p) pair_kept[p] = 0;
+    // AllPairs(only_with_pose), then the first RemoveDisconnectedViewPairs
+    std::vector<int> posed;
+    for (int p = 0; p < R; ++p) {
+      bool ok = !has_pose || has_pose[p];
+      for (int k = 0; k < 4; ++k) ok = ok && std::isfinite(qvec[4 * p + k]);
+      if (ok) posed.push_back(p);
+    }
+    std::vector<char> in_comp;
+    const std::vector<int> cp = largest_component(F, pair_images, posed, in_comp);
+    if (cp.empty()) {
+      return finish(fail(entry, PSFM_NO_ROTATIONS, "no image pair with a pose"));
+    }
+    std::vector<int> cidx(F, -1), cimg;
+    for (int f = 0; f < F; ++f) if (in_comp[f]) { cidx[f] = (int)cimg.size(); cimg.push_back(f); }
+    const int nc = (int)cimg.size(), n = nc - 1, Rc = (int)cp.size();
+    if (nc > kMaxComponentImages) return fail(entry, PSFM_ERR_UNSUPPORTED, "more than 8192 images in the kept component");
+    sm.gauge_image = cimg[0];
+    sm.num_images_connected = nc;
+    sm.num_pairs_connected = Rc;
+    std::vector<int> pa(Rc), pb(Rc);
+    std::vector<double> rq(4 * (size_t)Rc);
+    for (int i = 0; i < Rc; ++i) {
+      pa[i] = cidx[pair_images[2 * cp[i]]];
+      pb[i] = cidx[pair_images[2 * cp[i] + 1]];
+      for (int k = 0; k < 4; ++k) rq[4 * i + k] = qvec[4 * (size_t)cp[i] + k];
+    }
+    // OrientationsFromMaximumSpanningTree: Kruskal on (-num_correspondences, image 1, image 2), then chaining from
+    // the gauge image (on a tree the traversal order does not change the result)
+    std::vector<int> order(Rc);
+    std::iota(order.begin(), order.end(), 0);
+    std::sort(order.begin(), order.end(), [&](int i, int j) {
+      const int ni = num_correspondences[cp[i]], nj = num_correspondences[cp[j]];
+      if (ni != nj) return ni > nj;
+      if (pa[i] != pa[j]) return pa[i] < pa[j];
+      return pb[i] < pb[j];
+    });
+    std::vector<std::vector<int>> tree(nc);
+    {
+      UnionFind uf(nc);
+      for (int i : order)
+        if (uf.unite(pa[i], pb[i])) { tree[pa[i]].push_back(i); tree[pb[i]].push_back(i); }
+    }
+    std::vector<double> Rq(4 * (size_t)nc, 0.0);
+    {
+      std::vector<char> done(nc, 0);
+      std::vector<int> queue(1, 0);
+      Rq[0] = 1.0;
+      done[0] = 1;
+      for (size_t h = 0; h < queue.size(); ++h) {
+        const int s = queue[h];
+        double Rs[3][3], Rr[3][3], Rn[3][3];
+        quat_to_matrix({Rq[4 * s], Rq[4 * s + 1], Rq[4 * s + 2], Rq[4 * s + 3]}, Rs);
+        for (int i : tree[s]) {
+          const bool src_first = pa[i] == s;
+          const int t = src_first ? pb[i] : pa[i];
+          if (done[t]) continue;
+          quat_to_matrix({rq[4 * i], rq[4 * i + 1], rq[4 * i + 2], rq[4 * i + 3]}, Rr);
+          for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) {
+              double v = 0.0;
+              for (int k = 0; k < 3; ++k) v += (src_first ? Rr[r][k] : Rr[k][r]) * Rs[k][c];
+              Rn[r][c] = v;
+            }
+          const Quat q = matrix_to_quat(Rn);
+          Rq[4 * t] = q.w; Rq[4 * t + 1] = q.x; Rq[4 * t + 2] = q.y; Rq[4 * t + 3] = q.z;
+          done[t] = 1;
+          queue.push_back(t);
+        }
       }
     }
-  }
-  // image -> incident pairs, in pair order; bit 0: the image is the pair's image 2 (+I in A), else image 1 (-I)
-  std::vector<int> inc_ptr(nc + 1, 0), inc(2 * (size_t)Rc);
-  for (int i = 0; i < Rc; ++i) { ++inc_ptr[pa[i] + 1]; ++inc_ptr[pb[i] + 1]; }
-  for (int c = 0; c < nc; ++c) inc_ptr[c + 1] += inc_ptr[c];
-  {
-    std::vector<int> fill(inc_ptr.begin(), inc_ptr.end() - 1);
-    for (int i = 0; i < Rc; ++i) { inc[fill[pa[i]]++] = 2 * i; inc[fill[pb[i]]++] = 2 * i + 1; }
-  }
-  if ((rc = require_device(entry)) != PSFM_OK) return rc;
-  const auto t1 = std::chrono::steady_clock::now();
-  std::vector<unsigned char> kept(Rc);
-  try {
+    // image -> incident pairs, in pair order; bit 0: the image is the pair's image 2 (+I in A), else image 1 (-I)
+    std::vector<int> inc_ptr(nc + 1, 0), inc(2 * (size_t)Rc);
+    for (int i = 0; i < Rc; ++i) { ++inc_ptr[pa[i] + 1]; ++inc_ptr[pb[i] + 1]; }
+    for (int c = 0; c < nc; ++c) inc_ptr[c + 1] += inc_ptr[c];
+    {
+      std::vector<int> fill(inc_ptr.begin(), inc_ptr.end() - 1);
+      for (int i = 0; i < Rc; ++i) { inc[fill[pa[i]]++] = 2 * i; inc[fill[pb[i]]++] = 2 * i + 1; }
+    }
+    if ((rc = require_device(entry)) != PSFM_OK) return rc;
+    const auto t1 = std::chrono::steady_clock::now();
+    std::vector<unsigned char> kept(Rc);
     const int lda = n + 1, np = dense_chol_panels(n), rmax = dense_chol_rmax(n);
     DBuf<int> d_pa, d_pb, d_inc_ptr, d_inc, d_fail;
     DBuf<double> d_rq, d_R, d_res, d_z, d_u, d_dz, d_w, d_wr, d_part, d_ipart, d_atv, d_x, d_A, d_xc, d_Lp, d_Ld;
@@ -589,37 +589,37 @@ extern "C" int psfm_estimate_global_rotations(int32_t num_images, int64_t num_pa
     PSFM_LAUNCH_CHECK();
     PSFM_CUDA(cudaMemcpy(Rq.data(), d_R.p, sizeof(double) * 4 * (size_t)nc, cudaMemcpyDeviceToHost));
     PSFM_CUDA(cudaMemcpy(kept.data(), d_kept.p, Rc, cudaMemcpyDeviceToHost));
-  } catch (const CudaFail& f) { return finish(f.code); }
-  const auto t2 = std::chrono::steady_clock::now();
-  // the second RemoveDisconnectedViewPairs; every image of the first component keeps its orientation
-  for (int c = 0; c < nc; ++c) {
-    has_orientation[cimg[c]] = 1;
-    for (int k = 0; k < 4; ++k) orientations[4 * (size_t)cimg[c] + k] = Rq[4 * c + k];
-  }
-  std::vector<int> filtered;
-  for (int i = 0; i < Rc; ++i) if (kept[i]) filtered.push_back(cp[i]);
-  std::vector<char> in_kept;
-  const std::vector<int> fin = largest_component(F, pair_images, filtered, in_kept);
-  for (int p : fin) pair_kept[p] = 1;
-  sm.num_pairs_kept = (int)fin.size();
-  sm.num_images_kept = (int)std::count(in_kept.begin(), in_kept.end(), 1);
-  const auto t3 = std::chrono::steady_clock::now();
-  const auto ms = [](auto a, auto b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
-  sm.host_ms = ms(t0, t1) + ms(t2, t3);
-  sm.device_ms = ms(t1, t2);
-  return finish(PSFM_OK);
+    const auto t2 = std::chrono::steady_clock::now();
+    // the second RemoveDisconnectedViewPairs; every image of the first component keeps its orientation
+    for (int c = 0; c < nc; ++c) {
+      has_orientation[cimg[c]] = 1;
+      for (int k = 0; k < 4; ++k) orientations[4 * (size_t)cimg[c] + k] = Rq[4 * c + k];
+    }
+    std::vector<int> filtered;
+    for (int i = 0; i < Rc; ++i) if (kept[i]) filtered.push_back(cp[i]);
+    std::vector<char> in_kept;
+    const std::vector<int> fin = largest_component(F, pair_images, filtered, in_kept);
+    for (int p : fin) pair_kept[p] = 1;
+    sm.num_pairs_kept = (int)fin.size();
+    sm.num_images_kept = (int)std::count(in_kept.begin(), in_kept.end(), 1);
+    const auto t3 = std::chrono::steady_clock::now();
+    const auto ms = [](auto a, auto b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
+    sm.host_ms = ms(t0, t1) + ms(t2, t3);
+    sm.device_ms = ms(t1, t2);
+    return finish(PSFM_OK);
+  }, finish);
 }
 
 // test entry: the stage's x update on one SPD matrix, dense_cholesky_launch then k_trsv, failure through Ctl.failed
 extern "C" int psfm_laplacian_solve(const double* A, const double* B, int32_t n, double* X) {
-  if (!A || !B || !X) { set_error("psfm_laplacian_solve: null argument"); return PSFM_ERR_INVALID; }
-  if (n < 1 || n > kMaxComponentImages - 1) {
-    set_error("psfm_laplacian_solve: needs 1 <= n <= 8191 (the stage's bound)");
-    return PSFM_ERR_INVALID;
-  }
-  const int rc = require_device("psfm_laplacian_solve");
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard("psfm_laplacian_solve", [&]() -> int {
+    if (!A || !B || !X) { set_error("psfm_laplacian_solve: null argument"); return PSFM_ERR_INVALID; }
+    if (n < 1 || n > kMaxComponentImages - 1) {
+      set_error("psfm_laplacian_solve: needs 1 <= n <= 8191 (the stage's bound)");
+      return PSFM_ERR_INVALID;
+    }
+    const int rc = require_device("psfm_laplacian_solve");
+    if (rc != PSFM_OK) return rc;
     const int lda = n + 1, np = dense_chol_panels(n), rmax = dense_chol_rmax(n);
     DBuf<double> d_A, d_b, d_x, d_xc, d_Lp, d_Ld;
     DBuf<int> d_fail, d_skip;
@@ -640,5 +640,5 @@ extern "C" int psfm_laplacian_solve(const double* A, const double* B, int32_t n,
     if (h.failed) { set_error("psfm_laplacian_solve: matrix is not positive definite"); return PSFM_ERR_INVALID; }
     PSFM_CUDA(cudaMemcpy(X, d_x.p, sizeof(double) * 3 * (size_t)n, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }

@@ -139,46 +139,40 @@ __global__ void k_body_frame(long long T, long long total, uint8_t* body) {
 
 namespace psfm {
 
-int track_npy_encode(const long long* ids, const long long* ptr, const int* frames, const double* xy, long long T,
-                     cudaStream_t st, psfm_track_npy** out, int64_t* nbytes) {
-  psfm_track_npy* R = new psfm_track_npy;
-  try {
-    DBuf<long long> bytes, off;
-    DBuf<uint8_t> tmp, body;
-    long long sum = 0;
-    if (T) {
-      bytes.alloc(T, st); off.alloc(T, st);
-      k_record_bytes<<<grid_of(T), 256, 0, st>>>(T, ids, ptr, frames, bytes.p);
-      PSFM_LAUNCH_CHECK();
-      size_t tb = 0;
-      PSFM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, bytes.p, off.p, T, st));
-      tmp.alloc(tb, st);
-      PSFM_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, bytes.p, off.p, T, st));
-      PSFM_LAUNCH_CHECK();
-      long long last[2];
-      PSFM_CUDA(cudaMemcpyAsync(&last[0], off.p + T - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
-      PSFM_CUDA(cudaMemcpyAsync(&last[1], bytes.p + T - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
-      PSFM_CUDA(cudaStreamSynchronize(st));
-      sum = last[0] + last[1];
-    }
-    R->bytes = T ? 3 + sum : 1;
-    body.alloc((size_t)R->bytes, st);
-    k_body_frame<<<1, 1, 0, st>>>(T, sum, body.p);
+void track_npy_encode(const long long* ids, const long long* ptr, const int* frames, const double* xy, long long T,
+                      cudaStream_t st, psfm_track_npy** out, int64_t* nbytes) {
+  std::unique_ptr<psfm_track_npy, decltype(&psfm_track_npy_destroy)> R(new psfm_track_npy, psfm_track_npy_destroy);
+  DBuf<long long> bytes, off;
+  DBuf<uint8_t> tmp, body;
+  long long sum = 0;
+  if (T) {
+    bytes.alloc(T, st); off.alloc(T, st);
+    k_record_bytes<<<grid_of(T), 256, 0, st>>>(T, ids, ptr, frames, bytes.p);
     PSFM_LAUNCH_CHECK();
-    if (T) {
-      k_write_records<<<grid_of(32 * T), 256, 0, st>>>(T, ids, ptr, frames, xy, off.p, body.p);
-      PSFM_LAUNCH_CHECK();
-    }
-    PSFM_CUDA(cudaMallocHost((void**)&R->host, (size_t)R->bytes));
-    PSFM_CUDA(cudaMemcpyAsync(R->host, body.p, (size_t)R->bytes, cudaMemcpyDeviceToHost, st));
+    size_t tb = 0;
+    PSFM_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, bytes.p, off.p, T, st));
+    tmp.alloc(tb, st);
+    PSFM_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, bytes.p, off.p, T, st));
+    PSFM_LAUNCH_CHECK();
+    long long last[2];
+    PSFM_CUDA(cudaMemcpyAsync(&last[0], off.p + T - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    PSFM_CUDA(cudaMemcpyAsync(&last[1], bytes.p + T - 1, sizeof(long long), cudaMemcpyDeviceToHost, st));
     PSFM_CUDA(cudaStreamSynchronize(st));
-  } catch (const CudaFail& f) {
-    psfm_track_npy_destroy(R);
-    return f.code;
+    sum = last[0] + last[1];
   }
-  *out = R;
+  R->bytes = T ? 3 + sum : 1;
+  body.alloc((size_t)R->bytes, st);
+  k_body_frame<<<1, 1, 0, st>>>(T, sum, body.p);
+  PSFM_LAUNCH_CHECK();
+  if (T) {
+    k_write_records<<<grid_of(32 * T), 256, 0, st>>>(T, ids, ptr, frames, xy, off.p, body.p);
+    PSFM_LAUNCH_CHECK();
+  }
+  PSFM_CUDA(cudaMallocHost((void**)&R->host, (size_t)R->bytes));
+  PSFM_CUDA(cudaMemcpyAsync(R->host, body.p, (size_t)R->bytes, cudaMemcpyDeviceToHost, st));
+  PSFM_CUDA(cudaStreamSynchronize(st));
   *nbytes = R->bytes;
-  return PSFM_OK;
+  *out = R.release();
 }
 
 }  // namespace psfm
@@ -186,30 +180,31 @@ int track_npy_encode(const long long* ids, const long long* ptr, const int* fram
 extern "C" int psfm_track_npy_create(const int64_t* ids, const int64_t* ptr, const int32_t* frame_ids, const double* xy,
                                      int64_t num_trajs, int64_t num_obs, psfm_track_npy** out, int64_t* nbytes) {
   const char* entry = "psfm_track_npy_create";
-  if (!out || !nbytes) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  *out = nullptr;
-  *nbytes = 0;
-  if (num_trajs < 0 || num_obs < 0 || !ptr) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
-  if ((num_trajs && !ids) || (num_obs && (!frame_ids || !xy))) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  // every check before the device sees a byte: the kernels index with ptr and trust the widths
-  if (ptr[0] != 0 || ptr[num_trajs] != num_obs) return fail(entry, PSFM_ERR_INVALID, "ptr must run from 0 to num_obs");
-  for (int64_t k = 0; k < num_trajs; ++k) {
-    if (ptr[k + 1] < ptr[k]) return fail(entry, PSFM_ERR_INVALID, "ptr is not monotone at trajectory " + std::to_string(k));
-    if (ids[k] < 0 || ids[k] > INT32_MAX) return fail(entry, PSFM_ERR_INVALID, "trajectory id outside [0, 2^31): " + std::to_string(ids[k]));
-  }
-  for (int64_t j = 0; j < num_obs; ++j)
-    if (frame_ids[j] < 0) return fail(entry, PSFM_ERR_INVALID, "negative frame id at observation " + std::to_string(j));
-  int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!out || !nbytes) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    *out = nullptr;
+    *nbytes = 0;
+    if (num_trajs < 0 || num_obs < 0 || !ptr) return fail(entry, PSFM_ERR_INVALID, "bad sizes");
+    if ((num_trajs && !ids) || (num_obs && (!frame_ids || !xy))) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    // every check before the device sees a byte: the kernels index with ptr and trust the widths
+    if (ptr[0] != 0 || ptr[num_trajs] != num_obs) return fail(entry, PSFM_ERR_INVALID, "ptr must run from 0 to num_obs");
+    for (int64_t k = 0; k < num_trajs; ++k) {
+      if (ptr[k + 1] < ptr[k]) return fail(entry, PSFM_ERR_INVALID, "ptr is not monotone at trajectory " + std::to_string(k));
+      if (ids[k] < 0 || ids[k] > INT32_MAX) return fail(entry, PSFM_ERR_INVALID, "trajectory id outside [0, 2^31): " + std::to_string(ids[k]));
+    }
+    for (int64_t j = 0; j < num_obs; ++j)
+      if (frame_ids[j] < 0) return fail(entry, PSFM_ERR_INVALID, "negative frame id at observation " + std::to_string(j));
+    int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     DBuf<long long> dids, dptr; DBuf<int> dfr; DBuf<double> dxy;
     dids.alloc(num_trajs); dptr.alloc(num_trajs + 1); dfr.alloc(num_obs); dxy.alloc(2 * num_obs);
     dids.upload((const long long*)ids, num_trajs, nullptr);
     dptr.upload((const long long*)ptr, num_trajs + 1, nullptr);
     dfr.upload(frame_ids, num_obs, nullptr);
     dxy.upload(xy, 2 * num_obs, nullptr);
-    return track_npy_encode(dids.p, dptr.p, dfr.p, dxy.p, num_trajs, nullptr, out, nbytes);
-  } catch (const CudaFail& f) { return f.code; }
+    track_npy_encode(dids.p, dptr.p, dfr.p, dxy.p, num_trajs, nullptr, out, nbytes);
+    return PSFM_OK;
+  });
 }
 
 extern "C" const uint8_t* psfm_track_npy_data(const psfm_track_npy* h) { return h ? h->host : nullptr; }

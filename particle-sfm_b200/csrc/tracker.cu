@@ -308,11 +308,11 @@ struct FlagToInt {
 }  // namespace
 
 extern "C" int psfm_grid_sample(const float* map, int32_t h, int32_t w, int32_t channels, const double* xy, int32_t n, float* out) {
-  if (!map || !xy || !out || h < 2 || w < 2 || channels < 1 || channels > 2 || n < 0) return PSFM_ERR_INVALID;
-  int rc = require_device("psfm_grid_sample");
-  if (rc != PSFM_OK) return rc;
-  if (n == 0) return PSFM_OK;
-  try {
+  return guard("psfm_grid_sample", [&]() -> int {
+    if (!map || !xy || !out || h < 2 || w < 2 || channels < 1 || channels > 2 || n < 0) return PSFM_ERR_INVALID;
+    int rc = require_device("psfm_grid_sample");
+    if (rc != PSFM_OK) return rc;
+    if (n == 0) return PSFM_OK;
     DBuf<float> dm, dout; DBuf<double> dxy;
     dm.alloc((size_t)h * w * channels); dxy.alloc(2 * (size_t)n); dout.alloc((size_t)n * channels);
     dm.upload(map, dm.n, nullptr); dxy.upload(xy, dxy.n, nullptr);
@@ -320,14 +320,14 @@ extern "C" int psfm_grid_sample(const float* map, int32_t h, int32_t w, int32_t 
     PSFM_LAUNCH_CHECK();
     PSFM_CUDA(cudaMemcpy(out, dout.p, sizeof(float) * dout.n, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_flow_check(const float* flow_f, const float* flow_b, int32_t h, int32_t w, float thres, float* err, uint8_t* occ) {
-  if (!flow_f || !flow_b || !occ || h < 2 || w < 2) return PSFM_ERR_INVALID;
-  int rc = require_device("psfm_flow_check");
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard("psfm_flow_check", [&]() -> int {
+    if (!flow_f || !flow_b || !occ || h < 2 || w < 2) return PSFM_ERR_INVALID;
+    int rc = require_device("psfm_flow_check");
+    if (rc != PSFM_OK) return rc;
     const size_t hw = (size_t)h * w;
     DBuf<float> df, db, de; DBuf<unsigned char> dof;
     df.alloc(2 * hw); db.alloc(2 * hw); de.alloc(hw); dof.alloc(hw);
@@ -337,15 +337,15 @@ extern "C" int psfm_flow_check(const float* flow_f, const float* flow_b, int32_t
     if (err) PSFM_CUDA(cudaMemcpy(err, de.p, sizeof(float) * hw, cudaMemcpyDeviceToHost));
     PSFM_CUDA(cudaMemcpy(occ, dof.p, hw, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_tracker_step(const float* flow, const uint8_t* occ, int32_t h, int32_t w, const double* cur_xy, int32_t n,
                                  int32_t sample_ratio, double* next_xy, uint8_t* flags, uint8_t* reseed_mask) {
-  if (!flow || !occ || !cur_xy || !next_xy || !flags || h < 2 || w < 2 || n < 0 || sample_ratio < 1) return PSFM_ERR_INVALID;
-  int rc = require_device("psfm_tracker_step");
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard("psfm_tracker_step", [&]() -> int {
+    if (!flow || !occ || !cur_xy || !next_xy || !flags || h < 2 || w < 2 || n < 0 || sample_ratio < 1) return PSFM_ERR_INVALID;
+    int rc = require_device("psfm_tracker_step");
+    if (rc != PSFM_OK) return rc;
     const size_t hw = (size_t)h * w;
     const int gh = (h + sample_ratio - 1) / sample_ratio, gw = (w + sample_ratio - 1) / sample_ratio;
     DBuf<float> df; DBuf<unsigned char> dof, dfl, docc, dmask; DBuf<double> dcur, dnext, dkept;
@@ -370,16 +370,16 @@ extern "C" int psfm_tracker_step(const float* flow, const uint8_t* occ, int32_t 
       PSFM_CUDA(cudaMemcpy(reseed_mask, dmask.p, (size_t)gh * gw, cudaMemcpyDeviceToHost));
     }
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 extern "C" int psfm_tracker_buffer_inputs(const float* flow01, const float* flow02, const uint8_t* occ02, int32_t h, int32_t w,
                                           const double* x0, int32_t n, double upper_flow, double* ref1, double* ref2, double* scale) {
-  if (!flow01 || !flow02 || !occ02 || !x0 || !ref1 || !ref2 || !scale || h < 2 || w < 2 || n < 0) return PSFM_ERR_INVALID;
-  int rc = require_device("psfm_tracker_buffer_inputs");
-  if (rc != PSFM_OK) return rc;
-  if (n == 0) return PSFM_OK;
-  try {
+  return guard("psfm_tracker_buffer_inputs", [&]() -> int {
+    if (!flow01 || !flow02 || !occ02 || !x0 || !ref1 || !ref2 || !scale || h < 2 || w < 2 || n < 0) return PSFM_ERR_INVALID;
+    int rc = require_device("psfm_tracker_buffer_inputs");
+    if (rc != PSFM_OK) return rc;
+    if (n == 0) return PSFM_OK;
     const size_t hw = (size_t)h * w;
     DBuf<float> d1, d2; DBuf<unsigned char> dof; DBuf<double> dx, r1, r2, sc;
     d1.alloc(2 * hw); d2.alloc(2 * hw); dof.alloc(hw); dx.alloc(2 * (size_t)n); r1.alloc(2 * (size_t)n); r2.alloc(2 * (size_t)n); sc.alloc(n);
@@ -390,7 +390,7 @@ extern "C" int psfm_tracker_buffer_inputs(const float* flow01, const float* flow
     PSFM_CUDA(cudaMemcpy(ref2, r2.p, sizeof(double) * 2 * (size_t)n, cudaMemcpyDeviceToHost));
     PSFM_CUDA(cudaMemcpy(scale, sc.p, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 // ------------------------------------------------------------------ resident stage: host side
@@ -465,8 +465,9 @@ int tracker_usable(const psfm_tracker* T, bool args_ok, const char* fn) {
   return PSFM_OK;
 }
 
+// a failure left the device state unknown (T is NULL when the argument check itself threw)
 int tracker_broken(psfm_tracker* T, int code) {
-  T->failed = true;
+  if (T) T->failed = true;
   return code;
 }
 
@@ -474,16 +475,16 @@ int tracker_broken(psfm_tracker* T, int code) {
 
 extern "C" int psfm_flow_check_device(const float* d_flow_f, const float* d_flow_b, int32_t h, int32_t w, float thres, float* d_err,
                                       uint8_t* d_occ, void* stream) {
-  if (!d_flow_f || !d_flow_b || !d_occ) return fail("psfm_flow_check_device", PSFM_ERR_INVALID, "null argument");
-  if (h < 2 || w < 2) return fail("psfm_flow_check_device", PSFM_ERR_INVALID, "bad sizes");
-  int rc = require_device("psfm_flow_check_device");
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard("psfm_flow_check_device", [&]() -> int {
+    if (!d_flow_f || !d_flow_b || !d_occ) return fail("psfm_flow_check_device", PSFM_ERR_INVALID, "null argument");
+    if (h < 2 || w < 2) return fail("psfm_flow_check_device", PSFM_ERR_INVALID, "bad sizes");
+    int rc = require_device("psfm_flow_check_device");
+    if (rc != PSFM_OK) return rc;
     const size_t hw = (size_t)h * w;
     k_flow_check<<<grid_of(hw), 256, 0, (cudaStream_t)stream>>>(d_flow_f, d_flow_b, h, w, thres, d_err, d_occ);
     PSFM_LAUNCH_CHECK();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
 
 namespace {
@@ -496,52 +497,49 @@ int tracker_create(const char* entry, int32_t h, int32_t w, int32_t sample_ratio
   if (path_consistency != 0 && path_consistency != 1) return fail(entry, PSFM_ERR_INVALID, "path_consistency must be 0 or 1");
   int rc = require_device(entry);
   if (rc != PSFM_OK) return rc;
-  psfm_tracker* T = new psfm_tracker;
-  try {
-    T->h = h; T->w = w; T->ratio = sample_ratio; T->num_frames = num_frames;
-    T->path_consistency = path_consistency != 0;
-    T->gh = (h + sample_ratio - 1) / sample_ratio; T->gw = (w + sample_ratio - 1) / sample_ratio;
-    T->st = (cudaStream_t)stream;
-    T->hoff.assign(1, 0);
-    T->hcnt.assign(1, 0);
-    const size_t G = (size_t)T->gh * T->gw;
-    T->occ.alloc((size_t)h * w, T->st);
-    T->mask.alloc(G, T->st);
-    T->mpos.alloc(G, T->st);
-    T->d_counts.alloc(3, T->st);
-    T->totals.alloc(2, T->st);
-    PSFM_CUDA(cudaMallocHost((void**)&T->h_counts, 3 * sizeof(int)));
-    PSFM_CUDA(cudaMallocHost((void**)&T->h_totals, 2 * sizeof(long long)));
-  } catch (const CudaFail& f) {
-    psfm_tracker_destroy(T);
-    return f.code;
-  }
-  *out = T;
+  std::unique_ptr<psfm_tracker, decltype(&psfm_tracker_destroy)> T(new psfm_tracker, psfm_tracker_destroy);
+  T->h = h; T->w = w; T->ratio = sample_ratio; T->num_frames = num_frames;
+  T->path_consistency = path_consistency != 0;
+  T->gh = (h + sample_ratio - 1) / sample_ratio; T->gw = (w + sample_ratio - 1) / sample_ratio;
+  T->st = (cudaStream_t)stream;
+  T->hoff.assign(1, 0);
+  T->hcnt.assign(1, 0);
+  const size_t G = (size_t)T->gh * T->gw;
+  T->occ.alloc((size_t)h * w, T->st);
+  T->mask.alloc(G, T->st);
+  T->mpos.alloc(G, T->st);
+  T->d_counts.alloc(3, T->st);
+  T->totals.alloc(2, T->st);
+  PSFM_CUDA(cudaMallocHost((void**)&T->h_counts, 3 * sizeof(int)));
+  PSFM_CUDA(cudaMallocHost((void**)&T->h_totals, 2 * sizeof(long long)));
+  *out = T.release();
   return PSFM_OK;
 }
 
 }  // namespace
 
 extern "C" int psfm_tracker_create(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, void* stream, psfm_tracker** out) {
-  return tracker_create("psfm_tracker_create", h, w, sample_ratio, num_frames, 1, stream, out);
+  const char* entry = "psfm_tracker_create";
+  return guard(entry, [&] { return tracker_create(entry, h, w, sample_ratio, num_frames, 1, stream, out); });
 }
 
 extern "C" int psfm_tracker_create_mode(int32_t h, int32_t w, int32_t sample_ratio, int32_t num_frames, int32_t path_consistency,
                                         void* stream, psfm_tracker** out) {
-  return tracker_create("psfm_tracker_create_mode", h, w, sample_ratio, num_frames, path_consistency, stream, out);
+  const char* entry = "psfm_tracker_create_mode";
+  return guard(entry, [&] { return tracker_create(entry, h, w, sample_ratio, num_frames, path_consistency, stream, out); });
 }
 
 extern "C" int psfm_tracker_advance(psfm_tracker* T, const float* d_flow, const uint8_t* d_occ, const float* d_flow_prev,
                                     const float* d_flow2_prev, const uint8_t* d_occ2_prev, int32_t* counts) {
   const char* entry = "psfm_tracker_advance";
-  int rc = tracker_usable(T, d_flow && d_occ, entry);
-  if (rc != PSFM_OK) return rc;
-  if (T->finished) return fail(entry, PSFM_ERR_INVALID, "the track set was already assembled");
-  if (T->n_buf > 0) return fail(entry, PSFM_ERR_INVALID, "the buffered set of the previous frame was not optimised");
-  if (T->t + 1 >= T->num_frames) return fail(entry, PSFM_ERR_INVALID, "more frames than the tracker was created for");
-  if (T->path_consistency && T->t >= 1 && (!d_flow_prev || !d_flow2_prev || !d_occ2_prev))
-    return fail(entry, PSFM_ERR_INVALID, "from frame 1 on, flows[t-1], flows_f2[t-1] and occ_maps_s2[t-1] are needed");
-  try {
+  return guard(entry, [&]() -> int {
+    int rc = tracker_usable(T, d_flow && d_occ, entry);
+    if (rc != PSFM_OK) return rc;
+    if (T->finished) return fail(entry, PSFM_ERR_INVALID, "the track set was already assembled");
+    if (T->n_buf > 0) return fail(entry, PSFM_ERR_INVALID, "the buffered set of the previous frame was not optimised");
+    if (T->t + 1 >= T->num_frames) return fail(entry, PSFM_ERR_INVALID, "more frames than the tracker was created for");
+    if (T->path_consistency && T->t >= 1 && (!d_flow_prev || !d_flow2_prev || !d_occ2_prev))
+      return fail(entry, PSFM_ERR_INVALID, "from frame 1 on, flows[t-1], flows_f2[t-1] and occ_maps_s2[t-1] are needed");
     cudaStream_t st = T->st;
     const int t = T->t, G = T->gh * T->gw, H = T->h, W = T->w;
     const int seeds = t == 0 ? G : T->seeds, base = T->n_active, n = base + seeds;
@@ -632,7 +630,7 @@ extern "C" int psfm_tracker_advance(psfm_tracker* T, const float* d_flow, const 
     }
     if (counts) { counts[0] = survivors; counts[1] = T->seeds; counts[2] = T->n_buf; }
     return PSFM_OK;
-  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+  }, [&](int code) { return tracker_broken(T, code); });
 }
 
 namespace {
@@ -649,11 +647,11 @@ int tracker_writeback(psfm_tracker* T) {
 }  // namespace
 
 extern "C" int psfm_tracker_optimize(psfm_tracker* T, const psfm_traj_options* opts, psfm_traj_summary* summary) {
-  if (summary) memset(summary, 0, sizeof(*summary));
-  int rc = tracker_usable(T, true, "psfm_tracker_optimize");
-  if (rc != PSFM_OK) return rc;
-  if (T->n_buf <= 0) return fail("psfm_tracker_optimize", PSFM_ERR_INVALID, "no buffered trajectory");
-  try {
+  return guard("psfm_tracker_optimize", [&]() -> int {
+    if (summary) memset(summary, 0, sizeof(*summary));
+    int rc = tracker_usable(T, true, "psfm_tracker_optimize");
+    if (rc != PSFM_OK) return rc;
+    if (T->n_buf <= 0) return fail("psfm_tracker_optimize", PSFM_ERR_INVALID, "no buffered trajectory");
     // HP1 runs on the tracker's stream, after k_buffer_inputs.  NULL (the legacy default stream) is passed as
     // cudaStreamLegacy: a NULL stream would make solve_device use the HP1 workspace's non-blocking stream, which
     // is not ordered after the legacy stream's work.
@@ -661,14 +659,14 @@ extern "C" int psfm_tracker_optimize(psfm_tracker* T, const psfm_traj_options* o
                             summary, T->st ? T->st : cudaStreamLegacy);
     if (rc != PSFM_OK) return tracker_broken(T, rc);
     return tracker_writeback(T);
-  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+  }, [&](int code) { return tracker_broken(T, code); });
 }
 
 extern "C" int psfm_tracker_get_buffer(psfm_tracker* T, double* uv12, double* ref1, double* ref2, double* scale) {
-  int rc = tracker_usable(T, uv12 && ref1 && ref2 && scale, "psfm_tracker_get_buffer");
-  if (rc != PSFM_OK) return rc;
-  if (T->n_buf <= 0) return fail("psfm_tracker_get_buffer", PSFM_ERR_INVALID, "no buffered trajectory");
-  try {
+  return guard("psfm_tracker_get_buffer", [&]() -> int {
+    int rc = tracker_usable(T, uv12 && ref1 && ref2 && scale, "psfm_tracker_get_buffer");
+    if (rc != PSFM_OK) return rc;
+    if (T->n_buf <= 0) return fail("psfm_tracker_get_buffer", PSFM_ERR_INVALID, "no buffered trajectory");
     const size_t n = T->n_buf;
     PSFM_CUDA(cudaMemcpyAsync(uv12, T->buv.p, 4 * n * sizeof(double), cudaMemcpyDeviceToHost, T->st));
     PSFM_CUDA(cudaMemcpyAsync(ref1, T->bref1.p, 2 * n * sizeof(double), cudaMemcpyDeviceToHost, T->st));
@@ -676,27 +674,27 @@ extern "C" int psfm_tracker_get_buffer(psfm_tracker* T, double* uv12, double* re
     PSFM_CUDA(cudaMemcpyAsync(scale, T->bscale.p, n * sizeof(double), cudaMemcpyDeviceToHost, T->st));
     T->sync();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+  }, [&](int code) { return tracker_broken(T, code); });
 }
 
 extern "C" int psfm_tracker_set_buffer(psfm_tracker* T, const double* uv12) {
-  int rc = tracker_usable(T, uv12 != nullptr, "psfm_tracker_set_buffer");
-  if (rc != PSFM_OK) return rc;
-  if (T->n_buf <= 0) return fail("psfm_tracker_set_buffer", PSFM_ERR_INVALID, "no buffered trajectory");
-  try {
+  return guard("psfm_tracker_set_buffer", [&]() -> int {
+    int rc = tracker_usable(T, uv12 != nullptr, "psfm_tracker_set_buffer");
+    if (rc != PSFM_OK) return rc;
+    if (T->n_buf <= 0) return fail("psfm_tracker_set_buffer", PSFM_ERR_INVALID, "no buffered trajectory");
     PSFM_CUDA(cudaMemcpyAsync(T->bout.p, uv12, 4 * (size_t)T->n_buf * sizeof(double), cudaMemcpyHostToDevice, T->st));
     rc = tracker_writeback(T);
     T->sync();        // uv12 is the caller's (possibly pageable) memory
     return rc;
-  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+  }, [&](int code) { return tracker_broken(T, code); });
 }
 
 extern "C" int psfm_tracker_finish(psfm_tracker* T, int32_t traj_min_len, int64_t* num_trajs, int64_t* num_obs) {
-  int rc = tracker_usable(T, num_trajs && num_obs, "psfm_tracker_finish");
-  if (rc != PSFM_OK) return rc;
-  if (T->finished) return fail("psfm_tracker_finish", PSFM_ERR_INVALID, "already finished");
-  if (T->n_buf > 0) return fail("psfm_tracker_finish", PSFM_ERR_INVALID, "the buffered set of the last frame was not optimised");
-  try {
+  return guard("psfm_tracker_finish", [&]() -> int {
+    int rc = tracker_usable(T, num_trajs && num_obs, "psfm_tracker_finish");
+    if (rc != PSFM_OK) return rc;
+    if (T->finished) return fail("psfm_tracker_finish", PSFM_ERR_INVALID, "already finished");
+    if (T->n_buf > 0) return fail("psfm_tracker_finish", PSFM_ERR_INVALID, "the buffered set of the last frame was not optimised");
     cudaStream_t st = T->st;
     const int t = T->t;
     if (T->n_active) {
@@ -734,14 +732,14 @@ extern "C" int psfm_tracker_finish(psfm_tracker* T, int32_t traj_min_len, int64_
     *num_trajs = T->res_trajs;
     *num_obs = T->res_obs;
     return PSFM_OK;
-  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+  }, [&](int code) { return tracker_broken(T, code); });
 }
 
 extern "C" int psfm_tracker_result(psfm_tracker* T, int64_t* ids, int64_t* ptr, int32_t* frame_ids, double* xy) {
-  int rc = tracker_usable(T, ids && ptr && frame_ids && xy, "psfm_tracker_result");
-  if (rc != PSFM_OK) return rc;
-  if (!T->finished) return fail("psfm_tracker_result", PSFM_ERR_INVALID, "call psfm_tracker_finish first");
-  try {
+  return guard("psfm_tracker_result", [&]() -> int {
+    int rc = tracker_usable(T, ids && ptr && frame_ids && xy, "psfm_tracker_result");
+    if (rc != PSFM_OK) return rc;
+    if (!T->finished) return fail("psfm_tracker_result", PSFM_ERR_INVALID, "call psfm_tracker_finish first");
     const size_t nt = T->res_trajs, m = T->res_obs;
     if (T->next_id == 0) { ptr[0] = 0; return PSFM_OK; }
     PSFM_CUDA(cudaMemcpyAsync(ids, T->ids.p, nt * sizeof(int64_t), cudaMemcpyDeviceToHost, T->st));
@@ -750,18 +748,20 @@ extern "C" int psfm_tracker_result(psfm_tracker* T, int64_t* ids, int64_t* ptr, 
     PSFM_CUDA(cudaMemcpyAsync(xy, T->res_xy.p, 2 * m * sizeof(double), cudaMemcpyDeviceToHost, T->st));
     T->sync();
     return PSFM_OK;
-  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+  }, [&](int code) { return tracker_broken(T, code); });
 }
 
 extern "C" int psfm_tracker_track_npy(psfm_tracker* T, psfm_track_npy** out, int64_t* nbytes) {
-  int rc = tracker_usable(T, out && nbytes, "psfm_tracker_track_npy");
-  if (rc != PSFM_OK) return rc;
-  *out = nullptr;
-  *nbytes = 0;
-  if (!T->finished) return fail("psfm_tracker_track_npy", PSFM_ERR_INVALID, "call psfm_tracker_finish first");
-  // the tracker's ids are retire ranks (< 2^31, int counters), its frame ids times, its ptr an exclusive scan
-  rc = track_npy_encode(T->ids.p, T->ptr.p, T->res_frames.p, T->res_xy.p, T->res_trajs, T->st, out, nbytes);
-  return rc == PSFM_OK ? rc : tracker_broken(T, rc);
+  return guard("psfm_tracker_track_npy", [&]() -> int {
+    int rc = tracker_usable(T, out && nbytes, "psfm_tracker_track_npy");
+    if (rc != PSFM_OK) return rc;
+    *out = nullptr;
+    *nbytes = 0;
+    if (!T->finished) return fail("psfm_tracker_track_npy", PSFM_ERR_INVALID, "call psfm_tracker_finish first");
+    // the tracker's ids are retire ranks (< 2^31, int counters), its frame ids times, its ptr an exclusive scan
+    track_npy_encode(T->ids.p, T->ptr.p, T->res_frames.p, T->res_xy.p, T->res_trajs, T->st, out, nbytes);
+    return PSFM_OK;
+  }, [&](int code) { return tracker_broken(T, code); });
 }
 
 namespace {
@@ -776,14 +776,14 @@ __global__ void k_widen(long long n, const int* in, long long* out) {
 extern "C" int psfm_tracker_matches(psfm_tracker* T, int32_t num_images, int32_t sample_k, psfm_matches** out,
                                     int64_t* num_pairs, int64_t* num_matches) {
   const char* entry = "psfm_tracker_matches";
-  int rc = tracker_usable(T, out && num_pairs && num_matches, entry);
-  if (rc != PSFM_OK) return rc;
-  *out = nullptr;
-  if (!T->finished) return fail(entry, PSFM_ERR_INVALID, "call psfm_tracker_finish first");
-  if (num_images < T->num_frames) return fail(entry, PSFM_ERR_INVALID, "num_images is below the tracker's number of frames");
-  if (sample_k < 1) return fail(entry, PSFM_ERR_INVALID, "sample_k must be >= 1");
-  if (T->res_obs > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 samples");
-  try {
+  return guard(entry, [&]() -> int {
+    int rc = tracker_usable(T, out && num_pairs && num_matches, entry);
+    if (rc != PSFM_OK) return rc;
+    *out = nullptr;
+    if (!T->finished) return fail(entry, PSFM_ERR_INVALID, "call psfm_tracker_finish first");
+    if (num_images < T->num_frames) return fail(entry, PSFM_ERR_INVALID, "num_images is below the tracker's number of frames");
+    if (sample_k < 1) return fail(entry, PSFM_ERR_INVALID, "sample_k must be >= 1");
+    if (T->res_obs > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "more than 2^31 - 1 samples");
     // the tracker's ptr and xy are read where they are; its int32 frame ids are widened to the build's int64
     psfm::DBuf<long long> frames;
     psfm::TrackSetDev in;
@@ -798,7 +798,7 @@ extern "C" int psfm_tracker_matches(psfm_tracker* T, int32_t num_images, int32_t
     }
     rc = psfm::matches_build(entry, in, num_images, sample_k, T->st, out, num_pairs, num_matches);
     return rc == PSFM_OK ? rc : tracker_broken(T, rc);
-  } catch (const CudaFail& f) { return tracker_broken(T, f.code); }
+  }, [&](int code) { return tracker_broken(T, code); });
 }
 
 extern "C" void psfm_tracker_destroy(psfm_tracker* T) {

@@ -568,13 +568,9 @@ int solve_device(const double* d_uv12, const double* d_ref1, const double* d_ref
                  const float* d_flow12, int n, int w, int h, const psfm_traj_options* opts, double* d_out,
                  psfm_traj_summary* summary, cudaStream_t stream) {
   std::lock_guard<std::mutex> lock(g_ws.mu);
-  try {
-    g_ws.ensure((size_t)n, (size_t)(n + CH - 1) / CH);
-    return launch_solve(g_ws, d_uv12, d_ref1, d_ref2, d_scale, d_flow12, n, w, h, opts, d_out, summary,
-                        stream ? stream : g_ws.stream);
-  } catch (const CudaFail& f) {
-    return f.code;
-  }
+  g_ws.ensure((size_t)n, (size_t)(n + CH - 1) / CH);
+  return launch_solve(g_ws, d_uv12, d_ref1, d_ref2, d_scale, d_flow12, n, w, h, opts, d_out, summary,
+                      stream ? stream : g_ws.stream);
 }
 
 }  // namespace traj
@@ -599,27 +595,29 @@ extern "C" int psfm_traj_optimize_device(const double* d_uv12, const double* d_r
                                          const double* d_scale, const float* d_flow12, int32_t n, int32_t w,
                                          int32_t h, const psfm_traj_options* opts, double* d_out_uv12,
                                          psfm_traj_summary* summary, void* stream) {
-  if (summary) memset(summary, 0, sizeof(*summary));
-  if (n < 0 || w <= 0 || h <= 0) { set_error("psfm_traj_optimize: bad sizes"); return PSFM_ERR_INVALID; }
-  if (n == 0) return PSFM_OK;
-  int rc = require_device("psfm_traj_optimize_device");
-  if (rc != PSFM_OK) return rc;
-  return traj::solve_device(d_uv12, d_ref1, d_ref2, d_scale, d_flow12, n, w, h, opts, d_out_uv12, summary,
-                            (cudaStream_t)stream);
+  return guard("psfm_traj_optimize_device", [&]() -> int {
+    if (summary) memset(summary, 0, sizeof(*summary));
+    if (n < 0 || w <= 0 || h <= 0) { set_error("psfm_traj_optimize: bad sizes"); return PSFM_ERR_INVALID; }
+    if (n == 0) return PSFM_OK;
+    int rc = require_device("psfm_traj_optimize_device");
+    if (rc != PSFM_OK) return rc;
+    return traj::solve_device(d_uv12, d_ref1, d_ref2, d_scale, d_flow12, n, w, h, opts, d_out_uv12, summary,
+                              (cudaStream_t)stream);
+  });
 }
 
 extern "C" int psfm_traj_optimize(const double* uv12, const double* ref1, const double* ref2, const double* scale,
                                   const float* flow12, int32_t n, int32_t w, int32_t h,
                                   const psfm_traj_options* opts, double* out_uv12, psfm_traj_summary* summary) {
-  if (summary) memset(summary, 0, sizeof(*summary));
-  if (n < 0 || w <= 0 || h <= 0) { set_error("psfm_traj_optimize: bad sizes"); return PSFM_ERR_INVALID; }
-  if (n == 0) return PSFM_OK;
-  int rc = require_device("psfm_traj_optimize");
-  if (rc != PSFM_OK) return rc;
-  traj::Workspace& ws = traj::g_ws;
-  std::lock_guard<std::mutex> lock(ws.mu);
-  const auto t0 = std::chrono::steady_clock::now();
-  try {
+  return guard("psfm_traj_optimize", [&]() -> int {
+    if (summary) memset(summary, 0, sizeof(*summary));
+    if (n < 0 || w <= 0 || h <= 0) { set_error("psfm_traj_optimize: bad sizes"); return PSFM_ERR_INVALID; }
+    if (n == 0) return PSFM_OK;
+    int rc = require_device("psfm_traj_optimize");
+    if (rc != PSFM_OK) return rc;
+    traj::Workspace& ws = traj::g_ws;
+    std::lock_guard<std::mutex> lock(ws.mu);
+    const auto t0 = std::chrono::steady_clock::now();
     ws.ensure((size_t)n, (size_t)(n + traj::CH - 1) / traj::CH);
     const size_t nf = 2 * (size_t)w * h;
     if (nf > ws.cap_flow) { ws.flow.alloc(nf); ws.cap_flow = nf; }
@@ -634,10 +632,8 @@ extern "C" int psfm_traj_optimize(const double* uv12, const double* ref1, const 
     if (rc != PSFM_OK) return rc;
     PSFM_CUDA(cudaMemcpyAsync(out_uv12, ws.out.p, sizeof(double) * 4 * (size_t)n, cudaMemcpyDeviceToHost, st));
     PSFM_CUDA(cudaStreamSynchronize(st));
-  } catch (const CudaFail& f) {
-    return f.code;
-  }
-  if (summary)
-    summary->total_ms = 1e3 * std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-  return PSFM_OK;
+    if (summary)
+      summary->total_ms = 1e3 * std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    return PSFM_OK;
+  });
 }

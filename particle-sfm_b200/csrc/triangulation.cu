@@ -688,79 +688,79 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
                                          const double* orientations, const double* image_tvec, const uint8_t* registered,
                                          const psfm_triangulator_options* opts, psfm_triangulation** out,
                                          int64_t* num_points3D, int64_t* num_track_elements) {
-  const auto t0 = std::chrono::steady_clock::now();
-  const long long launches0 = g_launch_count.load();
-  const char* entry = "psfm_triangulation_create";
-  if (!out) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  *out = nullptr;
-  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
-  if (rc != PSFM_OK) return rc;
-  if (!keypoint_ptr || (num_images > 0 && (!image_camera || !orientations || !image_tvec || !registered)) ||
-      (num_cameras > 0 && (!cameras || !camera_size)) || (num_pairs > 0 && (!pair_images || !inlier_ptr)))
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  psfm_triangulator_options o;
-  psfm_triangulator_default_options(&o);
-  if (opts) o = *opts;
-  if (!(o.max_transitivity >= 0 && o.create_max_angle_error > 0 && o.continue_max_angle_error > 0 && o.min_angle > 0 &&
-        o.min_focal_length_ratio > 0 && o.max_focal_length_ratio > 0 && o.max_extra_param >= 0 &&
-        std::isfinite(o.create_max_angle_error) && std::isfinite(o.continue_max_angle_error) && std::isfinite(o.min_angle) &&
-        std::isfinite(o.min_focal_length_ratio) && std::isfinite(o.max_focal_length_ratio) && std::isfinite(o.max_extra_param)))
-    return fail(entry, PSFM_ERR_INVALID, "options fail the IncrementalTriangulator::Options Check()");
-  if (o.max_transitivity != 1) return fail(entry, PSFM_ERR_UNSUPPORTED, "max_transitivity != 1 is not supported");
-  const int F = num_images, R = (int)num_pairs;
-  if ((rc = check_keypoint_ptr(entry, F, keypoint_ptr)) != PSFM_OK) return rc;
-  const long long K = keypoint_ptr[F];
-  if (K >= 0x7fffffffLL) return fail(entry, PSFM_ERR_UNSUPPORTED, "2^31 - 1 keypoints or more");
-  if (K > 0 && !keypoints) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if ((rc = check_image_cameras(entry, F, image_camera, num_cameras)) != PSFM_OK) return rc;
-  if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
-  if (R > 0) {
-    if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
-    if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
-    if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
-    if (inlier_ptr[R] > 0 && !inlier_matches) return fail(entry, PSFM_ERR_INVALID, "null argument");
-    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
-  }
-  // per image: P = [R | t], the projection centre -R' t, qvec, tvec; eligible = registered with a non-bogus camera
-  // (Camera::HasBogusParams, SIMPLE_PINHOLE: principal point in [0, w] x [0, h], f / max(w, h) in the ratio range)
-  std::vector<double> img((size_t)kImg * F, 0.0);
-  std::vector<unsigned char> elig(F, 0);
-  for (int f = 0; f < F; ++f) {
-    if (!registered[f]) continue;
-    const double* q = orientations + 4 * (size_t)f;
-    const double* t = image_tvec + 3 * (size_t)f;
-    for (int i = 0; i < 4; ++i)
-      if (!std::isfinite(q[i])) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
-    for (int i = 0; i < 3; ++i)
-      if (!std::isfinite(t[i])) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
-    const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-    if (!(n > 0.0)) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
-    const double w = q[0] / n, x = q[1] / n, y = q[2] / n, z = q[3] / n;
-    const double Rm[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y),
-                          2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x),
-                          2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)};
-    double* T = img.data() + (size_t)kImg * f;
-    for (int r = 0; r < 3; ++r) {
-      for (int cc = 0; cc < 3; ++cc) T[4 * r + cc] = Rm[3 * r + cc];
-      T[4 * r + 3] = t[r];
+  return guard("psfm_triangulation_create", [&]() -> int {
+    const auto t0 = std::chrono::steady_clock::now();
+    const long long launches0 = g_launch_count.load();
+    const char* entry = "psfm_triangulation_create";
+    if (!out) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    *out = nullptr;
+    int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+    if (rc != PSFM_OK) return rc;
+    if (!keypoint_ptr || (num_images > 0 && (!image_camera || !orientations || !image_tvec || !registered)) ||
+        (num_cameras > 0 && (!cameras || !camera_size)) || (num_pairs > 0 && (!pair_images || !inlier_ptr)))
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    psfm_triangulator_options o;
+    psfm_triangulator_default_options(&o);
+    if (opts) o = *opts;
+    if (!(o.max_transitivity >= 0 && o.create_max_angle_error > 0 && o.continue_max_angle_error > 0 && o.min_angle > 0 &&
+          o.min_focal_length_ratio > 0 && o.max_focal_length_ratio > 0 && o.max_extra_param >= 0 &&
+          std::isfinite(o.create_max_angle_error) && std::isfinite(o.continue_max_angle_error) && std::isfinite(o.min_angle) &&
+          std::isfinite(o.min_focal_length_ratio) && std::isfinite(o.max_focal_length_ratio) && std::isfinite(o.max_extra_param)))
+      return fail(entry, PSFM_ERR_INVALID, "options fail the IncrementalTriangulator::Options Check()");
+    if (o.max_transitivity != 1) return fail(entry, PSFM_ERR_UNSUPPORTED, "max_transitivity != 1 is not supported");
+    const int F = num_images, R = (int)num_pairs;
+    if ((rc = check_keypoint_ptr(entry, F, keypoint_ptr)) != PSFM_OK) return rc;
+    const long long K = keypoint_ptr[F];
+    if (K >= 0x7fffffffLL) return fail(entry, PSFM_ERR_UNSUPPORTED, "2^31 - 1 keypoints or more");
+    if (K > 0 && !keypoints) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if ((rc = check_image_cameras(entry, F, image_camera, num_cameras)) != PSFM_OK) return rc;
+    if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
+    if (R > 0) {
+      if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
+      if ((rc = check_pair_images(entry, R, pair_images, F)) != PSFM_OK) return rc;
+      if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
+      if (inlier_ptr[R] > 0 && !inlier_matches) return fail(entry, PSFM_ERR_INVALID, "null argument");
+      if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
     }
-    for (int cc = 0; cc < 3; ++cc) T[12 + cc] = -(Rm[cc] * t[0] + Rm[3 + cc] * t[1] + Rm[6 + cc] * t[2]);
-    for (int i = 0; i < 4; ++i) T[15 + i] = q[i];
-    for (int i = 0; i < 3; ++i) T[19 + i] = t[i];
-    const int cam = image_camera[f];
-    const double fl = cameras[3 * cam], cx = cameras[3 * cam + 1], cy = cameras[3 * cam + 2];
-    const double wd = camera_size[2 * cam], ht = camera_size[2 * cam + 1];
-    const bool bogus_pp = cx < 0 || cx > wd || cy < 0 || cy > ht;
-    const double ratio = fl / std::max(wd, ht);
-    elig[f] = !(bogus_pp || ratio < o.min_focal_length_ratio || ratio > o.max_focal_length_ratio);
-  }
-  if ((rc = require_device(entry)) != PSFM_OK) return rc;
-  const long long N = R > 0 ? inlier_ptr[R] : 0, E = 2 * N;
-  psfm_triangulation_summary sm;
-  memset(&sm, 0, sizeof(sm));
-  sm.host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  auto h = new psfm_triangulation();
-  try {
+    // per image: P = [R | t], the projection centre -R' t, qvec, tvec; eligible = registered with a non-bogus camera
+    // (Camera::HasBogusParams, SIMPLE_PINHOLE: principal point in [0, w] x [0, h], f / max(w, h) in the ratio range)
+    std::vector<double> img((size_t)kImg * F, 0.0);
+    std::vector<unsigned char> elig(F, 0);
+    for (int f = 0; f < F; ++f) {
+      if (!registered[f]) continue;
+      const double* q = orientations + 4 * (size_t)f;
+      const double* t = image_tvec + 3 * (size_t)f;
+      for (int i = 0; i < 4; ++i)
+        if (!std::isfinite(q[i])) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
+      for (int i = 0; i < 3; ++i)
+        if (!std::isfinite(t[i])) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
+      const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+      if (!(n > 0.0)) return fail(entry, PSFM_ERR_INVALID, "a registered image with a non-finite pose");
+      const double w = q[0] / n, x = q[1] / n, y = q[2] / n, z = q[3] / n;
+      const double Rm[9] = {1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y),
+                            2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x),
+                            2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)};
+      double* T = img.data() + (size_t)kImg * f;
+      for (int r = 0; r < 3; ++r) {
+        for (int cc = 0; cc < 3; ++cc) T[4 * r + cc] = Rm[3 * r + cc];
+        T[4 * r + 3] = t[r];
+      }
+      for (int cc = 0; cc < 3; ++cc) T[12 + cc] = -(Rm[cc] * t[0] + Rm[3 + cc] * t[1] + Rm[6 + cc] * t[2]);
+      for (int i = 0; i < 4; ++i) T[15 + i] = q[i];
+      for (int i = 0; i < 3; ++i) T[19 + i] = t[i];
+      const int cam = image_camera[f];
+      const double fl = cameras[3 * cam], cx = cameras[3 * cam + 1], cy = cameras[3 * cam + 2];
+      const double wd = camera_size[2 * cam], ht = camera_size[2 * cam + 1];
+      const bool bogus_pp = cx < 0 || cx > wd || cy < 0 || cy > ht;
+      const double ratio = fl / std::max(wd, ht);
+      elig[f] = !(bogus_pp || ratio < o.min_focal_length_ratio || ratio > o.max_focal_length_ratio);
+    }
+    if ((rc = require_device(entry)) != PSFM_OK) return rc;
+    const long long N = R > 0 ? inlier_ptr[R] : 0, E = 2 * N;
+    psfm_triangulation_summary sm;
+    memset(&sm, 0, sizeof(sm));
+    sm.host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    std::unique_ptr<psfm_triangulation> h(new psfm_triangulation());
     Event ev[5];
     // the keypoints, their images and keypoint_ptr stay with the handle for psfm_ba_create_from_triangulation
     DBuf<long long>& d_kp_ptr = h->kp_ptr;
@@ -925,35 +925,32 @@ extern "C" int psfm_triangulation_create(int32_t num_images, const int64_t* keyp
     sm.num_ransac_trials = (long long)cnt_h[kCntTrials];
     sm.num_local_estimates = (long long)cnt_h[kCntLocal];
     h->P = P; h->E = NE; h->K = K;
-  } catch (const CudaFail& f) {
-    delete h;
-    return f.code;
-  }
-  sm.num_launches = g_launch_count.load() - launches0;
-  h->summary = sm;
-  *out = h;
-  if (num_points3D) *num_points3D = h->P;
-  if (num_track_elements) *num_track_elements = h->E;
-  return PSFM_OK;
+    sm.num_launches = g_launch_count.load() - launches0;
+    h->summary = sm;
+    if (num_points3D) *num_points3D = h->P;
+    if (num_track_elements) *num_track_elements = h->E;
+    *out = h.release();
+    return PSFM_OK;
+  });
 }
 
 extern "C" int psfm_triangulation_result(const psfm_triangulation* h, double* xyz, int64_t* track_ptr, int32_t* track_image,
                                          int32_t* track_point2D, int64_t* point3D_of_keypoint,
                                          psfm_triangulation_summary* summary) {
-  if (!h) {
-    set_error("psfm_triangulation_result: null handle");
-    return PSFM_ERR_INVALID;
-  }
-  try {
+  return guard("psfm_triangulation_result", [&]() -> int {
+    if (!h) {
+      set_error("psfm_triangulation_result: null handle");
+      return PSFM_ERR_INVALID;
+    }
     if (xyz && h->P) PSFM_CUDA(cudaMemcpy(xyz, h->xyz.p, sizeof(double) * 3 * (size_t)h->P, cudaMemcpyDeviceToHost));
     if (track_ptr) PSFM_CUDA(cudaMemcpy(track_ptr, h->track_ptr.p, sizeof(int64_t) * (size_t)(h->P + 1), cudaMemcpyDeviceToHost));
     if (track_image && h->E) PSFM_CUDA(cudaMemcpy(track_image, h->track_image.p, sizeof(int32_t) * (size_t)h->E, cudaMemcpyDeviceToHost));
     if (track_point2D && h->E) PSFM_CUDA(cudaMemcpy(track_point2D, h->track_p2d.p, sizeof(int32_t) * (size_t)h->E, cudaMemcpyDeviceToHost));
     if (point3D_of_keypoint && h->K)
       PSFM_CUDA(cudaMemcpy(point3D_of_keypoint, h->kp_points.p, sizeof(int64_t) * (size_t)h->K, cudaMemcpyDeviceToHost));
-  } catch (const CudaFail& f) { return f.code; }
-  if (summary) *summary = h->summary;
-  return PSFM_OK;
+    if (summary) *summary = h->summary;
+    return PSFM_OK;
+  });
 }
 
 extern "C" void psfm_triangulation_destroy(psfm_triangulation* h) { delete h; }

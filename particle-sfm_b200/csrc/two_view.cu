@@ -457,26 +457,26 @@ extern "C" int psfm_two_view_relative_poses(int32_t num_images, const int64_t* k
                                             const uint32_t* inlier_matches, double* qvec, double* tvec, double* tri_angle,
                                             int32_t* config_out, int64_t* num_points3D, uint8_t* estimated) {
   const char* entry = "psfm_two_view_relative_poses";
-  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
-  if (rc != PSFM_OK) return rc;
-  if (num_pairs > 0 && (!keypoint_ptr || !image_camera || !cameras || !pair_images || !config || !E || !F || !H ||
-                        !inlier_ptr || !qvec || !tvec || !tri_angle || !config_out || !num_points3D || !estimated))
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  const int R = (int)num_pairs;
-  if (R > 0) {
-    // no check_distinct_pairs: this stage accepts self pairs and repeated pairs
-    if ((rc = check_keypoint_ptr(entry, num_images, keypoint_ptr)) != PSFM_OK) return rc;
-    if ((rc = check_image_cameras(entry, num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
-    if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
-    if ((rc = check_pair_images(entry, R, pair_images, num_images)) != PSFM_OK) return rc;
-    if (inlier_ptr[R] > 0 && (!inlier_matches || (keypoint_ptr[num_images] > 0 && !keypoints)))
+  return guard(entry, [&]() -> int {
+    int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+    if (rc != PSFM_OK) return rc;
+    if (num_pairs > 0 && (!keypoint_ptr || !image_camera || !cameras || !pair_images || !config || !E || !F || !H ||
+                          !inlier_ptr || !qvec || !tvec || !tri_angle || !config_out || !num_points3D || !estimated))
       return fail(entry, PSFM_ERR_INVALID, "null argument");
-    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
-  }
-  if ((rc = require_device(entry)) != PSFM_OK) return rc;
-  if (R == 0) return PSFM_OK;
-  const long long N = inlier_ptr[R], K = keypoint_ptr[num_images];
-  try {
+    const int R = (int)num_pairs;
+    if (R > 0) {
+      // no check_distinct_pairs: this stage accepts self pairs and repeated pairs
+      if ((rc = check_keypoint_ptr(entry, num_images, keypoint_ptr)) != PSFM_OK) return rc;
+      if ((rc = check_image_cameras(entry, num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
+      if ((rc = check_match_ptr(entry, "inlier_ptr", R, inlier_ptr)) != PSFM_OK) return rc;
+      if ((rc = check_pair_images(entry, R, pair_images, num_images)) != PSFM_OK) return rc;
+      if (inlier_ptr[R] > 0 && (!inlier_matches || (keypoint_ptr[num_images] > 0 && !keypoints)))
+        return fail(entry, PSFM_ERR_INVALID, "null argument");
+      if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, inlier_ptr, inlier_matches)) != PSFM_OK) return rc;
+    }
+    if ((rc = require_device(entry)) != PSFM_OK) return rc;
+    if (R == 0) return PSFM_OK;
+    const long long N = inlier_ptr[R], K = keypoint_ptr[num_images];
     DBuf<int> d_pairs, d_config, d_cam, d_ncand, d_chosen, d_cfg_out;
     DBuf<double> d_cams, d_E, d_F, d_H, d_cand, d_q, d_t, d_tri;
     DBuf<long long> d_iptr, d_kp_ptr, d_np3;
@@ -546,5 +546,5 @@ extern "C" int psfm_two_view_relative_poses(int32_t num_images, const int64_t* k
     PSFM_LAUNCH_CHECK();
     PSFM_CUDA(cudaMemcpy(tri_angle, d_tri.p, sizeof(double) * (size_t)R, cudaMemcpyDeviceToHost));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }

@@ -829,90 +829,86 @@ int verify_graph(const char* entry, std::chrono::steady_clock::time_point t0, lo
       sizes[4 * p + 2 * k + 1] = camera_size[2 * c + 1];
     }
   sm.host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  try {
-    Event ev[4];
-    DBuf<long long> up_kp_ptr, up_mptr, d_iptr, d_count;
-    DBuf<float2> up_kps;
-    DBuf<int2> up_pairs, d_sizes;
-    DBuf<uint2> up_m, d_out;
-    DBuf<float4> d_pts;
-    DBuf<int> d_inl, d_config, d_trials, d_rounds;
-    DBuf<double> d_F, d_H;
-    const long long *kp_ptr, *mptr;
-    const float2* kps;
-    const int2* pairs;
-    const uint2* m;
-    if (g.table) {
-      kp_ptr = g.table->d_keypoint_ptr.p; kps = g.table->keypoints.p; mptr = g.table->d_match_ptr.p;
-      pairs = g.table->pairs.p; m = g.table->matches.p;
-    } else {
-      up_kp_ptr.alloc(g.num_images + 1); up_kps.alloc(g.K); up_mptr.alloc(R + 1); up_pairs.alloc(R); up_m.alloc(M);
-      up_kp_ptr.upload(reinterpret_cast<const long long*>(g.keypoint_ptr), g.num_images + 1, nullptr);
-      up_kps.upload(reinterpret_cast<const float2*>(g.keypoints), g.K, nullptr);
-      up_mptr.upload(reinterpret_cast<const long long*>(g.match_ptr), R + 1, nullptr);
-      up_pairs.upload(reinterpret_cast<const int2*>(g.pair_images), R, nullptr);
-      up_m.upload(reinterpret_cast<const uint2*>(g.matches), M, nullptr);
-      kp_ptr = up_kp_ptr.p; kps = up_kps.p; mptr = up_mptr.p; pairs = up_pairs.p; m = up_m.p;
-    }
-    d_iptr.alloc(R + 1); d_count.alloc(R); d_sizes.alloc(2 * (size_t)R); d_pts.alloc(M); d_inl.alloc(M);
-    d_config.alloc(R); d_trials.alloc(3 * (size_t)R); d_rounds.alloc(3 * (size_t)R); d_F.alloc(9 * (size_t)R);
-    d_H.alloc(9 * (size_t)R);
-    d_sizes.upload(reinterpret_cast<const int2*>(sizes.data()), 2 * (size_t)R, nullptr);
-    PSFM_CUDA(cudaEventRecord(ev[0], nullptr));
-    k_gather<<<R, 256>>>(R, mptr, pairs, kp_ptr, kps, m, d_pts.p);
-    PSFM_LAUNCH_CHECK();
-    PSFM_CUDA(cudaEventRecord(ev[1], nullptr));
-    Args a;
-    a.R = R; a.mptr = mptr; a.pts = d_pts.p; a.sizes = d_sizes.p; a.inl_idx = d_inl.p; a.config = d_config.p;
-    a.F = d_F.p; a.H = d_H.p; a.count = d_count.p; a.trials = d_trials.p; a.rounds = d_rounds.p;
-    a.thr = o.max_error * o.max_error;
-    a.confidence = o.confidence; a.multiplier = o.dyn_num_trials_multiplier;
-    const int ks[3] = {kSevenPointSamples, kHomographySamples, kTranslationSamples};
-    for (int k = 0; k < 3; ++k) {
-      const double ratio = k == kKindW ? o.watermark_min_inlier_ratio : o.min_inlier_ratio;
-      const long long cap = compute_num_trials((long long)(ratio * kCapNumSamples), kCapNumSamples, ks[k], o.confidence,
-                                               o.dyn_num_trials_multiplier);
-      a.max_trials[k] = std::min<long long>(o.max_num_trials, cap);
-    }
-    a.min_trials = o.min_num_trials; a.min_num_inliers = o.min_num_inliers; a.max_H_ratio = o.max_H_inlier_ratio;
-    a.detect_watermark = o.detect_watermark != 0; a.wm_ratio = o.watermark_min_inlier_ratio;
-    a.wm_border = o.watermark_border_size; a.seed = (u64)o.random_seed;
-    k_verify<<<R, kThreads>>>(a);
-    PSFM_LAUNCH_CHECK();
-    PSFM_CUDA(cudaEventRecord(ev[2], nullptr));
-    std::vector<long long> cnt(R);
-    PSFM_CUDA(cudaMemcpy(cnt.data(), d_count.p, sizeof(long long) * R, cudaMemcpyDeviceToHost));
-    for (int p = 0; p < R; ++p) inlier_ptr[p + 1] = inlier_ptr[p] + cnt[p];
-    const long long N = inlier_ptr[R];
-    d_iptr.upload(reinterpret_cast<const long long*>(inlier_ptr), R + 1, nullptr);
-    d_out.alloc(N);
-    k_compact<<<R, 256>>>(R, mptr, d_iptr.p, d_inl.p, m, d_out.p);
-    PSFM_LAUNCH_CHECK();
-    PSFM_CUDA(cudaEventRecord(ev[3], nullptr));
-    PSFM_CUDA(cudaEventSynchronize(ev[3]));
-    if (N) PSFM_CUDA(cudaMemcpy(inlier_matches, d_out.p, sizeof(uint2) * N, cudaMemcpyDeviceToHost));
-    PSFM_CUDA(cudaMemcpy(config, d_config.p, sizeof(int) * R, cudaMemcpyDeviceToHost));
-    PSFM_CUDA(cudaMemcpy(F, d_F.p, sizeof(double) * 9 * R, cudaMemcpyDeviceToHost));
-    PSFM_CUDA(cudaMemcpy(H, d_H.p, sizeof(double) * 9 * R, cudaMemcpyDeviceToHost));
-    memset(E, 0, sizeof(double) * 9 * (size_t)R);
-    std::vector<int> tr(3 * (size_t)R), rd(3 * (size_t)R);
-    PSFM_CUDA(cudaMemcpy(tr.data(), d_trials.p, sizeof(int) * 3 * R, cudaMemcpyDeviceToHost));
-    PSFM_CUDA(cudaMemcpy(rd.data(), d_rounds.p, sizeof(int) * 3 * R, cudaMemcpyDeviceToHost));
-    if (pair_trials) memcpy(pair_trials, tr.data(), sizeof(int) * 3 * (size_t)R);
-    for (int p = 0; p < R; ++p) {
-      for (int k = 0; k < 3; ++k) {
-        sm.num_trials[k] += tr[3 * p + k];
-        sm.num_local_rounds[k] += rd[3 * p + k];
-      }
-      if (config[p] >= 0 && config[p] < 8) sm.num_config[config[p]] += 1;
-    }
-    for (int k = 0; k < 3; ++k) sm.num_trials_scored[k] = sm.num_trials[k];
-    float ms[3];
-    for (int i = 0; i < 3; ++i) PSFM_CUDA(cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]));
-    sm.gather_ms = ms[0]; sm.ransac_ms = ms[1]; sm.compact_ms = ms[2];
-  } catch (const CudaFail& f) {
-    return f.code;
+  Event ev[4];
+  DBuf<long long> up_kp_ptr, up_mptr, d_iptr, d_count;
+  DBuf<float2> up_kps;
+  DBuf<int2> up_pairs, d_sizes;
+  DBuf<uint2> up_m, d_out;
+  DBuf<float4> d_pts;
+  DBuf<int> d_inl, d_config, d_trials, d_rounds;
+  DBuf<double> d_F, d_H;
+  const long long *kp_ptr, *mptr;
+  const float2* kps;
+  const int2* pairs;
+  const uint2* m;
+  if (g.table) {
+    kp_ptr = g.table->d_keypoint_ptr.p; kps = g.table->keypoints.p; mptr = g.table->d_match_ptr.p;
+    pairs = g.table->pairs.p; m = g.table->matches.p;
+  } else {
+    up_kp_ptr.alloc(g.num_images + 1); up_kps.alloc(g.K); up_mptr.alloc(R + 1); up_pairs.alloc(R); up_m.alloc(M);
+    up_kp_ptr.upload(reinterpret_cast<const long long*>(g.keypoint_ptr), g.num_images + 1, nullptr);
+    up_kps.upload(reinterpret_cast<const float2*>(g.keypoints), g.K, nullptr);
+    up_mptr.upload(reinterpret_cast<const long long*>(g.match_ptr), R + 1, nullptr);
+    up_pairs.upload(reinterpret_cast<const int2*>(g.pair_images), R, nullptr);
+    up_m.upload(reinterpret_cast<const uint2*>(g.matches), M, nullptr);
+    kp_ptr = up_kp_ptr.p; kps = up_kps.p; mptr = up_mptr.p; pairs = up_pairs.p; m = up_m.p;
   }
+  d_iptr.alloc(R + 1); d_count.alloc(R); d_sizes.alloc(2 * (size_t)R); d_pts.alloc(M); d_inl.alloc(M);
+  d_config.alloc(R); d_trials.alloc(3 * (size_t)R); d_rounds.alloc(3 * (size_t)R); d_F.alloc(9 * (size_t)R);
+  d_H.alloc(9 * (size_t)R);
+  d_sizes.upload(reinterpret_cast<const int2*>(sizes.data()), 2 * (size_t)R, nullptr);
+  PSFM_CUDA(cudaEventRecord(ev[0], nullptr));
+  k_gather<<<R, 256>>>(R, mptr, pairs, kp_ptr, kps, m, d_pts.p);
+  PSFM_LAUNCH_CHECK();
+  PSFM_CUDA(cudaEventRecord(ev[1], nullptr));
+  Args a;
+  a.R = R; a.mptr = mptr; a.pts = d_pts.p; a.sizes = d_sizes.p; a.inl_idx = d_inl.p; a.config = d_config.p;
+  a.F = d_F.p; a.H = d_H.p; a.count = d_count.p; a.trials = d_trials.p; a.rounds = d_rounds.p;
+  a.thr = o.max_error * o.max_error;
+  a.confidence = o.confidence; a.multiplier = o.dyn_num_trials_multiplier;
+  const int ks[3] = {kSevenPointSamples, kHomographySamples, kTranslationSamples};
+  for (int k = 0; k < 3; ++k) {
+    const double ratio = k == kKindW ? o.watermark_min_inlier_ratio : o.min_inlier_ratio;
+    const long long cap = compute_num_trials((long long)(ratio * kCapNumSamples), kCapNumSamples, ks[k], o.confidence,
+                                             o.dyn_num_trials_multiplier);
+    a.max_trials[k] = std::min<long long>(o.max_num_trials, cap);
+  }
+  a.min_trials = o.min_num_trials; a.min_num_inliers = o.min_num_inliers; a.max_H_ratio = o.max_H_inlier_ratio;
+  a.detect_watermark = o.detect_watermark != 0; a.wm_ratio = o.watermark_min_inlier_ratio;
+  a.wm_border = o.watermark_border_size; a.seed = (u64)o.random_seed;
+  k_verify<<<R, kThreads>>>(a);
+  PSFM_LAUNCH_CHECK();
+  PSFM_CUDA(cudaEventRecord(ev[2], nullptr));
+  std::vector<long long> cnt(R);
+  PSFM_CUDA(cudaMemcpy(cnt.data(), d_count.p, sizeof(long long) * R, cudaMemcpyDeviceToHost));
+  for (int p = 0; p < R; ++p) inlier_ptr[p + 1] = inlier_ptr[p] + cnt[p];
+  const long long N = inlier_ptr[R];
+  d_iptr.upload(reinterpret_cast<const long long*>(inlier_ptr), R + 1, nullptr);
+  d_out.alloc(N);
+  k_compact<<<R, 256>>>(R, mptr, d_iptr.p, d_inl.p, m, d_out.p);
+  PSFM_LAUNCH_CHECK();
+  PSFM_CUDA(cudaEventRecord(ev[3], nullptr));
+  PSFM_CUDA(cudaEventSynchronize(ev[3]));
+  if (N) PSFM_CUDA(cudaMemcpy(inlier_matches, d_out.p, sizeof(uint2) * N, cudaMemcpyDeviceToHost));
+  PSFM_CUDA(cudaMemcpy(config, d_config.p, sizeof(int) * R, cudaMemcpyDeviceToHost));
+  PSFM_CUDA(cudaMemcpy(F, d_F.p, sizeof(double) * 9 * R, cudaMemcpyDeviceToHost));
+  PSFM_CUDA(cudaMemcpy(H, d_H.p, sizeof(double) * 9 * R, cudaMemcpyDeviceToHost));
+  memset(E, 0, sizeof(double) * 9 * (size_t)R);
+  std::vector<int> tr(3 * (size_t)R), rd(3 * (size_t)R);
+  PSFM_CUDA(cudaMemcpy(tr.data(), d_trials.p, sizeof(int) * 3 * R, cudaMemcpyDeviceToHost));
+  PSFM_CUDA(cudaMemcpy(rd.data(), d_rounds.p, sizeof(int) * 3 * R, cudaMemcpyDeviceToHost));
+  if (pair_trials) memcpy(pair_trials, tr.data(), sizeof(int) * 3 * (size_t)R);
+  for (int p = 0; p < R; ++p) {
+    for (int k = 0; k < 3; ++k) {
+      sm.num_trials[k] += tr[3 * p + k];
+      sm.num_local_rounds[k] += rd[3 * p + k];
+    }
+    if (config[p] >= 0 && config[p] < 8) sm.num_config[config[p]] += 1;
+  }
+  for (int k = 0; k < 3; ++k) sm.num_trials_scored[k] = sm.num_trials[k];
+  float ms[3];
+  for (int i = 0; i < 3; ++i) PSFM_CUDA(cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]));
+  sm.gather_ms = ms[0]; sm.ransac_ms = ms[1]; sm.compact_ms = ms[2];
   sm.num_launches = g_launch_count.load() - launches0;
   if (summary) *summary = sm;
   return PSFM_OK;
@@ -927,41 +923,43 @@ extern "C" int psfm_verify_two_view_geometries(int32_t num_images, const int64_t
                                                const psfm_verification_options* opts, int32_t* config, double* F, double* E,
                                                double* H, int64_t* inlier_ptr, uint32_t* inlier_matches,
                                                int32_t* pair_trials, psfm_verification_summary* summary) {
-  const auto t0 = std::chrono::steady_clock::now();
-  const long long launches0 = g_launch_count.load();
-  const char* entry = "psfm_verify_two_view_geometries";
-  int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
-  if (rc != PSFM_OK) return rc;
-  if (!keypoint_ptr || (num_images > 0 && !image_camera) || (num_cameras > 0 && !camera_size) ||
-      (num_pairs > 0 && (!pair_images || !match_ptr || !config || !F || !E || !H)) || !inlier_ptr)
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  psfm_verification_options o;
-  if ((rc = check_options(entry, opts, &o)) != PSFM_OK) return rc;
-  const int Fimg = num_images, R = (int)num_pairs;
-  if ((rc = check_keypoint_ptr(entry, Fimg, keypoint_ptr)) != PSFM_OK) return rc;
-  const long long K = keypoint_ptr[Fimg];
-  if (K > 0 && !keypoints) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if ((rc = check_image_cameras(entry, Fimg, image_camera, num_cameras)) != PSFM_OK) return rc;
-  if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
-  long long M = 0;
-  if (R > 0) {
-    if ((rc = check_match_ptr(entry, "match_ptr", R, match_ptr)) != PSFM_OK) return rc;
-    for (int p = 0; p < R; ++p)
-      if (match_ptr[p + 1] - match_ptr[p] > 0x7fffffffLL)
-        return fail(entry, PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
-    if ((rc = check_pair_images(entry, R, pair_images, Fimg)) != PSFM_OK) return rc;
-    if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
-    M = match_ptr[R];
-    if (M > 0 && (!matches || !inlier_matches)) return fail(entry, PSFM_ERR_INVALID, "null argument");
-    if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, match_ptr, matches)) != PSFM_OK) return rc;
-    if ((rc = check_prior_focal_length(entry, R, pair_images, image_camera, prior_focal_length)) != PSFM_OK) return rc;
-  }
-  Graph g;
-  g.num_images = Fimg; g.R = R; g.K = K; g.M = M;
-  g.keypoint_ptr = keypoint_ptr; g.keypoints = keypoints; g.pair_images = pair_images; g.match_ptr = match_ptr;
-  g.matches = matches;
-  return verify_graph(entry, t0, launches0, g, image_camera, camera_size, o, config, F, E, H, inlier_ptr, inlier_matches,
-                      pair_trials, summary);
+  return guard("psfm_verify_two_view_geometries", [&]() -> int {
+    const auto t0 = std::chrono::steady_clock::now();
+    const long long launches0 = g_launch_count.load();
+    const char* entry = "psfm_verify_two_view_geometries";
+    int rc = check_sizes(entry, num_images, num_cameras, num_pairs);
+    if (rc != PSFM_OK) return rc;
+    if (!keypoint_ptr || (num_images > 0 && !image_camera) || (num_cameras > 0 && !camera_size) ||
+        (num_pairs > 0 && (!pair_images || !match_ptr || !config || !F || !E || !H)) || !inlier_ptr)
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    psfm_verification_options o;
+    if ((rc = check_options(entry, opts, &o)) != PSFM_OK) return rc;
+    const int Fimg = num_images, R = (int)num_pairs;
+    if ((rc = check_keypoint_ptr(entry, Fimg, keypoint_ptr)) != PSFM_OK) return rc;
+    const long long K = keypoint_ptr[Fimg];
+    if (K > 0 && !keypoints) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if ((rc = check_image_cameras(entry, Fimg, image_camera, num_cameras)) != PSFM_OK) return rc;
+    if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
+    long long M = 0;
+    if (R > 0) {
+      if ((rc = check_match_ptr(entry, "match_ptr", R, match_ptr)) != PSFM_OK) return rc;
+      for (int p = 0; p < R; ++p)
+        if (match_ptr[p + 1] - match_ptr[p] > 0x7fffffffLL)
+          return fail(entry, PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
+      if ((rc = check_pair_images(entry, R, pair_images, Fimg)) != PSFM_OK) return rc;
+      if ((rc = check_distinct_pairs(entry, R, pair_images)) != PSFM_OK) return rc;
+      M = match_ptr[R];
+      if (M > 0 && (!matches || !inlier_matches)) return fail(entry, PSFM_ERR_INVALID, "null argument");
+      if ((rc = check_match_keypoints(entry, R, pair_images, keypoint_ptr, match_ptr, matches)) != PSFM_OK) return rc;
+      if ((rc = check_prior_focal_length(entry, R, pair_images, image_camera, prior_focal_length)) != PSFM_OK) return rc;
+    }
+    Graph g;
+    g.num_images = Fimg; g.R = R; g.K = K; g.M = M;
+    g.keypoint_ptr = keypoint_ptr; g.keypoints = keypoints; g.pair_images = pair_images; g.match_ptr = match_ptr;
+    g.matches = matches;
+    return verify_graph(entry, t0, launches0, g, image_camera, camera_size, o, config, F, E, H, inlier_ptr, inlier_matches,
+                        pair_trials, summary);
+  });
 }
 
 extern "C" int psfm_match_table_verify(const psfm_match_table* t, const int32_t* image_camera, int32_t num_cameras,
@@ -969,46 +967,48 @@ extern "C" int psfm_match_table_verify(const psfm_match_table* t, const int32_t*
                                        const psfm_verification_options* opts, int32_t* config, double* F, double* E,
                                        double* H, int64_t* inlier_ptr, uint32_t* inlier_matches, int32_t* pair_trials,
                                        psfm_verification_summary* summary) {
-  const auto t0 = std::chrono::steady_clock::now();
-  const long long launches0 = g_launch_count.load();
-  const char* entry = "psfm_match_table_verify";
-  if (!t) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  int rc = check_sizes(entry, t->num_images, num_cameras, t->num_pairs);
-  if (rc != PSFM_OK) return rc;
-  const int R = (int)t->num_pairs;
-  if ((t->num_images > 0 && !image_camera) || (num_cameras > 0 && !camera_size) ||
-      (R > 0 && (!config || !F || !E || !H)) || !inlier_ptr || (t->num_matches > 0 && !inlier_matches))
-    return fail(entry, PSFM_ERR_INVALID, "null argument");
-  psfm_verification_options o;
-  if ((rc = check_options(entry, opts, &o)) != PSFM_OK) return rc;
-  if ((rc = check_image_cameras(entry, t->num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
-  if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
-  for (int p = 0; p < R; ++p)
-    if (t->match_ptr[p + 1] - t->match_ptr[p] > 0x7fffffffLL)
-      return fail(entry, PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
-  if ((rc = check_prior_focal_length(entry, R, t->pair_images.data(), image_camera, prior_focal_length)) != PSFM_OK)
-    return rc;
-  Graph g;
-  g.num_images = t->num_images; g.R = R; g.K = t->num_keypoints; g.M = t->num_matches;
-  g.keypoint_ptr = reinterpret_cast<const int64_t*>(t->keypoint_ptr.data());
-  g.match_ptr = reinterpret_cast<const int64_t*>(t->match_ptr.data());
-  g.pair_images = t->pair_images.data();
-  g.table = t;
-  return verify_graph(entry, t0, launches0, g, image_camera, camera_size, o, config, F, E, H, inlier_ptr, inlier_matches,
-                      pair_trials, summary);
+  return guard("psfm_match_table_verify", [&]() -> int {
+    const auto t0 = std::chrono::steady_clock::now();
+    const long long launches0 = g_launch_count.load();
+    const char* entry = "psfm_match_table_verify";
+    if (!t) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    int rc = check_sizes(entry, t->num_images, num_cameras, t->num_pairs);
+    if (rc != PSFM_OK) return rc;
+    const int R = (int)t->num_pairs;
+    if ((t->num_images > 0 && !image_camera) || (num_cameras > 0 && !camera_size) ||
+        (R > 0 && (!config || !F || !E || !H)) || !inlier_ptr || (t->num_matches > 0 && !inlier_matches))
+      return fail(entry, PSFM_ERR_INVALID, "null argument");
+    psfm_verification_options o;
+    if ((rc = check_options(entry, opts, &o)) != PSFM_OK) return rc;
+    if ((rc = check_image_cameras(entry, t->num_images, image_camera, num_cameras)) != PSFM_OK) return rc;
+    if ((rc = check_camera_sizes(entry, num_cameras, camera_size)) != PSFM_OK) return rc;
+    for (int p = 0; p < R; ++p)
+      if (t->match_ptr[p + 1] - t->match_ptr[p] > 0x7fffffffLL)
+        return fail(entry, PSFM_ERR_UNSUPPORTED, "a pair with 2^31 or more matches");
+    if ((rc = check_prior_focal_length(entry, R, t->pair_images.data(), image_camera, prior_focal_length)) != PSFM_OK)
+      return rc;
+    Graph g;
+    g.num_images = t->num_images; g.R = R; g.K = t->num_keypoints; g.M = t->num_matches;
+    g.keypoint_ptr = reinterpret_cast<const int64_t*>(t->keypoint_ptr.data());
+    g.match_ptr = reinterpret_cast<const int64_t*>(t->match_ptr.data());
+    g.pair_images = t->pair_images.data();
+    g.table = t;
+    return verify_graph(entry, t0, launches0, g, image_camera, camera_size, o, config, F, E, H, inlier_ptr, inlier_matches,
+                        pair_trials, summary);
+  });
 }
 
 extern "C" int psfm_verification_local_model(int32_t kind, const float* points, int64_t n, const double* best,
                                              double max_squared_error, double* null_vector, double* normalization,
                                              double* local_model) {
   const char* entry = "psfm_verification_local_model";
-  if (!points || !best || !null_vector || !normalization || !local_model) return fail(entry, PSFM_ERR_INVALID, "null argument");
-  if (kind != kKindF && kind != kKindH) return fail(entry, PSFM_ERR_INVALID, "kind must be 0 (F) or 1 (H)");
-  if (n < 1 || n > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "needs 1 <= n < 2^31");
-  if (!(max_squared_error >= 0.0)) return fail(entry, PSFM_ERR_INVALID, "max_squared_error must be >= 0");
-  const int rc = require_device(entry);
-  if (rc != PSFM_OK) return rc;
-  try {
+  return guard(entry, [&]() -> int {
+    if (!points || !best || !null_vector || !normalization || !local_model) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (kind != kKindF && kind != kKindH) return fail(entry, PSFM_ERR_INVALID, "kind must be 0 (F) or 1 (H)");
+    if (n < 1 || n > 0x7fffffffLL) return fail(entry, PSFM_ERR_INVALID, "needs 1 <= n < 2^31");
+    if (!(max_squared_error >= 0.0)) return fail(entry, PSFM_ERR_INVALID, "max_squared_error must be >= 0");
+    const int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
     DBuf<float4> d_pts;
     DBuf<double> d_best, d_out;
     d_pts.alloc(n); d_best.alloc(9); d_out.alloc(24);
@@ -1023,5 +1023,5 @@ extern "C" int psfm_verification_local_model(int32_t kind, const float* points, 
     memcpy(normalization, out + 9, 6 * sizeof(double));
     memcpy(local_model, out + 15, 9 * sizeof(double));
     return PSFM_OK;
-  } catch (const CudaFail& f) { return f.code; }
+  });
 }
