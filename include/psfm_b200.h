@@ -917,7 +917,7 @@ int psfm_laplacian_solve(const double* A, const double* B, int32_t n, double* X)
 int psfm_spd_inverse(const double* A, int32_t n, double* X);
 
 /* Test entries of the small null-vector solvers of the geometry stages (csrc/dlt.cuh) and of the verification's local
-   step.  Each returns PSFM_OK, PSFM_ERR_INVALID on a bad argument (psfm_last_error says which), PSFM_ERR_NO_DEVICE
+   step, minimal estimators and cubic.  Each returns PSFM_OK, PSFM_ERR_INVALID on a bad argument (psfm_last_error says which), PSFM_ERR_NO_DEVICE
    without a device; argument checks come first.
    psfm_null_vectors: one solver per thread on `count` (1 .. 2^24) row-major N x N matrices A, its raw outputs in out:
      PSFM_NV_JACOBI_3, _4   one_sided_jacobi<N>: A V [N][N], then V [N][N]
@@ -929,7 +929,13 @@ int psfm_spd_inverse(const double* A, int32_t n, double* X);
      CTA, k_verify's code path) for kind 0 (eight-point F) or 1 (normalised DLT H) on the inliers of `best` [9]
      (residual <= max_squared_error) among n points [n][4] = (x1, y1, x2, y2).  null_vector [9]: the normalised
      solve's null vector (unit norm, any sign); normalization [6]: (s1, c1x, c1y, s2, c2x, c2y), T = [s 0 -s cx;
-     0 s -s cy; 0 0 1]; local_model [9]: the denormalised model that k_verify scores next (F after the rank-2 step). */
+     0 s -s cy; 0 0 1]; local_model [9]: the denormalised model that k_verify scores next (F after the rank-2 step).
+   psfm_verification_minimal: the verification's minimal estimators (k_verify's own functions), one sample per thread
+     on `count` (1 .. 2^24) samples of points [count][K][4] = (x1, y1, x2, y2).  Kind 0: seven_point on K = 7
+     correspondences, models [count][3][9] (F(2,2) = 1, ordered by (F00, F01, ...), zero rows past num_models[t] <= 3);
+     kind 1: homography_minimal (the normalised DLT) on K = 4, models [count][1][9], num_models[t] = 1.
+   psfm_verification_cubic: the seven-point step's cubic_real_roots on `count` (1 .. 2^24) coefficient rows
+     [count][4] = (c3, c2, c1, c0): roots [count][3] (zero past num_roots[t] <= 3). */
 #define PSFM_NV_JACOBI_3 0
 #define PSFM_NV_JACOBI_4 1
 #define PSFM_NV_DLT_POINT 2
@@ -940,6 +946,8 @@ int psfm_null_vectors(int32_t form, const double* A, int64_t count, double* out)
 int psfm_verification_local_model(int32_t kind, const float* points, int64_t n, const double* best,
                                   double max_squared_error, double* null_vector, double* normalization,
                                   double* local_model);
+int psfm_verification_minimal(int32_t kind, const float* points, int64_t count, double* models, int32_t* num_models);
+int psfm_verification_cubic(const double* coeffs, int64_t count, double* roots, int32_t* num_roots);
 
 /* ------------------------------------------------------------------------- */
 /* RAFT's correlation, lookup, upsampling and flow image on the device          */

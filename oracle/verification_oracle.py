@@ -12,7 +12,8 @@ or on an arbitrary basis, the same way on the device:
 * Sampler: each trial's sample is drawn from a SplitMix64 stream keyed by (random_seed, pair, kind, trial) (`sample`);
   the same distribution as COLMAP's RandomSampler, not the same draws.
 * The seven-point models come from the real roots of det(lambda a + b) = 0 for an orthonormal basis (a, b) of the
-  null space, solved in closed form (`cubic_real_roots`) with one Newton step; a model whose unit-norm form has
+  null space (of det(a + mu b) = 0 when its leading coefficient det(b) is the larger one), solved by `cubic_real_roots`
+  with one Newton step per root; a model whose unit-norm form has
   |F(2,2)| < 1e-10 is dropped; the others are scaled to F(2,2) = 1 and ordered by (F(0,0), F(0,1), ...).
 * Stored F and H have unit Frobenius norm with the largest-magnitude entry positive (the first one on a tie).
 Numpy's SVD stands where COLMAP uses Eigen's.  Every decision that rounding could flip records its margin
@@ -130,41 +131,76 @@ def _margin(margins, key, value):
 
 
 # ------------------------------------------------------------------------------------------------------- estimators
+def _newton_step(c3, c2, c1, c0, x):
+    """One Newton step, kept only when it lowers |p| (at a near-multiple root p' is rounding noise)."""
+    f = ((c3 * x + c2) * x + c1) * x + c0
+    df = (3.0 * c3 * x + 2.0 * c2) * x + c1
+    if df == 0.0:
+        return x
+    y = x - f / df
+    g = ((c3 * y + c2) * y + c1) * y + c0
+    return y if abs(g) < abs(f) else x
+
+
+def _stable_quadratic(a, b, c, d):
+    """The roots of a x^2 + b x + c (a != 0) for a discriminant d >= 0, without cancellation."""
+    h = -0.5 * (b + math.copysign(math.sqrt(d), b))
+    return [h / a, c / h if h != 0.0 else 0.0]
+
+
+def _quadratic_margin(margins, a, b, c, d):
+    if margins is not None:
+        scale = b * b + abs(4.0 * a * c)
+        _margin(margins, "cubic", abs(d) / scale if scale > 0 else 1.0)
+
+
 def cubic_real_roots(c3, c2, c1, c0, margins=None):
-    """Real roots of c3 x^3 + c2 x^2 + c1 x + c0 in closed form (Cardano / trigonometric), one Newton step each."""
+    """Real roots of c3 x^3 + c2 x^2 + c1 x + c0, one Newton step each.  One real root r from the depressed cubic's
+    closed form (Cardano with the two cube roots added without cancellation, or the trigonometric form's largest-magnitude
+    root); after its Newton step r is deflated out (from the constant term when it is the largest root, from the leading
+    term otherwise), and the quadratic left decides whether there are two more real roots and gives them in the stable
+    form.  The depressed form yields no other root: once c3 is small its shift -c2 / 3 c3 swamps the moderate roots.
+    margins["cubic"]: the relative discriminant of the quadratic that decides the count."""
+    c3, c2, c1, c0 = float(c3), float(c2), float(c1), float(c0)
     if c3 == 0.0:
         if c2 == 0.0:
             return [] if c1 == 0.0 else [-c0 / c1]
         d = c1 * c1 - 4.0 * c2 * c0
+        _quadratic_margin(margins, c2, c1, c0, d)
         if d < 0:
             return []
-        s = math.sqrt(d)
-        return [(-c1 + s) / (2.0 * c2), (-c1 - s) / (2.0 * c2)]
+        return _stable_quadratic(c2, c1, c0, d)
     b, c, d = c2 / c3, c1 / c3, c0 / c3
     p = c - b * b / 3.0
     q = 2.0 * b * b * b / 27.0 - b * c / 3.0 + d
     disc = (q / 2.0) * (q / 2.0) + (p / 3.0) * (p / 3.0) * (p / 3.0)
-    if margins is not None:
-        scale = (q / 2.0) * (q / 2.0) + abs(p / 3.0) ** 3
-        _margin(margins, "cubic", abs(disc) / scale if scale > 0 else 1.0)
     shift = -b / 3.0
+    r = shift
     if disc > 0:
-        s = math.sqrt(disc)
-        roots = [np.cbrt(-q / 2.0 + s) + np.cbrt(-q / 2.0 - s) + shift]
-    elif p == 0.0:
-        roots = [shift]
-    else:
-        r = 2.0 * math.sqrt(-p / 3.0)
+        A = -math.copysign(float(np.cbrt(abs(q) / 2.0 + math.sqrt(disc))), q)
+        r = (A - p / (3.0 * A) if A != 0.0 else 0.0) + shift
+    elif p != 0.0:
+        rr = 2.0 * math.sqrt(-p / 3.0)
         a = 3.0 * q / (2.0 * p) * math.sqrt(-3.0 / p)
         phi = math.acos(min(1.0, max(-1.0, a))) / 3.0
-        roots = [r * math.cos(phi - 2.0 * math.pi * k / 3.0) + shift for k in range(3)]
-    out = []
-    for x in roots:
-        x = float(x)
-        f = ((c3 * x + c2) * x + c1) * x + c0
-        df = (3.0 * c3 * x + 2.0 * c2) * x + c1
-        out.append(x - f / df if df != 0.0 else x)
-    return out
+        r = 0.0
+        for k in range(3):
+            t = rr * math.cos(phi - 2.0 * math.pi * k / 3.0) + shift
+            if abs(t) > abs(r):
+                r = t
+    r = _newton_step(c3, c2, c1, c0, r)
+    if r != 0.0 and abs(c3 * r * r * r) >= abs(c0):         # c3 x^2 + e1 x + e0 = p(x) / (x - r)
+        e0 = -c0 / r
+        e1 = (e0 - c1) / r
+    else:
+        e1 = c2 + c3 * r
+        e0 = c1 + e1 * r
+    dq = e1 * e1 - 4.0 * c3 * e0
+    _quadratic_margin(margins, c3, e1, e0, dq)
+    if dq < 0:
+        return [r]
+    x1, x2 = _stable_quadratic(c3, e1, e0, dq)
+    return [r, _newton_step(c3, c2, c1, c0, x1), _newton_step(c3, c2, c1, c0, x2)]
 
 
 def _det3(f):
@@ -183,9 +219,11 @@ def seven_point(x1, x2, margins=None):
     c3 = _det3(a)
     c2 = 0.5 * (d1 + dm) - d0
     c1 = 0.5 * (d1 - dm) - c3
+    # when |c3| < |d0| the pencil is solved as det(a + mu b), whose leading coefficient d0 is the larger one
+    flip = abs(c3) < abs(d0)
     models = []
-    for lam in cubic_real_roots(c3, c2, c1, d0, margins):
-        F = lam * a + b
+    for lam in (cubic_real_roots(d0, c1, c2, c3, margins) if flip else cubic_real_roots(c3, c2, c1, d0, margins)):
+        F = a + lam * b if flip else lam * a + b
         Fn = F / np.linalg.norm(F)
         if margins is not None:
             _margin(margins, "f22", abs(abs(Fn[8]) - RECALLED["min_f22"]) / RECALLED["min_f22"])

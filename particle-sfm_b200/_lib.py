@@ -34,7 +34,7 @@ EXPORTS = [
     "psfm_triangulator_default_options", "psfm_triangulation_create", "psfm_triangulation_result",
     "psfm_triangulation_destroy", "psfm_verification_default_options", "psfm_verify_two_view_geometries",
     "psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse",
-    "psfm_null_vectors", "psfm_verification_local_model",
+    "psfm_null_vectors", "psfm_verification_local_model", "psfm_verification_minimal", "psfm_verification_cubic",
     "psfm_convert_create", "psfm_convert_result", "psfm_convert_destroy",
     "psfm_colors_create", "psfm_colors_add_images", "psfm_colors_result", "psfm_colors_destroy",
     "psfm_corr_pyramids", "psfm_corr_pyramid_floats", "psfm_corr_lookup", "psfm_flow_upsample", "psfm_flow_to_image",
@@ -171,6 +171,8 @@ def lib():
     L.psfm_spd_inverse.argtypes = [dp, C.c_int32, dp]
     L.psfm_null_vectors.argtypes = [C.c_int32, dp, C.c_int64, dp]
     L.psfm_verification_local_model.argtypes = [C.c_int32, fp, C.c_int64, dp, C.c_double, dp, dp, dp]
+    L.psfm_verification_minimal.argtypes = [C.c_int32, fp, C.c_int64, dp, ip]
+    L.psfm_verification_cubic.argtypes = [dp, C.c_int64, dp, ip]
     L.psfm_convert_create.argtypes = [C.c_int32, ip, C.c_int32, dp, dp, ip, i64p, dp, ip, C.c_int64, dp, u8p, C.c_int64,
                                       C.POINTER(vp), i64p, ip, C.POINTER(_abi.ConvertSummary)]
     L.psfm_convert_result.argtypes = [vp, C.c_int32, C.c_int32, dp, u8p, C.POINTER(_abi.ConvertSummary)]

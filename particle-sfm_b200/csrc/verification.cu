@@ -9,7 +9,8 @@
 // Device (R pairs, M raw matches):
 //   gather   k_gather: each match's two keypoints as one float4 (x1, y1, x2, y2), 16 B per match
 //   verify   k_verify: one CTA per pair.  The leader thread draws each trial's sample and builds its models (the
-//            seven-point null space by Householder QR of A', never A'A; the cubic in closed form; the DLT likewise);
+//            seven-point null space by Householder QR of A', never A'A; the cubic by one closed-form root, deflation
+//            and the stable quadratic; the DLT likewise);
 //            the CTA scores all models of the sample in one sweep over the pair's matches (per-thread partials, then a
 //            fixed-order block reduction); the leader applies the support comparison, the dynamic trial bound and the
 //            stopping test in model order.  Local optimisation sweeps the best model's inliers for their moments and
@@ -168,9 +169,31 @@ __device__ __forceinline__ double det3(const double* f) {
   return f[0] * (f[4] * f[8] - f[5] * f[7]) - f[1] * (f[3] * f[8] - f[5] * f[6]) + f[2] * (f[3] * f[7] - f[4] * f[6]);
 }
 
-// real roots of c3 x^3 + c2 x^2 + c1 x + c0 in closed form, one Newton step each (oracle: cubic_real_roots)
+// one Newton step, kept only when it lowers |p|: at a near-multiple root p' is rounding noise and the step can jump far
+__device__ __forceinline__ double newton_step(double c3, double c2, double c1, double c0, double x) {
+  const double f = ((c3 * x + c2) * x + c1) * x + c0;
+  const double df = (3.0 * c3 * x + 2.0 * c2) * x + c1;
+  if (df == 0.0) return x;
+  const double y = x - f / df;
+  const double g = ((c3 * y + c2) * y + c1) * y + c0;
+  return fabs(g) < fabs(f) ? y : x;
+}
+
+// the roots of a x^2 + b x + c (a != 0) for a discriminant d >= 0: h = -(b + sign(b) sqrt(d)) / 2 adds magnitudes, so
+// neither h / a nor c / h cancels
+__device__ __forceinline__ void stable_quadratic(double a, double b, double c, double d, double* x) {
+  const double h = -0.5 * (b + copysign(sqrt(d), b));
+  x[0] = h / a;
+  x[1] = h != 0.0 ? c / h : 0.0;
+}
+
+// Real roots of c3 x^3 + c2 x^2 + c1 x + c0, one Newton step each (oracle: cubic_real_roots).  One real root r comes
+// from the depressed cubic's closed form: Cardano with the two cube roots added without cancellation, or the
+// trigonometric form's largest-magnitude root.  After its Newton step r is deflated out, from the constant term when it
+// is the largest root and from the leading term otherwise (the stable direction each way), and the quadratic left
+// decides whether there are two more real roots and gives them in the stable form.  The depressed form yields no other
+// root: once c3 is small its shift -c2 / 3 c3 swamps the moderate roots, and its discriminant cancels.
 __device__ int cubic_real_roots(double c3, double c2, double c1, double c0, double* x) {
-  int n = 0;
   if (c3 == 0.0) {
     if (c2 == 0.0) {
       if (c1 == 0.0) return 0;
@@ -179,8 +202,7 @@ __device__ int cubic_real_roots(double c3, double c2, double c1, double c0, doub
     }
     const double d = c1 * c1 - 4.0 * c2 * c0;
     if (d < 0.0) return 0;
-    const double s = sqrt(d);
-    x[0] = (-c1 + s) / (2.0 * c2); x[1] = (-c1 - s) / (2.0 * c2);
+    stable_quadratic(c2, c1, c0, d, x);
     return 2;
   }
   const double b = c2 / c3, c = c1 / c3, d = c0 / c3;
@@ -188,23 +210,33 @@ __device__ int cubic_real_roots(double c3, double c2, double c1, double c0, doub
   const double q = 2.0 * b * b * b / 27.0 - b * c / 3.0 + d;
   const double disc = (q / 2.0) * (q / 2.0) + (p / 3.0) * (p / 3.0) * (p / 3.0);
   const double shift = -b / 3.0;
+  double r = shift;
   if (disc > 0.0) {
-    const double s = sqrt(disc);
-    x[n++] = cbrt(-q / 2.0 + s) + cbrt(-q / 2.0 - s) + shift;
-  } else if (p == 0.0) {
-    x[n++] = shift;
-  } else {
-    const double r = 2.0 * sqrt(-p / 3.0);
+    const double A = -copysign(cbrt(fabs(q) / 2.0 + sqrt(disc)), q);
+    r = (A != 0.0 ? A - p / (3.0 * A) : 0.0) + shift;
+  } else if (p != 0.0) {
+    const double rr = 2.0 * sqrt(-p / 3.0);
     const double a = 3.0 * q / (2.0 * p) * sqrt(-3.0 / p);
     const double phi = acos(fmin(1.0, fmax(-1.0, a))) / 3.0;
-    for (int k = 0; k < 3; ++k) x[n++] = r * cos(phi - 2.0 * M_PI * k / 3.0) + shift;
+    r = 0.0;
+    for (int k = 0; k < 3; ++k) {
+      const double t = rr * cos(phi - 2.0 * M_PI * k / 3.0) + shift;
+      if (fabs(t) > fabs(r)) r = t;
+    }
   }
-  for (int i = 0; i < n; ++i) {
-    const double f = ((c3 * x[i] + c2) * x[i] + c1) * x[i] + c0;
-    const double df = (3.0 * c3 * x[i] + 2.0 * c2) * x[i] + c1;
-    if (df != 0.0) x[i] -= f / df;
-  }
-  return n;
+  r = newton_step(c3, c2, c1, c0, r);
+  x[0] = r;
+  // c3 x^2 + e1 x + e0 = p(x) / (x - r); r is the largest root when |c3 r^3| >= |c0| = |c3 r r1 r2|
+  const bool backward = r != 0.0 && fabs(c3 * r * r * r) >= fabs(c0);
+  double e1, e0;
+  if (backward) { e0 = -c0 / r; e1 = (e0 - c1) / r; }
+  else { e1 = c2 + c3 * r; e0 = c1 + e1 * r; }
+  const double dq = e1 * e1 - 4.0 * c3 * e0;
+  if (dq < 0.0) return 1;
+  stable_quadratic(c3, e1, e0, dq, x + 1);
+  x[1] = newton_step(c3, c2, c1, c0, x[1]);
+  x[2] = newton_step(c3, c2, c1, c0, x[2]);
+  return 3;
 }
 
 __device__ bool lex_less(const double* u, const double* v) {
@@ -232,12 +264,15 @@ __device__ __noinline__ int seven_point(const float4* p, double (*models)[9]) {
   const double d0 = det3(b), d1 = det3(t1), dm = det3(tm), c3 = det3(a);
   const double c2 = 0.5 * (d1 + dm) - d0;
   const double c1 = 0.5 * (d1 - dm) - c3;
+  // det(lam a + b) = c3 lam^3 + c2 lam^2 + c1 lam + d0; when |c3| < |d0| the pencil is solved as det(a + mu b) =
+  // d0 mu^3 + c1 mu^2 + c2 mu + c3 instead, whose leading coefficient is the larger one (mu = 0 is F = a, lam = inf)
+  const bool flip = fabs(c3) < fabs(d0);
   double lam[3];
-  const int nr = cubic_real_roots(c3, c2, c1, d0, lam);
+  const int nr = flip ? cubic_real_roots(d0, c1, c2, c3, lam) : cubic_real_roots(c3, c2, c1, d0, lam);
   int nm = 0;
   for (int r = 0; r < nr; ++r) {
     double F[9], nrm = 0.0;
-    for (int i = 0; i < 9; ++i) { F[i] = lam[r] * a[i] + b[i]; nrm += F[i] * F[i]; }
+    for (int i = 0; i < 9; ++i) { F[i] = flip ? a[i] + lam[r] * b[i] : lam[r] * a[i] + b[i]; nrm += F[i] * F[i]; }
     if (fabs(F[8] / sqrt(nrm)) < kMinF22) continue;
     const double s = F[8];
     for (int i = 0; i < 9; ++i) F[i] /= s;
@@ -746,6 +781,36 @@ __global__ void __launch_bounds__(kThreads) k_local_model(const float4* __restri
   if (threadIdx.x < 6) out[9 + threadIdx.x] = s.lnorm[threadIdx.x];
 }
 
+// psfm_verification_minimal / psfm_verification_cubic: one sample (one cubic) per thread through the functions
+// k_verify calls
+constexpr int kMinimalBlock = 128;
+
+template <int KIND>
+__global__ void __launch_bounds__(kMinimalBlock) k_minimal(const float4* __restrict__ pts, long long count,
+                                                           double* __restrict__ models, int* __restrict__ num_models) {
+  const long long t = blockIdx.x * (long long)kMinimalBlock + threadIdx.x;
+  if (t >= count) return;
+  constexpr int K = KIND == kKindF ? kSevenPointSamples : kHomographySamples;
+  float4 p[K];
+  for (int i = 0; i < K; ++i) p[i] = pts[K * t + i];
+  double m[3][9];
+  const int nm = KIND == kKindF ? seven_point(p, m) : homography_minimal(p, m[0]);
+  constexpr int NM = KIND == kKindF ? 3 : 1;
+  for (int k = 0; k < NM; ++k)
+    for (int i = 0; i < 9; ++i) models[(NM * t + k) * 9 + i] = k < nm ? m[k][i] : 0.0;
+  num_models[t] = nm;
+}
+
+__global__ void __launch_bounds__(kMinimalBlock) k_cubic(const double* __restrict__ coeffs, long long count,
+                                                         double* __restrict__ roots, int* __restrict__ num_roots) {
+  const long long t = blockIdx.x * (long long)kMinimalBlock + threadIdx.x;
+  if (t >= count) return;
+  const double* c = coeffs + 4 * t;
+  double x[3] = {0.0, 0.0, 0.0};
+  num_roots[t] = cubic_real_roots(c[0], c[1], c[2], c[3], x);
+  for (int i = 0; i < 3; ++i) roots[3 * t + i] = x[i];
+}
+
 }  // namespace
 
 extern "C" void psfm_verification_default_options(psfm_verification_options* o) {
@@ -1022,6 +1087,50 @@ extern "C" int psfm_verification_local_model(int32_t kind, const float* points, 
     memcpy(null_vector, out, 9 * sizeof(double));
     memcpy(normalization, out + 9, 6 * sizeof(double));
     memcpy(local_model, out + 15, 9 * sizeof(double));
+    return PSFM_OK;
+  });
+}
+
+extern "C" int psfm_verification_minimal(int32_t kind, const float* points, int64_t count, double* models,
+                                         int32_t* num_models) {
+  const char* entry = "psfm_verification_minimal";
+  return guard(entry, [&]() -> int {
+    if (!points || !models || !num_models) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (kind != kKindF && kind != kKindH) return fail(entry, PSFM_ERR_INVALID, "kind must be 0 (F) or 1 (H)");
+    if (count < 1 || count > (1LL << 24)) return fail(entry, PSFM_ERR_INVALID, "needs 1 <= count <= 2^24");
+    const int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
+    const long long k = kind == kKindF ? kSevenPointSamples : kHomographySamples, nm = kind == kKindF ? 3 : 1;
+    DBuf<float4> d_pts;
+    DBuf<double> d_models;
+    DBuf<int> d_num;
+    d_pts.alloc(k * count); d_models.alloc(9 * nm * count); d_num.alloc(count);
+    d_pts.upload(reinterpret_cast<const float4*>(points), k * count, nullptr);
+    const unsigned grid = (unsigned)((count + kMinimalBlock - 1) / kMinimalBlock);
+    if (kind == kKindF) k_minimal<kKindF><<<grid, kMinimalBlock>>>(d_pts.p, count, d_models.p, d_num.p);
+    else k_minimal<kKindH><<<grid, kMinimalBlock>>>(d_pts.p, count, d_models.p, d_num.p);
+    PSFM_LAUNCH_CHECK();
+    PSFM_CUDA(cudaMemcpy(models, d_models.p, sizeof(double) * 9 * nm * count, cudaMemcpyDeviceToHost));
+    PSFM_CUDA(cudaMemcpy(num_models, d_num.p, sizeof(int) * count, cudaMemcpyDeviceToHost));
+    return PSFM_OK;
+  });
+}
+
+extern "C" int psfm_verification_cubic(const double* coeffs, int64_t count, double* roots, int32_t* num_roots) {
+  const char* entry = "psfm_verification_cubic";
+  return guard(entry, [&]() -> int {
+    if (!coeffs || !roots || !num_roots) return fail(entry, PSFM_ERR_INVALID, "null argument");
+    if (count < 1 || count > (1LL << 24)) return fail(entry, PSFM_ERR_INVALID, "needs 1 <= count <= 2^24");
+    const int rc = require_device(entry);
+    if (rc != PSFM_OK) return rc;
+    DBuf<double> d_c, d_x;
+    DBuf<int> d_n;
+    d_c.alloc(4 * count); d_x.alloc(3 * count); d_n.alloc(count);
+    d_c.upload(coeffs, 4 * count, nullptr);
+    k_cubic<<<(unsigned)((count + kMinimalBlock - 1) / kMinimalBlock), kMinimalBlock>>>(d_c.p, count, d_x.p, d_n.p);
+    PSFM_LAUNCH_CHECK();
+    PSFM_CUDA(cudaMemcpy(roots, d_x.p, sizeof(double) * 3 * count, cudaMemcpyDeviceToHost));
+    PSFM_CUDA(cudaMemcpy(num_roots, d_n.p, sizeof(int) * count, cudaMemcpyDeviceToHost));
     return PSFM_OK;
   });
 }

@@ -147,17 +147,23 @@ def test_no_cpu_fallback_of_the_initialisation_ops():
 
 def _null_vector_entries(form=0, A=np.eye(3), count=1, kind=0, n=8, best=np.eye(3).reshape(9), thr=16.0,
                          points=np.zeros((8, 4), np.float32), out=True, only=None):
-    """The two null-vector test entries on the same kind of arguments: (name, status, psfm_last_error).  The outputs
-    are sized for one good call; a call with more is refused before it reads or writes anything."""
+    """The null-vector and minimal-solver test entries on the same kind of arguments: (name, status,
+    psfm_last_error).  The outputs are sized for one good call; a call with more is refused before it reads or writes
+    anything."""
     L = _lib.lib()
     o = np.zeros(171) if out else None
     v, T, m = (np.zeros(9), np.zeros(6), np.zeros(9)) if out else (None, None, None)
+    nums = np.zeros(1, np.int32)
+    num = nums.ctypes.data_as(C.POINTER(C.c_int32)) if out else None
     pts = None if points is None else points.ctypes.data_as(C.POINTER(C.c_float))
     res = []
     for name, call in (("psfm_null_vectors", lambda: L.psfm_null_vectors(form, _lib.dptr(A), count, _lib.dptr(o))),
                        ("psfm_verification_local_model",
                         lambda: L.psfm_verification_local_model(kind, pts, n, _lib.dptr(best), thr, _lib.dptr(v),
-                                                                _lib.dptr(T), _lib.dptr(m)))):
+                                                                _lib.dptr(T), _lib.dptr(m))),
+                       ("psfm_verification_minimal",
+                        lambda: L.psfm_verification_minimal(kind, pts, count, _lib.dptr(o), num)),
+                       ("psfm_verification_cubic", lambda: L.psfm_verification_cubic(_lib.dptr(A), count, _lib.dptr(o), num))):
         if only is None or name in only:
             rc = call()
             res.append((name, rc, L.psfm_last_error().decode()))
@@ -165,14 +171,18 @@ def _null_vector_entries(form=0, A=np.eye(3), count=1, kind=0, n=8, best=np.eye(
 
 
 NULL_VECTOR_BAD = {
-    "null_input": (dict(A=None, points=None), {"psfm_null_vectors", "psfm_verification_local_model"}),
-    "null_output": (dict(out=False), {"psfm_null_vectors", "psfm_verification_local_model"}),
+    "null_input": (dict(A=None, points=None), {"psfm_null_vectors", "psfm_verification_local_model",
+                                               "psfm_verification_minimal", "psfm_verification_cubic"}),
+    "null_output": (dict(out=False), {"psfm_null_vectors", "psfm_verification_local_model", "psfm_verification_minimal",
+                                      "psfm_verification_cubic"}),
     "null_best": (dict(best=None), {"psfm_verification_local_model"}),
     "form_negative": (dict(form=-1), {"psfm_null_vectors"}),
     "form_unknown": (dict(form=6), {"psfm_null_vectors"}),
-    "count0": (dict(count=0), {"psfm_null_vectors"}),
-    "count_above_2e24": (dict(count=(1 << 24) + 1), {"psfm_null_vectors"}),
-    "kind_watermark": (dict(kind=2), {"psfm_verification_local_model"}),
+    "count0": (dict(count=0), {"psfm_null_vectors", "psfm_verification_minimal", "psfm_verification_cubic"}),
+    "count_above_2e24": (dict(count=(1 << 24) + 1), {"psfm_null_vectors", "psfm_verification_minimal",
+                                                      "psfm_verification_cubic"}),
+    "kind_negative": (dict(kind=-1), {"psfm_verification_local_model", "psfm_verification_minimal"}),
+    "kind_watermark": (dict(kind=2), {"psfm_verification_local_model", "psfm_verification_minimal"}),
     "n0": (dict(n=0), {"psfm_verification_local_model"}),
     "n2e31": (dict(n=1 << 31), {"psfm_verification_local_model"}),
     "threshold_negative": (dict(thr=-1.0), {"psfm_verification_local_model"}),

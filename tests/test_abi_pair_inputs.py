@@ -224,7 +224,8 @@ def _no_device_calls():
     })
     for name in ("psfm_blocked_cholesky_solve", "psfm_laplacian_solve", "psfm_spd_inverse"):
         calls[name] = lambda n=name: _dense_chol_entries(np.eye(4), np.ones(4), 4, 4, 4, 0, only={n})[0][1:]
-    for name in ("psfm_null_vectors", "psfm_verification_local_model"):
+    for name in ("psfm_null_vectors", "psfm_verification_local_model", "psfm_verification_minimal",
+                 "psfm_verification_cubic"):
         calls[name] = lambda n=name: _null_vector_entries(only={n})[0][1:]
     return calls
 
@@ -232,7 +233,8 @@ def _no_device_calls():
 NO_DEVICE_ENTRIES = list(STAGES) + ["psfm_ba_solve", "psfm_traj_optimize", "psfm_known_rotation_translations",
                                     "psfm_triangulate_tracks", "psfm_matches_create", "psfm_tracker_create",
                                     "psfm_convert_create", "psfm_blocked_cholesky_solve", "psfm_laplacian_solve",
-                                    "psfm_spd_inverse", "psfm_null_vectors", "psfm_verification_local_model"]
+                                    "psfm_spd_inverse", "psfm_null_vectors", "psfm_verification_local_model",
+                                    "psfm_verification_minimal", "psfm_verification_cubic"]
 
 
 @pytest.mark.skipif(device_count() > 0, reason="checks the refusal without a device")
